@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native LZ4 block codec (see BASELINE.json).
+"""bench.py -- headline benchmark of the H100-native LZ4 block codec (see BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 The metric is "GB/s uncompressed (encode+decode) on batched 64 KiB blocks": a STEP is one
@@ -18,7 +18,7 @@ the barrier and the max-over-ranks time reduction).
 The JSON line carries, beyond the base contract:
   decode / encode  device-timed throughput of each direction (CUDA events around the launches)
   roofline         the decode step (the kernel the north_star target names): algorithmic bytes
-                   (compressed read + raw written) / CUDA-event time vs the measured HBM peak;
+                   (compressed read + raw written) / CUDA-event time vs the HBM peak;
                    roofline.encode is the same for the encoder (the kernel that dominates the step)
   e2e              the same step through the C-ABI calls with HOST (pinned) buffers: H2D and D2H
                    inside the timed region; e2e.decode / e2e.encode split it
@@ -28,6 +28,10 @@ The JSON line carries, beyond the base contract:
 `--impl reference` times the reference's own CPU implementation (oracle/_ref: the upstream C
 engine the C# code is a port of and is tested bit-identical against; else the oracle port) with
 all host threads on the SAME config; it never loads libk4lz4.
+
+`--dump-outputs DIR` (impl ours, rank 0) writes what the last timed step returned to its caller, as
+float32 .npy files: the per-block result lengths of both passes in full, and the bytes of a fixed,
+seeded sample of DUMP_BLOCKS blocks (compressed bytes padded with -1 up to the slot size; decoded bytes).
 """
 from __future__ import annotations
 
@@ -56,6 +60,8 @@ SEED = 1234
 CHUNK_BLOCKS = 1024             # generator streams are 64 MiB long
 METRIC = "GB/s uncompressed (encode+decode) on batched 64KiB blocks @1/2/4/8 GPU vs CPU ref"
 ALL_CPUS = os.sched_getaffinity(0)     # before any NUMA binding
+DUMP_BLOCKS = 64                # --dump-outputs: 64 x (64 KiB + slot) as float32 = 34 MB with the length arrays
+DUMP_SEED = 20240607
 
 
 # ---- pure helpers (unit-tested on CPU, tests/test_host_logic.py) --------------------------------
@@ -94,7 +100,7 @@ def workload_config(blocks_per_gpu: int) -> dict:
         "generator": "reference datagen RDG_genBuffer(matchProba 0.63 decode / 0.55 encode, litProba 0, "
                      "seed 1234 + chunk) in 64 MiB chunks, cut into 64 KiB blocks",
         "compressed_layout": "decode input tightly packed + int64 offsets; encode output in compressBound slots",
-        "l2": "each pass touches > 6 GB >> 126 MB L2; no flush needed",
+        "l2": "each pass touches > 6 GB >> 50 MB L2; no flush needed",
     }
 
 
@@ -103,16 +109,33 @@ def measured_peak_gbs() -> tuple[float, str]:
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
-def profiled_traffic() -> dict | None:
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of every kernel of the step, from the
-    committed `ncu --set full` capture of this command (profiles/traffic.json); None if absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        return None
+def dump_sample(n_blocks: int) -> np.ndarray:
+    """The fixed block indices whose bytes --dump-outputs writes (same for every run with the same --blocks)."""
+    k = min(DUMP_BLOCKS, n_blocks)
+    return np.sort(np.random.default_rng(DUMP_SEED).choice(n_blocks, size=k, replace=False))
+
+
+def dump_outputs(out_dir: str, slots, enc_len, out, out_len, n_blocks: int) -> None:
+    """Writes the last timed step's results (device tensors) as float32 .npy files under out_dir."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    idx = torch.from_numpy(dump_sample(n_blocks)).to(slots.device)
+    el = enc_len.to(torch.int64)
+    enc = slots.view(n_blocks, BOUND)[idx].to(torch.float32)
+    pos = torch.arange(BOUND, device=slots.device).unsqueeze(0)
+    enc[pos >= el[idx].unsqueeze(1)] = -1.0                   # bytes past the returned length are not output
+    arrays = {
+        "encode_len": enc_len.to(torch.float32),
+        "encode_bytes_sample": enc,
+        "decode_len": out_len.to(torch.float32),
+        "decode_bytes_sample": out.view(n_blocks, BLOCK)[idx].to(torch.float32),
+        "sample_blocks": idx.to(torch.float64),
+    }
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy())
 
 
 def gen_blocks(n_blocks: int, match_proba: float, first_block: int, out: np.ndarray | None = None) -> np.ndarray:
@@ -468,6 +491,8 @@ def run_ours(args) -> None:
         e0.record(); encode_pass(); e1.record(); decode_pass(); e2.record()
     torch.cuda.synchronize()
     launches = L.k4lz4_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, slots, enc_len, out, out_len, nb)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
@@ -498,7 +523,6 @@ def run_ours(args) -> None:
     algo_enc = enc_bytes + nb * BLOCK
     ach_dec = algo_dec / (dec_ms_mean / 1e3) / 1e9
     ach_enc = algo_enc / (enc_ms_mean / 1e3) / 1e9
-    traffic = profiled_traffic()
 
     # ---- e2e: the same step through the C ABI with HOST (pinned) buffers ----
     e2e_steps = max(1, min(args.steps, 3))
@@ -652,8 +676,6 @@ def run_ours(args) -> None:
                        "ratio": round(ratio_enc, 4)},
             "roofline": {"bound": "hbm", "kernel": "k4::decode_tile_kernel (+ its two near-empty follow-up launches): the decode pass",
                          "achieved": round(ach_dec, 1), "peak": peak, "unit": "GB/s", "frac": round(ach_dec / peak, 4),
-                         "traffic": (traffic or {}).get("decode_bytes_per_launch"),
-                         "traffic_split": (traffic or {}).get("decode_split"),
                          "algorithmic_bytes_per_launch": algo_dec, "kernel_ms": round(dec_ms_mean, 4),
                          "read_only_frac": round(comp_bytes / (dec_ms_mean / 1e3) / 1e9 / peak, 4),
                          "peak_source": peak_src,
@@ -661,7 +683,6 @@ def run_ours(args) -> None:
                                         "encode": round(sum(enc_ms) / (sum(dec_ms) + sum(enc_ms)), 4)},
                          "encode": {"kernel": "k4::encode kernel: the encode pass (dominates the step by time)",
                                     "achieved": round(ach_enc, 1), "frac": round(ach_enc / peak, 4),
-                                    "traffic": (traffic or {}).get("encode_bytes_per_launch"),
                                     "algorithmic_bytes_per_launch": algo_enc, "kernel_ms": round(enc_ms_mean, 4)}},
             "e2e": e2e,
             "gpu_launches": int(launches),
@@ -691,7 +712,11 @@ def main():
                          "runs on rank 0 whenever more than one GPU is visible)")
     ap.add_argument("--lib", default=None, help="development only: another build of libk4lz4.so (A/B runs of kernel variants)")
     ap.add_argument("--no-aux", action="store_true", help="development only: skip the aux legs (pickler, all-devices call)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs (lengths, seeded sample of block bytes) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference_arm(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * k4lz4.h -- C ABI of libk4lz4: a B200-native (sm_100a CUDA) LZ4 *block* codec that is a
+ * k4lz4.h -- C ABI of libk4lz4: an H100-native (sm_90a CUDA) LZ4 *block* codec that is a
  * drop-in for ONE hot path of K4os.Compression.LZ4:
  *     LZ4Codec.Encode(..., LZ4Level.L00_FAST)   LZ4Codec.Decode(...)   LZ4Pickler.Pickle/Unpickle
  * over batches of independent blocks.  Plain C: pointers and sizes only.

@@ -1,4 +1,4 @@
-"""k4os.compression.lz4_b200 -- B200-native (sm_100a CUDA) drop-in for one hot path of
+"""k4os.compression.lz4_b200 -- H100-native (sm_90a CUDA) drop-in for one hot path of
 K4os.Compression.LZ4: ``LZ4Codec.Encode`` at ``L00_FAST``, ``LZ4Codec.Decode`` and
 ``LZ4Pickler.Pickle/Unpickle`` over batches of independent blocks (plus ``Decode`` with a
 dictionary, ``PartialDecode`` and the independent-block ``LZ4BlockEncoder`` / ``LZ4BlockDecoder``

@@ -1,4 +1,4 @@
-// decode_tile.cuh -- the batched LZ4 block decoder for B200: ONE kernel, ONE CTA per block.
+// decode_tile.cuh -- the batched LZ4 block decoder for H100: ONE kernel, ONE CTA per block.
 //
 // A CTA (512 threads) owns one block.  Everything a block needs lives in shared memory: the
 // compressed stream (pulled in by one TMA bulk copy), the 64 KiB output tile (left through one
@@ -155,8 +155,8 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 // ---- shared memory by 32-bit shared-space address -----------------------------------------------
 // Every hot access goes through these: with generic pointers into the dynamic shared array nvcc
 // re-materialises the shared-window base (S2R SR_CgaCtaId, MOV, LEA, IADD) in front of EVERY
-// predicated byte access -- measured: 4-5 extra instructions per byte moved, 210 K warp instructions
-// per block instead of ~50 K (profiles/ncu_r02_*).  A shared address computed once costs nothing.
+// predicated byte access (4-5 extra instructions per byte moved in the SASS).  A shared address
+// computed once costs nothing.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t lds8(uint32_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ uint32_t lds16(uint32_t a) { uint32_t v; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
@@ -263,7 +263,7 @@ __device__ __forceinline__ int jt_hop(const uint32_t sJ, const uint32_t sStg, co
 // first token position >= end and ORs `bad`.  The only serial dependency is table byte -> next position
 // -> table byte: the loads that give a sequence's decoded size are issued BEHIND the next table load and
 // consumed one hop later, so a hop costs one shared-memory round trip (the kernel keeps the LSU queue
-// busy: a dependent load takes hundreds of cycles there, profiles/ncu_r02b_*).
+// busy: a dependent load can take hundreds of cycles there).
 template <class F>
 __device__ __forceinline__ int jt_walk(const uint32_t sJ, const uint32_t sStg, int p, const int end, const int n,
                                        uint32_t& bad, F f) {

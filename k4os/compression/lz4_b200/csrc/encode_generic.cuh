@@ -26,7 +26,7 @@ constexpr int ENC_TAG_BYTES = K4_ENC_TAGS ? 8192 : 0;   // one filter byte per u
 constexpr int ENC_SLOT_BYTES = ENC_TABLE_BYTES + ENC_TAG_BYTES;   // shared memory per warp
 // the global-table encoder warps (encode_tile.cuh) filter their candidate reads by a tag: see TAGMODE there
 #ifndef K4_ENC_GTAG
-#define K4_ENC_GTAG 2        // measured: 39.4 -> 40.6 GB/s on configs[2] (32-bit slots: position | 16-bit tag)
+#define K4_ENC_GTAG 2        // 32-bit slots: position | 16-bit tag
 #endif
 constexpr int ENC_GTAG = K4_ENC_GTAG;
 constexpr int ENC_GSLOT_BYTES = ENC_GTAG == 2 ? 2 * ENC_TABLE_BYTES : (ENC_GTAG ? ENC_TABLE_BYTES + ENC_TABLE_BYTES / 2 : ENC_TABLE_BYTES);
@@ -230,7 +230,7 @@ constexpr int ENC_WARPS_PER_CTA = K4_ENC_TAGS ? 9 : 7;   // pickle_kernel: 2 CTA
 #define K4_ENC_SM_WARPS 8       // shared-memory tables: 8 x (16 KiB + 1 KiB the hardware reserves per CTA); the rest of the 256 KiB stays L1
 #endif
 #ifndef K4_ENC_GM_WARPS
-#define K4_ENC_GM_WARPS 22      // global-memory tables (sweep in DESIGN.md 4.2)
+#define K4_ENC_GM_WARPS 22      // global-memory tables (H100 sweep in DESIGN.md 7.2)
 #endif
 constexpr int ENC_SM_WARPS = K4_ENC_SM_WARPS;
 constexpr int ENC_GM_WARPS = K4_ENC_GM_WARPS;

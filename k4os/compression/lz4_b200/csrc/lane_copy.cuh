@@ -3,8 +3,7 @@
 // Every lane of a warp owns one short run (a literal run or a match of at most LC_MAX bytes) at
 // arbitrary byte alignment on both sides.  Copying it byte by byte costs one load and one store
 // instruction (and one shared-memory wavefront each) per byte of the LONGEST run of the warp; the
-// shared-memory pipe and the issue slots are what the tile decoder runs out of
-// (profiles/ncu_r02b_decode_summary.txt).  Here a lane copies
+// shared-memory pipe and the issue slots are what the tile decoder runs out of.  Here a lane copies
 //     up to 3 head bytes until its destination is word aligned,
 //     whole destination words, each built from two aligned source words by a funnel shift,
 //     up to 3 tail bytes,

@@ -9,21 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
 def port():
     import oracle
     return oracle.Port()
-
-
-@pytest.fixture(scope="session")
-def ref():
-    import oracle
-    if not oracle.have_ref():
-        pytest.skip("oracle/_ref/libk4ref.so not built (reference absent)")
-    return oracle.Ref()
 
 
 @pytest.fixture(scope="session")

@@ -13,6 +13,9 @@
    produced -- like the reference's own rows (playground/SharedSources/app.cpp:94-97) -- by the
    upstream C engine orig/lib/lz4.c compiled as-is (oracle/_ref/libk4ref.so), including
    limited-output capacities and the expected return codes.
+3. ref_digests.json: for each differential test of tests/test_oracle.py, the SHA-256 of the reference
+   engine's results over that test's cases; the tests compare the restatement with it where
+   oracle/_ref is not built.
 """
 import base64
 import hashlib
@@ -78,6 +81,25 @@ def main():
                "lz4_version": R.version(), "rows": rows},
               open(os.path.join(HERE, "encode_rows.json"), "w"), indent=0)
     print(len(rows), "encode rows; issue64 ok")
+
+    # 3. ref_digests.json: one digest per differential test of tests/test_oracle.py over the reference
+    # engine's results, so that those tests also run where oracle/_ref cannot be built
+    from tests import test_oracle as T
+    digests = {}
+
+    def record(name, port, results_of):
+        digests[name] = T._digest(results_of(R))
+    T._pin, saved = record, T._pin
+    try:
+        port = oracle.Port()
+        for fn in (T.test_port_equals_reference_engine, T.test_malformed_decode_matches_reference_engine,
+                   T.test_datagen_port_matches_reference_generator, T.test_dictionary_decode_matches_reference_engine,
+                   T.test_partial_decode_matches_reference_engine, T.test_xxh32_restatement_matches_upstream):
+            fn(port)
+    finally:
+        T._pin = saved
+    json.dump(digests, open(os.path.join(HERE, "ref_digests.json"), "w"), indent=1, sort_keys=True)
+    print(len(digests), "reference digests")
 
 
 if __name__ == "__main__":

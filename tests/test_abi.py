@@ -56,6 +56,18 @@ def test_synth_host_is_deterministic(native):
     assert not np.array_equal(a[:4096], a[4096:8192])
 
 
+def test_library_holds_sm90a_code_only(native):
+    """The shipped library is Hopper code: an sm_90a cubin, no other architecture."""
+    import subprocess
+    from k4os.compression.lz4_b200 import _native, build
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    cuobjdump = os.path.join(os.path.dirname(nvcc), "cuobjdump")
+    out = subprocess.run([cuobjdump, "--list-elf", _native.SO_PATH], capture_output=True, text=True, check=True).stdout
+    archs = set(re.findall(r"\.(sm_\w+)\.cubin", out))
+    assert archs == {"sm_90a"}, out
+    assert "arch=compute_90a,code=sm_90a" in build.NVCC_FLAGS
+
+
 def test_product_never_imports_oracle():
     """The product package must not reference oracle/ (checked textually over its sources)."""
     pkg = os.path.join(ROOT, "k4os")

@@ -54,6 +54,32 @@ def test_shard_ranges_cover_everything():
             assert max(sizes) - min(sizes) <= 1
 
 
+def test_bench_dump_outputs_format(tmp_path):
+    """--dump-outputs: float .npy files, a sample fixed by the seed, bytes past a returned length masked,
+    at most 64 MB at the default batch size."""
+    import torch
+    sys.path.insert(0, ROOT)
+    import bench
+    nb = 100
+    assert np.array_equal(bench.dump_sample(nb), bench.dump_sample(nb)) and len(bench.dump_sample(nb)) == bench.DUMP_BLOCKS
+    slots = torch.randint(0, 256, (nb * bench.BOUND,), dtype=torch.uint8)
+    enc_len = torch.randint(1, bench.BOUND, (nb,), dtype=torch.int32)
+    out = torch.randint(0, 256, (nb * bench.BLOCK,), dtype=torch.uint8)
+    out_len = torch.full((nb,), bench.BLOCK, dtype=torch.int32)
+    bench.dump_outputs(str(tmp_path), slots, enc_len, out, out_len, nb)
+    files = {p.stem: np.load(p) for p in tmp_path.glob("*.npy")}
+    assert set(files) == {"encode_len", "encode_bytes_sample", "decode_len", "decode_bytes_sample", "sample_blocks"}
+    assert all(a.dtype in (np.float32, np.float64) for a in files.values())
+    idx = files["sample_blocks"].astype(np.int64)
+    assert np.array_equal(idx, bench.dump_sample(nb))
+    for row, b in zip(files["encode_bytes_sample"], idx):
+        n = int(enc_len[b])
+        assert np.array_equal(row[:n], slots.view(nb, bench.BOUND)[b, :n].numpy()) and (row[n:] == -1).all()
+    assert np.array_equal(files["decode_bytes_sample"], out.view(nb, bench.BLOCK)[idx].numpy())
+    full = bench.BLOCKS_PER_GPU
+    assert 4 * (2 * full + bench.DUMP_BLOCKS * (bench.BOUND + bench.BLOCK)) + 8 * bench.DUMP_BLOCKS <= 64 << 20
+
+
 def test_two_rank_gloo_sharding_and_timing_reduce():
     """world_size 2 on CPU (gloo): the N>1 plumbing of bench.py -- shard, max-over-ranks
     timing reduce, sum of units -- without touching a GPU."""
