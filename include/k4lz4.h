@@ -226,6 +226,13 @@ K4LZ4_API int64_t k4lz4_launch_count(void);
  * Synchronises the device.  Diagnostics only (tests assert that clean data stays on the tile path). */
 K4LZ4_API int32_t k4lz4_decode_stats(int32_t device, uint64_t *out4, int32_t reset);
 
+/* Encoder path counters of `device` since the last reset: out4[0] blocks encoded by a warp with its
+ * hash table in shared memory, [1] by a warp with its table in global memory (only launched when a
+ * call has more blocks than the shared-memory warps take in one round), [2] blocks of >= 65 547
+ * bytes (the u32-table engine, either warp kind), [3] 0.  Empty blocks are not counted.
+ * Synchronises the device.  Diagnostics only. */
+K4LZ4_API int32_t k4lz4_encode_stats(int32_t device, uint64_t *out4, int32_t reset);
+
 #ifdef __cplusplus
 }
 #endif

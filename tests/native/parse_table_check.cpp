@@ -29,8 +29,12 @@ Seq ref_seq(const uint8_t* s, int n, int p) {
 // [4] first failing position + 1 (0 = none), [5] wrong lanes of a simulated speculative parse, [6] lanes
 extern "C" int jt_check(const uint8_t* stream, int n, int shift, int fill, int seg, int warm, long long* stats) {
     std::vector<uint8_t> stage((size_t)shift + n + 64, (uint8_t)fill);
+    if (fill > 255) {        // pseudo-random bytes seeded by `fill`: the big-stage kernel sees the previous block's bytes
+        uint32_t x = (uint32_t)fill * 2654435761u;
+        for (auto& b : stage) { x = x * 1664525u + 1013904223u; b = (uint8_t)(x >> 24); }
+    }
     memcpy(stage.data() + shift, stream, (size_t)n);
-    const uint8_t* s = stage.data() + shift;                 // s[p] = stream byte p; bytes at >= n are `fill`
+    const uint8_t* s = stage.data() + shift;                 // s[p] = stream byte p; bytes at >= n (and < 0) are `fill`
     std::vector<uint8_t> J((size_t)shift + n + 64, 0);
     auto ld8 = [&](int q) -> uint32_t { return s[q]; };
     const int nWords = (shift + n + 3) >> 2;

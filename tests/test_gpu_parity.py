@@ -381,9 +381,10 @@ def test_tile_path_with_oversized_capacity(k4):
 
 def test_decode_paths_cover_every_engine(k4):
     """Incompressible blocks (compressed size > 65535 / > the small stage), a block of more than
-    16384 sequences and a multi-megabyte length-byte run all take their designated engine and agree
-    with the oracle."""
+    16384 sequences (valid under a large capacity; only the exact decoder takes it) and multi-megabyte
+    length-byte runs all take their designated engine and agree with the oracle."""
     import oracle
+    from tests import lz4_blocks as LB
     port = oracle.Port()
     rnd = inputs.gen("random", 65536, 1)                                   # -> 65 794 compressed bytes: generic
     mid = inputs.gen("random", 45000, 2) + inputs.gen("repeat", 20536, 7)  # ~45 KB compressed: big stage
@@ -394,6 +395,10 @@ def test_decode_paths_cover_every_engine(k4):
     caps.append(65536)
     streams.append(b"\x0F" + b"\x01\x00" + b"\xFF" * (9 << 20) + b"\x00" + b"\x50abcde")
     caps.append(65536)
+    dense, _ = LB.dense_block(17000, np.random.default_rng(9), term=5)    # 17 000 sequences, 68 002 bytes
+    assert LB.tile_route(dense, 80000).n_seq > LB.DT_NMAX
+    streams.append(dense)
+    caps.append(80000)
     k4.batch.decode_stats(0, reset=True)
     dec, dl = k4.batch.decode_batch_host(streams, caps)
     st = k4.batch.decode_stats(0, reset=True)
@@ -402,7 +407,8 @@ def test_decode_paths_cover_every_engine(k4):
         assert int(dl[i]) == r, (i, int(dl[i]), r)
         if r > 0:
             assert dec[i] == ref
-    assert st["generic"] >= 3 and st["tile_big"] == 1, st
+    assert int(dl[-1]) == 68002
+    assert st["generic"] == 4 and st["tile_big"] == 1 and st["tile"] == 0, st
 
 
 def test_dictionary_decode_gpu(k4):

@@ -1,7 +1,8 @@
 """CPU test of the decoder's jump table (csrc/parse_table.cuh): the SAME header the CUDA kernel uses is
 compiled for the host and compared, position by position, with a strict restatement of the block format's
 length decoding -- on valid streams (oracle encoder), mutated streams and random bytes, at every stage
-alignment, with 0x00 / 0xFF behind the end of the stream."""
+alignment, with 0x00 / 0xFF or random bytes (what the big-stage kernel leaves from the previous block) behind
+the end of the stream."""
 import ctypes as C
 import os
 import subprocess
@@ -55,7 +56,7 @@ def test_table_matches_format_on_valid_streams(chk):
     tot = np.zeros(8, dtype=np.int64)
     for s in _streams():
         for shift in (0, 1, 2, 3, 7, 15):
-            for fill in (0x00, 0xFF):
+            for fill in (0x00, 0xFF, 0x100 + shift):            # > 255: pseudo-random bytes seeded by it
                 fails, st = chk(s, shift, fill)
                 assert fails == 0, (len(s), shift, fill, int(st[4]) - 1)
                 tot += st
@@ -72,13 +73,13 @@ def test_table_on_mutated_and_random_streams(chk):
         s = bytearray(base[it % len(base)][: int(rng.integers(20, 6000))])
         for _ in range(int(rng.integers(1, 12))):
             s[int(rng.integers(0, len(s)))] = int(rng.choice([0, 15, 0xF0, 0xFF, 0xEF, 0xFE, int(rng.integers(0, 256))]))
-        fails, st = chk(bytes(s), int(rng.integers(0, 16)), int(rng.choice([0, 0xFF, 0xF0])))
+        fails, st = chk(bytes(s), int(rng.integers(0, 16)), int(rng.choice([0, 0xFF, 0xF0, 0x100 + it])))
         assert fails == 0, (it, int(st[4]) - 1)
         n_checked += int(st[0])
     for it in range(100):
         p = rng.choice([0.02, 0.2, 0.5])
         s = np.where(rng.random(3000) < p, 0xFF, rng.integers(0, 256, 3000)).astype(np.uint8).tobytes()
-        fails, st = chk(s, it % 16, 0xFF)
+        fails, st = chk(s, it % 16, 0xFF if it % 2 else 0x1000 + it)
         assert fails == 0, (it, int(st[4]) - 1)
     assert n_checked > 100_000
 
