@@ -49,6 +49,10 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_partial_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* targetLen,
             int* outLen, int nBlocks, int memKind, void* cudaStream, int device);
+        // LZ4ChainDecoder.DecodeBlock over many streams, one block each (prefix mode of LZ4_decompress_safe_continue)
+        [DllImport(Lib)] public static extern int k4lz4_decode_chain_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* prefixLen, int* outLen, int nBlocks, int memKind, void* cudaStream, int device);
         // LL.Enforce32 semantics (LL.tools.cs:29-36) for inputs >= 65 547 bytes
         [DllImport(Lib)] public static extern int k4lz4_encode_x32(byte* src, int srcLen, byte* dst, int dstCap, int level);
         [DllImport(Lib)] public static extern int k4lz4_encode_batch_x32(

@@ -141,6 +141,26 @@ K4LZ4_API int32_t k4lz4_partial_decode_batch(const uint8_t *srcBase, const int64
                                              int32_t *outLen, int32_t nBlocks,
                                              int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- chained (linked) blocks: LZ4ChainDecoder, one block per stream per call ------------------ */
+
+/* LZ4ChainDecoder.Decode -> LLxx.LZ4_decompress_safe_continue in prefix mode
+ * (LZ4ChainDecoder.cs:45-61,142-143; LL64.dec.cs:479-498,558-592).
+ * Block i decodes srcBase[srcOff[i] .. +srcLen[i]) to dstBase[dstOff[i] .. +dstCap[i]); the
+ * prefixLen[i] bytes directly in front of it, dstBase[dstOff[i]-prefixLen[i] .. dstOff[i]), are the
+ * stream's history (what the reference keeps as lz4sd->prefixSize).  Values >= 65535 all mean
+ * "withPrefix64k"; only the last 65535 bytes are ever read.  History bytes are read, never written.
+ * outLen[i] = bytes decoded, or -1 where LZ4ChainDecoder.Decode would throw (decoded < 0).
+ * Like memcpy's buffers, the blocks of one call must not overlap: no block's
+ * [dstOff - prefixLen, dstOff + dstCap) may overlap another block's destination in the same call (one
+ * block per stream per call meets this).  Clean blocks of at most 64 KiB output take the shared-memory
+ * tile kernel; the rest the exact warp-per-block engine.  memKind == K4LZ4_MEM_HOST stages each block's
+ * history in front of its device slot and runs on one GPU (`device`, K4LZ4_ALL_DEVICES = GPU 0).
+ * A negative prefixLen is K4LZ4_E_ARG with host memory, outLen = -1 with device memory. */
+K4LZ4_API int32_t k4lz4_decode_chain_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           const int32_t *prefixLen, int32_t *outLen, int32_t nBlocks,
+                                           int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- XXH32: the checksum of the LZ4 Frame container (SURVEY 8f row 2) ------------------------ */
 
 /* XXH32 of one buffer on the host (frame header byte, serial content checksum) --

@@ -260,6 +260,32 @@ def decode_dict_batch_host(blocks: Sequence, caps: Sequence[int], dicts: Sequenc
     return [dst[doff[i]:doff[i] + max(int(out[i]), 0)].tobytes() for i in range(n)], out
 
 
+def decode_chain_batch_host(src: np.ndarray, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, prefix_len,
+                            device: int = 0) -> np.ndarray:
+    """LZ4ChainDecoder's block decode over a batch of streams (k4lz4_decode_chain_batch, host memory).
+    Block i decodes into dst[dst_off[i] .. + dst_cap[i]); the prefix_len[i] bytes in front of it are its
+    stream's history (LZ4_decompress_safe_continue in prefix mode).  No two blocks' [dst_off - prefix_len,
+    dst_off + dst_cap) may overlap another block's destination.  Returns int32 results: bytes decoded or -1."""
+    src_off, dst_off = _i64(src_off), _i64(dst_off)
+    src_len, dst_cap, prefix_len = _i32(src_len), _i32(dst_cap), _i32(prefix_len)
+    n = int(src_len.shape[0])
+    out = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_decode_chain_batch(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
+                                             dst.ctypes.data, dst_off.ctypes.data, dst_cap.ctypes.data,
+                                             prefix_len.ctypes.data, out.ctypes.data, n, N.MEM_HOST, None,
+                                             int(device)))
+    return out
+
+
+def decode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int,
+                              dst_off_ptr: int, dst_cap_ptr: int, prefix_len_ptr: int, out_len_ptr: int, n: int,
+                              stream: int = 0, device: int = -1) -> None:
+    """Device-pointer form of decode_chain_batch_host: only enqueues the kernels on `stream`."""
+    N.check(N.lib().k4lz4_decode_chain_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
+                                             prefix_len_ptr, out_len_ptr, int(n), N.MEM_DEVICE, stream or None,
+                                             int(device)))
+
+
 def partial_decode_batch_host(blocks: Sequence, targets: Sequence[int], device: int = 0):
     """LZ4Codec.PartialDecode over a batch (k4lz4_partial_decode_batch, host memory)."""
     src, so, sl = _pack(blocks)

@@ -115,10 +115,13 @@ __device__ __forceinline__ void warp_copy_match_window(uint8_t* dst, int64_t op,
 // The general form of decode_block_warp: external dictionary (LZ4_decompress_safe_usingDict,
 // LL64.dec.cs:523-546 -> forceExtDict :510-521; the prefix variants read the same bytes and reject
 // the same offsets) and/or partial decoding (LZ4_decompress_safe_partial :548-556 with
-// dstCapacity == targetOutputSize, LLxx.cs:29-39; paths :256-280, :301-307, :387-406).
+// dstCapacity == targetOutputSize, LLxx.cs:29-39; paths :256-280, :301-307, :387-406), or prefix mode:
+// `prefix` bytes of history lie directly in front of dst (LZ4_decompress_safe_withSmallPrefix /
+// _withPrefix64k, LL64.dec.cs:479-498, as LZ4_decompress_safe_continue calls them :558-592): lowPrefix =
+// dst - prefix, dictSize = 0; prefix >= 65535 is withPrefix64k, whose shortcut test (:213) no offset fails.
 __device__ int decode_block_warp_general(const uint8_t* __restrict__ src, int n, uint8_t* __restrict__ dst,
                                          int outputSize, bool partial,
-                                         const uint8_t* __restrict__ dict, int dictSize) {
+                                         const uint8_t* __restrict__ dict, int dictSize, int prefix = 0) {
     const int lane = lane_id();
     int64_t ip = 0, op = 0;
     const int64_t iend = n, oend = outputSize;
@@ -126,6 +129,7 @@ __device__ int decode_block_warp_general(const uint8_t* __restrict__ src, int n,
     const bool checkOffset = dictSize < 65536;                       // :147
     const bool extDict = dict != nullptr && dictSize > 0;
     if (!extDict) dictSize = 0;
+    const int64_t lowPrefix = extDict ? 0 : -(int64_t)(prefix < 65535 ? prefix : 65535);   // relative to dst
 
     if (outputSize == 0) {                                           // :162-168
         if (partial) return 0;
@@ -170,7 +174,7 @@ __device__ int decode_block_warp_general(const uint8_t* __restrict__ src, int n,
         const int64_t match = op - offset;
         len = token & 15;
 
-        if (shortcut && len != 15 && offset >= 8 && match >= 0) {    // :211-220 (match >= lowPrefix == dst)
+        if (shortcut && len != 15 && offset >= 8 && match >= lowPrefix) {   // :211-220
             len += MINMATCH;
             warp_copy_match(dst, op, match, (int)len, offset, lane);
             op += len;
@@ -185,8 +189,8 @@ __device__ int decode_block_warp_general(const uint8_t* __restrict__ src, int n,
             }
         }
         len += MINMATCH;
-        if (checkOffset && match + dictSize < 0) return -1;          // :338
-        if (match < 0) {
+        if (checkOffset && match + dictSize < lowPrefix) return -1;  // :338
+        if (match < lowPrefix) {
             if (!extDict) return -1;                                  // (unreachable with checkOffset on)
             if (op + len > oend - LASTLITERALS) {                     // :343-347
                 if (partial) len = (oend - op) < len ? (oend - op) : len;

@@ -361,13 +361,36 @@ __device__ __forceinline__ void lanes_copy(const uint32_t d, const uint32_t s, c
     if (ovl) for (int j = 0; j < len; j++) sts8(d + j, lds8(s + j));
 }
 
+// ---- copies from the stream's history (global memory in front of the block's destination) ---------
+// Same shapes as lanes_copy / warp_copy, source in global memory: the history of a chained block is read
+// where it lies (at most 64 KiB per stream, read-only during the call), never staged.
+__device__ __forceinline__ void lanes_copy_hist(const uint32_t d, const uint8_t* __restrict__ s, const int len) {
+    const int top = __reduce_max_sync(FULL, len);
+    for (int base = 0; base < top; base += 8) {
+        const int left = len - base;
+        uint32_t v[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) if (j < left) v[j] = __ldg(s + base + j);
+#pragma unroll
+        for (int j = 0; j < 8; j++) if (j < left) sts8(d + base + j, v[j]);
+    }
+}
+__device__ __forceinline__ void warp_copy_hist(const uint32_t d, const uint8_t* __restrict__ s, const int len, const int lane) {
+    for (int i = lane; i < len; i += 32) sts8(d + (uint32_t)i, __ldg(s + i));
+}
+
 // ---- the tile decoder ---------------------------------------------------------------------------
 // All DT_THREADS threads of the CTA call it with the same arguments.  Requires 1 <= n <= DT_MAX_SRC,
-// (src & 15) + n + 16 <= STAGE, cap >= 1.  Returns the decoded size (> 0) after the bytes have been
-// written to gdst, or -1 -- nothing written -- when the block has to go to the exact decoder.
+// (src & 15) + n + 16 <= STAGE, cap >= 1, 0 <= P <= 65535.  Returns the decoded size (> 0) after the
+// bytes have been written to gdst, or -1 -- nothing written -- when the block has to go to the exact decoder.
+// P is the length of the stream's history, gdst[-P .. 0) (prefix mode of LZ4_decompress_safe_continue,
+// LL64.dec.cs:479-498: lowPrefix = dst - P; 65535 stands for every P >= 65535, withPrefix64k).  A match
+// whose source starts before the block is split the way the reference splits an external-dictionary match
+// (LL64.dec.cs:359-374): the history part is copied from global memory in the far phase, the remainder is
+// a match at d' = off with source 0 and is scheduled like any other.  With P = 0 nothing changes.
 template <int STAGE>
 __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__ src, const int n,
-                                 uint8_t* __restrict__ gdst, const int cap, uint32_t& barParity) {
+                                 uint8_t* __restrict__ gdst, const int cap, const int P, uint32_t& barParity) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int shift = (int)(reinterpret_cast<uintptr_t>(src) & 15);
     uint8_t* const stg = S.stage + shift;                       // stg[p] == src[p]
@@ -527,14 +550,20 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
                 if (!(fl & SQ_LAST) || op + lit > cap) bad = true;
             } else {
                 if ((fl & SQ_LAST) || litPos + lit > n - 8 || op + lit > cap - MFLIMIT) bad = true;   // :247
-                if (off == 0 || off > op + lit || op + lit + ml > cap - LASTLITERALS) bad = true;     // :338, :427-433
+                if (off == 0 || off > op + lit + P || op + lit + ml > cap - LASTLITERALS) bad = true;   // :338, :427-433
             }
             if (bad) { lit = 0; ml = 0; }
         }
         DT_PROF(5);
 
+        // history part of a match whose source starts before the block: hl bytes from gdst + d - off
+        int d = op + lit;                                        // match destination
+        const int hl = P > 0 && off > d ? (off - d < ml ? off - d : ml) : 0;
+        const int hd = d;
+        d += hl;                                                 // the remainder: at d = off, source 0
+        ml -= hl;
+
         // classification of the match
-        const int d = op + lit;                                  // match destination
         const int a = d - off;                                   // match source
         const int srcEnd = a + ml < d ? a + ml : d;              // bytes read from outside the match itself: [a, srcEnd)
         const bool nearM = ml > 0 && srcEnd > Sr;
@@ -545,6 +574,16 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
         for (unsigned m = __ballot_sync(FULL, lit > DT_LSHORT); m; m &= m - 1) {
             const int l = __ffs(m) - 1;
             warp_copy(sT + (uint32_t)__shfl_sync(FULL, op, l), sStg + (uint32_t)__shfl_sync(FULL, litPos, l), __shfl_sync(FULL, lit, l), lane);
+        }
+        if (P > 0) {
+            // history parts: nothing else of this step reads or writes [hd, hd + hl) before barrier #1, and a
+            // near remainder that reads it (off < its length) runs behind that barrier
+            lanes_copy_hist(sT + (uint32_t)hd, gdst + (hd - off), hl <= DT_LSHORT ? hl : 0);
+            for (unsigned m = __ballot_sync(FULL, hl > DT_LSHORT); m; m &= m - 1) {
+                const int l = __ffs(m) - 1;
+                const int ld = __shfl_sync(FULL, hd, l);
+                warp_copy_hist(sT + (uint32_t)ld, gdst + (ld - __shfl_sync(FULL, off, l)), __shfl_sync(FULL, hl, l), lane);
+            }
         }
         DT_PROF(6);
 #if K4_DT_LATEBAR
@@ -694,17 +733,36 @@ __device__ __forceinline__ bool decode_trivial(int n, int cap, int32_t* outLen) 
     return false;
 }
 
+// LZ4ChainDecoder.Decode has no LZ4Codec post-processing: the engine's own special cases (LL64.dec.cs:162-172)
+__device__ __forceinline__ int chain_trivial(int n, int cap, const uint8_t* src) {
+    if (n <= 0 || cap < 0) return -1;
+    return (n == 1 && src[0] == 0) ? 0 : -1;                       // cap == 0
+}
+// the block's history length (prefix mode); every value >= 65535 reads the same bytes (withPrefix64k)
+__device__ __forceinline__ int chain_prefix(const int32_t* prefixLen, int b) {
+    if (!prefixLen) return 0;
+    const int p = prefixLen[b];
+    return p < 65535 ? p : 65535;
+}
+
 // launch 1: one CTA per block, small stage, two CTAs per SM
 __global__ void __launch_bounds__(DT_THREADS, 2)
 decode_tile_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
                    const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
                    const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                   int32_t* __restrict__ outLen, DecodeLists wl) {
+                   const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TileSmem<STAGE_SMALL>& S = *reinterpret_cast<TileSmem<STAGE_SMALL>*>(smem_raw);
     const int b = blockIdx.x;
     const int n = srcLen[b], cap = dstCap[b];
-    if (n <= 0 || cap <= 0) { if (threadIdx.x == 0) decode_trivial(n, cap, &outLen[b]); return; }
+    const int P = chain_prefix(prefixLen, b);
+    if (n <= 0 || cap <= 0 || P < 0) {
+        if (threadIdx.x == 0) {
+            if (!prefixLen) decode_trivial(n, cap, &outLen[b]);
+            else outLen[b] = P < 0 ? -1 : chain_trivial(n, cap, srcBase + srcOff[b]);
+        }
+        return;
+    }
     const uint8_t* src = srcBase + srcOff[b];
     const int shift = (int)(reinterpret_cast<uintptr_t>(src) & 15);
     if (n > DT_MAX_SRC) { if (threadIdx.x == 0) wl_push(wl.gen, &wl.counts[1], (uint32_t)b); return; }
@@ -712,7 +770,7 @@ decode_tile_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);
     __syncthreads();
     uint32_t parity = 0;
-    const int r = tile_decode_block<STAGE_SMALL>(S, src, n, dstBase + dstOff[b], cap, parity);
+    const int r = tile_decode_block<STAGE_SMALL>(S, src, n, dstBase + dstOff[b], cap, P, parity);
     if (threadIdx.x == 0) {
         if (r > 0) { outLen[b] = r; atomicAdd(&g_decode_stats[0], 1ull); }
         else wl_push(wl.gen, &wl.counts[1], (uint32_t)b);
@@ -724,7 +782,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1)
 decode_tile_big_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
                        const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                       int32_t* __restrict__ outLen, DecodeLists wl) {
+                       const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TileSmem<STAGE_BIG>& S = *reinterpret_cast<TileSmem<STAGE_BIG>*>(smem_raw);
     const uint32_t count = wl.counts[0];
@@ -735,7 +793,8 @@ decode_tile_big_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __res
     for (uint32_t e = blockIdx.x; e < count; e += gridDim.x) {
         const int b = (int)wl.big[e];
         const uint8_t* src = srcBase + srcOff[b];
-        const int r = tile_decode_block<STAGE_BIG>(S, src, srcLen[b], dstBase + dstOff[b], dstCap[b], parity);
+        const int r = tile_decode_block<STAGE_BIG>(S, src, srcLen[b], dstBase + dstOff[b], dstCap[b],
+                                                   chain_prefix(prefixLen, b), parity);
         if (threadIdx.x == 0) {
             if (r > 0) { outLen[b] = r; atomicAdd(&g_decode_stats[1], 1ull); }
             else wl_push(wl.gen, &wl.counts[1], (uint32_t)b);
@@ -749,12 +808,18 @@ __global__ void __launch_bounds__(128)
 decode_rest_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
                    const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
                    const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                   int32_t* __restrict__ outLen, DecodeLists wl) {
+                   const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
     const uint32_t count = wl.counts[1];
     const uint32_t nwarps = gridDim.x * (blockDim.x >> 5);
     for (uint32_t e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < count; e += nwarps) {
         const int b = (int)wl.gen[e];
-        const int r = codec_decode_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b]);
+        int r;
+        if (!prefixLen) r = codec_decode_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b]);
+        else {                                   // LZ4_decompress_safe_continue in prefix mode, raw engine result
+            r = decode_block_warp_general(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b], false,
+                                          nullptr, 0, chain_prefix(prefixLen, b));
+            r = r < 0 ? -1 : r;
+        }
         if (lane_id() == 0) { outLen[b] = r; atomicAdd(&g_decode_stats[2], 1ull); }
     }
 }
@@ -802,11 +867,14 @@ inline DecodeDev* decode_dev(int dev) {
     return d;
 }
 
-// Enqueues the decode of n blocks on `st` (current device).  Returns the number of kernels
-// launched, or -1 with *err set.
+// Enqueues the decode of n blocks on `st` (current device).  prefixLen (device array, may be null:
+// independent blocks) gives each block's history length, the bytes in front of its destination; with it the
+// results are those of LZ4_decompress_safe_continue in prefix mode (bytes decoded or -1).  Returns the
+// number of kernels launched, or -1 with *err set.
 inline int decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                          uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
-                         int32_t* outLen, int n, cudaStream_t st, cudaError_t* err) {
+                         int32_t* outLen, int n, cudaStream_t st, cudaError_t* err,
+                         const int32_t* prefixLen = nullptr) {
     int dev = 0;
     cudaGetDevice(&dev);
     DecodeDev* D = decode_dev(dev);
@@ -821,13 +889,14 @@ inline int decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const in
     e = cudaMemsetAsync(wl.counts, 0, 4 * sizeof(uint32_t), st);
     if (e == cudaSuccess) {
         decode_tile_kernel<<<n, DT_THREADS, sizeof(TileSmem<STAGE_SMALL>), st>>>(
-            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, wl);
+            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
         const int gridBig = n < D->sms ? n : D->sms;
         decode_tile_big_kernel<<<gridBig, DT_THREADS, sizeof(TileSmem<STAGE_BIG>), st>>>(
-            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, wl);
+            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
         const int want = (n + 3) / 4;
         const int gridRest = want < D->sms * 8 ? want : D->sms * 8;
-        decode_rest_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, wl);
+        decode_rest_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen,
+                                                      outLen, wl);
         e = cudaGetLastError();
     }
     cudaFreeAsync(scratch, st);

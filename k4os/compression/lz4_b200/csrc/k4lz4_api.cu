@@ -771,6 +771,100 @@ int run_general(const GeneralArgs& g, int memKind, void* stream, int device) {
     return K4LZ4_OK;
 }
 
+// ---- chained blocks (LZ4ChainDecoder): tile path with a history window, simple host staging ---------
+
+struct ChainArgs {
+    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
+    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap; const int32_t* prefixLen;
+    int32_t* outLen; int32_t n;
+};
+
+int launch_chain(const ChainArgs& c, cudaStream_t st) {
+    cudaError_t de = cudaSuccess;
+    const int nl = k4::decode_launch(c.srcBase, c.srcOff, c.srcLen, c.dstBase, c.dstOff, c.dstCap, c.outLen, c.n,
+                                     st, &de, c.prefixLen);
+    if (nl < 0) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain decode launch failed: %s", cudaGetErrorString(de)); }
+    g_launches += nl;
+    CU_TRY(cudaGetLastError());
+    return K4LZ4_OK;
+}
+
+// host pointers: per chunk, every block's history (its last <= 65535 bytes: all the decoder reads) is staged
+// directly in front of its device slot; one H2D per array, one decode, one D2H, exact scatter
+int run_chain_host(const ChainArgs& c, int device) {
+    const int ndev = device_count_cached();
+    if (ndev <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
+    const int dev = device >= 0 ? device : 0;
+    if (dev >= ndev) return fail(K4LZ4_E_ARG, "device %d out of range (%d visible)", dev, ndev);
+    DeviceGuard guard(dev);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
+    const int64_t CH = 256ll << 20;
+    auto hist = [&](int64_t i) { return (int64_t)std::min<int32_t>(c.prefixLen[i], 65535); };
+    int64_t i = 0;
+    while (i < c.n) {
+        int64_t j = i, bytes = 0;
+        while (j < c.n) {
+            const int64_t add = std::max<int32_t>(c.srcLen[j], 0) + std::max<int32_t>(c.dstCap[j], 0) + hist(j) + 16;
+            if (j > i && bytes + add > CH) break;
+            bytes += add; j++;
+        }
+        const int64_t nb = j - i;
+        std::vector<int64_t> so(nb), doff(nb);
+        std::vector<int32_t> sl(nb), dc(nb), pl(nb), res(nb);
+        int64_t sTot = 0, dTot = 0;
+        for (int64_t k = 0; k < nb; k++) {
+            sl[k] = c.srcLen[i + k]; dc[k] = c.dstCap[i + k]; pl[k] = (int32_t)hist(i + k);
+            so[k] = sTot; sTot += std::max<int32_t>(sl[k], 0);
+            doff[k] = (dTot + pl[k] + 15) & ~int64_t(15);           // slot = [history | destination], 16-aligned
+            dTot = doff[k] + std::max<int32_t>(dc[k], 0);
+        }
+        std::vector<uint8_t> hs((size_t)sTot + 16), hd((size_t)dTot + 16);
+        for (int64_t k = 0; k < nb; k++) {
+            if (sl[k] > 0) memcpy(hs.data() + so[k], c.srcBase + c.srcOff[i + k], (size_t)sl[k]);
+            if (pl[k] > 0) memcpy(hd.data() + doff[k] - pl[k], c.dstBase + c.dstOff[i + k] - pl[k], (size_t)pl[k]);
+        }
+        DevMem dS, dO, dM;
+        CU_TRY(dS.alloc((size_t)sTot + 16)); CU_TRY(dO.alloc((size_t)dTot + 16));
+        CU_TRY(dM.alloc((size_t)nb * (8 * 2 + 4 * 4)));
+        int64_t* mSo = (int64_t*)dM.p; int64_t* mDo = mSo + nb;
+        int32_t* mSl = (int32_t*)(mDo + nb); int32_t* mDc = mSl + nb; int32_t* mPl = mDc + nb; int32_t* mRes = mPl + nb;
+        CU_TRY(cudaMemcpy(dS.p, hs.data(), (size_t)sTot, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(dO.p, hd.data(), (size_t)dTot, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(mSo, so.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(mDo, doff.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(mSl, sl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(mDc, dc.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(mPl, pl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
+        ChainArgs d{(const uint8_t*)dS.p, mSo, mSl, (uint8_t*)dO.p, mDo, mDc, mPl, mRes, (int32_t)nb};
+        const int rc = launch_chain(d, nullptr);
+        if (rc != K4LZ4_OK) return rc;
+        CU_TRY(cudaMemcpy(res.data(), mRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
+        CU_TRY(cudaMemcpy(hd.data(), dO.p, (size_t)dTot, cudaMemcpyDeviceToHost));
+        for (int64_t k = 0; k < nb; k++) {
+            c.outLen[i + k] = res[k];
+            if (res[k] > 0) memcpy(c.dstBase + c.dstOff[i + k], hd.data() + doff[k], (size_t)res[k]);
+        }
+        i = j;
+    }
+    return K4LZ4_OK;
+}
+
+int run_chain(const ChainArgs& c, int memKind, void* stream, int device) {
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (c.n < 0) return fail(K4LZ4_E_ARG, "negative block count");
+    if (c.n > 0 && (!c.srcBase || !c.srcOff || !c.srcLen || !c.dstBase || !c.dstOff || !c.dstCap || !c.prefixLen || !c.outLen))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST)                   // device arrays cannot be checked here: there a negative prefix gives -1
+        for (int32_t i = 0; i < c.n; i++)
+            if (c.prefixLen[i] < 0) return fail(K4LZ4_E_ARG, "negative prefix length at block %d", i);
+    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
+    if (c.n == 0) return K4LZ4_OK;
+    if (memKind == K4LZ4_MEM_HOST) return run_chain_host(c, device);
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    return launch_chain(c, (cudaStream_t)stream);
+}
+
 }  // namespace
 
 // ---- exported C ABI ------------------------------------------------------------------------
@@ -870,6 +964,14 @@ int32_t k4lz4_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, c
                                 int32_t device) {
     GeneralArgs g{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, dictBase, dictOff, dictLen, outLen, nBlocks, false};
     return run_general(g, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                 const int32_t* prefixLen, int32_t* outLen, int32_t nBlocks,
+                                 int32_t memKind, void* cudaStream, int32_t device) {
+    ChainArgs c{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, nBlocks};
+    return run_chain(c, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_partial_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,

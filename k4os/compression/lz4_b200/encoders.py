@@ -9,16 +9,21 @@ list of compressed blocks and decodes them with ONE `k4lz4_decode_batch` call.  
 and return value equal what the reference's per-block call produces (independent blocks: no
 dictionary, fresh table per block -- LZ4BlockEncoder.cs:18-23).  Chained encoders (dependent
 blocks) stay with the managed engine: they are not data parallel.
+
+`LZ4ChainDecoder` (Encoders/LZ4ChainDecoder.cs) decodes dependent blocks.  One stream's blocks are serial, but
+the blocks of MANY streams are not: `LZ4ChainDecoder.DecodeMany` advances many decoders by one block each with
+ONE `k4lz4_decode_chain_batch` call.
 """
 from __future__ import annotations
 
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_batch_host, encode_batch_flat_host
 from .codec import LZ4Codec, LZ4Level
 
 K1 = 1024
+K64 = 65536
 
 
 def _round_up(v: int, step: int) -> int:      # Mem.RoundUp
@@ -243,3 +248,166 @@ class LZ4BlockDecoder:
     def _check(self) -> None:
         if self._disposed:
             raise RuntimeError("ObjectDisposedException")
+
+
+class LZ4ChainDecoder:
+    """LZ4ChainDecoder(blockSize, extraBlocks) -- LZ4ChainDecoder.cs:26-36: the same ring buffer of
+    64 KiB + (1 + extraBlocks) * blockSize + 32 bytes, the same CopyDict / ApplyDict bookkeeping, and the
+    prefix size LZ4_streamDecode_t would hold (LL64.dec.cs:558-592; the reference's decoder only ever takes
+    the prefix branches of LZ4_decompress_safe_continue, so the end of the prefix is always the write
+    position).  Decoding runs on the GPU; DecodeMany advances many decoders with one call."""
+
+    def __init__(self, blockSize: int = 65536, extraBlocks: int = 0):
+        self._block = _round_up(max(int(blockSize), K1), K1)
+        extra = max(int(extraBlocks), 0)
+        self._out_len = K64 + (1 + extra) * self._block + 32
+        self._out = np.zeros(self._out_len + 8, dtype=np.uint8)
+        self._index = 0
+        self._prefix = 0                  # lz4sd->prefixSize
+        self._disposed = False
+
+    @property
+    def BlockSize(self) -> int:
+        return self._block
+
+    @property
+    def BytesReady(self) -> int:
+        return self._index
+
+    @property
+    def PrefixSize(self) -> int:
+        """The history length the next Decode passes to the GPU (LZ4_streamDecode_t.prefixSize)."""
+        return self._prefix
+
+    def Decode(self, source, blockSize: int = 0) -> int:
+        """LZ4ChainDecoder.cs:45-61: decodes one block behind the previous output; returns its length."""
+        return LZ4ChainDecoder.DecodeMany([self], [(source, blockSize)])[0]
+
+    @staticmethod
+    def DecodeMany(decoders, blocks, device: int = 0) -> list:
+        """Decode() on every decoder at once: decoders[i] decodes blocks[i] (compressed bytes, or a tuple
+        (bytes, blockSize)), all of them in ONE GPU call.  The decoders must be distinct.  Returns the decoded
+        lengths.  If a block is malformed its decoder's write position does not move (Decode throws before
+        `_outputIndex += decoded`) and InvalidOperationException is raised after every other decoder has been
+        advanced."""
+        decoders = list(decoders)
+        if len(decoders) != len(blocks):
+            raise ValueError("one block per decoder")
+        if len({id(d) for d in decoders}) != len(decoders):
+            raise ValueError("a decoder may take only one block per call")
+        n = len(decoders)
+        if n == 0:
+            return []
+        srcs, caps = [], []
+        for d, b in zip(decoders, blocks):
+            d._check()
+            data, bs = (b if isinstance(b, tuple) else (b, 0))
+            bs = int(bs) if int(bs) > 0 else d._block
+            if K64 + bs > d._out_len:
+                raise RuntimeError("InvalidOperationException")       # the block cannot fit behind the dictionary
+            d._prepare(bs)
+            srcs.append(bytes(data))
+            caps.append(bs)
+        # one slot per decoder: [history (<= 64 KiB) | block capacity], 16-aligned
+        hist = [min(d._prefix, d._index, 65535) for d in decoders]
+        doff = np.zeros(n, dtype=np.int64)
+        at = 0
+        for i in range(n):
+            doff[i] = (at + hist[i] + 15) // 16 * 16
+            at = int(doff[i]) + caps[i]
+        dst = np.zeros(at + 16, dtype=np.uint8)
+        for i, d in enumerate(decoders):
+            if hist[i]:
+                dst[doff[i] - hist[i]:doff[i]] = d._out[d._index - hist[i]:d._index]
+        lens = np.array([len(x) for x in srcs], dtype=np.int32)
+        soff = np.zeros(n, dtype=np.int64)
+        soff[1:] = np.cumsum(lens[:-1], dtype=np.int64)
+        src = np.frombuffer(b"".join(srcs) or b"\x00", dtype=np.uint8)
+        out = decode_chain_batch_host(src, soff, lens, dst, doff, np.array(caps, dtype=np.int32),
+                                      np.array(hist, dtype=np.int32), device)
+        res, failed = [], False
+        for i, d in enumerate(decoders):
+            r = int(out[i])
+            if r < 0:
+                failed = True
+                res.append(r)
+                continue
+            d._out[d._index:d._index + r] = dst[doff[i]:doff[i] + r]
+            d._index += r
+            if r > 0:                                                  # LL64.dec.cs:566-590
+                d._prefix = r if d._prefix == 0 else d._prefix + r
+            res.append(r)
+        if failed:
+            raise RuntimeError("InvalidOperationException")
+        return res
+
+    def Inject(self, source) -> int:
+        """LZ4ChainDecoder.cs:64-93."""
+        self._check()
+        src = np.frombuffer(bytes(source), dtype=np.uint8)
+        length = int(src.size)
+        if length <= 0:
+            return 0
+        if length > max(self._block, K64):
+            raise RuntimeError("InvalidOperationException")
+        if self._index + length < self._out_len:
+            self._out[self._index:self._index + length] = src
+            self._index = self._apply_dict(self._index + length)
+        elif length >= K64:
+            self._out[:length] = src
+            self._index = self._apply_dict(length)
+        else:
+            tail = min(K64 - length, self._index)
+            self._out[:tail] = self._out[self._index - tail:self._index].copy()
+            self._out[tail:tail + length] = src
+            self._index = self._apply_dict(tail + length)
+        return length
+
+    def Drain(self, target, offset: int, length: int) -> None:
+        """LZ4ChainDecoder.cs:96-103 (offset is negative: counted from the write position)."""
+        self._check()
+        offset = self._index + offset
+        if offset < 0 or length < 0 or offset + length > self._index:
+            raise RuntimeError("InvalidOperationException")
+        t = np.frombuffer(target, dtype=np.uint8) if not isinstance(target, np.ndarray) else target
+        t[:length] = self._out[offset:offset + length]
+
+    def Peek(self, offset: int) -> np.ndarray:
+        """LZ4ChainDecoder.cs:106-115: the bytes from `offset` (negative) to the write position."""
+        self._check()
+        offset = self._index + offset
+        if offset < 0 or offset > self._index:
+            raise RuntimeError("InvalidOperationException")
+        return self._out[offset:self._index]
+
+    def Dispose(self) -> None:
+        self._disposed = True
+
+    # -- LZ4ChainDecoder.cs:117-140 --------------------------------------------------------------------------
+    def _prepare(self, block_size: int) -> None:
+        if self._index + block_size <= self._out_len:
+            return
+        self._index = self._copy_dict(self._index)
+
+    def _copy_dict(self, index: int) -> int:
+        start = max(index - K64, 0)
+        size = index - start
+        self._out[:size] = self._out[start:index].copy()
+        self._prefix = size                                            # LZ4_setStreamDecode(ctx, buffer, size)
+        return size
+
+    def _apply_dict(self, index: int) -> int:
+        self._prefix = index - max(index - K64, 0)                    # LZ4_setStreamDecode(ctx, buffer + start, size)
+        return index
+
+    def _check(self) -> None:
+        if self._disposed:
+            raise RuntimeError("ObjectDisposedException")
+
+
+class LZ4Decoder:
+    """LZ4Decoder.Create -- Encoders/LZ4Decoder.cs:13-15."""
+
+    @staticmethod
+    def Create(chaining: bool, blockSize: int, extraBlocks: int = 0):
+        return LZ4ChainDecoder(blockSize, extraBlocks) if chaining else LZ4BlockDecoder(blockSize)

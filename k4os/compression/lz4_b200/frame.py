@@ -10,9 +10,10 @@ independent blocks (`Chaining = false`), `L00_FAST`:
 All blocks of a frame go through ONE k4lz4_encode_batch / k4lz4_decode_batch call and ONE
 k4lz4_xxh32_batch call; only the serial parts (header byte, content checksum, byte layout) run
 on the host.  Frames are interoperable with upstream lz4 (tests decode them with
-orig/lib/lz4frame.c and decode upstream's frames here).  Chained blocks, content size and
-dictionary ids are the managed engine's business (the reference itself throws NotImplemented for
-the last two, LZ4FrameWriter.cs:89-95).
+orig/lib/lz4frame.c and decode upstream's frames here).  Frames of linked blocks (the reference's
+default, LZ4EncoderSettings.ChainBlocks) are READ on the GPU as well, batched across frames
+(read_frames); writing them, content size and dictionary ids are the managed engine's business
+(the reference itself throws NotImplemented for the last two, LZ4FrameWriter.cs:89-95).
 """
 from __future__ import annotations
 
@@ -21,7 +22,7 @@ import struct
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_batch_host, encode_batch_flat_host
 
 MAGIC = 0x184D2204
 _BLOCK_SIZES = {4: 1 << 16, 5: 1 << 18, 6: 1 << 20, 7: 1 << 22}
@@ -94,78 +95,160 @@ def write_frame(data, block_size: int = 65536, block_checksum: bool = False,
     return b"".join(out)
 
 
-def read_frame(frame, device: int = 0) -> bytes:
-    """Decodes one frame of independent blocks (LZ4FrameReader.blocking.cs:57-144); raises
-    InvalidDataException on a bad magic number, header checksum, block or content checksum."""
-    f = bytes(frame)
-    if len(f) < 7 or struct.unpack_from("<I", f, 0)[0] != MAGIC:
-        raise InvalidDataException("LZ4 frame magic number expected")
-    flg, bd = f[4], f[5]
-    if (flg >> 6) & 0x11 != 1:                                   # sic: the reference masks with 0x11, :85
-        raise InvalidDataException(f"LZ4 frame version unknown: {(flg >> 6) & 0x11}")
-    chaining = ((flg >> 5) & 1) == 0
-    block_checksum = bool((flg >> 4) & 1)
-    has_size = bool((flg >> 3) & 1)
-    content_checksum = bool((flg >> 2) & 1)
-    if flg & 1:
-        raise NotImplementedError("Predefined dictionaries feature is not implemented")   # :108-110
-    p = 6 + (8 if has_size else 0)
-    if len(f) < p + 1 or ((xxh32(f[4:p]) >> 8) & 0xFF) != f[p]:
-        raise InvalidDataException("Invalid LZ4 frame header checksum")
-    p += 1
-    if chaining:
-        raise NotImplementedError("chained blocks are decoded by the managed engine (dependent blocks)")
-    max_block = _BLOCK_SIZES.get((bd >> 4) & 7, 1 << 16)        # LZ4FrameReader.cs:55-59
-    pos, lens, raws, sums = [], [], [], []
-    while True:
-        if p + 4 > len(f):
-            raise InvalidDataException("Unexpected end of stream")
-        code = struct.unpack_from("<I", f, p)[0]
-        p += 4
-        if code == 0:
-            break
-        blen = code & 0x7FFFFFFF
-        if p + blen + (4 if block_checksum else 0) > len(f):
-            raise InvalidDataException("Unexpected end of stream")
-        pos.append(p); lens.append(blen); raws.append(bool(code & 0x80000000))
-        p += blen
-        if block_checksum:
-            sums.append(struct.unpack_from("<I", f, p)[0])
+class _Frame:
+    """A parsed frame: header flags and the position, length and raw flag of every block."""
+
+    def __init__(self, f: bytes):
+        if len(f) < 7 or struct.unpack_from("<I", f, 0)[0] != MAGIC:
+            raise InvalidDataException("LZ4 frame magic number expected")
+        flg, bd = f[4], f[5]
+        if (flg >> 6) & 0x11 != 1:                               # sic: the reference masks with 0x11, :85
+            raise InvalidDataException(f"LZ4 frame version unknown: {(flg >> 6) & 0x11}")
+        self.chaining = ((flg >> 5) & 1) == 0
+        self.block_checksum = bool((flg >> 4) & 1)
+        has_size = bool((flg >> 3) & 1)
+        content_checksum = bool((flg >> 2) & 1)
+        if flg & 1:
+            raise NotImplementedError("Predefined dictionaries feature is not implemented")   # :108-110
+        p = 6 + (8 if has_size else 0)
+        if len(f) < p + 1 or ((xxh32(f[4:p]) >> 8) & 0xFF) != f[p]:
+            raise InvalidDataException("Invalid LZ4 frame header checksum")
+        p += 1
+        self.max_block = _BLOCK_SIZES.get((bd >> 4) & 7, 1 << 16)    # LZ4FrameReader.cs:55-59
+        pos, lens, raws, sums = [], [], [], []
+        while True:
+            if p + 4 > len(f):
+                raise InvalidDataException("Unexpected end of stream")
+            code = struct.unpack_from("<I", f, p)[0]
             p += 4
-    expect_content = None
-    if content_checksum:
-        if p + 4 > len(f):
-            raise InvalidDataException("Unexpected end of stream")
-        expect_content = struct.unpack_from("<I", f, p)[0]
+            if code == 0:
+                break
+            blen = code & 0x7FFFFFFF
+            if p + blen + (4 if self.block_checksum else 0) > len(f):
+                raise InvalidDataException("Unexpected end of stream")
+            pos.append(p); lens.append(blen); raws.append(bool(code & 0x80000000))
+            p += blen
+            if self.block_checksum:
+                sums.append(struct.unpack_from("<I", f, p)[0])
+                p += 4
+        self.expect_content = None
+        if content_checksum:
+            if p + 4 > len(f):
+                raise InvalidDataException("Unexpected end of stream")
+            self.expect_content = struct.unpack_from("<I", f, p)[0]
+        self.f, self.pos, self.lens, self.raws, self.sums = f, pos, lens, raws, sums
+
+    def check_blocks(self, device: int) -> None:
+        if self.block_checksum and self.pos:
+            base = np.frombuffer(self.f, dtype=np.uint8)
+            got = xxh32_batch(base, np.array(self.pos, dtype=np.int64), np.array(self.lens, dtype=np.int32), 0, device)
+            if (got != np.array(self.sums, dtype=np.uint32)).any():
+                raise InvalidDataException("Invalid block checksum")
+
+    def check_content(self, content: bytes) -> bytes:
+        if self.expect_content is not None and xxh32(content) != self.expect_content:
+            raise InvalidDataException("Invalid content checksum")
+        return content
+
+
+def _read_independent(fr: _Frame, device: int) -> bytes:
+    f, pos, lens, max_block = fr.f, fr.pos, fr.lens, fr.max_block
     nb = len(pos)
     if nb == 0:
-        content = b""
-    else:
-        base = np.frombuffer(f, dtype=np.uint8)
-        off = np.array(pos, dtype=np.int64)
-        ln = np.array(lens, dtype=np.int32)
-        if block_checksum:
-            got = xxh32_batch(base, off, ln, 0, device)
-            if (got != np.array(sums, dtype=np.uint32)).any():
-                raise InvalidDataException("Invalid block checksum")
-        is_raw = np.array(raws, dtype=bool)
-        caps = np.full(nb, max_block + 8, dtype=np.int32)       # LZ4BlockDecoder.cs:26
-        doff = np.arange(nb, dtype=np.int64) * (max_block + 8)
-        dst = np.zeros(nb * (max_block + 8) + 16, dtype=np.uint8)
-        dec_len = np.where(is_raw, 0, ln).astype(np.int32)       # raw blocks are injected, not decoded
-        out_len = decode_batch_flat_host(base, off, dec_len, dst, doff, caps, device)
-        parts = []
-        for i in range(nb):
-            if is_raw[i]:
-                if lens[i] > max_block + 8:
+        return b""
+    base = np.frombuffer(f, dtype=np.uint8)
+    off = np.array(pos, dtype=np.int64)
+    ln = np.array(lens, dtype=np.int32)
+    fr.check_blocks(device)
+    is_raw = np.array(fr.raws, dtype=bool)
+    caps = np.full(nb, max_block + 8, dtype=np.int32)           # LZ4BlockDecoder.cs:26
+    doff = np.arange(nb, dtype=np.int64) * (max_block + 8)
+    dst = np.zeros(nb * (max_block + 8) + 16, dtype=np.uint8)
+    dec_len = np.where(is_raw, 0, ln).astype(np.int32)           # raw blocks are injected, not decoded
+    out_len = decode_batch_flat_host(base, off, dec_len, dst, doff, caps, device)
+    parts = []
+    for i in range(nb):
+        if is_raw[i]:
+            if lens[i] > max_block + 8:
+                raise InvalidDataException("block larger than the declared block size")
+            parts.append(f[pos[i]:pos[i] + lens[i]])
+        else:
+            r = int(out_len[i])
+            if r < 0 or (r == 0 and lens[i] > 0):
+                raise InvalidDataException("corrupted block")   # InvalidOperationException in LZ4BlockDecoder.cs:50-51
+            parts.append(dst[doff[i]:doff[i] + r].tobytes())
+    return b"".join(parts)
+
+
+def _read_linked(frames: list, device: int) -> list:
+    """Linked-block frames, batched ACROSS frames: step k decodes block k of every frame that has one with ONE
+    k4lz4_decode_chain_batch call.  A block decodes with dstCap = the frame's maximum block size and the
+    frame's output so far as history (LZ4ChainDecoder, LZ4FrameReader.cs:93-106); a raw block is history too
+    (Inject, :93-96)."""
+    for fr in frames:
+        fr.check_blocks(device)
+    outs = [bytearray() for _ in frames]
+    steps = max((len(fr.pos) for fr in frames), default=0)
+    for k in range(steps):
+        todo = []
+        for j, fr in enumerate(frames):
+            if k >= len(fr.pos):
+                continue
+            blk = fr.f[fr.pos[k]:fr.pos[k] + fr.lens[k]]
+            if fr.raws[k]:
+                if fr.lens[k] > max(fr.max_block, 65536):            # LZ4ChainDecoder.Inject, :69-70
                     raise InvalidDataException("block larger than the declared block size")
-                parts.append(f[pos[i]:pos[i] + lens[i]])
+                outs[j] += blk
             else:
-                r = int(out_len[i])
-                if r < 0 or (r == 0 and lens[i] > 0):
-                    raise InvalidDataException("corrupted block")   # InvalidOperationException in LZ4BlockDecoder.cs:50-51
-                parts.append(dst[doff[i]:doff[i] + r].tobytes())
-        content = b"".join(parts)
-    if expect_content is not None and xxh32(content) != expect_content:
-        raise InvalidDataException("Invalid content checksum")
-    return content
+                todo.append((j, blk))
+        if not todo:
+            continue
+        n = len(todo)
+        hist = [min(len(outs[j]), 65535) for j, _ in todo]
+        caps = [frames[j].max_block for j, _ in todo]
+        doff = np.zeros(n, dtype=np.int64)
+        at = 0
+        for i in range(n):
+            doff[i] = (at + hist[i] + 15) // 16 * 16
+            at = int(doff[i]) + caps[i]
+        dst = np.zeros(at + 16, dtype=np.uint8)
+        for i, (j, _) in enumerate(todo):
+            if hist[i]:
+                dst[doff[i] - hist[i]:doff[i]] = np.frombuffer(bytes(outs[j][-hist[i]:]), dtype=np.uint8)
+        lens = np.array([len(b) for _, b in todo], dtype=np.int32)
+        soff = np.zeros(n, dtype=np.int64)
+        soff[1:] = np.cumsum(lens[:-1], dtype=np.int64)
+        src = np.frombuffer(b"".join(b for _, b in todo) or b"\x00", dtype=np.uint8)
+        res = decode_chain_batch_host(src, soff, lens, dst, doff, np.array(caps, dtype=np.int32),
+                                      np.array(hist, dtype=np.int32), device)
+        for i, (j, _) in enumerate(todo):
+            r = int(res[i])
+            if r < 0:
+                raise InvalidDataException("corrupted block")   # InvalidOperationException in LZ4ChainDecoder.cs:55-56
+            outs[j] += dst[doff[i]:doff[i] + r].tobytes()
+    return [fr.check_content(bytes(o)) for fr, o in zip(frames, outs)]
+
+
+def read_frames(frames, device: int = 0) -> list:
+    """Decodes many frames, linked or independent; returns their contents in order.  Independent frames are
+    read as by read_frame; the linked ones together, one block of every frame per GPU call.  Raises like
+    read_frame for the first bad frame."""
+    parsed = [_Frame(bytes(f)) for f in frames]
+    out = [None] * len(parsed)
+    linked = [i for i, fr in enumerate(parsed) if fr.chaining]
+    for i, fr in enumerate(parsed):
+        if not fr.chaining:
+            out[i] = fr.check_content(_read_independent(fr, device))
+    for i, content in zip(linked, _read_linked([parsed[i] for i in linked], device)):
+        out[i] = content
+    return out
+
+
+def read_frame(frame, device: int = 0) -> bytes:
+    """Decodes one frame (LZ4FrameReader.blocking.cs:57-144); raises InvalidDataException on a bad magic
+    number, header checksum, block or content checksum or a corrupted block.  A frame of linked blocks goes
+    through read_frames."""
+    fr = _Frame(bytes(frame))
+    if fr.chaining:
+        return read_frames([fr.f], device)[0]
+    return fr.check_content(_read_independent(fr, device))

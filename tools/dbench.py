@@ -4,6 +4,11 @@ checks the result (decode: against the raw input; encode: round trip).
     python tools/dbench.py [--blocks N] [--data datagen|synth] [--mp 630] [--reps 5] [--what decode|encode|both]
 --data datagen: the reference's generator (oracle/: RDG_genBuffer, matchProba = mp/1000, seed 1234 + chunk)
 --data synth  : the library's own device generator
+    python tools/dbench.py --what chain [--streams 264,1024,4096] [--chain-blocks 16]
+S streams x B linked 64 KiB blocks of datagen, compressed by upstream's chained encoder
+(LZ4_compress_fast_continue, oracle/_ref/): one k4lz4_decode_chain_batch call per step decodes block k of every
+stream behind its history; GB/s of decoded output over all B steps, next to one k4lz4_decode_batch call over
+the same raw bytes compressed as independent blocks.
 """
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -20,7 +25,11 @@ ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--what", default="decode")
 ap.add_argument("--check", type=int, default=0, help="encode: compare every CHECK-th block with the oracle engine (bit-exact)")
 ap.add_argument("--lib", default=None, help="alternative build of libk4lz4.so (e.g. a -DK4_DT_PROFILE build under scratch/)")
+ap.add_argument("--streams", default="264,1024,4096", help="chain: stream counts")
+ap.add_argument("--chain-blocks", type=int, default=16, help="chain: linked blocks per stream")
 a = ap.parse_args()
+if a.what == "chain":
+    a.blocks = max(int(x) for x in a.streams.split(",")) * a.chain_blocks
 if a.lib:
     N.SO_PATH = os.path.abspath(a.lib)
 dev = torch.device("cuda", 0)
@@ -116,3 +125,51 @@ if a.what in ("decode", "both"):
     algo = (int(clen.sum()) + nb * bs)
     print(f"decode[{a.data}{a.mp}]: {ms:.3f} ms (median {med:.3f})  {nb*bs/ms/1e6:.1f} GB/s out  {algo/ms/1e6:.1f} GB/s algorithmic  "
           f"ok={ok} ratio {ratio:.3f} stats {stats}", flush=True)
+if a.what == "chain":
+    from concurrent.futures import ThreadPoolExecutor
+    from tests import chain_ref as CR
+    Bk = a.chain_blocks
+    up = CR.Upstream()
+    hraw = raw.cpu().numpy()
+    S_all = nb // Bk
+    with ThreadPoolExecutor(max_workers=min(64, os.cpu_count() or 1)) as ex:
+        comp = list(ex.map(lambda s_: up.encode_chain(hraw[s_ * Bk * bs:(s_ + 1) * Bk * bs].tobytes(), bs), range(S_all)))
+    for S in (int(x) for x in a.streams.split(",")):
+        steps = []
+        for k in range(Bk):
+            blocks = [comp[s_][k] for s_ in range(S)]
+            ln = np.array([len(b) for b in blocks], dtype=np.int32)
+            so = np.zeros(S, dtype=np.int64)
+            so[1:] = np.cumsum(ln[:-1])
+            steps.append((torch.from_numpy(np.frombuffer(b"".join(blocks), dtype=np.uint8).copy()).to(dev),
+                          torch.from_numpy(so).to(dev), torch.from_numpy(ln).to(dev),
+                          torch.arange(S, dtype=torch.int64, device=dev) * (Bk * bs) + k * bs,
+                          torch.full((S,), bs, dtype=torch.int32, device=dev),
+                          torch.full((S,), k * bs, dtype=torch.int32, device=dev)))
+        out = torch.zeros(S * Bk * bs, dtype=torch.uint8, device=dev)
+        olen = torch.zeros(S, dtype=torch.int32, device=dev)
+        def chain():
+            for t_src, t_so, t_ln, t_do, t_cap, t_pre in steps:
+                B.decode_chain_batch_device(t_src.data_ptr(), t_so.data_ptr(), t_ln.data_ptr(), out.data_ptr(),
+                                            t_do.data_ptr(), t_cap.data_ptr(), t_pre.data_ptr(), olen.data_ptr(), S, st)
+        B.decode_stats(0, reset=True)
+        chain(); torch.cuda.synchronize()
+        stats = B.decode_stats(0, reset=True)
+        ok = bool(torch.equal(out, raw[:S * Bk * bs]))
+        ms, med = timeit(chain, a.reps)
+        cbytes = sum(len(comp[s_][k]) for s_ in range(S) for k in range(Bk))
+        # the same raw bytes as independent blocks (the GPU encoder's output), one call
+        n2 = S * Bk
+        poff = torch.cumsum(clen[:n2].to(torch.int64), 0) - clen[:n2].to(torch.int64)
+        packed = torch.empty(int(clen[:n2].sum()) + 64, dtype=torch.uint8, device=dev)
+        B.copy_blocks_device(slots.data_ptr(), coff.data_ptr(), packed.data_ptr(), poff.data_ptr(), clen.data_ptr(), n2, st)
+        out2 = torch.zeros(n2 * bs, dtype=torch.uint8, device=dev)
+        olen2 = torch.zeros(n2, dtype=torch.int32, device=dev)
+        def indep():
+            B.decode_batch_device(packed.data_ptr(), poff.data_ptr(), clen.data_ptr(), out2.data_ptr(), roff.data_ptr(),
+                                  rlen.data_ptr(), olen2.data_ptr(), n2, st)
+        ms2, med2 = timeit(indep, a.reps)
+        ok2 = bool(torch.equal(out2, raw[:n2 * bs]))
+        print(f"chain[{a.data}{a.mp}] S={S} B={Bk}: {ms:.3f} ms (median {med:.3f})  {n2*bs/ms/1e6:.1f} GB/s out  "
+              f"ratio {cbytes/(n2*bs):.3f} ok={ok} stats {stats} | independent, one call: {ms2:.3f} ms "
+              f"{n2*bs/ms2/1e6:.1f} GB/s ok={ok2}", flush=True)
