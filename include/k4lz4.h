@@ -17,8 +17,14 @@
  *     and never collide with codec results; k4lz4_last_error() gives the message;
  *   - bytes of a destination block at index >= its returned length are never written
  *     (SpanTests.cs:36-37, PartialDecompressionTests.cs:33-35);
+ *   - every batched call checks its arguments before the machine, in this order: an unknown
+ *     memKind, a negative block count, a required pointer that is NULL while nBlocks > 0, and the
+ *     host-memory contents (a negative prefixLen, a level outside 0..255) give K4LZ4_E_ARG; then
+ *     no device gives K4LZ4_E_NODEVICE; then nBlocks == 0 returns K4LZ4_OK; then a device index
+ *     >= k4lz4_device_count() gives K4LZ4_E_ARG and a failed cudaSetDevice K4LZ4_E_CUDA.  So a
+ *     caller's mistake gets the same code with or without a GPU;
  *   - the library never falls back to a CPU codec: without a usable CUDA device every
- *     compute entry point returns K4LZ4_E_NODEVICE.
+ *     compute call with valid arguments returns K4LZ4_E_NODEVICE.
  */
 #ifndef K4LZ4_H
 #define K4LZ4_H

@@ -64,50 +64,49 @@ def _pack(bufs: Sequence) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
     return np.ascontiguousarray(base), offs, lens
 
 
+def _slots(caps) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Slots of max(cap, 0) bytes back to back in one 0xCD-filled buffer -> (buffer, offsets, int32 caps)."""
+    dc = _i32(caps)
+    do = np.zeros(len(dc), dtype=np.int64)
+    if len(dc):
+        do[1:] = np.cumsum(np.maximum(dc[:-1], 0), dtype=np.int64)
+    return np.full(int(np.maximum(dc, 0).sum()) + 1, 0xCD, dtype=np.uint8), do, dc
+
+
+def _slices(dst: np.ndarray, do, out) -> list:
+    """The bytes each block produced: dst[do[i] .. +out[i]), empty where out[i] <= 0."""
+    return [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(len(out))]
+
+
 def encode_batch_host(blocks: Sequence, caps: Sequence[int] | None = None, level: int = 0,
                       device: int = 0):
     """-> (list[bytes], outLen int32[n]); caps default to MaximumOutputSize(len)."""
     src, so, sl = _pack(blocks)
     if caps is None:
         caps = [N.lib().k4lz4_max_output_size(int(x)) for x in sl]
-    dc = _i32(caps)
-    do = np.zeros(len(dc), dtype=np.int64)
-    if len(dc):
-        do[1:] = np.cumsum(np.maximum(dc[:-1], 0), dtype=np.int64)
-    dst = np.full(int(np.maximum(dc, 0).sum()) + 1, 0xCD, dtype=np.uint8)
+    dst, do, dc = _slots(caps)
     out = encode_batch_flat_host(src, so, sl, dst, do, dc, level, device)
-    res = [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(len(dc))]
-    return res, out
+    return _slices(dst, do, out), out
 
 
 def decode_batch_host(blocks: Sequence, caps: Sequence[int], device: int = 0):
     """-> (list[bytes], outLen int32[n])."""
     src, so, sl = _pack(blocks)
-    dc = _i32(caps)
-    do = np.zeros(len(dc), dtype=np.int64)
-    if len(dc):
-        do[1:] = np.cumsum(np.maximum(dc[:-1], 0), dtype=np.int64)
-    dst = np.full(int(np.maximum(dc, 0).sum()) + 1, 0xCD, dtype=np.uint8)
+    dst, do, dc = _slots(caps)
     out = decode_batch_flat_host(src, so, sl, dst, do, dc, device)
-    res = [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(len(dc))]
-    return res, out
+    return _slices(dst, do, out), out
 
 
 def pickle_batch_host(messages: Sequence, level: int = 0, device: int = 0):
     """LZ4Pickler.Pickle over a batch -> (list[bytes], outLen int32[n])."""
     src, so, sl = _pack(messages)
     n = len(sl)
-    bound = np.where(sl > 0, sl.astype(np.int64) + 1, 0)
-    do = np.zeros(n, dtype=np.int64)
-    if n:
-        do[1:] = np.cumsum(bound[:-1])
-    dst = np.full(int(bound.sum()) + 1, 0xCD, dtype=np.uint8)
+    dst, do, _ = _slots(np.where(sl > 0, sl + 1, 0))
     out = np.full(n, -1, dtype=np.int32)
     N.check(N.lib().k4lz4_pickle_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
                                        dst.ctypes.data, do.ctypes.data, out.ctypes.data,
                                        n, int(level), N.MEM_HOST, None, int(device)))
-    res = [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(n)]
-    return res, out
+    return _slices(dst, do, out), out
 
 
 def pickle_writer_batch_host(messages: Sequence, level: int = 0, device: int = 0):
@@ -116,17 +115,12 @@ def pickle_writer_batch_host(messages: Sequence, level: int = 0, device: int = 0
     src, so, sl = _pack(messages)
     n = len(sl)
     L = N.lib()
-    bound = np.array([L.k4lz4_pickle_writer_bound(int(v)) for v in sl], dtype=np.int64)
-    do = np.zeros(n, dtype=np.int64)
-    if n:
-        do[1:] = np.cumsum(bound[:-1])
-    dst = np.full(int(bound.sum()) + 1, 0xCD, dtype=np.uint8)
+    dst, do, _ = _slots([L.k4lz4_pickle_writer_bound(int(v)) for v in sl])
     out = np.full(n, -1, dtype=np.int32)
     N.check(L.k4lz4_pickle_writer_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
                                         dst.ctypes.data, do.ctypes.data, out.ctypes.data,
                                         n, int(level), N.MEM_HOST, None, int(device)))
-    res = [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(n)]
-    return res, out
+    return _slices(dst, do, out), out
 
 
 def unpickled_size_batch_host(pickles: Sequence, device: int = 0) -> np.ndarray:
@@ -146,19 +140,15 @@ def unpickle_batch_host(pickles: Sequence, outputs: Sequence[np.ndarray] | None 
     n = len(sl)
     if outputs is None:
         sizes = unpickled_size_batch_host(pickles, device)
-        dl = np.where(sizes > 0, sizes, 0).astype(np.int32)
+        dst, do, dl = _slots(np.where(sizes > 0, sizes, 0))
     else:
-        dl = np.array([o.shape[0] for o in outputs], dtype=np.int32)
-    do = np.zeros(n, dtype=np.int64)
-    if n:
-        do[1:] = np.cumsum(dl[:-1], dtype=np.int64)
-    dst = np.full(int(dl.sum()) + 1, 0xCD, dtype=np.uint8)
+        dst, do, dl = _slots([o.shape[0] for o in outputs])
     out = np.full(n, -1, dtype=np.int32)
     N.check(N.lib().k4lz4_unpickle_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
                                          dst.ctypes.data, do.ctypes.data, dl.ctypes.data,
                                          out.ctypes.data, n, N.MEM_HOST, None, int(device)))
     if outputs is None:
-        res = [dst[do[i]:do[i] + out[i]].tobytes() if out[i] > 0 else b"" for i in range(n)]
+        res = _slices(dst, do, out)
         # a message whose header was corrupt reports R_CORRUPT in `sizes`; keep that verdict
         out = np.where(sizes == N.R_CORRUPT, N.R_CORRUPT, out).astype(np.int32)
         return res, out
@@ -247,17 +237,12 @@ def decode_dict_batch_host(blocks: Sequence, caps: Sequence[int], dicts: Sequenc
     Returns (list of bytes, int32 results)."""
     src, so, sl = _pack(blocks)
     dic, do, dl = _pack(dicts)
-    n = len(sl)
-    caps = _i32(caps)
-    doff = np.zeros(n, dtype=np.int64)
-    if n > 1:
-        doff[1:] = np.cumsum(np.maximum(caps[:-1], 0).astype(np.int64))
-    dst = np.zeros(int(np.maximum(caps, 0).sum()) + 16, dtype=np.uint8)
-    out = np.zeros(n, dtype=np.int32)
+    dst, doff, caps = _slots(caps)
+    out = np.full(len(sl), -1, dtype=np.int32)
     N.check(N.lib().k4lz4_decode_dict_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
                                             doff.ctypes.data, caps.ctypes.data, dic.ctypes.data, do.ctypes.data,
-                                            dl.ctypes.data, out.ctypes.data, n, N.MEM_HOST, None, int(device)))
-    return [dst[doff[i]:doff[i] + max(int(out[i]), 0)].tobytes() for i in range(n)], out
+                                            dl.ctypes.data, out.ctypes.data, len(sl), N.MEM_HOST, None, int(device)))
+    return _slices(dst, doff, out), out
 
 
 def decode_chain_batch_host(src: np.ndarray, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, prefix_len,
@@ -277,6 +262,26 @@ def decode_chain_batch_host(src: np.ndarray, src_off, src_len, dst: np.ndarray, 
     return out
 
 
+def decode_chain_blocks_host(blocks: Sequence, histories: Sequence, caps: Sequence[int], device: int = 0):
+    """Block i decodes behind histories[i] (its stream's output so far; the decoder reads the last 65 535 bytes)
+    into at most caps[i] bytes, in one call; slot i is [history | capacity], 16-aligned.
+    -> (int32 results: bytes decoded or -1, list of the decoded bytes)."""
+    src, so, sl = _pack(blocks)
+    dc = _i32(caps)
+    hl = np.array([min(len(h), 65535) for h in histories], dtype=np.int32)
+    do = np.zeros(len(dc), dtype=np.int64)
+    at = 0
+    for i in range(len(dc)):
+        do[i] = (at + int(hl[i]) + 15) // 16 * 16
+        at = int(do[i]) + max(int(dc[i]), 0)
+    dst = np.zeros(at + 16, dtype=np.uint8)
+    for i, h in enumerate(histories):
+        if hl[i]:
+            dst[do[i] - hl[i]:do[i]] = np.frombuffer(bytes(h[len(h) - int(hl[i]):]), dtype=np.uint8)
+    out = decode_chain_batch_host(src, so, sl, dst, do, dc, hl, device)
+    return out, _slices(dst, do, out)
+
+
 def decode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int,
                               dst_off_ptr: int, dst_cap_ptr: int, prefix_len_ptr: int, out_len_ptr: int, n: int,
                               stream: int = 0, device: int = -1) -> None:
@@ -290,13 +295,9 @@ def partial_decode_batch_host(blocks: Sequence, targets: Sequence[int], device: 
     """LZ4Codec.PartialDecode over a batch (k4lz4_partial_decode_batch, host memory)."""
     src, so, sl = _pack(blocks)
     n = len(sl)
-    tg = _i32(targets)
-    doff = np.zeros(n, dtype=np.int64)
-    if n > 1:
-        doff[1:] = np.cumsum(np.maximum(tg[:-1], 0).astype(np.int64))
-    dst = np.zeros(int(np.maximum(tg, 0).sum()) + 16, dtype=np.uint8)
-    out = np.zeros(n, dtype=np.int32)
+    dst, doff, tg = _slots(targets)
+    out = np.full(n, -1, dtype=np.int32)
     N.check(N.lib().k4lz4_partial_decode_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
                                                doff.ctypes.data, tg.ctypes.data, out.ctypes.data, n,
                                                N.MEM_HOST, None, int(device)))
-    return [dst[doff[i]:doff[i] + max(int(out[i]), 0)].tobytes() for i in range(n)], out
+    return _slices(dst, doff, out), out

@@ -827,61 +827,20 @@ decode_rest_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
 // ------------------------------------------------------------------------------------------------
 // launcher (host)
 // ------------------------------------------------------------------------------------------------
-// Per-device state of the decoder: a PRIVATE stream-ordered memory pool for the work lists (the
-// process-wide default pool is never touched), the SM count, the kernels' shared-memory opt-in.
-struct DecodeDev {
-    std::once_flag once;
-    cudaMemPool_t pool = nullptr;
-    int sms = 0;
-    cudaError_t err = cudaSuccess;
-    cudaStream_t helper = nullptr;   // side stream of the encoder (encode_launch)
-};
-
-inline DecodeDev* decode_dev(int dev) {
-    static DecodeDev devs[64];
-    if (dev < 0 || dev >= 64) return nullptr;
-    DecodeDev* d = &devs[dev];
-    std::call_once(d->once, [d, dev] {
-        cudaError_t e = cudaDeviceGetAttribute(&d->sms, cudaDevAttrMultiProcessorCount, dev);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(decode_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(TileSmem<STAGE_SMALL>));
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(decode_tile_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(TileSmem<STAGE_BIG>));
-        if (e == cudaSuccess) {
-            cudaMemPoolProps props = {};
-            props.allocType = cudaMemAllocationTypePinned;
-            props.handleTypes = cudaMemHandleTypeNone;
-            props.location.type = cudaMemLocationTypeDevice;
-            props.location.id = dev;
-            e = cudaMemPoolCreate(&d->pool, &props);
-            if (e == cudaSuccess) {
-                unsigned long long keep = 256ull << 20;         // cache up to 256 MiB of work lists and encoder tables
-                cudaMemPoolSetAttribute(d->pool, cudaMemPoolAttrReleaseThreshold, &keep);
-            }
-        }
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&d->helper, cudaStreamNonBlocking);
-        d->err = e;
-    });
-    return d;
-}
-
 // Enqueues the decode of n blocks on `st` (current device).  prefixLen (device array, may be null:
 // independent blocks) gives each block's history length, the bytes in front of its destination; with it the
-// results are those of LZ4_decompress_safe_continue in prefix mode (bytes decoded or -1).  Returns the
-// number of kernels launched, or -1 with *err set.
-inline int decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
-                         uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
-                         int32_t* outLen, int n, cudaStream_t st, cudaError_t* err,
-                         const int32_t* prefixLen = nullptr) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    DecodeDev* D = decode_dev(dev);
-    if (!D || D->err != cudaSuccess) { *err = D ? D->err : cudaErrorInvalidDevice; return -1; }
+// results are those of LZ4_decompress_safe_continue in prefix mode (bytes decoded or -1).  On success
+// DECODE_LAUNCHES kernels were launched.  The work lists come from `pool`, a private stream-ordered
+// pool of the current device (the process-wide default pool is never touched); `sms` is its SM count.  The
+// tile kernels must have been granted their dynamic shared memory (sizeof(TileSmem<...>)).
+constexpr int DECODE_LAUNCHES = 3;
+inline cudaError_t decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                 const int32_t* prefixLen, int32_t* outLen, int n, cudaStream_t st,
+                                 cudaMemPool_t pool, int sms) {
     uint32_t* scratch = nullptr;
-    cudaError_t e = cudaMallocFromPoolAsync((void**)&scratch, ((size_t)2 * n + 4) * sizeof(uint32_t), D->pool, st);
-    if (e != cudaSuccess) { *err = e; return -1; }
+    cudaError_t e = cudaMallocFromPoolAsync((void**)&scratch, ((size_t)2 * n + 4) * sizeof(uint32_t), pool, st);
+    if (e != cudaSuccess) return e;
     DecodeLists wl;
     wl.counts = scratch;
     wl.big = scratch + 4;
@@ -890,18 +849,17 @@ inline int decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const in
     if (e == cudaSuccess) {
         decode_tile_kernel<<<n, DT_THREADS, sizeof(TileSmem<STAGE_SMALL>), st>>>(
             srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
-        const int gridBig = n < D->sms ? n : D->sms;
+        const int gridBig = n < sms ? n : sms;
         decode_tile_big_kernel<<<gridBig, DT_THREADS, sizeof(TileSmem<STAGE_BIG>), st>>>(
             srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
         const int want = (n + 3) / 4;
-        const int gridRest = want < D->sms * 8 ? want : D->sms * 8;
+        const int gridRest = want < sms * 8 ? want : sms * 8;
         decode_rest_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen,
                                                       outLen, wl);
         e = cudaGetLastError();
     }
     cudaFreeAsync(scratch, st);
-    if (e != cudaSuccess) { *err = e; return -1; }
-    return 3;
+    return e;
 }
 
 }  // namespace k4

@@ -1,9 +1,10 @@
 // k4lz4_api.cu -- the C ABI of libk4lz4 (include/k4lz4.h): argument handling, the
-// device-resident launch path, the host-buffer staging path (chunked, double-buffered,
-// NCCL-free multi-GPU split of the block list) and the synthetic workload generator.
+// device-resident launch path, the host-buffer staging paths (chunked, double-buffered,
+// NCCL-free multi-GPU split of the block list for the codec; one synchronous routine for the
+// rest) and the synthetic workload generator.
 //
 // There is deliberately NO CPU codec in this library: without a usable CUDA device every
-// compute entry point fails with K4LZ4_E_NODEVICE.
+// compute call with valid arguments fails with K4LZ4_E_NODEVICE.
 #include "../../../../include/k4lz4.h"
 
 #include <cuda_runtime.h>
@@ -19,7 +20,6 @@
 #include <cstdio>
 #include <cstring>
 #include <functional>
-#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -67,131 +67,68 @@ int device_count_cached() {
     return n;
 }
 
-// ---- kernel launchers (device pointers) ---------------------------------------------------
+// ---- one batch description, one argument check ------------------------------------------------
 
-enum Op { OP_ENCODE = 0, OP_DECODE = 1, OP_PICKLE = 2, OP_UNPICKLE = 3, OP_USIZE = 4, OP_PICKLEW = 5 };
-
-std::once_flag g_attr_once[64];
-
-void set_func_attrs(int dev) {
-    if (dev < 0 || dev >= 64) return;
-    std::call_once(g_attr_once[dev], [] {
-        cudaFuncSetAttribute(k4::pickle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES);
-        // both encoder kernels ask for the same shared-memory / L1 split (they share SMs): just enough for the
-        // shared-memory tables (+1 KiB the hardware reserves per CTA), the rest stays L1 for the input windows
-        const int carve = (k4::ENC_SM_WARPS * (k4::ENC_SLOT_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
-        cudaFuncSetAttribute(k4::encode_spec_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
-        cudaFuncSetAttribute(k4::encode_spec_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
-    });
-}
-
-// Enqueues the block encoder: a shared-memory-table kernel on `st` and, when the batch is big enough for
-// it to pay, a global-memory-table kernel on a helper stream that runs beside it (fork / join by events).
-// Both are persistent and pull blocks from one device counter.  The workspace (counter + the global
-// tables) comes from the private stream-ordered pool.
-cudaError_t encode_launch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
-                          uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
-                          int32_t* outLen, int n, int level, cudaStream_t st, int* launches) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    k4::DecodeDev* D = k4::decode_dev(dev);
-    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
-    const int wave = D->sms * k4::ENC_SM_WARPS;
-    const int gridS = n < wave ? n : wave;
-    // The global-table warps need longer per block than the shared-memory warps: a batch that the latter
-    // finish in one round goes to them alone.
-    const bool useG = k4::ENC_GM_WARPS > 0 && n > wave;
-    const int gridG = useG ? D->sms * k4::ENC_GM_WARPS : 0;
-    const size_t tabBytes = (size_t)gridG * k4::ENC_GSLOT_BYTES;
-    uint8_t* ws = nullptr;
-    cudaError_t e = cudaMallocFromPoolAsync((void**)&ws, 256 + tabBytes, D->pool, st);
-    if (e != cudaSuccess) return e;
-    uint32_t* counter = reinterpret_cast<uint32_t*>(ws);
-    e = cudaMemsetAsync(ws, 0, 4, st);
-    cudaEvent_t fork = nullptr, join = nullptr;
-    if (e == cudaSuccess && useG) {
-        // ONE side stream per device: the global-table kernels of consecutive chunks run one after the other, so an
-        // SM never holds more than ENC_GM_WARPS of them (CTAs of a queued launch would otherwise fill the SM's spare
-        // CTA slots and crowd out the mix; measured slower)
-        cudaStream_t hs = D->helper;
-        e = cudaEventCreateWithFlags(&fork, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&join, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventRecord(fork, st);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(hs, fork, 0);
-        if (e == cudaSuccess) {
-            k4::encode_spec_gtab_kernel<<<gridG, 32, 0, hs>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen,
-                                                             n, level, counter, ws + 256, wave);
-            e = cudaGetLastError();
-            if (launches) (*launches)++;
-        }
-        if (e == cudaSuccess) e = cudaEventRecord(join, hs);
-    }
-    if (e == cudaSuccess && gridS > 0) {
-        k4::encode_spec_kernel<<<gridS, 32, k4::ENC_SLOT_BYTES, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap,
-                                                                      outLen, n, level, counter);
-        e = cudaGetLastError();
-        if (launches) (*launches)++;
-    }
-    if (join && e == cudaSuccess) e = cudaStreamWaitEvent(st, join, 0);
-    if (fork) cudaEventDestroy(fork);
-    if (join) cudaEventDestroy(join);
-    cudaFreeAsync(ws, st);
-    return e;
-}
-
-struct DevArgs {
-    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
-    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap;
-    int32_t* outLen; int n; int level;
+enum Op {
+    OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY
 };
 
-cudaError_t launch_op(Op op, const DevArgs& a, cudaStream_t st) {
-    if (a.n <= 0) return cudaSuccess;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    set_func_attrs(dev);
-    switch (op) {
-    case OP_ENCODE: {
-        int nl = 0;
-        const cudaError_t ee = encode_launch(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.dstCap,
-                                             a.outLen, a.n, a.level, st, &nl);
-        g_launches += nl;
-        if (ee != cudaSuccess) { (void)cudaGetLastError(); return ee; }
-        break;
-    }
-    case OP_DECODE: {
-        cudaError_t de = cudaSuccess;
-        const int nl = k4::decode_launch(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
-                                         a.dstCap, a.outLen, a.n, st, &de);
-        if (nl < 0) { (void)cudaGetLastError(); return de != cudaSuccess ? de : cudaErrorUnknown; }
-        g_launches += nl;
-        break;
-    }
-    case OP_PICKLE:
-    case OP_PICKLEW: {
-        const int ctas = (a.n + k4::ENC_WARPS_PER_CTA - 1) / k4::ENC_WARPS_PER_CTA;
-        k4::pickle_kernel<<<ctas, k4::ENC_WARPS_PER_CTA * 32,
-                            k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES, st>>>(
-            a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.outLen, a.n, a.level, op == OP_PICKLEW ? 1 : 0);
-        g_launches++;
-        break;
-    }
-    case OP_UNPICKLE: {
-        const int ctas = (a.n + 3) / 4;
-        k4::unpickle_kernel<<<ctas, 128, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
-                                                  a.dstCap, a.outLen, a.n);
-        g_launches++;
-        break;
-    }
-    case OP_USIZE: {
-        const int ctas = (a.n + 255) / 256;
-        k4::unpickled_size_kernel<<<ctas, 256, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.outLen, a.n);
-        g_launches++;
-        break;
-    }
-    }
-    return cudaGetLastError();
+// Block i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]) and outLen[i].
+// The optional parts are null / 0 unless the op reads them.
+struct Batch {
+    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
+    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap;
+    int32_t* outLen;                  // OP_XXH32: the uint32 checksums
+    int64_t n;
+    int level = 0;                    // OP_ENCODE: 0..255; OP_PICKLE(W): passed through
+    bool x32 = false;                 // OP_ENCODE: reproduce the 32-bit engine (k4lz4_encode*_x32)
+    const uint8_t* dictBase = nullptr; const int64_t* dictOff = nullptr; const int32_t* dictLen = nullptr;
+    const int32_t* prefixLen = nullptr;   // OP_CHAIN: history in front of each destination
+    bool partial = false;             // OP_GENERAL: PartialDecode semantics (dstCap = target length)
+    uint32_t seed = 0;                // OP_XXH32
+};
+
+// The pointers each op needs when n > 0, besides srcBase / srcOff / srcLen.  A dictionary is optional
+// wherever it is read: with dictBase set, dictOff and dictLen are required too.
+struct Needs { bool dst, cap, out, prefix, level; };
+constexpr Needs NEEDS[] = {
+    /* OP_ENCODE   */ {true,  true,  true,  false, true},
+    /* OP_DECODE   */ {true,  true,  true,  false, false},
+    /* OP_CHAIN    */ {true,  true,  true,  true,  false},
+    /* OP_GENERAL  */ {true,  true,  true,  false, false},
+    /* OP_PICKLE   */ {true,  false, true,  false, false},
+    /* OP_PICKLEW  */ {true,  false, true,  false, false},
+    /* OP_UNPICKLE */ {true,  true,  true,  false, false},
+    /* OP_USIZE    */ {false, false, true,  false, false},
+    /* OP_XXH32    */ {false, false, true,  false, false},
+    /* OP_COPY     */ {true,  false, false, false, false},
+};
+static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_COPY + 1, "one row per op");
+
+// The machine part of check(): a device must exist, an empty batch is then done (the caller returns OK for
+// n == 0), and `device` (K4LZ4_ALL_DEVICES or the current device when negative) must name a visible GPU.
+int check_device(int device, int64_t n) {
+    const int ndev = device_count_cached();
+    if (ndev <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
+    if (n == 0) return K4LZ4_OK;
+    if (device >= ndev) return fail(K4LZ4_E_ARG, "device %d out of range (%d visible)", device, ndev);
+    return K4LZ4_OK;
+}
+
+// Every batched export: the arguments first, then the machine, so that a caller's mistake gets the same
+// code with or without a GPU.
+int check(Op op, const Batch& b, int memKind, int device) {
+    const Needs& w = NEEDS[op];
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
+    if (b.n > 0 && (!b.srcBase || !b.srcOff || !b.srcLen || (w.out && !b.outLen) || (w.dst && (!b.dstBase || !b.dstOff)) ||
+                    (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen))))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (w.prefix && memKind == K4LZ4_MEM_HOST)       // device arrays cannot be checked here: there a negative prefix gives -1
+        for (int64_t i = 0; i < b.n; i++)
+            if (b.prefixLen[i] < 0) return fail(K4LZ4_E_ARG, "negative prefix length at block %lld", (long long)i);
+    if (w.level && (b.level < 0 || b.level > 0xFF)) return fail(K4LZ4_E_ARG, "bad level %d", b.level);
+    return check_device(device, b.n);
 }
 
 struct DeviceGuard {
@@ -206,53 +143,28 @@ struct DeviceGuard {
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
-int run_device(Op op, const DevArgs& a, void* stream, int device) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (a.n < 0) return fail(K4LZ4_E_ARG, "negative block count");
-    if (a.n == 0) return K4LZ4_OK;
-    if (!a.srcBase || !a.srcOff || !a.srcLen || !a.outLen) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (op != OP_USIZE && (!a.dstBase || !a.dstOff)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if ((op == OP_ENCODE || op == OP_DECODE || op == OP_UNPICKLE) && !a.dstCap)
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    DeviceGuard g(device);
-    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    CU_TRY(launch_op(op, a, (cudaStream_t)stream));
-    return K4LZ4_OK;
-}
+// ---- per-device state ---------------------------------------------------------------------------
 
-// ---- host-buffer path ----------------------------------------------------------------------
-
-struct DBuf {
+struct Buf {           // grows, never shrinks: device memory, or pinned host memory
+    bool pinned = false;
     void* p = nullptr; size_t cap = 0;
+    cudaError_t alloc(size_t n) { return pinned ? cudaHostAlloc(&p, n, cudaHostAllocDefault) : cudaMalloc(&p, n); }
     cudaError_t ensure(size_t n) {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
+        if (p) { if (pinned) cudaFreeHost(p); else cudaFree(p); }
         p = nullptr; cap = 0;
         size_t want = n + n / 4 + 4096;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) { e = cudaMalloc(&p, n); want = n; }
-        if (e == cudaSuccess) cap = want; else p = nullptr;
-        return e;
-    }
-};
-struct HBuf {   // pinned host
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr; cap = 0;
-        size_t want = n + n / 4 + 4096;
-        cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
-        if (e != cudaSuccess) { e = cudaHostAlloc(&p, n, cudaHostAllocDefault); want = n; }
+        cudaError_t e = alloc(want);
+        if (e != cudaSuccess) { e = alloc(n); want = n; }
         if (e == cudaSuccess) cap = want; else p = nullptr;
         return e;
     }
 };
 
-struct Slot {          // one in-flight chunk
+struct Slot {          // one in-flight chunk of the pipelined host path
     cudaStream_t stream = nullptr;
-    DBuf dSrc, dDst, dMeta, dPack, dPackOff;
-    HBuf hSrc, hDst, hMeta, hPackOff;
+    Buf dSrc, dDst, dMeta, dPack, dPackOff;
+    Buf hSrc{true}, hDst{true}, hMeta{true}, hPackOff{true};
     const int64_t* dDstOffArr = nullptr;   // device copies of the chunk's dst offsets / results (inside dMeta)
     const int32_t* dOutLenArr = nullptr;
     bool compact = false;             // stage 2 gathered the produced bytes on the device first
@@ -265,35 +177,181 @@ struct Slot {          // one in-flight chunk
     int64_t dstBytes = 0;             // device-side extent of the destination region of the chunk
     bool direct = false;              // stage 2 copied straight into the caller's buffer
     int state = 0;                    // 0 idle, 3 inputs on their way, 1 kernel + outLen enqueued, 2 data D2H enqueued
-    DevArgs launch{};                 // the chunk's kernel arguments (state 3 -> 1)
+    Batch launch{};                   // the chunk's kernel arguments (state 3 -> 1)
 };
 
 constexpr int ENC_BIG_WAVES = 6;        // encode chunks in the middle of a batch: this many waves of blocks
 constexpr int NSLOT = 4;                // chunks in flight per device (see run_host_slice)
 
-struct DevCtx {
-    int dev = -1;
+// Everything the library keeps per GPU, set up once on first use with that GPU current: its SM count, a
+// PRIVATE stream-ordered memory pool for the decoder's work lists and the encoder's tables (the process-wide
+// default pool is never touched), the encoder's helper stream, the kernels' function attributes and the
+// slots of the pipelined host path (guarded by `mu`).
+struct Dev {
+    std::once_flag once;
+    cudaError_t err = cudaSuccess;
+    int sms = 0;
+    cudaMemPool_t pool = nullptr;
+    cudaStream_t helper = nullptr;    // side stream of the encoder (encode_launch)
     std::mutex mu;
     Slot slot[NSLOT];
-    bool init = false;
 };
 
-DevCtx* get_ctx(int dev) {
-    static std::mutex m;
-    static std::vector<std::unique_ptr<DevCtx>> ctxs;
-    std::lock_guard<std::mutex> lk(m);
-    if ((int)ctxs.size() <= dev) ctxs.resize(dev + 1);
-    if (!ctxs[dev]) { ctxs[dev].reset(new DevCtx()); ctxs[dev]->dev = dev; }
-    return ctxs[dev].get();
+Dev* dev_state(int dev) {
+    static Dev devs[64];
+    if (dev < 0 || dev >= 64) return nullptr;
+    Dev* d = &devs[dev];
+    std::call_once(d->once, [d, dev] {
+        // best effort, as their results never decide anything: the pickler's shared memory, and the split of
+        // shared memory / L1 both encoder kernels ask for (they share SMs): just enough for the shared-memory
+        // tables (+1 KiB the hardware reserves per CTA), the rest stays L1 for the input windows
+        cudaFuncSetAttribute(k4::pickle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES);
+        const int carve = (k4::ENC_SM_WARPS * (k4::ENC_SLOT_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
+        cudaFuncSetAttribute(k4::encode_spec_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
+        cudaFuncSetAttribute(k4::encode_spec_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
+        cudaError_t e = cudaDeviceGetAttribute(&d->sms, cudaDevAttrMultiProcessorCount, dev);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(k4::decode_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(k4::TileSmem<k4::STAGE_SMALL>));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(k4::decode_tile_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(k4::TileSmem<k4::STAGE_BIG>));
+        if (e == cudaSuccess) {
+            cudaMemPoolProps props = {};
+            props.allocType = cudaMemAllocationTypePinned;
+            props.handleTypes = cudaMemHandleTypeNone;
+            props.location.type = cudaMemLocationTypeDevice;
+            props.location.id = dev;
+            e = cudaMemPoolCreate(&d->pool, &props);
+            if (e == cudaSuccess) {
+                unsigned long long keep = 256ull << 20;         // cache up to 256 MiB of work lists and encoder tables
+                cudaMemPoolSetAttribute(d->pool, cudaMemPoolAttrReleaseThreshold, &keep);
+            }
+        }
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&d->helper, cudaStreamNonBlocking);
+        for (auto& s : d->slot)
+            if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking);
+        d->err = e;
+    });
+    return d;
 }
 
-struct HostArgs {
-    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
-    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap;
-    int32_t* outLen; int level;
-};
+// ---- kernel launchers (device pointers, current device) ------------------------------------------
 
-inline int64_t dst_room(Op op, const HostArgs& a, int64_t i) {
+// Enqueues the block encoder: a shared-memory-table kernel on `st` and, when the batch is big enough for
+// it to pay, a global-memory-table kernel on a helper stream that runs beside it (fork / join by events).
+// Both are persistent and pull blocks from one device counter.  The workspace (counter + the global
+// tables) comes from the private stream-ordered pool.
+cudaError_t encode_launch(const Batch& a, int level, const Dev& D, cudaStream_t st, int* launches) {
+    const int n = (int)a.n;
+    const int wave = D.sms * k4::ENC_SM_WARPS;
+    const int gridS = n < wave ? n : wave;
+    // The global-table warps need longer per block than the shared-memory warps: a batch that the latter
+    // finish in one round goes to them alone.
+    const bool useG = k4::ENC_GM_WARPS > 0 && n > wave;
+    const int gridG = useG ? D.sms * k4::ENC_GM_WARPS : 0;
+    const size_t tabBytes = (size_t)gridG * k4::ENC_GSLOT_BYTES;
+    uint8_t* ws = nullptr;
+    cudaError_t e = cudaMallocFromPoolAsync((void**)&ws, 256 + tabBytes, D.pool, st);
+    if (e != cudaSuccess) return e;
+    uint32_t* counter = reinterpret_cast<uint32_t*>(ws);
+    e = cudaMemsetAsync(ws, 0, 4, st);
+    cudaEvent_t fork = nullptr, join = nullptr;
+    if (e == cudaSuccess && useG) {
+        // ONE side stream per device: the global-table kernels of consecutive chunks run one after the other, so an
+        // SM never holds more than ENC_GM_WARPS of them (CTAs of a queued launch would otherwise fill the SM's spare
+        // CTA slots and crowd out the mix; measured slower)
+        cudaStream_t hs = D.helper;
+        e = cudaEventCreateWithFlags(&fork, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&join, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventRecord(fork, st);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(hs, fork, 0);
+        if (e == cudaSuccess) {
+            k4::encode_spec_gtab_kernel<<<gridG, 32, 0, hs>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
+                                                             a.dstCap, a.outLen, n, level, counter, ws + 256, wave);
+            e = cudaGetLastError();
+            (*launches)++;
+        }
+        if (e == cudaSuccess) e = cudaEventRecord(join, hs);
+    }
+    if (e == cudaSuccess && gridS > 0) {
+        k4::encode_spec_kernel<<<gridS, 32, k4::ENC_SLOT_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
+                                                                      a.dstOff, a.dstCap, a.outLen, n, level, counter);
+        e = cudaGetLastError();
+        (*launches)++;
+    }
+    if (join && e == cudaSuccess) e = cudaStreamWaitEvent(st, join, 0);
+    if (fork) cudaEventDestroy(fork);
+    if (join) cudaEventDestroy(join);
+    cudaFreeAsync(ws, st);
+    return e;
+}
+
+// Every kernel of the codec is launched here, on `st` of the current device.
+cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
+    if (a.n <= 0) return cudaSuccess;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const Dev* D = dev_state(dev);
+    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
+    const int n = (int)a.n;
+    switch (op) {
+    case OP_ENCODE: {
+        int nl = 0;
+        const cudaError_t ee = encode_launch(a, a.level | (a.x32 ? k4::ENC_FLAG_X32 : 0), *D, st, &nl);
+        g_launches += nl;
+        if (ee != cudaSuccess) { (void)cudaGetLastError(); return ee; }
+        break;
+    }
+    case OP_DECODE:
+    case OP_CHAIN: {
+        const cudaError_t de = k4::decode_launch(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.dstCap,
+                                                 op == OP_CHAIN ? a.prefixLen : nullptr, a.outLen, n, st, D->pool, D->sms);
+        if (de != cudaSuccess) { (void)cudaGetLastError(); return de; }
+        g_launches += k4::DECODE_LAUNCHES;
+        break;
+    }
+    case OP_GENERAL:
+        k4::decode_general_kernel<<<(n + 3) / 4, 128, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
+                                                               a.dstCap, a.dictBase, a.dictOff, a.dictLen, a.outLen,
+                                                               n, a.partial ? 1 : 0);
+        g_launches++;
+        break;
+    case OP_PICKLE:
+    case OP_PICKLEW: {
+        const int ctas = (n + k4::ENC_WARPS_PER_CTA - 1) / k4::ENC_WARPS_PER_CTA;
+        k4::pickle_kernel<<<ctas, k4::ENC_WARPS_PER_CTA * 32,
+                            k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES, st>>>(
+            a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.outLen, n, a.level, op == OP_PICKLEW ? 1 : 0);
+        g_launches++;
+        break;
+    }
+    case OP_UNPICKLE:
+        k4::unpickle_kernel<<<(n + 3) / 4, 128, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
+                                                         a.dstCap, a.outLen, n);
+        g_launches++;
+        break;
+    case OP_USIZE:
+        k4::unpickled_size_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.outLen, n);
+        g_launches++;
+        break;
+    case OP_XXH32:
+        k4::xxh32_batch_kernel<<<(unsigned)(((int64_t)n * 4 + 127) / 128), 128, 0, st>>>(
+            a.srcBase, a.srcOff, a.srcLen, a.seed, reinterpret_cast<uint32_t*>(a.outLen), n);
+        g_launches++;
+        break;
+    case OP_COPY:      // srcLen[i] bytes of block i
+        k4::copy_blocks_kernel<<<n, 256, 0, st>>>(a.srcBase, a.srcOff, a.dstBase, a.dstOff, a.srcLen, n);
+        g_launches++;
+        break;
+    }
+    return cudaGetLastError();
+}
+
+// ---- pipelined host path: encode / decode / pickle / unpickle --------------------------------------
+
+inline int64_t dst_room(Op op, const Batch& a, int64_t i) {
     switch (op) {
     case OP_PICKLE: return a.srcLen[i] <= 0 ? 0 : (int64_t)a.srcLen[i] + 1;
     case OP_PICKLEW: return a.srcLen[i] <= 0 ? 0 : (int64_t)a.srcLen[i] + 1 + k4::pickle_diff_width(a.srcLen[i]);
@@ -306,7 +364,7 @@ inline int64_t dst_room(Op op, const HostArgs& a, int64_t i) {
     default: return a.dstCap[i] < 0 ? 0 : a.dstCap[i];
     }
 }
-inline int64_t src_size(const HostArgs& a, int64_t i) { return a.srcLen[i] < 0 ? 0 : a.srcLen[i]; }
+inline int64_t src_size(const Batch& a, int64_t i) { return a.srcLen[i] < 0 ? 0 : a.srcLen[i]; }
 
 void parallel_for_blocks(int64_t b0, int64_t b1, int64_t bytesHint, const std::function<void(int64_t, int64_t)>& fn);
 int launch_chunk(Op op, Slot& s);
@@ -315,7 +373,7 @@ constexpr int64_t CHUNK_BYTES = 192ll << 20;   // src + dst payload per in-fligh
 
 // Copies every produced byte of chunk [b0,b1) from the pinned staging buffer into the
 // caller's destination; bytes at index >= outLen[i] are never touched.
-void scatter_chunk(Op op, const HostArgs& a, Slot& s) {
+void scatter_chunk(Op op, const Batch& a, Slot& s) {
     if (op == OP_USIZE) return;
     const uint8_t* stage = (const uint8_t*)s.hDst.p;
     int64_t total = 0;
@@ -335,7 +393,7 @@ void scatter_chunk(Op op, const HostArgs& a, Slot& s) {
 // data D2H.  When every block filled its whole slot and the slots are contiguous (the decode
 // case) the bytes go straight into the caller's buffer in one copy; otherwise through the pinned
 // staging buffer and a host-side scatter (stage 3) that leaves bytes >= outLen[i] untouched.
-int stage2_slot(Op op, const HostArgs& a, Slot& s) {
+int stage2_slot(Op op, const Batch& a, Slot& s) {
     if (s.state == 3) { int rc = launch_chunk(op, s); if (rc != K4LZ4_OK) return rc; }
     if (s.state != 1) return K4LZ4_OK;
     CU_TRY(cudaStreamSynchronize(s.stream));
@@ -375,18 +433,16 @@ int stage2_slot(Op op, const HostArgs& a, Slot& s) {
         CU_TRY(s.hDst.ensure((size_t)total + 16));
         memcpy(s.hPackOff.p, s.compactOff.data(), (size_t)nb * 8);
         CU_TRY(cudaMemcpyAsync(s.dPackOff.p, s.hPackOff.p, (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
-        k4::copy_blocks_kernel<<<(unsigned)nb, 256, 0, s.stream>>>(
-            (const uint8_t*)s.dDst.p, s.dDstOffArr, (uint8_t*)s.dPack.p, (const int64_t*)s.dPackOff.p,
-            s.dOutLenArr, (int)nb);
-        g_launches++;
-        CU_TRY(cudaGetLastError());
+        Batch g{(const uint8_t*)s.dDst.p, s.dDstOffArr, s.dOutLenArr, (uint8_t*)s.dPack.p,
+                (const int64_t*)s.dPackOff.p, nullptr, nullptr, nb};
+        CU_TRY(launch_op(OP_COPY, g, s.stream));
         CU_TRY(cudaMemcpyAsync(s.hDst.p, s.dPack.p, (size_t)total, cudaMemcpyDeviceToHost, s.stream));
     }
     return K4LZ4_OK;
 }
 
 // stage 3: data has landed
-int stage3_slot(Op op, const HostArgs& a, Slot& s) {
+int stage3_slot(Op op, const Batch& a, Slot& s) {
     if (s.state == 1 || s.state == 3) { int rc = stage2_slot(op, a, s); if (rc != K4LZ4_OK) return rc; }
     if (s.state != 2) return K4LZ4_OK;
     s.state = 0;
@@ -396,7 +452,7 @@ int stage3_slot(Op op, const HostArgs& a, Slot& s) {
 }
 
 // stage 1a: stage the chunk's inputs and block table on the device (asynchronous copies on the slot's stream)
-int enqueue_chunk(Op op, const HostArgs& a, Slot& s, int64_t b0, int64_t b1) {
+int enqueue_chunk(Op op, const Batch& a, Slot& s, int64_t b0, int64_t b1) {
     const int64_t nb = b1 - b0;
     s.b0 = b0; s.b1 = b1;
     // extents
@@ -458,8 +514,10 @@ int enqueue_chunk(Op op, const HostArgs& a, Slot& s, int64_t b0, int64_t b1) {
         CU_TRY(cudaMemcpyAsync(s.dSrc.p, srcPacked ? (const void*)s.hSrc.p : (const void*)(a.srcBase + sLo),
                                (size_t)srcBytes, cudaMemcpyHostToDevice, st));
     CU_TRY(cudaMemcpyAsync(s.dMeta.p, s.hMeta.p, (size_t)nb * 24, cudaMemcpyHostToDevice, st));
-    s.launch = DevArgs{(const uint8_t*)s.dSrc.p, dSrcOff, dSrcLen, (uint8_t*)s.dDst.p, dDstOff, dDstCap,
-                       dOutLen, (int)nb, a.level};
+    s.launch = a;
+    s.launch.srcBase = (const uint8_t*)s.dSrc.p; s.launch.srcOff = dSrcOff; s.launch.srcLen = dSrcLen;
+    s.launch.dstBase = (uint8_t*)s.dDst.p; s.launch.dstOff = dDstOff; s.launch.dstCap = dDstCap;
+    s.launch.outLen = dOutLen; s.launch.n = nb;
     s.dDstOffArr = dDstOff;
     s.dOutLenArr = dOutLen;
     s.state = 3;
@@ -477,26 +535,18 @@ int launch_chunk(Op op, Slot& s) {
     return K4LZ4_OK;
 }
 
-// blocks the encoder finishes in about one shared-memory-warp block time on `dev` (a global-table warp counts half)
-int64_t enc_wave_blocks(int dev) {
-    static int sms[64] = {0};
-    if (dev < 0 || dev >= 64) return 1;
-    if (!sms[dev]) { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) v = 0; sms[dev] = v > 0 ? v : -1; }
-    return sms[dev] > 0 ? (int64_t)sms[dev] * (k4::ENC_SM_WARPS + (k4::ENC_GM_WARPS + 1) / 2) : 1;
-}
-
 // One device, blocks [b0, b1): chunked + double-buffered (H2D/kernel/D2H of chunk c overlap
 // the host-side scatter of chunk c-1 and the copies of chunk c+1 on the other stream).
-int run_host_slice(Op op, const HostArgs& a, int64_t b0, int64_t b1, int dev) {
+int run_host_slice(Op op, const Batch& a, int64_t b0, int64_t b1, int dev) {
     if (b1 <= b0) return K4LZ4_OK;
-    DevCtx* ctx = get_ctx(dev);
-    std::lock_guard<std::mutex> lk(ctx->mu);
     DeviceGuard g(dev);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
-    if (!ctx->init) {
-        for (auto& s : ctx->slot) CU_TRY(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-        ctx->init = true;
-    }
+    Dev* ctx = dev_state(dev);
+    if (!ctx) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
+    if (ctx->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed: %s", dev, cudaGetErrorString(ctx->err));
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    // blocks the encoder finishes in about one shared-memory-warp block time (a global-table warp counts half)
+    const int64_t W = (int64_t)ctx->sms * (k4::ENC_SM_WARPS + (k4::ENC_GM_WARPS + 1) / 2);
     int rc = K4LZ4_OK;
     // Chunk boundaries.  Encode: a warp works on one block for milliseconds; consecutive chunks' kernels
     // overlap (one-warp CTAs leave individually and the next launch, on another stream, moves in), so a
@@ -507,7 +557,7 @@ int run_host_slice(Op op, const HostArgs& a, int64_t b0, int64_t b1, int dev) {
         int64_t bytes = 0, j = i;
         int64_t limit = CHUNK_BYTES, maxBlocks = INT64_MAX;
         if (op == OP_ENCODE) {
-            const int64_t W = enc_wave_blocks(dev), rem = b1 - i;
+            const int64_t rem = b1 - i;
             limit = 2560ll << 20;
             if (c == 0) maxBlocks = W;
             else if (c == 1) maxBlocks = 2 * W;
@@ -615,16 +665,9 @@ void bind_thread_near_gpu(int dev) {
 #endif
 }
 
-int run_host(Op op, const HostArgs& a, int64_t n, int device) {
+int run_host(Op op, const Batch& a, int device) {
+    const int64_t n = a.n;
     const int ndev = device_count_cached();
-    if (ndev <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (n < 0) return fail(K4LZ4_E_ARG, "negative block count");
-    if (n == 0) return K4LZ4_OK;
-    if (!a.srcBase || !a.srcOff || !a.srcLen || !a.outLen) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (op != OP_USIZE && (!a.dstBase || !a.dstOff)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if ((op == OP_ENCODE || op == OP_DECODE || op == OP_UNPICKLE) && !a.dstCap)
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (device >= ndev) return fail(K4LZ4_E_ARG, "device %d out of range (%d visible)", device, ndev);
     if (device >= 0 || ndev == 1) return run_host_slice(op, a, 0, n, device >= 0 ? device : 0);
 
     // K4LZ4_ALL_DEVICES: contiguous split balanced by bytes, one host thread per GPU
@@ -651,218 +694,135 @@ int run_host(Op op, const HostArgs& a, int64_t n, int device) {
     return K4LZ4_OK;
 }
 
-int run(Op op, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen, uint8_t* dstBase,
-        const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int64_t n, int level,
-        int memKind, void* stream, int device) {
-    if (memKind == K4LZ4_MEM_DEVICE) {
-        if (n > INT32_MAX) return fail(K4LZ4_E_ARG, "too many blocks");
-        DevArgs d{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, (int)n, level};
-        return run_device(op, d, stream, device);
-    }
-    if (memKind == K4LZ4_MEM_HOST) {
-        HostArgs h{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, level};
-        return run_host(op, h, n, device);
-    }
-    return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-}
+// ---- synchronous host path: dictionary / partial / chained decode and XXH32 ------------------------
 
-// ---- dictionary / partial decode (SURVEY 8f rows 3 and 4): exactness first, simple staging ------
-
-struct GeneralArgs {
-    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
-    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap;
-    const uint8_t* dictBase; const int64_t* dictOff; const int32_t* dictLen;   // all three may be null
-    int32_t* outLen; int64_t n; bool partial;
-};
-
-cudaError_t launch_general(const GeneralArgs& g, cudaStream_t st) {
-    if (g.n <= 0) return cudaSuccess;
-    const long long ctas = (g.n + 3) / 4;
-    k4::decode_general_kernel<<<(unsigned)ctas, 128, 0, st>>>(g.srcBase, g.srcOff, g.srcLen, g.dstBase, g.dstOff,
-                                                              g.dstCap, g.dictBase, g.dictOff, g.dictLen, g.outLen,
-                                                              (int)g.n, g.partial ? 1 : 0);
-    g_launches++;
-    return cudaGetLastError();
-}
-
-struct DevMem {
-    void* p = nullptr;
+struct DevMem {         // the call's device buffer: grows with the chunks, freed when the call returns
+    void* p = nullptr; size_t cap = 0;
     ~DevMem() { if (p) cudaFree(p); }
-    cudaError_t alloc(size_t n) { return cudaMalloc(&p, n ? n : 1); }
+    cudaError_t ensure(size_t n) {
+        if (n <= cap) return cudaSuccess;
+        if (p) cudaFree(p);
+        cap = 0;
+        const cudaError_t e = cudaMalloc(&p, n);
+        if (e == cudaSuccess) cap = n; else p = nullptr;
+        return e;
+    }
 };
 
-// host pointers: pack the blocks of a chunk, one H2D per array, one kernel, one D2H, exact scatter
-int run_general_host(const GeneralArgs& g, int device) {
-    const int ndev = device_count_cached();
-    if (ndev <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (g.n < 0) return fail(K4LZ4_E_ARG, "negative block count");
-    if (g.n == 0) return K4LZ4_OK;
-    if (!g.srcBase || !g.srcOff || !g.srcLen || !g.dstBase || !g.dstOff || !g.dstCap || !g.outLen)
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (g.dictBase && (!g.dictOff || !g.dictLen)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    const int dev = device >= 0 ? device : 0;
-    if (dev >= ndev) return fail(K4LZ4_E_ARG, "device %d out of range (%d visible)", dev, ndev);
+constexpr int64_t STAGE_BYTES = 256ll << 20;   // staged payload per chunk
+
+// One GPU, no pipelining: per chunk of at most STAGE_BYTES, everything the kernel reads is packed into one
+// host buffer -- the block table, the sources, the dictionaries (when the batch has them) and, with a
+// prefix, the destination slots [history | capacity] (16-aligned, history filled in: all the decoder reads
+// of a stream is its last <= 65535 bytes) -- and goes up in one copy.  The results and the destination
+// region come back, and exactly outLen[i] > 0 bytes of each block are copied to the caller.  A batch
+// without dstCap (XXH32) has no destination: its per-block result is the whole output.
+int run_staged(Op op, const Batch& b, int dev) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
-    const int64_t CH = 256ll << 20;
-    int64_t i = 0;
-    while (i < g.n) {
-        int64_t j = i, bytes = 0;
-        while (j < g.n) {
-            const int64_t add = std::max<int64_t>(g.srcLen[j], 0) + std::max<int64_t>(g.dstCap[j], 0) +
-                                (g.dictBase ? std::max<int64_t>(g.dictLen[j], 0) : 0);
-            if (j > i && bytes + add > CH) break;
-            bytes += add; j++;
+    const bool dict = b.dictBase != nullptr, prefix = b.prefixLen != nullptr, dst = b.dstCap != nullptr;
+    auto hist = [&](int64_t i) -> int64_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
+    auto cap = [&](int64_t i) -> int64_t { return dst ? std::max<int32_t>(b.dstCap[i], 0) : 0; };
+    auto dlen = [&](int64_t i) -> int64_t { return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0; };
+    auto up = [](int64_t x) { return (x + 255) & ~int64_t(255); };
+    std::vector<uint8_t> h;          // reused by every chunk: the kernel reads only bytes the chunk has written
+    DevMem d;
+    for (int64_t i = 0, j; i < b.n; i = j) {
+        int64_t bytes = 0;
+        for (j = i; j < b.n; j++) {
+            const int64_t add = src_size(b, j) + dlen(j) + cap(j) + (prefix ? hist(j) + 16 : 0);
+            if (j > i && bytes + add > STAGE_BYTES) break;
+            bytes += add;
         }
         const int64_t nb = j - i;
-        std::vector<int64_t> so(nb), doff(nb), dio(nb);
-        std::vector<int32_t> sl(nb), dc(nb), dl(nb), res(nb);
-        int64_t sTot = 0, dTot = 0, diTot = 0;
+        // block table: srcOff dstOff dictOff (int64) | srcLen dstCap dictLen prefixLen outLen (int32)
+        int64_t sTot = 0, diTot = 0, dTot = 0;
         for (int64_t k = 0; k < nb; k++) {
-            sl[k] = g.srcLen[i + k]; dc[k] = g.dstCap[i + k] < 0 ? 0 : g.dstCap[i + k];
-            dl[k] = g.dictBase ? std::max<int32_t>(g.dictLen[i + k], 0) : 0;
-            so[k] = sTot; doff[k] = dTot; dio[k] = diTot;
-            sTot += std::max<int32_t>(sl[k], 0); dTot += dc[k]; diTot += dl[k];
+            sTot += src_size(b, i + k); diTot += dlen(i + k);
+            dTot = (prefix ? (dTot + hist(i + k) + 15) & ~int64_t(15) : dTot) + cap(i + k);
         }
-        std::vector<uint8_t> hs((size_t)sTot + 16), hd((size_t)diTot + 16), ho((size_t)dTot + 16);
+        const int64_t srcAt = up(nb * (3 * 8 + 5 * 4)), dictAt = up(srcAt + sTot), dstAt = up(dictAt + diTot);
+        const int64_t total = dstAt + dTot;
+        if (h.size() < (size_t)total + 16) h.resize((size_t)total + 16);
+        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* dio = doff + nb;
+        int32_t* sl = (int32_t*)(dio + nb); int32_t* dc = sl + nb; int32_t* dl = dc + nb; int32_t* pl = dl + nb;
+        int32_t* res = pl + nb;
+        for (int64_t k = 0, sp = 0, dip = 0, dp = 0; k < nb; k++) {
+            const int64_t x = i + k;
+            sl[k] = b.srcLen[x]; dc[k] = dst ? b.dstCap[x] : 0; dl[k] = (int32_t)dlen(x); pl[k] = (int32_t)hist(x);
+            so[k] = sp; dio[k] = dip;
+            doff[k] = prefix ? (dp + pl[k] + 15) & ~int64_t(15) : dp;
+            if (sl[k] > 0) memcpy(h.data() + srcAt + sp, b.srcBase + b.srcOff[x], (size_t)sl[k]);
+            if (dl[k] > 0) memcpy(h.data() + dictAt + dip, b.dictBase + b.dictOff[x], (size_t)dl[k]);
+            if (pl[k] > 0) memcpy(h.data() + dstAt + doff[k] - pl[k], b.dstBase + b.dstOff[x] - pl[k], (size_t)pl[k]);
+            sp += src_size(b, x); dip += dl[k]; dp = doff[k] + cap(x);
+        }
+        CU_TRY(d.ensure((size_t)total + 16));
+        uint8_t* D = (uint8_t*)d.p;
+        CU_TRY(cudaMemcpy(D, h.data(), (size_t)(prefix ? total : dstAt), cudaMemcpyHostToDevice));
+        int32_t* dRes = (int32_t*)(D + ((uint8_t*)res - h.data()));
+        Batch kb = b;                                // the same batch, on the device
+        kb.srcBase = D + srcAt; kb.srcOff = (int64_t*)D; kb.srcLen = (int32_t*)(D + ((uint8_t*)sl - h.data()));
+        kb.dstBase = D + dstAt; kb.dstOff = kb.srcOff + nb; kb.dstCap = dst ? kb.srcLen + nb : nullptr;
+        kb.dictBase = dict ? D + dictAt : nullptr; kb.dictOff = kb.srcOff + 2 * nb; kb.dictLen = kb.srcLen + 2 * nb;
+        kb.prefixLen = prefix ? kb.srcLen + 3 * nb : nullptr;
+        kb.outLen = dRes; kb.n = nb;
+        CU_TRY(launch_op(op, kb, nullptr));
+        CU_TRY(cudaMemcpy(b.outLen + i, dRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
+        if (!dst || dTot == 0) continue;
+        CU_TRY(cudaMemcpy(h.data() + dstAt, D + dstAt, (size_t)dTot, cudaMemcpyDeviceToHost));
         for (int64_t k = 0; k < nb; k++) {
-            if (sl[k] > 0) memcpy(hs.data() + so[k], g.srcBase + g.srcOff[i + k], (size_t)sl[k]);
-            if (dl[k] > 0) memcpy(hd.data() + dio[k], g.dictBase + g.dictOff[i + k], (size_t)dl[k]);
+            const int32_t r = b.outLen[i + k];
+            if (r > 0) memcpy(b.dstBase + b.dstOff[i + k], h.data() + dstAt + doff[k], (size_t)r);
         }
-        DevMem dS, dD, dO, dM;
-        CU_TRY(dS.alloc((size_t)sTot + 16)); CU_TRY(dD.alloc((size_t)diTot + 16)); CU_TRY(dO.alloc((size_t)dTot + 16));
-        CU_TRY(dM.alloc((size_t)nb * (8 * 3 + 4 * 4)));
-        int64_t* mSo = (int64_t*)dM.p; int64_t* mDo = mSo + nb; int64_t* mDio = mDo + nb;
-        int32_t* mSl = (int32_t*)(mDio + nb); int32_t* mDc = mSl + nb; int32_t* mDl = mDc + nb; int32_t* mRes = mDl + nb;
-        CU_TRY(cudaMemcpy(dS.p, hs.data(), (size_t)sTot, cudaMemcpyHostToDevice));
-        if (diTot) CU_TRY(cudaMemcpy(dD.p, hd.data(), (size_t)diTot, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mSo, so.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDo, doff.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDio, dio.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mSl, sl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDc, dc.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDl, dl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        GeneralArgs d{(const uint8_t*)dS.p, mSo, mSl, (uint8_t*)dO.p, mDo, mDc,
-                      g.dictBase ? (const uint8_t*)dD.p : nullptr, mDio, mDl, mRes, nb, g.partial};
-        CU_TRY(launch_general(d, nullptr));
-        CU_TRY(cudaMemcpy(res.data(), mRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
-        if (dTot) CU_TRY(cudaMemcpy(ho.data(), dO.p, (size_t)dTot, cudaMemcpyDeviceToHost));
-        for (int64_t k = 0; k < nb; k++) {
-            g.outLen[i + k] = res[k];
-            if (res[k] > 0) memcpy(g.dstBase + g.dstOff[i + k], ho.data() + doff[k], (size_t)res[k]);
-        }
-        i = j;
     }
     return K4LZ4_OK;
 }
 
-int run_general(const GeneralArgs& g, int memKind, void* stream, int device) {
-    if (memKind == K4LZ4_MEM_HOST) return run_general_host(g, device);
-    if (memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (g.n < 0 || g.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count");
-    if (g.n == 0) return K4LZ4_OK;
-    if (!g.srcBase || !g.srcOff || !g.srcLen || !g.dstBase || !g.dstOff || !g.dstCap || !g.outLen)
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (g.dictBase && (!g.dictOff || !g.dictLen)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    CU_TRY(launch_general(g, (cudaStream_t)stream));
+int run(Op op, const Batch& b, int memKind, void* stream, int device) {
+    const int rc = check(op, b, memKind, device);
+    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    if (memKind == K4LZ4_MEM_HOST)
+        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32) ? run_staged(op, b, device < 0 ? 0 : device)
+                                                                        : run_host(op, b, device);
+    DeviceGuard g(device);
+    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    CU_TRY(launch_op(op, b, (cudaStream_t)stream));
     return K4LZ4_OK;
 }
 
-// ---- chained blocks (LZ4ChainDecoder): tile path with a history window, simple host staging ---------
-
-struct ChainArgs {
-    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
-    uint8_t* dstBase; const int64_t* dstOff; const int32_t* dstCap; const int32_t* prefixLen;
-    int32_t* outLen; int32_t n;
-};
-
-int launch_chain(const ChainArgs& c, cudaStream_t st) {
-    cudaError_t de = cudaSuccess;
-    const int nl = k4::decode_launch(c.srcBase, c.srcOff, c.srcLen, c.dstBase, c.dstOff, c.dstCap, c.outLen, c.n,
-                                     st, &de, c.prefixLen);
-    if (nl < 0) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain decode launch failed: %s", cudaGetErrorString(de)); }
-    g_launches += nl;
-    CU_TRY(cudaGetLastError());
-    return K4LZ4_OK;
+// One block in host memory through the batched path, after the reference's answers that need no device.
+int32_t run_one(Op op, const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap, int level = 0,
+                bool x32 = false, const uint8_t* dict = nullptr, int32_t dictLen = 0, bool partial = false) {
+    if (srcLen <= 0) return 0;                       // LZ4Codec.cs:45-46,108-109,129-130,150-151
+    if (op == OP_ENCODE && level >= 3) return K4LZ4_R_DELEGATE;
+    if (!src || (!dst && dstCap > 0) || (!dict && dictLen > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (dstCap <= 0) return -1;                      // nothing fits in an empty target (LL64.dec.cs:162-168; LZ4Codec.cs:135)
+    int64_t zero = 0; int32_t out = -1;
+    Batch b{src, &zero, &srcLen, dst, &zero, &dstCap, &out, 1};
+    // the encoder reads bits 0-7 of its level word as the level and bit 8 as the 32-bit switch: a level
+    // below 0 reaches it as that word
+    const int word = level | (x32 ? k4::ENC_FLAG_X32 : 0);
+    b.level = word & 0xFF; b.x32 = (word & k4::ENC_FLAG_X32) != 0;
+    if (dictLen > 0) { b.dictBase = dict; b.dictOff = &zero; b.dictLen = &dictLen; }
+    b.partial = partial;
+    const int rc = run(op, b, K4LZ4_MEM_HOST, nullptr, 0);
+    return rc != K4LZ4_OK ? rc : out;
 }
 
-// host pointers: per chunk, every block's history (its last <= 65535 bytes: all the decoder reads) is staged
-// directly in front of its device slot; one H2D per array, one decode, one D2H, exact scatter
-int run_chain_host(const ChainArgs& c, int device) {
-    const int ndev = device_count_cached();
-    if (ndev <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    const int dev = device >= 0 ? device : 0;
-    if (dev >= ndev) return fail(K4LZ4_E_ARG, "device %d out of range (%d visible)", dev, ndev);
-    DeviceGuard guard(dev);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
-    const int64_t CH = 256ll << 20;
-    auto hist = [&](int64_t i) { return (int64_t)std::min<int32_t>(c.prefixLen[i], 65535); };
-    int64_t i = 0;
-    while (i < c.n) {
-        int64_t j = i, bytes = 0;
-        while (j < c.n) {
-            const int64_t add = std::max<int32_t>(c.srcLen[j], 0) + std::max<int32_t>(c.dstCap[j], 0) + hist(j) + 16;
-            if (j > i && bytes + add > CH) break;
-            bytes += add; j++;
-        }
-        const int64_t nb = j - i;
-        std::vector<int64_t> so(nb), doff(nb);
-        std::vector<int32_t> sl(nb), dc(nb), pl(nb), res(nb);
-        int64_t sTot = 0, dTot = 0;
-        for (int64_t k = 0; k < nb; k++) {
-            sl[k] = c.srcLen[i + k]; dc[k] = c.dstCap[i + k]; pl[k] = (int32_t)hist(i + k);
-            so[k] = sTot; sTot += std::max<int32_t>(sl[k], 0);
-            doff[k] = (dTot + pl[k] + 15) & ~int64_t(15);           // slot = [history | destination], 16-aligned
-            dTot = doff[k] + std::max<int32_t>(dc[k], 0);
-        }
-        std::vector<uint8_t> hs((size_t)sTot + 16), hd((size_t)dTot + 16);
-        for (int64_t k = 0; k < nb; k++) {
-            if (sl[k] > 0) memcpy(hs.data() + so[k], c.srcBase + c.srcOff[i + k], (size_t)sl[k]);
-            if (pl[k] > 0) memcpy(hd.data() + doff[k] - pl[k], c.dstBase + c.dstOff[i + k] - pl[k], (size_t)pl[k]);
-        }
-        DevMem dS, dO, dM;
-        CU_TRY(dS.alloc((size_t)sTot + 16)); CU_TRY(dO.alloc((size_t)dTot + 16));
-        CU_TRY(dM.alloc((size_t)nb * (8 * 2 + 4 * 4)));
-        int64_t* mSo = (int64_t*)dM.p; int64_t* mDo = mSo + nb;
-        int32_t* mSl = (int32_t*)(mDo + nb); int32_t* mDc = mSl + nb; int32_t* mPl = mDc + nb; int32_t* mRes = mPl + nb;
-        CU_TRY(cudaMemcpy(dS.p, hs.data(), (size_t)sTot, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(dO.p, hd.data(), (size_t)dTot, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mSo, so.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDo, doff.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mSl, sl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mDc, dc.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        CU_TRY(cudaMemcpy(mPl, pl.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
-        ChainArgs d{(const uint8_t*)dS.p, mSo, mSl, (uint8_t*)dO.p, mDo, mDc, mPl, mRes, (int32_t)nb};
-        const int rc = launch_chain(d, nullptr);
-        if (rc != K4LZ4_OK) return rc;
-        CU_TRY(cudaMemcpy(res.data(), mRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
-        CU_TRY(cudaMemcpy(hd.data(), dO.p, (size_t)dTot, cudaMemcpyDeviceToHost));
-        for (int64_t k = 0; k < nb; k++) {
-            c.outLen[i + k] = res[k];
-            if (res[k] > 0) memcpy(c.dstBase + c.dstOff[i + k], hd.data() + doff[k], (size_t)res[k]);
-        }
-        i = j;
-    }
+// Counter array `sym` (4 x u64) of `device`, after the device is idle.
+int read_stats(const void* sym, int32_t device, uint64_t* out4, int32_t reset) {
+    if (!out4) return fail(K4LZ4_E_ARG, "null pointer argument");
+    const int rc = check_device(device, 1);
+    if (rc != K4LZ4_OK) return rc;
+    DeviceGuard g(device);
+    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    unsigned long long v[4] = {0, 0, 0, 0};
+    CU_TRY(cudaDeviceSynchronize());
+    CU_TRY(cudaMemcpyFromSymbol(v, sym, sizeof(v)));
+    for (int i = 0; i < 4; i++) out4[i] = v[i];
+    if (reset) { unsigned long long z[4] = {0, 0, 0, 0}; CU_TRY(cudaMemcpyToSymbol(sym, z, sizeof(z))); }
     return K4LZ4_OK;
-}
-
-int run_chain(const ChainArgs& c, int memKind, void* stream, int device) {
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (c.n < 0) return fail(K4LZ4_E_ARG, "negative block count");
-    if (c.n > 0 && (!c.srcBase || !c.srcOff || !c.srcLen || !c.dstBase || !c.dstOff || !c.dstCap || !c.prefixLen || !c.outLen))
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST)                   // device arrays cannot be checked here: there a negative prefix gives -1
-        for (int32_t i = 0; i < c.n; i++)
-            if (c.prefixLen[i] < 0) return fail(K4LZ4_E_ARG, "negative prefix length at block %d", i);
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (c.n == 0) return K4LZ4_OK;
-    if (memKind == K4LZ4_MEM_HOST) return run_chain_host(c, device);
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    return launch_chain(c, (cudaStream_t)stream);
 }
 
 }  // namespace
@@ -877,29 +837,11 @@ const char* k4lz4_last_error(void) { return t_err.c_str(); }
 int64_t k4lz4_launch_count(void) { return g_launches.load(); }
 
 int32_t k4lz4_decode_stats(int32_t device, uint64_t* out4, int32_t reset) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (!out4) return fail(K4LZ4_E_ARG, "null pointer argument");
-    DeviceGuard g(device);
-    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    unsigned long long v[4] = {0, 0, 0, 0};
-    CU_TRY(cudaDeviceSynchronize());
-    CU_TRY(cudaMemcpyFromSymbol(v, k4::g_decode_stats, sizeof(v)));
-    for (int i = 0; i < 4; i++) out4[i] = v[i];
-    if (reset) { unsigned long long z[4] = {0, 0, 0, 0}; CU_TRY(cudaMemcpyToSymbol(k4::g_decode_stats, z, sizeof(z))); }
-    return K4LZ4_OK;
+    return read_stats((const void*)&k4::g_decode_stats, device, out4, reset);
 }
 
 int32_t k4lz4_encode_stats(int32_t device, uint64_t* out4, int32_t reset) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (!out4) return fail(K4LZ4_E_ARG, "null pointer argument");
-    DeviceGuard g(device);
-    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    unsigned long long v[4] = {0, 0, 0, 0};
-    CU_TRY(cudaDeviceSynchronize());
-    CU_TRY(cudaMemcpyFromSymbol(v, k4::g_encode_stats, sizeof(v)));
-    for (int i = 0; i < 4; i++) out4[i] = v[i];
-    if (reset) { unsigned long long z[4] = {0, 0, 0, 0}; CU_TRY(cudaMemcpyToSymbol(k4::g_encode_stats, z, sizeof(z))); }
-    return K4LZ4_OK;
+    return read_stats((const void*)&k4::g_encode_stats, device, out4, reset);
 }
 
 #ifdef K4_DT_PROFILE
@@ -918,43 +860,24 @@ int32_t k4lz4_max_output_size(int32_t length) { return k4::max_output_size(lengt
 int32_t k4lz4_pickle_bound(int32_t length) { return length <= 0 ? 0 : length + 1; }
 
 int32_t k4lz4_encode(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap, int32_t level) {
-    if (srcLen <= 0) return 0;                       // LZ4Codec.cs:45-46
-    if (level >= 3) return K4LZ4_R_DELEGATE;
-    if (!src || (!dst && dstCap > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (dstCap <= 0) return -1;                      // nothing fits in an empty target
-    int64_t so = 0, dof = 0; int32_t out = -1;
-    int rc = run(OP_ENCODE, src, &so, &srcLen, dst, &dof, &dstCap, &out, 1, level, K4LZ4_MEM_HOST, nullptr, 0);
-    return rc != K4LZ4_OK ? rc : out;
+    return run_one(OP_ENCODE, src, srcLen, dst, dstCap, level);
+}
+
+int32_t k4lz4_encode_x32(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap, int32_t level) {
+    return run_one(OP_ENCODE, src, srcLen, dst, dstCap, level, true);
 }
 
 int32_t k4lz4_decode(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap) {
-    if (srcLen <= 0) return 0;                       // LZ4Codec.cs:108-109
-    if (!src || (!dst && dstCap > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (dstCap <= 0) return -1;                      // LL64.dec.cs:162-168 gives 0 or -1 => -1
-    int64_t so = 0, dof = 0; int32_t out = -1;
-    int rc = run(OP_DECODE, src, &so, &srcLen, dst, &dof, &dstCap, &out, 1, 0, K4LZ4_MEM_HOST, nullptr, 0);
-    return rc != K4LZ4_OK ? rc : out;
+    return run_one(OP_DECODE, src, srcLen, dst, dstCap);
 }
 
 int32_t k4lz4_decode_dict(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap,
                           const uint8_t* dict, int32_t dictLen) {
-    if (srcLen <= 0) return 0;                       // LZ4Codec.cs:150-151
-    if (!src || (!dst && dstCap > 0) || (!dict && dictLen > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (dstCap <= 0) return -1;
-    int64_t zero = 0; int32_t out = -1;
-    GeneralArgs g{src, &zero, &srcLen, dst, &zero, &dstCap, dictLen > 0 ? dict : nullptr, &zero, &dictLen, &out, 1, false};
-    const int rc = run_general(g, K4LZ4_MEM_HOST, nullptr, 0);
-    return rc != K4LZ4_OK ? rc : out;
+    return run_one(OP_GENERAL, src, srcLen, dst, dstCap, 0, false, dict, dictLen);
 }
 
 int32_t k4lz4_partial_decode(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t targetLen) {
-    if (srcLen <= 0) return 0;                       // LZ4Codec.cs:129-130
-    if (!src || (!dst && targetLen > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (targetLen <= 0) return -1;                   // engine returns 0 -> -1 (LZ4Codec.cs:135)
-    int64_t zero = 0; int32_t out = -1;
-    GeneralArgs g{src, &zero, &srcLen, dst, &zero, &targetLen, nullptr, nullptr, nullptr, &out, 1, true};
-    const int rc = run_general(g, K4LZ4_MEM_HOST, nullptr, 0);
-    return rc != K4LZ4_OK ? rc : out;
+    return run_one(OP_GENERAL, src, srcLen, dst, targetLen, 0, false, nullptr, 0, true);
 }
 
 int32_t k4lz4_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -962,59 +885,50 @@ int32_t k4lz4_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, c
                                 const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen,
                                 int32_t* outLen, int32_t nBlocks, int32_t memKind, void* cudaStream,
                                 int32_t device) {
-    GeneralArgs g{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, dictBase, dictOff, dictLen, outLen, nBlocks, false};
-    return run_general(g, memKind, cudaStream, device);
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
+    b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
+    return run(OP_GENERAL, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                  uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
                                  const int32_t* prefixLen, int32_t* outLen, int32_t nBlocks,
                                  int32_t memKind, void* cudaStream, int32_t device) {
-    ChainArgs c{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, nBlocks};
-    return run_chain(c, memKind, cudaStream, device);
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
+    b.prefixLen = prefixLen;
+    return run(OP_CHAIN, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_partial_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                    uint8_t* dstBase, const int64_t* dstOff, const int32_t* targetLen,
                                    int32_t* outLen, int32_t nBlocks, int32_t memKind, void* cudaStream,
                                    int32_t device) {
-    GeneralArgs g{srcBase, srcOff, srcLen, dstBase, dstOff, targetLen, nullptr, nullptr, nullptr, outLen, nBlocks, true};
-    return run_general(g, memKind, cudaStream, device);
-}
-
-int32_t k4lz4_encode_x32(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap, int32_t level) {
-    if (srcLen <= 0) return 0;
-    if (level >= 3) return K4LZ4_R_DELEGATE;
-    if (!src || (!dst && dstCap > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (dstCap <= 0) return -1;
-    int64_t so = 0, dof = 0; int32_t out = -1;
-    int rc = run(OP_ENCODE, src, &so, &srcLen, dst, &dof, &dstCap, &out, 1, level | k4::ENC_FLAG_X32, K4LZ4_MEM_HOST, nullptr, 0);
-    return rc != K4LZ4_OK ? rc : out;
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, targetLen, outLen, nBlocks};
+    b.partial = true;
+    return run(OP_GENERAL, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_encode_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
                                int32_t* outLen, int32_t nBlocks, int32_t level, int32_t memKind,
                                void* cudaStream, int32_t device) {
-    if (level < 0 || level > 0xFF) return fail(K4LZ4_E_ARG, "bad level");
-    return run(OP_ENCODE, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level | k4::ENC_FLAG_X32,
-               memKind, cudaStream, device);
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level, true};
+    return run(OP_ENCODE, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_encode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                            uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
                            int32_t* outLen, int32_t nBlocks, int32_t level, int32_t memKind,
                            void* cudaStream, int32_t device) {
-    if (level < 0 || level > 0xFF) return fail(K4LZ4_E_ARG, "bad level");
-    return run(OP_ENCODE, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level,
-               memKind, cudaStream, device);
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level};
+    return run(OP_ENCODE, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                            uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
                            int32_t* outLen, int32_t nBlocks, int32_t memKind, void* cudaStream,
                            int32_t device) {
-    return run(OP_DECODE, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, 0,
+    return run(OP_DECODE, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks},
                memKind, cudaStream, device);
 }
 
@@ -1022,7 +936,7 @@ int32_t k4lz4_pickle_batch(const uint8_t* srcBase, const int64_t* srcOff, const 
                            uint8_t* dstBase, const int64_t* dstOff, int32_t* outLen,
                            int32_t nMessages, int32_t level, int32_t memKind, void* cudaStream,
                            int32_t device) {
-    return run(OP_PICKLE, srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level,
+    return run(OP_PICKLE, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level},
                memKind, cudaStream, device);
 }
 
@@ -1032,14 +946,14 @@ int32_t k4lz4_pickle_writer_batch(const uint8_t* srcBase, const int64_t* srcOff,
                                   uint8_t* dstBase, const int64_t* dstOff, int32_t* outLen,
                                   int32_t nMessages, int32_t level, int32_t memKind, void* cudaStream,
                                   int32_t device) {
-    return run(OP_PICKLEW, srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level,
+    return run(OP_PICKLEW, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level},
                memKind, cudaStream, device);
 }
 
 int32_t k4lz4_unpickled_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                    int32_t* outSize, int32_t nMessages, int32_t memKind,
                                    void* cudaStream, int32_t device) {
-    return run(OP_USIZE, srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nMessages, 0,
+    return run(OP_USIZE, Batch{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nMessages},
                memKind, cudaStream, device);
 }
 
@@ -1047,7 +961,7 @@ int32_t k4lz4_unpickle_batch(const uint8_t* srcBase, const int64_t* srcOff, cons
                              uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstLen,
                              int32_t* outLen, int32_t nMessages, int32_t memKind, void* cudaStream,
                              int32_t device) {
-    return run(OP_UNPICKLE, srcBase, srcOff, srcLen, dstBase, dstOff, dstLen, outLen, nMessages, 0,
+    return run(OP_UNPICKLE, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, dstLen, outLen, nMessages},
                memKind, cudaStream, device);
 }
 
@@ -1057,37 +971,9 @@ uint32_t k4lz4_xxh32(const uint8_t* data, int64_t length, uint32_t seed) {
 
 int32_t k4lz4_xxh32_batch(const uint8_t* base, const int64_t* off, const int32_t* len, uint32_t seed,
                           uint32_t* out, int32_t nBlocks, int32_t memKind, void* cudaStream, int32_t device) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
-    if (nBlocks < 0 || !base || !off || !len || !out) return fail(K4LZ4_E_ARG, "bad xxh32 arguments");
-    if (nBlocks == 0) return K4LZ4_OK;
-    DeviceGuard g(memKind == K4LZ4_MEM_HOST && device < 0 ? 0 : device);
-    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    const unsigned ctas = (unsigned)(((int64_t)nBlocks * 4 + 127) / 128);
-    if (memKind == K4LZ4_MEM_DEVICE) {
-        k4::xxh32_batch_kernel<<<ctas, 128, 0, (cudaStream_t)cudaStream>>>(base, off, len, seed, out, nBlocks);
-        g_launches++;
-        CU_TRY(cudaGetLastError());
-        return K4LZ4_OK;
-    }
-    if (memKind != K4LZ4_MEM_HOST) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    // host memory: pack, one H2D, one kernel, one D2H (checksums are a side channel of the frame writer)
-    std::vector<int64_t> po((size_t)nBlocks);
-    int64_t tot = 0;
-    for (int i = 0; i < nBlocks; i++) { po[(size_t)i] = tot; tot += len[i] > 0 ? len[i] : 0; }
-    std::vector<uint8_t> pk((size_t)tot + 16);
-    for (int i = 0; i < nBlocks; i++) if (len[i] > 0) memcpy(pk.data() + po[(size_t)i], base + off[i], (size_t)len[i]);
-    DevMem dB, dM;
-    CU_TRY(dB.alloc((size_t)tot + 16));
-    CU_TRY(dM.alloc((size_t)nBlocks * 16));
-    int64_t* dOff = (int64_t*)dM.p; int32_t* dLen = (int32_t*)(dOff + nBlocks); uint32_t* dOut = (uint32_t*)(dLen + nBlocks);
-    CU_TRY(cudaMemcpy(dB.p, pk.data(), (size_t)tot, cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(dOff, po.data(), (size_t)nBlocks * 8, cudaMemcpyHostToDevice));
-    CU_TRY(cudaMemcpy(dLen, len, (size_t)nBlocks * 4, cudaMemcpyHostToDevice));
-    k4::xxh32_batch_kernel<<<ctas, 128>>>((const uint8_t*)dB.p, dOff, dLen, seed, dOut, nBlocks);
-    g_launches++;
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpy(out, dOut, (size_t)nBlocks * 4, cudaMemcpyDeviceToHost));
-    return K4LZ4_OK;
+    Batch b{base, off, len, nullptr, nullptr, nullptr, reinterpret_cast<int32_t*>(out), nBlocks};
+    b.seed = seed;
+    return run(OP_XXH32, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_synth_host(uint8_t* base, int64_t nBlocks, int32_t blockSize, int32_t matchPermille,
@@ -1108,9 +994,9 @@ int32_t k4lz4_synth_host(uint8_t* base, int64_t nBlocks, int32_t blockSize, int3
 
 int32_t k4lz4_synth_device(uint8_t* base, int64_t nBlocks, int32_t blockSize, int32_t matchPermille,
                            uint64_t seed, int64_t firstBlock, void* cudaStream, int32_t device) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
     if (!base || nBlocks < 0 || blockSize <= 0) return fail(K4LZ4_E_ARG, "bad synth arguments");
-    if (nBlocks == 0) return K4LZ4_OK;
+    const int rc = check_device(device, nBlocks);
+    if (rc != K4LZ4_OK || nBlocks == 0) return rc;
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
     const int threads = 64;
@@ -1125,16 +1011,14 @@ int32_t k4lz4_synth_device(uint8_t* base, int64_t nBlocks, int32_t blockSize, in
 int32_t k4lz4_copy_blocks_device(const uint8_t* srcBase, const int64_t* srcOff, uint8_t* dstBase,
                                  const int64_t* dstOff, const int32_t* len, int32_t nBlocks,
                                  void* cudaStream, int32_t device) {
-    if (device_count_cached() <= 0) return fail(K4LZ4_E_NODEVICE, "no CUDA device available");
     if (nBlocks < 0 || !srcBase || !srcOff || !dstBase || !dstOff || !len)
         return fail(K4LZ4_E_ARG, "bad copy_blocks arguments");
-    if (nBlocks == 0) return K4LZ4_OK;
+    const int rc = check_device(device, nBlocks);
+    if (rc != K4LZ4_OK || nBlocks == 0) return rc;
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    k4::copy_blocks_kernel<<<nBlocks, 256, 0, (cudaStream_t)cudaStream>>>(srcBase, srcOff, dstBase,
-                                                                         dstOff, len, nBlocks);
-    g_launches++;
-    CU_TRY(cudaGetLastError());
+    CU_TRY(launch_op(OP_COPY, Batch{srcBase, srcOff, len, dstBase, dstOff, nullptr, nullptr, nBlocks},
+                     (cudaStream_t)cudaStream));
     return K4LZ4_OK;
 }
 

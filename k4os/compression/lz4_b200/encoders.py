@@ -19,7 +19,7 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, decode_chain_batch_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host
 from .codec import LZ4Codec, LZ4Level
 
 K1 = 1024
@@ -308,23 +308,8 @@ class LZ4ChainDecoder:
             d._prepare(bs)
             srcs.append(bytes(data))
             caps.append(bs)
-        # one slot per decoder: [history (<= 64 KiB) | block capacity], 16-aligned
-        hist = [min(d._prefix, d._index, 65535) for d in decoders]
-        doff = np.zeros(n, dtype=np.int64)
-        at = 0
-        for i in range(n):
-            doff[i] = (at + hist[i] + 15) // 16 * 16
-            at = int(doff[i]) + caps[i]
-        dst = np.zeros(at + 16, dtype=np.uint8)
-        for i, d in enumerate(decoders):
-            if hist[i]:
-                dst[doff[i] - hist[i]:doff[i]] = d._out[d._index - hist[i]:d._index]
-        lens = np.array([len(x) for x in srcs], dtype=np.int32)
-        soff = np.zeros(n, dtype=np.int64)
-        soff[1:] = np.cumsum(lens[:-1], dtype=np.int64)
-        src = np.frombuffer(b"".join(srcs) or b"\x00", dtype=np.uint8)
-        out = decode_chain_batch_host(src, soff, lens, dst, doff, np.array(caps, dtype=np.int32),
-                                      np.array(hist, dtype=np.int32), device)
+        hist = [d._out[d._index - min(d._prefix, d._index, 65535):d._index] for d in decoders]
+        out, data = decode_chain_blocks_host(srcs, hist, caps, device)
         res, failed = [], False
         for i, d in enumerate(decoders):
             r = int(out[i])
@@ -332,7 +317,7 @@ class LZ4ChainDecoder:
                 failed = True
                 res.append(r)
                 continue
-            d._out[d._index:d._index + r] = dst[doff[i]:doff[i] + r]
+            d._out[d._index:d._index + r] = np.frombuffer(data[i], dtype=np.uint8)
             d._index += r
             if r > 0:                                                  # LL64.dec.cs:566-590
                 d._prefix = r if d._prefix == 0 else d._prefix + r

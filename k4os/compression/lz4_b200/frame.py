@@ -22,7 +22,7 @@ import struct
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, decode_chain_batch_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host
 
 MAGIC = 0x184D2204
 _BLOCK_SIZES = {4: 1 << 16, 5: 1 << 18, 6: 1 << 20, 7: 1 << 22}
@@ -203,29 +203,12 @@ def _read_linked(frames: list, device: int) -> list:
                 todo.append((j, blk))
         if not todo:
             continue
-        n = len(todo)
-        hist = [min(len(outs[j]), 65535) for j, _ in todo]
-        caps = [frames[j].max_block for j, _ in todo]
-        doff = np.zeros(n, dtype=np.int64)
-        at = 0
-        for i in range(n):
-            doff[i] = (at + hist[i] + 15) // 16 * 16
-            at = int(doff[i]) + caps[i]
-        dst = np.zeros(at + 16, dtype=np.uint8)
+        res, data = decode_chain_blocks_host([b for _, b in todo], [outs[j] for j, _ in todo],
+                                             [frames[j].max_block for j, _ in todo], device)
         for i, (j, _) in enumerate(todo):
-            if hist[i]:
-                dst[doff[i] - hist[i]:doff[i]] = np.frombuffer(bytes(outs[j][-hist[i]:]), dtype=np.uint8)
-        lens = np.array([len(b) for _, b in todo], dtype=np.int32)
-        soff = np.zeros(n, dtype=np.int64)
-        soff[1:] = np.cumsum(lens[:-1], dtype=np.int64)
-        src = np.frombuffer(b"".join(b for _, b in todo) or b"\x00", dtype=np.uint8)
-        res = decode_chain_batch_host(src, soff, lens, dst, doff, np.array(caps, dtype=np.int32),
-                                      np.array(hist, dtype=np.int32), device)
-        for i, (j, _) in enumerate(todo):
-            r = int(res[i])
-            if r < 0:
+            if res[i] < 0:
                 raise InvalidDataException("corrupted block")   # InvalidOperationException in LZ4ChainDecoder.cs:55-56
-            outs[j] += dst[doff[i]:doff[i] + r].tobytes()
+            outs[j] += data[i]
     return [fr.check_content(bytes(o)) for fr, o in zip(frames, outs)]
 
 

@@ -5,6 +5,7 @@ import os
 import re
 
 import numpy as np
+import pytest
 
 from tests.conftest import ROOT, has_gpu
 
@@ -107,3 +108,68 @@ def test_cpp_mirror_header_compiles_and_links(native, tmp_path):
     subprocess.run([gxx, "-std=c++17", "-I", os.path.join(ROOT, "include"), str(src), "-L", libdir, "-lk4lz4",
                     f"-Wl,-rpath,{libdir}", "-o", str(exe)], check=True, capture_output=True)
     assert subprocess.run([str(exe)]).returncode == 0
+
+
+# Every batched export, called with its pointer arguments all null (`ptrs(None)`) or all pointing at
+# zeroed host arrays (empty blocks, zero capacities and prefixes).
+def _export_calls(L):
+    return {
+        "encode_batch": lambda p, n, mk, d: L.k4lz4_encode_batch(*p(7), n, 0, mk, None, d),
+        "encode_batch_x32": lambda p, n, mk, d: L.k4lz4_encode_batch_x32(*p(7), n, 0, mk, None, d),
+        "decode_batch": lambda p, n, mk, d: L.k4lz4_decode_batch(*p(7), n, mk, None, d),
+        "pickle_batch": lambda p, n, mk, d: L.k4lz4_pickle_batch(*p(6), n, 0, mk, None, d),
+        "pickle_writer_batch": lambda p, n, mk, d: L.k4lz4_pickle_writer_batch(*p(6), n, 0, mk, None, d),
+        "unpickle_batch": lambda p, n, mk, d: L.k4lz4_unpickle_batch(*p(7), n, mk, None, d),
+        "unpickled_size_batch": lambda p, n, mk, d: L.k4lz4_unpickled_size_batch(*p(4), n, mk, None, d),
+        "decode_dict_batch": lambda p, n, mk, d: L.k4lz4_decode_dict_batch(*p(10), n, mk, None, d),
+        "partial_decode_batch": lambda p, n, mk, d: L.k4lz4_partial_decode_batch(*p(7), n, mk, None, d),
+        "decode_chain_batch": lambda p, n, mk, d: L.k4lz4_decode_chain_batch(*p(8), n, mk, None, d),
+        "xxh32_batch": lambda p, n, mk, d: L.k4lz4_xxh32_batch(*p(3), 0, *p(1), n, mk, None, d),
+    }
+
+
+_EXPORTS = sorted(_export_calls(None))
+
+
+@pytest.mark.parametrize("case", ["negative_count", "null_pointer", "empty_nulls", "device_out_of_range"])
+@pytest.mark.parametrize("mem", ["host", "device", "unknown"])
+@pytest.mark.parametrize("export", _EXPORTS)
+def test_argument_error_matrix(native, export, mem, case):
+    """One check for every batched export: argument errors first (E_ARG with or without a GPU), then the
+    machine (E_NODEVICE without a GPU), then an empty batch (OK), then the device index.  No row reaches a
+    device: the pointers are null or zeroed host arrays that are rejected before any copy or launch."""
+    from k4os.compression.lz4_b200 import _native as N
+    keep = [np.zeros(16, dtype=np.int64) for _ in range(10)]
+    real = lambda k: [a.ctypes.data for a in keep[:k]]
+    null = lambda k: [None] * k
+    mk = {"host": N.MEM_HOST, "device": N.MEM_DEVICE, "unknown": 7}[mem]
+    ndev = native.k4lz4_device_count()
+    ptrs, n, dev = {"negative_count": (null, -1, 0), "null_pointer": (null, 1, 0), "empty_nulls": (null, 0, 0),
+                    "device_out_of_range": (real, 1, ndev)}[case]
+    rc = _export_calls(native)[export](ptrs, n, mk, dev)
+    if mem == "unknown" or case in ("negative_count", "null_pointer"):
+        want = N.E_ARG
+    elif not has_gpu():
+        want = N.E_NODEVICE
+    else:
+        want = N.OK if case == "empty_nulls" else N.E_ARG
+    assert rc == want, (export, mem, case, rc, native.k4lz4_last_error())
+
+
+def test_device_only_calls_check_arguments_first(native):
+    """synth_device, copy_blocks_device and the two stats calls: argument errors are E_ARG with or without a
+    GPU; a device index out of range is E_ARG on a GPU."""
+    from k4os.compression.lz4_b200 import _native as N
+    assert native.k4lz4_synth_device(None, 1, 4096, 500, 1, 0, None, 0) == N.E_ARG
+    assert native.k4lz4_synth_device(None, -1, 4096, 500, 1, 0, None, 0) == N.E_ARG
+    assert native.k4lz4_copy_blocks_device(None, None, None, None, None, 1, None, 0) == N.E_ARG
+    assert native.k4lz4_copy_blocks_device(None, None, None, None, None, -1, None, 0) == N.E_ARG
+    assert native.k4lz4_decode_stats(0, None, 0) == N.E_ARG
+    assert native.k4lz4_encode_stats(0, None, 0) == N.E_ARG
+    keep = np.zeros(16, dtype=np.int64)
+    p, ndev = keep.ctypes.data, native.k4lz4_device_count()
+    want = N.E_ARG if has_gpu() else N.E_NODEVICE
+    assert native.k4lz4_synth_device(p, 1, 4096, 500, 1, 0, None, ndev) == want
+    assert native.k4lz4_copy_blocks_device(p, p, p, p, p, 1, None, ndev) == want
+    assert native.k4lz4_decode_stats(ndev, p, 0) == want
+    assert native.k4lz4_encode_stats(ndev, p, 0) == want

@@ -49,4 +49,9 @@ dd, dr = k4.batch.decode_dict_batch_host(enc[:3], [bs] * 3, [dic] * 3)
 assert dd == blocks[:3]
 pd, pr = k4.batch.partial_decode_batch_host(enc[:3], [1000, 65536, 5])
 assert pd == [blocks[0][:1000], blocks[1], blocks[2][:5]]
+cr, cd = k4.batch.decode_chain_blocks_host(enc[:3], [b"", blocks[5], blocks[6][:100]], [bs] * 3)
+assert cd == blocks[:3]
+from k4os.compression.lz4_b200 import frame
+xs = frame.xxh32_batch(raw, [0, bs, 7], [bs, 100, 0])
+assert xs.tolist() == [port.xxh32(raw[:bs].tobytes()), port.xxh32(raw[bs:bs + 100].tobytes()), port.xxh32(b"")]
 print("san workload ok:", k4.batch.decode_stats(0))
