@@ -53,6 +53,12 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_decode_chain_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* prefixLen, int* outLen, int nBlocks, int memKind, void* cudaStream, int device);
+        // LZ4FastChainEncoder.Encode (LZ4_compress_fast_continue, prefix mode) for one block of each of many streams;
+        // state = K4LZ4_CHAIN_STATE_BYTES (16 400) per stream, all zero for a new one
+        [DllImport(Lib)] public static extern int k4lz4_encode_chain_batch(
+            byte* srcBase, long* srcOff, int* srcLen, int* prefixLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* stateBase, long* stateOff, int* outLen, int nBlocks, int level, int memKind, void* cudaStream,
+            int device);
         // LL.Enforce32 semantics (LL.tools.cs:29-36) for inputs >= 65 547 bytes
         [DllImport(Lib)] public static extern int k4lz4_encode_x32(byte* src, int srcLen, byte* dst, int dstCap, int level);
         [DllImport(Lib)] public static extern int k4lz4_encode_batch_x32(

@@ -19,7 +19,8 @@
  *     (SpanTests.cs:36-37, PartialDecompressionTests.cs:33-35);
  *   - every batched call checks its arguments before the machine, in this order: an unknown
  *     memKind, a negative block count, a required pointer that is NULL while nBlocks > 0, and the
- *     host-memory contents (a negative prefixLen, a level outside 0..255) give K4LZ4_E_ARG; then
+ *     host-memory contents (a negative prefixLen, a state offset that is not a multiple of 16, a
+ *     level outside 0..255) give K4LZ4_E_ARG; then
  *     no device gives K4LZ4_E_NODEVICE; then nBlocks == 0 returns K4LZ4_OK; then a device index
  *     >= k4lz4_device_count() gives K4LZ4_E_ARG and a failed cudaSetDevice K4LZ4_E_CUDA.  So a
  *     caller's mistake gets the same code with or without a GPU;
@@ -167,6 +168,33 @@ K4LZ4_API int32_t k4lz4_decode_chain_batch(const uint8_t *srcBase, const int64_t
                                            const int32_t *prefixLen, int32_t *outLen, int32_t nBlocks,
                                            int32_t memKind, void *cudaStream, int32_t device);
 
+/* LZ4FastChainEncoder.Encode -> LLxx.LZ4_compress_fast_continue(state, src, dst, n, dstCap, 1)
+ * (Encoders/LZ4FastChainEncoder.cs:35-41, Engine/x64/LL64.fast.cs:582-667) with the stream's history
+ * contiguous in front of the source (the prefix mode the reference's ring buffer sets up).
+ * Block i encodes srcBase[srcOff[i] .. +srcLen[i]) into dstBase[dstOff[i] .. +dstCap[i]); the prefixLen[i]
+ * bytes directly in front of the source are the stream's history, and the state record at
+ * stateBase + stateOff[i] (K4LZ4_CHAIN_STATE_BYTES, 16-aligned) is read and advanced.  The dictionary the
+ * block sees is min(state.dictSize, prefixLen[i]) bytes, which is LZ4_saveDict's clamp: a caller that moves
+ * its history (a ring buffer) passes the bytes it kept and never writes the state.  At most 65 535 history
+ * bytes are read, never written.  Every block size up to 2 GiB uses the same u32 table (hash5).
+ * outLen[i] = bytes written; 0 for srcLen <= 0 and K4LZ4_R_DELEGATE for level >= 3, both with the state
+ * untouched; -1 where LZ4FastChainEncoder.Encode would throw (the engine returned 0: the block does not fit
+ * dstCap), with the state advanced exactly as the reference's is.
+ * No two blocks of one call may share a state record, and no block's destination or state record may
+ * overlap another block's source, history, destination or state (one block per stream per call meets
+ * this).  memKind == K4LZ4_MEM_HOST stages [history | source], the state and the destination slot of each
+ * block, copies back exactly outLen > 0 bytes and every state record whole, and runs on one GPU (`device`,
+ * K4LZ4_ALL_DEVICES = GPU 0).  A negative prefixLen or a misaligned state offset is K4LZ4_E_ARG with host
+ * memory, outLen = -1 (state untouched) with device memory.  Counted in k4lz4_encode_stats out4[3]. */
+#define K4LZ4_CHAIN_STATE_BYTES 16400  /* uint32 hashTable[4096]; uint32 currentOffset; uint32 dictSize; uint32 reserved[2];
+                                          all zero = a new stream (LZ4_createStream / PinnedMemory.Alloc) */
+K4LZ4_API int32_t k4lz4_encode_chain_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           const int32_t *prefixLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           uint8_t *stateBase, const int64_t *stateOff,
+                                           int32_t *outLen, int32_t nBlocks, int32_t level,
+                                           int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- XXH32: the checksum of the LZ4 Frame container (SURVEY 8f row 2) ------------------------ */
 
 /* XXH32 of one buffer on the host (frame header byte, serial content checksum) --
@@ -255,7 +283,8 @@ K4LZ4_API int32_t k4lz4_decode_stats(int32_t device, uint64_t *out4, int32_t res
 /* Encoder path counters of `device` since the last reset: out4[0] blocks encoded by a warp with its
  * hash table in shared memory, [1] by a warp with its table in global memory (only launched when a
  * call has more blocks than the shared-memory warps take in one round), [2] blocks of >= 65 547
- * bytes (the u32-table engine, either warp kind), [3] 0.  Empty blocks are not counted.
+ * bytes (the u32-table engine, either warp kind), [3] chained blocks (k4lz4_encode_chain_batch, any
+ * size).  Empty blocks, delegated levels and rejected arguments are not counted.
  * Synchronises the device.  Diagnostics only. */
 K4LZ4_API int32_t k4lz4_encode_stats(int32_t device, uint64_t *out4, int32_t reset);
 

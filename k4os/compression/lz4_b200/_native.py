@@ -13,6 +13,7 @@ R_DELEGATE = -2
 R_CORRUPT = -1000
 MEM_HOST, MEM_DEVICE = 0, 1
 ALL_DEVICES = -1
+CHAIN_STATE_BYTES = 16400                 # K4LZ4_CHAIN_STATE_BYTES
 
 _vp, _i32, _i64, _u32, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64
 _BATCH = [_vp] * 7                        # srcBase srcOff srcLen dstBase dstOff dstCap outLen
@@ -39,6 +40,7 @@ SIGNATURES = {
     "k4lz4_partial_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_decode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),
+    "k4lz4_encode_chain_batch": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_unpickle_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_pickle_batch": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_pickle_writer_batch": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),

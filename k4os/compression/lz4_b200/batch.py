@@ -229,7 +229,7 @@ def encode_stats(device: int = 0, reset: bool = False) -> dict:
     """Encoder path counters (k4lz4_encode_stats): which kind of warp encoded how many blocks."""
     v = (C.c_uint64 * 4)()
     N.check(N.lib().k4lz4_encode_stats(device, C.addressof(v), int(reset)))
-    return {"smem": int(v[0]), "gtab": int(v[1]), "generic": int(v[2])}
+    return {"smem": int(v[0]), "gtab": int(v[1]), "generic": int(v[2]), "chain": int(v[3])}
 
 
 def decode_dict_batch_host(blocks: Sequence, caps: Sequence[int], dicts: Sequence, device: int = 0):
@@ -301,3 +301,31 @@ def partial_decode_batch_host(blocks: Sequence, targets: Sequence[int], device: 
                                                doff.ctypes.data, tg.ctypes.data, out.ctypes.data, n,
                                                N.MEM_HOST, None, int(device)))
     return _slices(dst, doff, out), out
+
+
+def encode_chain_batch_host(src: np.ndarray, src_off, src_len, prefix_len, dst: np.ndarray, dst_off, dst_cap,
+                            state: np.ndarray, state_off, level: int = 0, device: int = 0) -> np.ndarray:
+    """LZ4FastChainEncoder's block encode over a batch of streams (k4lz4_encode_chain_batch, host memory).
+    Block i encodes src[src_off[i] .. + src_len[i]) behind the prefix_len[i] bytes in front of it (its stream's
+    history) into dst[dst_off[i] .. + dst_cap[i]), reading and advancing the 16 400-byte state record at
+    state[state_off[i]] (16-aligned; all zero = a new stream).  One block per stream per call.  Returns int32
+    results: bytes written, 0 for an empty block, -1 where Encode would throw (state advanced), R_DELEGATE for
+    level >= 3."""
+    src_off, dst_off, state_off = _i64(src_off), _i64(dst_off), _i64(state_off)
+    src_len, dst_cap, prefix_len = _i32(src_len), _i32(dst_cap), _i32(prefix_len)
+    n = int(src_len.shape[0])
+    out = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_encode_chain_batch(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
+                                             prefix_len.ctypes.data, dst.ctypes.data, dst_off.ctypes.data,
+                                             dst_cap.ctypes.data, state.ctypes.data, state_off.ctypes.data,
+                                             out.ctypes.data, n, int(level), N.MEM_HOST, None, int(device)))
+    return out
+
+
+def encode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, prefix_len_ptr: int, dst_ptr: int,
+                              dst_off_ptr: int, dst_cap_ptr: int, state_ptr: int, state_off_ptr: int,
+                              out_len_ptr: int, n: int, level: int = 0, stream: int = 0, device: int = -1) -> None:
+    """Device-pointer form of encode_chain_batch_host: only enqueues the kernel on `stream`."""
+    N.check(N.lib().k4lz4_encode_chain_batch(src_ptr, src_off_ptr, src_len_ptr, prefix_len_ptr, dst_ptr, dst_off_ptr,
+                                             dst_cap_ptr, state_ptr, state_off_ptr, out_len_ptr, int(n), int(level),
+                                             N.MEM_DEVICE, stream or None, int(device)))

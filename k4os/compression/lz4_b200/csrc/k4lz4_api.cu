@@ -30,6 +30,7 @@
 #include "decode_tile.cuh"
 #include "encode_generic.cuh"
 #include "encode_tile.cuh"
+#include "encode_chain.cuh"
 #include "pickle.cuh"
 #include "synth.cuh"
 #include "copy_blocks.cuh"
@@ -70,7 +71,8 @@ int device_count_cached() {
 // ---- one batch description, one argument check ------------------------------------------------
 
 enum Op {
-    OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY
+    OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY,
+    OP_ENCCHAIN
 };
 
 // Block i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]) and outLen[i].
@@ -83,27 +85,29 @@ struct Batch {
     int level = 0;                    // OP_ENCODE: 0..255; OP_PICKLE(W): passed through
     bool x32 = false;                 // OP_ENCODE: reproduce the 32-bit engine (k4lz4_encode*_x32)
     const uint8_t* dictBase = nullptr; const int64_t* dictOff = nullptr; const int32_t* dictLen = nullptr;
-    const int32_t* prefixLen = nullptr;   // OP_CHAIN: history in front of each destination
+    const int32_t* prefixLen = nullptr;   // OP_CHAIN: history in front of each destination; OP_ENCCHAIN: of each source
+    uint8_t* stateBase = nullptr; const int64_t* stateOff = nullptr;   // OP_ENCCHAIN: K4LZ4_CHAIN_STATE_BYTES per block
     bool partial = false;             // OP_GENERAL: PartialDecode semantics (dstCap = target length)
     uint32_t seed = 0;                // OP_XXH32
 };
 
 // The pointers each op needs when n > 0, besides srcBase / srcOff / srcLen.  A dictionary is optional
 // wherever it is read: with dictBase set, dictOff and dictLen are required too.
-struct Needs { bool dst, cap, out, prefix, level; };
+struct Needs { bool dst, cap, out, prefix, level, state; };
 constexpr Needs NEEDS[] = {
-    /* OP_ENCODE   */ {true,  true,  true,  false, true},
-    /* OP_DECODE   */ {true,  true,  true,  false, false},
-    /* OP_CHAIN    */ {true,  true,  true,  true,  false},
-    /* OP_GENERAL  */ {true,  true,  true,  false, false},
-    /* OP_PICKLE   */ {true,  false, true,  false, false},
-    /* OP_PICKLEW  */ {true,  false, true,  false, false},
-    /* OP_UNPICKLE */ {true,  true,  true,  false, false},
-    /* OP_USIZE    */ {false, false, true,  false, false},
-    /* OP_XXH32    */ {false, false, true,  false, false},
-    /* OP_COPY     */ {true,  false, false, false, false},
+    /* OP_ENCODE   */ {true,  true,  true,  false, true,  false},
+    /* OP_DECODE   */ {true,  true,  true,  false, false, false},
+    /* OP_CHAIN    */ {true,  true,  true,  true,  false, false},
+    /* OP_GENERAL  */ {true,  true,  true,  false, false, false},
+    /* OP_PICKLE   */ {true,  false, true,  false, false, false},
+    /* OP_PICKLEW  */ {true,  false, true,  false, false, false},
+    /* OP_UNPICKLE */ {true,  true,  true,  false, false, false},
+    /* OP_USIZE    */ {false, false, true,  false, false, false},
+    /* OP_XXH32    */ {false, false, true,  false, false, false},
+    /* OP_COPY     */ {true,  false, false, false, false, false},
+    /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true},
 };
-static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_COPY + 1, "one row per op");
+static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_ENCCHAIN + 1, "one row per op");
 
 // The machine part of check(): a device must exist, an empty batch is then done (the caller returns OK for
 // n == 0), and `device` (K4LZ4_ALL_DEVICES or the current device when negative) must name a visible GPU.
@@ -122,11 +126,15 @@ int check(Op op, const Batch& b, int memKind, int device) {
     if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
     if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
     if (b.n > 0 && (!b.srcBase || !b.srcOff || !b.srcLen || (w.out && !b.outLen) || (w.dst && (!b.dstBase || !b.dstOff)) ||
-                    (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen))))
+                    (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen)) ||
+                    (w.state && (!b.stateBase || !b.stateOff))))
         return fail(K4LZ4_E_ARG, "null pointer argument");
     if (w.prefix && memKind == K4LZ4_MEM_HOST)       // device arrays cannot be checked here: there a negative prefix gives -1
         for (int64_t i = 0; i < b.n; i++)
             if (b.prefixLen[i] < 0) return fail(K4LZ4_E_ARG, "negative prefix length at block %lld", (long long)i);
+    if (w.state && memKind == K4LZ4_MEM_HOST)        // likewise: on the device a misaligned state record gives -1
+        for (int64_t i = 0; i < b.n; i++)
+            if (b.stateOff[i] & 15) return fail(K4LZ4_E_ARG, "state offset not a multiple of 16 at block %lld", (long long)i);
     if (w.level && (b.level < 0 || b.level > 0xFF)) return fail(K4LZ4_E_ARG, "bad level %d", b.level);
     return check_device(device, b.n);
 }
@@ -345,6 +353,19 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
         k4::copy_blocks_kernel<<<n, 256, 0, st>>>(a.srcBase, a.srcOff, a.dstBase, a.dstOff, a.srcLen, n);
         g_launches++;
         break;
+    case OP_ENCCHAIN: {   // one persistent warp kind; its counter comes from the private pool
+        uint32_t* counter = nullptr;
+        cudaError_t e = cudaMallocFromPoolAsync((void**)&counter, 256, D->pool, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(counter, 0, 4, st);
+        if (e != cudaSuccess) { (void)cudaGetLastError(); return e; }
+        const int wave = D->sms * k4::ENC_CHAIN_WARPS;
+        k4::encode_chain_kernel<<<n < wave ? n : wave, 32, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.prefixLen,
+                                                                    a.dstBase, a.dstOff, a.dstCap, a.stateBase,
+                                                                    a.stateOff, a.outLen, n, a.level, counter);
+        g_launches++;
+        cudaFreeAsync(counter, st);
+        break;
+    }
     }
     return cudaGetLastError();
 }
@@ -714,61 +735,81 @@ constexpr int64_t STAGE_BYTES = 256ll << 20;   // staged payload per chunk
 // One GPU, no pipelining: per chunk of at most STAGE_BYTES, everything the kernel reads is packed into one
 // host buffer -- the block table, the sources, the dictionaries (when the batch has them) and, with a
 // prefix, the destination slots [history | capacity] (16-aligned, history filled in: all the decoder reads
-// of a stream is its last <= 65535 bytes) -- and goes up in one copy.  The results and the destination
-// region come back, and exactly outLen[i] > 0 bytes of each block are copied to the caller.  A batch
-// without dstCap (XXH32) has no destination: its per-block result is the whole output.
+// of a stream is its last <= 65535 bytes) -- and goes up in one copy.  The chained encoder's history goes in
+// front of its source instead ([history | source], 16-aligned) and its state records (16-aligned) go up and
+// come back whole.  The results and the destination region come back, and exactly outLen[i] > 0 bytes of
+// each block are copied to the caller.  A batch without dstCap (XXH32) has no destination: its per-block
+// result is the whole output.
 int run_staged(Op op, const Batch& b, int dev) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
     const bool dict = b.dictBase != nullptr, prefix = b.prefixLen != nullptr, dst = b.dstCap != nullptr;
+    const bool enc = op == OP_ENCCHAIN;
+    constexpr int64_t SB = K4LZ4_CHAIN_STATE_BYTES;
     auto hist = [&](int64_t i) -> int64_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
-    auto cap = [&](int64_t i) -> int64_t { return dst ? std::max<int32_t>(b.dstCap[i], 0) : 0; };
+    auto cap = [&](int64_t i) -> int64_t {      // the encoder never writes more than compressBound(srcLen)
+        const int64_t c = dst ? std::max<int32_t>(b.dstCap[i], 0) : 0;
+        return enc ? std::min<int64_t>(c, b.srcLen[i] > 0 ? k4::max_output_size(b.srcLen[i]) : 0) : c;
+    };
     auto dlen = [&](int64_t i) -> int64_t { return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0; };
     auto up = [](int64_t x) { return (x + 255) & ~int64_t(255); };
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
     std::vector<uint8_t> h;          // reused by every chunk: the kernel reads only bytes the chunk has written
     DevMem d;
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
         for (j = i; j < b.n; j++) {
-            const int64_t add = src_size(b, j) + dlen(j) + cap(j) + (prefix ? hist(j) + 16 : 0);
+            const int64_t add = src_size(b, j) + dlen(j) + cap(j) + (prefix ? hist(j) + 16 : 0) + (enc ? SB : 0);
             if (j > i && bytes + add > STAGE_BYTES) break;
             bytes += add;
         }
         const int64_t nb = j - i;
-        // block table: srcOff dstOff dictOff (int64) | srcLen dstCap dictLen prefixLen outLen (int32)
+        // block table: srcOff dstOff dictOff stateOff (int64) | srcLen dstCap dictLen prefixLen outLen (int32)
         int64_t sTot = 0, diTot = 0, dTot = 0;
         for (int64_t k = 0; k < nb; k++) {
-            sTot += src_size(b, i + k); diTot += dlen(i + k);
-            dTot = (prefix ? (dTot + hist(i + k) + 15) & ~int64_t(15) : dTot) + cap(i + k);
+            sTot = (enc ? a16(sTot + hist(i + k)) : sTot) + src_size(b, i + k);
+            diTot += dlen(i + k);
+            dTot = (prefix && !enc ? a16(dTot + hist(i + k)) : dTot) + cap(i + k);
         }
-        const int64_t srcAt = up(nb * (3 * 8 + 5 * 4)), dictAt = up(srcAt + sTot), dstAt = up(dictAt + diTot);
+        const int64_t stTot = enc ? nb * SB : 0;
+        const int64_t srcAt = up(nb * (4 * 8 + 5 * 4)), dictAt = up(srcAt + sTot), stateAt = up(dictAt + diTot);
+        const int64_t dstAt = up(stateAt + stTot);
         const int64_t total = dstAt + dTot;
         if (h.size() < (size_t)total + 16) h.resize((size_t)total + 16);
-        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* dio = doff + nb;
-        int32_t* sl = (int32_t*)(dio + nb); int32_t* dc = sl + nb; int32_t* dl = dc + nb; int32_t* pl = dl + nb;
+        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* dio = doff + nb; int64_t* sto = dio + nb;
+        int32_t* sl = (int32_t*)(sto + nb); int32_t* dc = sl + nb; int32_t* dl = dc + nb; int32_t* pl = dl + nb;
         int32_t* res = pl + nb;
         for (int64_t k = 0, sp = 0, dip = 0, dp = 0; k < nb; k++) {
-            const int64_t x = i + k;
-            sl[k] = b.srcLen[x]; dc[k] = dst ? b.dstCap[x] : 0; dl[k] = (int32_t)dlen(x); pl[k] = (int32_t)hist(x);
-            so[k] = sp; dio[k] = dip;
-            doff[k] = prefix ? (dp + pl[k] + 15) & ~int64_t(15) : dp;
-            if (sl[k] > 0) memcpy(h.data() + srcAt + sp, b.srcBase + b.srcOff[x], (size_t)sl[k]);
+            const int64_t x = i + k, hl = hist(x);
+            sl[k] = b.srcLen[x]; dc[k] = dst ? b.dstCap[x] : 0; dl[k] = (int32_t)dlen(x);
+            pl[k] = enc ? b.prefixLen[x] : (int32_t)hl;   // the encoder's dictSize clamp needs the caller's value
+            so[k] = enc ? a16(sp + hl) : sp; dio[k] = dip; sto[k] = k * SB;
+            doff[k] = prefix && !enc ? a16(dp + hl) : dp;
+            if (enc && hl > 0) memcpy(h.data() + srcAt + so[k] - hl, b.srcBase + b.srcOff[x] - hl, (size_t)hl);
+            if (sl[k] > 0) memcpy(h.data() + srcAt + so[k], b.srcBase + b.srcOff[x], (size_t)sl[k]);
             if (dl[k] > 0) memcpy(h.data() + dictAt + dip, b.dictBase + b.dictOff[x], (size_t)dl[k]);
-            if (pl[k] > 0) memcpy(h.data() + dstAt + doff[k] - pl[k], b.dstBase + b.dstOff[x] - pl[k], (size_t)pl[k]);
-            sp += src_size(b, x); dip += dl[k]; dp = doff[k] + cap(x);
+            if (enc) memcpy(h.data() + stateAt + sto[k], b.stateBase + b.stateOff[x], (size_t)SB);
+            else if (prefix && hl > 0) memcpy(h.data() + dstAt + doff[k] - hl, b.dstBase + b.dstOff[x] - hl, (size_t)hl);
+            sp = so[k] + src_size(b, x); dip += dl[k]; dp = doff[k] + cap(x);
         }
         CU_TRY(d.ensure((size_t)total + 16));
         uint8_t* D = (uint8_t*)d.p;
-        CU_TRY(cudaMemcpy(D, h.data(), (size_t)(prefix ? total : dstAt), cudaMemcpyHostToDevice));
+        CU_TRY(cudaMemcpy(D, h.data(), (size_t)(prefix && !enc ? total : dstAt), cudaMemcpyHostToDevice));
         int32_t* dRes = (int32_t*)(D + ((uint8_t*)res - h.data()));
         Batch kb = b;                                // the same batch, on the device
         kb.srcBase = D + srcAt; kb.srcOff = (int64_t*)D; kb.srcLen = (int32_t*)(D + ((uint8_t*)sl - h.data()));
         kb.dstBase = D + dstAt; kb.dstOff = kb.srcOff + nb; kb.dstCap = dst ? kb.srcLen + nb : nullptr;
         kb.dictBase = dict ? D + dictAt : nullptr; kb.dictOff = kb.srcOff + 2 * nb; kb.dictLen = kb.srcLen + 2 * nb;
         kb.prefixLen = prefix ? kb.srcLen + 3 * nb : nullptr;
+        kb.stateBase = enc ? D + stateAt : nullptr; kb.stateOff = enc ? kb.srcOff + 3 * nb : nullptr;
         kb.outLen = dRes; kb.n = nb;
         CU_TRY(launch_op(op, kb, nullptr));
         CU_TRY(cudaMemcpy(b.outLen + i, dRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
+        if (enc) {
+            CU_TRY(cudaMemcpy(h.data() + stateAt, D + stateAt, (size_t)stTot, cudaMemcpyDeviceToHost));
+            for (int64_t k = 0; k < nb; k++)
+                memcpy(b.stateBase + b.stateOff[i + k], h.data() + stateAt + sto[k], (size_t)SB);
+        }
         if (!dst || dTot == 0) continue;
         CU_TRY(cudaMemcpy(h.data() + dstAt, D + dstAt, (size_t)dTot, cudaMemcpyDeviceToHost));
         for (int64_t k = 0; k < nb; k++) {
@@ -783,8 +824,8 @@ int run(Op op, const Batch& b, int memKind, void* stream, int device) {
     const int rc = check(op, b, memKind, device);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     if (memKind == K4LZ4_MEM_HOST)
-        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32) ? run_staged(op, b, device < 0 ? 0 : device)
-                                                                        : run_host(op, b, device);
+        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN)
+                   ? run_staged(op, b, device < 0 ? 0 : device) : run_host(op, b, device);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
     CU_TRY(launch_op(op, b, (cudaStream_t)stream));
@@ -897,6 +938,16 @@ int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, 
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
     b.prefixLen = prefixLen;
     return run(OP_CHAIN, b, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_encode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 const int32_t* prefixLen, uint8_t* dstBase, const int64_t* dstOff,
+                                 const int32_t* dstCap, uint8_t* stateBase, const int64_t* stateOff,
+                                 int32_t* outLen, int32_t nBlocks, int32_t level, int32_t memKind, void* cudaStream,
+                                 int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level};
+    b.prefixLen = prefixLen; b.stateBase = stateBase; b.stateOff = stateOff;
+    return run(OP_ENCCHAIN, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_partial_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,

@@ -7,19 +7,21 @@ with the same member names and error behaviour, plus the one thing a GPU needs: 
 `batch_blocks` full blocks and encodes them with ONE `k4lz4_encode_batch` call; the decoder takes a
 list of compressed blocks and decodes them with ONE `k4lz4_decode_batch` call.  Every block's bytes
 and return value equal what the reference's per-block call produces (independent blocks: no
-dictionary, fresh table per block -- LZ4BlockEncoder.cs:18-23).  Chained encoders (dependent
-blocks) stay with the managed engine: they are not data parallel.
+dictionary, fresh table per block -- LZ4BlockEncoder.cs:18-23).
 
-`LZ4ChainDecoder` (Encoders/LZ4ChainDecoder.cs) decodes dependent blocks.  One stream's blocks are serial, but
-the blocks of MANY streams are not: `LZ4ChainDecoder.DecodeMany` advances many decoders by one block each with
-ONE `k4lz4_decode_chain_batch` call.
+`LZ4FastChainEncoder` (Encoders/LZ4FastChainEncoder.cs) encodes dependent blocks at L00_FAST, and
+`LZ4ChainDecoder` (Encoders/LZ4ChainDecoder.cs) decodes them.  One stream's blocks are serial, but the blocks
+of MANY streams are not: `LZ4FastChainEncoder.EncodeMany` and `LZ4ChainDecoder.DecodeMany` advance many
+encoders or decoders by one block each with ONE `k4lz4_encode_chain_batch` / `k4lz4_decode_chain_batch` call.
+The chained HC encoder stays with the managed engine.
+
 """
 from __future__ import annotations
 
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host, encode_chain_batch_host
 from .codec import LZ4Codec, LZ4Level
 
 K1 = 1024
@@ -388,6 +390,147 @@ class LZ4ChainDecoder:
     def _check(self) -> None:
         if self._disposed:
             raise RuntimeError("ObjectDisposedException")
+
+
+class LZ4FastChainEncoder:
+    """LZ4FastChainEncoder(blockSize, extraBlocks) -- LZ4FastChainEncoder.cs:14-41 over LZ4EncoderBase.cs:27-97:
+    the same input ring of 64 KiB + (1 + extraBlocks) * blockSize + 32 bytes, Topup / Encode / Commit, and
+    CopyDict = LZ4_saveDict (the last <= 64 KiB move to the front of the ring).  The LZ4_stream_t lives in a
+    16 400-byte state record (K4LZ4_CHAIN_STATE_BYTES, zero = LZ4_createStream); blocks are encoded on the GPU
+    by LZ4_compress_fast_continue's rules with the bytes in front of the block in the ring as history, and
+    EncodeMany advances many encoders with one call.  After a failed Encode (target too small) the state has
+    advanced as the reference's has; encoding the same bytes again would take upstream's external-dictionary
+    branch, which the GPU does not reproduce, so such an encoder should be discarded, as the exception suggests."""
+
+    def __init__(self, blockSize: int = 65536, extraBlocks: int = 0):
+        self._block = _round_up(max(int(blockSize), K1), K1)              # LZ4EncoderBase.cs:29-35
+        extra = max(int(extraBlocks), 0)
+        self._in_len = K64 + (1 + extra) * self._block + 32
+        self._in = np.zeros(self._in_len + 8, dtype=np.uint8)
+        self._index = 0                                                   # _inputIndex
+        self._pointer = 0                                                 # _inputPointer
+        self._state = np.zeros(N.CHAIN_STATE_BYTES, dtype=np.uint8)
+        self._disposed = False
+
+    @property
+    def BlockSize(self) -> int:
+        return self._block
+
+    @property
+    def BytesReady(self) -> int:
+        return self._pointer - self._index
+
+    @property
+    def State(self) -> np.ndarray:
+        """The stream state: uint32 hashTable[4096], currentOffset, dictSize, reserved[2] (a view)."""
+        return self._state.view(np.uint32)
+
+    def Topup(self, source) -> int:
+        """LZ4EncoderBase.cs:46-62: adds up to the rest of the current block; returns the bytes taken."""
+        self._check()
+        src = np.frombuffer(bytes(source), dtype=np.uint8) if not isinstance(source, np.ndarray) else source
+        if src.size == 0:
+            return 0
+        left = self._index + self._block - self._pointer
+        if left <= 0:
+            return 0
+        chunk = min(left, int(src.size))
+        self._in[self._pointer:self._pointer + chunk] = src[:chunk]
+        self._pointer += chunk
+        return chunk
+
+    def Encode(self, target, allowCopy: bool = False) -> int:
+        """LZ4EncoderBase.cs:65-88: encodes the pending bytes into `target` (a writable uint8 array; its length
+        is the capacity).  Returns the encoded length, -length when allowCopy stored the block raw, 0 when nothing
+        is pending; raises like the reference when the block does not fit."""
+        return LZ4FastChainEncoder.EncodeMany([self], [target], allowCopy)[0]
+
+    @staticmethod
+    def EncodeMany(encoders, targets, allowCopy: bool = False, device: int = 0) -> list:
+        """Encode() on every encoder at once: encoders[i] encodes its pending bytes into targets[i] (writable
+        uint8 arrays), all in ONE GPU call.  The encoders must be distinct.  Returns the per-encoder results of
+        Encode.  If a block does not fit, its encoder is not committed (Encode throws before Commit) and
+        InvalidOperationException is raised after every other encoder has been advanced."""
+        encoders = list(encoders)
+        if len(encoders) != len(targets):
+            raise ValueError("one target per encoder")
+        if len({id(e) for e in encoders}) != len(encoders):
+            raise ValueError("an encoder may take only one block per call")
+        for e in encoders:
+            e._check()
+        todo = [i for i, e in enumerate(encoders) if e._pointer - e._index > 0]
+        res = [0] * len(encoders)
+        if not todo:
+            return res
+        tg = [targets[i] if isinstance(targets[i], np.ndarray) else np.frombuffer(targets[i], dtype=np.uint8)
+              for i in todo]
+        # every ring and state goes up as it is: block k starts at ring k's _inputIndex, behind its history
+        rings = [encoders[i]._in for i in todo]
+        base = np.concatenate(rings)
+        roff = np.zeros(len(todo), dtype=np.int64)
+        roff[1:] = np.cumsum([r.size for r in rings[:-1]])
+        src_off = roff + np.array([encoders[i]._index for i in todo], dtype=np.int64)
+        src_len = np.array([encoders[i]._pointer - encoders[i]._index for i in todo], dtype=np.int32)
+        prefix = np.array([encoders[i]._index for i in todo], dtype=np.int32)
+        caps = np.array([t.size for t in tg], dtype=np.int32)
+        dst = np.zeros(int(caps.astype(np.int64).sum()) + 16, dtype=np.uint8)
+        doff = np.zeros(len(todo), dtype=np.int64)
+        doff[1:] = np.cumsum(caps[:-1].astype(np.int64))
+        state = np.concatenate([encoders[i]._state for i in todo])
+        soff = np.arange(len(todo), dtype=np.int64) * N.CHAIN_STATE_BYTES
+        out = encode_chain_batch_host(base, src_off, src_len, prefix, dst, doff, caps, state, soff, 0, device)
+        failed = False
+        for k, i in enumerate(todo):
+            e, r, n = encoders[i], int(out[k]), int(src_len[k])
+            e._state[:] = state[soff[k]:soff[k] + N.CHAIN_STATE_BYTES]  # the engine advanced it, fit or not
+            if r <= 0:                                                    # LZ4EncoderBase.cs:75-77
+                failed = True
+                res[i] = r
+                continue
+            if allowCopy and r >= n:                                      # :79-83
+                tg[k][:n] = e._in[e._index:e._index + n]
+                r = -n
+            else:
+                tg[k][:r] = dst[doff[k]:doff[k] + r]
+            e._commit()
+            res[i] = r
+        if failed:
+            raise RuntimeError("Failed to encode chunk. Target buffer too small.")   # InvalidOperationException
+        return res
+
+    def Dispose(self) -> None:
+        self._disposed = True
+
+    # -- LZ4EncoderBase.cs:90-97, LZ4FastChainEncoder.cs:40-41 ---------------------------------------------------
+    def _commit(self) -> None:
+        self._index = self._pointer
+        if self._index + self._block <= self._in_len:
+            return
+        self._index = self._pointer = self._copy_dict(self._pointer)
+
+    def _copy_dict(self, length: int) -> int:
+        """LZ4_saveDict(ctx, buffer, length): the last min(length, 64 KiB, dictSize) bytes move to the front.  The
+        state's dictSize is not written: the next block passes this length as its prefix, and the GPU clamps
+        dictSize to it the same way."""
+        size = min(length, K64, int(self.State[4097]))
+        self._in[:size] = self._in[self._index - size:self._index].copy()
+        return size
+
+    def _check(self) -> None:
+        if self._disposed:
+            raise RuntimeError("ObjectDisposedException")
+
+
+class LZ4Encoder:
+    """LZ4Encoder.Create -- Encoders/LZ4Encoder.cs:14-29."""
+
+    @staticmethod
+    def Create(chaining: bool, level: LZ4Level = LZ4Level.L00_FAST, blockSize: int = 65536, extraBlocks: int = 0):
+        if not chaining:
+            return LZ4BlockEncoder(level, blockSize)
+        if LZ4Level(level) < LZ4Level.L03_HC:
+            return LZ4FastChainEncoder(blockSize, extraBlocks)
+        raise NotImplementedError("LZ4HighChainEncoder (chained HC levels) stays with the managed engine")
 
 
 class LZ4Decoder:

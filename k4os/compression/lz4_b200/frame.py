@@ -11,9 +11,9 @@ All blocks of a frame go through ONE k4lz4_encode_batch / k4lz4_decode_batch cal
 k4lz4_xxh32_batch call; only the serial parts (header byte, content checksum, byte layout) run
 on the host.  Frames are interoperable with upstream lz4 (tests decode them with
 orig/lib/lz4frame.c and decode upstream's frames here).  Frames of linked blocks (the reference's
-default, LZ4EncoderSettings.ChainBlocks) are READ on the GPU as well, batched across frames
-(read_frames); writing them, content size and dictionary ids are the managed engine's business
-(the reference itself throws NotImplemented for the last two, LZ4FrameWriter.cs:89-95).
+default, LZ4EncoderSettings.ChainBlocks) are written (write_frames, L00_FAST) and read (read_frames) on the
+GPU as well, batched across frames; content size and dictionary ids are not written (the reference itself
+throws NotImplemented for them, LZ4FrameWriter.cs:89-95).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ import struct
 import numpy as np
 
 from . import _native as N
-from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host
+from .batch import decode_batch_flat_host, decode_chain_blocks_host, encode_batch_flat_host, encode_chain_batch_host
 
 MAGIC = 0x184D2204
 _BLOCK_SIZES = {4: 1 << 16, 5: 1 << 18, 6: 1 << 20, 7: 1 << 22}
@@ -54,9 +54,87 @@ def _block_size_code(block_size: int) -> int:                # LZ4FrameWriter.cs
     raise ValueError(f"Invalid block size {block_size} for stream")
 
 
+def _header(code: int, chaining: bool, block_checksum: bool, content_checksum: bool) -> list:
+    flg = (1 << 6) | (int(not chaining) << 5) | (int(block_checksum) << 4) | (int(content_checksum) << 2)
+    head = struct.pack("<IBB", MAGIC, flg, code << 4)
+    return [head, bytes([(xxh32(head[4:6]) >> 8) & 0xFF])]       # HC, LZ4FrameWriter.cs:100-102
+
+
+def _blocks(out: list, stored, raw, block_checksum: bool, device: int) -> None:
+    """Appends the blocks of a frame (length code with bit 31 = stored raw, data, [XXH32 of the stored bytes],
+    LZ4FrameWriter.cs:159-175) and the end mark."""
+    if block_checksum and stored:
+        base = np.frombuffer(b"".join(stored), dtype=np.uint8)
+        ln = np.array([len(b) for b in stored], dtype=np.int32)
+        off = np.zeros(len(stored), dtype=np.int64)
+        off[1:] = np.cumsum(ln[:-1].astype(np.int64))
+        sums = xxh32_batch(base, off, ln, 0, device)
+    for i, body in enumerate(stored):
+        out.append(struct.pack("<I", len(body) | (0x80000000 if raw[i] else 0)))
+        out.append(body)
+        if block_checksum:
+            out.append(struct.pack("<I", int(sums[i])))
+    out.append(struct.pack("<I", 0))                            # end mark, blocking.cs:94
+
+
+def write_frames(datas, block_size: int = 65536, block_checksum: bool = False, content_checksum: bool = False,
+                 level: int = 0, device: int = 0, chaining: bool = True) -> list:
+    """Many LZ4 frames, one per item of `datas` (LZ4FrameWriter with the default Chaining = true, L00_FAST).
+    Linked frames are encoded together: step k encodes block k of every frame that has one with ONE
+    k4lz4_encode_chain_batch call, each frame's earlier blocks being its history (LZ4FastChainEncoder).  A block
+    is encoded with capacity MaximumOutputSize(blockSize) and stored raw when it does not shrink
+    (LZ4FrameWriter.cs:105,130-157); a raw block stays history.  chaining=False writes independent frames
+    (write_frame).  Chained HC levels stay with the managed engine (NotImplementedError)."""
+    if not chaining:
+        return [write_frame(d, block_size, block_checksum, content_checksum, level, device) for d in datas]
+    if level >= 3:
+        raise NotImplementedError("LZ4HighChainEncoder (chained HC levels) stays with the managed engine")
+    srcs = [np.frombuffer(bytes(d), dtype=np.uint8) if not isinstance(d, np.ndarray) else d for d in datas]
+    code = _block_size_code(block_size)
+    bs = max(1024, (block_size + 1023) // 1024 * 1024)          # LZ4EncoderBase.cs:29
+    bound = N.lib().k4lz4_max_output_size(bs)
+    nf = len(srcs)
+    base = np.concatenate(srcs) if nf and sum(int(s.size) for s in srcs) else np.zeros(1, dtype=np.uint8)
+    foff = np.zeros(nf, dtype=np.int64)
+    if nf:
+        foff[1:] = np.cumsum([int(s.size) for s in srcs[:-1]])
+    nbs = [(int(s.size) + bs - 1) // bs for s in srcs]
+    state = np.zeros(nf * N.CHAIN_STATE_BYTES, dtype=np.uint8)
+    stored = [[] for _ in srcs]
+    raws = [[] for _ in srcs]
+    for k in range(max(nbs, default=0)):
+        fs = [j for j in range(nf) if k < nbs[j]]
+        so = np.array([foff[j] + k * bs for j in fs], dtype=np.int64)
+        sl = np.array([min(bs, int(srcs[j].size) - k * bs) for j in fs], dtype=np.int32)
+        pl = np.full(len(fs), min(k * bs, 0x7FFFFFFF), dtype=np.int32)   # the frame so far, in front
+        caps = np.full(len(fs), bound, dtype=np.int32)
+        doff = np.arange(len(fs), dtype=np.int64) * bound
+        dst = np.zeros(len(fs) * bound + 16, dtype=np.uint8)
+        st_off = np.array(fs, dtype=np.int64) * N.CHAIN_STATE_BYTES
+        enc = encode_chain_batch_host(base, so, sl, pl, dst, doff, caps, state, st_off, level, device)
+        if (enc <= 0).any():
+            raise RuntimeError("Failed to encode chunk. Target buffer too small.")   # LZ4EncoderBase.cs:75-77
+        for i, j in enumerate(fs):
+            raw = int(enc[i]) >= int(sl[i])                      # allowCopy, :79-83
+            body = base[so[i]:so[i] + sl[i]] if raw else dst[doff[i]:doff[i] + enc[i]]
+            stored[j].append(body.tobytes())
+            raws[j].append(raw)
+    frames = []
+    for j in range(nf):
+        out = _header(code, True, block_checksum, content_checksum)
+        _blocks(out, stored[j], raws[j], block_checksum, device)
+        if content_checksum:
+            out.append(struct.pack("<I", xxh32(srcs[j])))       # :95
+        frames.append(b"".join(out))
+    return frames
+
+
 def write_frame(data, block_size: int = 65536, block_checksum: bool = False,
-                content_checksum: bool = False, level: int = 0, device: int = 0) -> bytes:
-    """One LZ4 frame of independent blocks holding `data` (LZ4FrameWriter with Chaining = false)."""
+                content_checksum: bool = False, level: int = 0, device: int = 0, chaining: bool = False) -> bytes:
+    """One LZ4 frame holding `data`: independent blocks (LZ4FrameWriter with Chaining = false), or with
+    chaining=True linked blocks (write_frames)."""
+    if chaining:
+        return write_frames([data], block_size, block_checksum, content_checksum, level, device)[0]
     src = np.frombuffer(bytes(data), dtype=np.uint8) if not isinstance(data, np.ndarray) else data
     code = _block_size_code(block_size)
     bs = max(1024, (block_size + 1023) // 1024 * 1024)          # LZ4EncoderBase.cs:29

@@ -9,6 +9,12 @@ S streams x B linked 64 KiB blocks of datagen, compressed by upstream's chained 
 (LZ4_compress_fast_continue, oracle/_ref/): one k4lz4_decode_chain_batch call per step decodes block k of every
 stream behind its history; GB/s of decoded output over all B steps, next to one k4lz4_decode_batch call over
 the same raw bytes compressed as independent blocks.
+    python tools/dbench.py --what chain-encode [--streams 264,1024,4096] [--chain-blocks 16]
+S streams x B linked 64 KiB blocks of datagen: one k4lz4_encode_chain_batch call per step (device memory) encodes
+block k of every stream behind its history; GB/s of input over all B steps, next to one k4lz4_encode_batch call
+over the same raw bytes, with the encoder's path counters and a spot check against upstream's chained encoder.
+The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
+chained call also moves each block's history and its 16 400-byte state each way).
 """
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -28,7 +34,7 @@ ap.add_argument("--lib", default=None, help="alternative build of libk4lz4.so (e
 ap.add_argument("--streams", default="264,1024,4096", help="chain: stream counts")
 ap.add_argument("--chain-blocks", type=int, default=16, help="chain: linked blocks per stream")
 a = ap.parse_args()
-if a.what == "chain":
+if a.what in ("chain", "chain-encode"):
     a.blocks = max(int(x) for x in a.streams.split(",")) * a.chain_blocks
 if a.lib:
     N.SO_PATH = os.path.abspath(a.lib)
@@ -68,7 +74,8 @@ def timeit(fn, reps):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); fn(); e1.record(); torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
     return min(ts), float(np.median(ts))
-enc(); torch.cuda.synchronize()
+if a.what != "chain-encode":
+    enc(); torch.cuda.synchronize()
 ratio = float(clen.sum()) / (nb * bs)
 if a.what in ("encode", "both"):
     ms, med = timeit(enc, a.reps)
@@ -173,3 +180,69 @@ if a.what == "chain":
         print(f"chain[{a.data}{a.mp}] S={S} B={Bk}: {ms:.3f} ms (median {med:.3f})  {n2*bs/ms/1e6:.1f} GB/s out  "
               f"ratio {cbytes/(n2*bs):.3f} ok={ok} stats {stats} | independent, one call: {ms2:.3f} ms "
               f"{n2*bs/ms2/1e6:.1f} GB/s ok={ok2}", flush=True)
+if a.what == "chain-encode":
+    from tests import chain_ref as CR
+    Bk, SB = a.chain_blocks, N.CHAIN_STATE_BYTES
+    up = CR.Upstream()
+    hraw = raw.cpu().numpy()
+    print("gpu:", torch.cuda.get_device_name(0), flush=True)
+    for S in (int(x) for x in a.streams.split(",")):
+        n2 = S * Bk
+        state = torch.zeros(S * SB, dtype=torch.uint8, device=dev)
+        soff = torch.arange(S, dtype=torch.int64, device=dev) * SB
+        dstc = torch.empty(S * Bk * bound, dtype=torch.uint8, device=dev)
+        steps = [(torch.arange(S, dtype=torch.int64, device=dev) * (Bk * bs) + k * bs,
+                  torch.full((S,), k * bs, dtype=torch.int32, device=dev),
+                  torch.arange(S, dtype=torch.int64, device=dev) * (Bk * bound) + k * bound,
+                  torch.zeros(S, dtype=torch.int32, device=dev)) for k in range(Bk)]
+        rl, cc = rlen[:S], ccap[:S]
+        def chain():
+            state.zero_()
+            for t_so, t_pre, t_do, t_out in steps:
+                B.encode_chain_batch_device(raw.data_ptr(), t_so.data_ptr(), rl.data_ptr(), t_pre.data_ptr(),
+                                            dstc.data_ptr(), t_do.data_ptr(), cc.data_ptr(), state.data_ptr(),
+                                            soff.data_ptr(), t_out.data_ptr(), S, 0, st)
+        B.encode_stats(0, reset=True)
+        chain(); torch.cuda.synchronize()
+        stats = B.encode_stats(0, reset=True)
+        ms, med = timeit(chain, a.reps)
+        # spot check: streams 0 and S-1 against upstream's chained encoder
+        hd = dstc.cpu().numpy()
+        lens = [steps[k][3].cpu().numpy() for k in range(Bk)]
+        ok = True
+        for s_ in (0, S - 1):
+            want = up.encode_chain(hraw[s_ * Bk * bs:(s_ + 1) * Bk * bs].tobytes(), bs)
+            for k in range(Bk):
+                o = (s_ * Bk + k) * bound
+                ok &= int(lens[k][s_]) == len(want[k]) and hd[o:o + len(want[k])].tobytes() == want[k]
+        cbytes = sum(int(l.sum()) for l in lens)
+        def indep():
+            B.encode_batch_device(raw.data_ptr(), roff.data_ptr(), rlen.data_ptr(), slots.data_ptr(), coff.data_ptr(),
+                                  ccap.data_ptr(), clen.data_ptr(), n2, 0, st)
+        B.encode_stats(0, reset=True)
+        indep(); torch.cuda.synchronize()
+        stats2 = B.encode_stats(0, reset=True)
+        ms2, med2 = timeit(indep, a.reps)
+        # host memory: one step (block 1 of every stream, 64 KiB of history each) vs independent encode of it
+        import time
+        so = (np.arange(S, dtype=np.int64) * (Bk * bs) + bs)
+        hs = np.zeros(S * SB, dtype=np.uint8)
+        hso = np.arange(S, dtype=np.int64) * SB
+        hdst = np.empty(S * bound, dtype=np.uint8)
+        hdo = np.arange(S, dtype=np.int64) * bound
+        args = (hraw, so, np.full(S, bs, np.int32))
+        def host_chain():
+            B.encode_chain_batch_host(hraw, so, args[2], np.full(S, bs, np.int32), hdst, hdo, np.full(S, bound, np.int32), hs, hso)
+        def host_indep():
+            B.encode_batch_flat_host(hraw, so, args[2], hdst, hdo, np.full(S, bound, np.int32))
+        th = []
+        for fn in (host_chain, host_indep):
+            fn()
+            t = []
+            for _ in range(a.reps):
+                t0 = time.perf_counter(); fn(); t.append((time.perf_counter() - t0) * 1e3)
+            th.append(float(np.median(t)))
+        print(f"chain-encode[{a.data}{a.mp}] S={S} B={Bk}: {ms:.3f} ms (median {med:.3f})  {n2*bs/ms/1e6:.1f} GB/s in  "
+              f"ratio {cbytes/(n2*bs):.3f} ok={ok} stats {stats} | independent, one call: {ms2:.3f} ms "
+              f"{n2*bs/ms2/1e6:.1f} GB/s stats {stats2} | host memory, one step: chained {th[0]:.2f} ms, "
+              f"independent {th[1]:.2f} ms, state {2*S*SB/2**20:.1f} MiB moved", flush=True)
