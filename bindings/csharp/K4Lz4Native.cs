@@ -59,6 +59,23 @@ namespace K4os.Compression.LZ4.Engine.Native
             byte* srcBase, long* srcOff, int* srcLen, int* prefixLen, byte* dstBase, long* dstOff, int* dstCap,
             byte* stateBase, long* stateOff, int* outLen, int nBlocks, int level, int memKind, void* cudaStream,
             int device);
+        // chain groups: S LZ4FastChainEncoder / LZ4ChainDecoder streams whose rings and states stay on one GPU
+        // (kind 0 = encoder, 1 = decoder; streams[i] names the stream block i advances; not thread-safe)
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_create(
+            int kind, int nStreams, int blockSize, int device, void** group);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_destroy(void* group);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_reset(
+            void* group, int* streams, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_encode(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* dstCap, int* outLen, int n, int level, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_decode(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* dstCap, int* outLen, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_inject(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_state(void* group, int stream, byte* state);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_history(void* group, int stream, byte* dst, int cap);
         // LL.Enforce32 semantics (LL.tools.cs:29-36) for inputs >= 65 547 bytes
         [DllImport(Lib)] public static extern int k4lz4_encode_x32(byte* src, int srcLen, byte* dst, int dstCap, int level);
         [DllImport(Lib)] public static extern int k4lz4_encode_batch_x32(

@@ -195,6 +195,75 @@ K4LZ4_API int32_t k4lz4_encode_chain_batch(const uint8_t *srcBase, const int64_t
                                            int32_t *outLen, int32_t nBlocks, int32_t level,
                                            int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- chain groups: chained streams whose context stays on the GPU ---------------------------- */
+
+/*
+ * A chain group holds S chained streams of one direction on one device: per stream a history ring of
+ * 128 KiB + max(blockSize, 64 KiB) bytes, its write position and, for encoders, its 16 400-byte state record
+ * (an LZ4FastChainEncoder's LZ4_stream_t, Encoders/LZ4FastChainEncoder.cs:14-41) and a "failed" flag.  A call
+ * advances any subset of the streams by one block each; only the blocks' own bytes cross PCIe (memKind
+ * K4LZ4_MEM_HOST), or nothing does (K4LZ4_MEM_DEVICE: the call only enqueues work on `cudaStream` and never
+ * synchronises the host).  A block sees the last min(bytes so far, 65 536) bytes of its stream as history; that
+ * gives exactly the bytes the reference's ring buffers give for any blockSize / extraBlocks.
+ *
+ * streams[i] names the stream block i advances.  Encoder groups: block i is srcBase[srcOff[i] .. +srcLen[i]),
+ * srcLen[i] <= blockSize, and outLen[i] is what k4lz4_encode_chain_batch returns for it (0 for an empty block
+ * and K4LZ4_R_DELEGATE for level >= 3, both leaving the stream untouched; -1 where Encode would throw, after
+ * which the stream returns -1 until it is reset, as the reference's encoder should then be discarded).
+ * Decoder groups: block i decodes into dstBase[dstOff[i] .. +dstCap[i]), dstCap[i] <= blockSize, and outLen[i]
+ * is what k4lz4_decode_chain_batch returns (a failed block leaves its stream as it was, like
+ * LZ4ChainDecoder.Decode).  A block whose stream index is out of range (device memory), whose length exceeds
+ * blockSize or whose encoder stream has failed gets -1 and changes nothing.
+ *
+ * Host memory: sources go up packed in one copy, results and produced bytes come down compacted; bytes of a
+ * destination at index >= outLen[i] are never written.  The group's pinned staging buffers grow and never
+ * shrink.  Device memory: every array (streams included) lives on the group's device; encoded bytes are written
+ * straight into the destination (a block that does not fit may write anything below its dstCap, as
+ * k4lz4_encode_chain_batch does), decoded bytes are copied there from the ring.
+ *
+ * Arguments, in this order, give K4LZ4_E_ARG: a null group or a group of the other kind; an unknown memKind;
+ * a negative count; a required pointer that is NULL while n > 0; with host memory a stream index out of range or
+ * listed twice in one call; a level outside 0..255.  A group is bound to the device it was created on.  Like the
+ * reference's encoder and decoder objects, a group is not thread-safe: calls on one group must not run
+ * concurrently, and device-memory calls on different CUDA streams must be ordered by the caller.  With device
+ * memory, listing a stream twice in one call is undefined.  Counted in k4lz4_encode_stats out4[3] and
+ * k4lz4_decode_stats like the chained batch calls.
+ */
+typedef struct k4lz4_chain_group k4lz4_chain_group;
+#define K4LZ4_CHAIN_ENCODER 0
+#define K4LZ4_CHAIN_DECODER 1
+
+/* kind K4LZ4_CHAIN_ENCODER or K4LZ4_CHAIN_DECODER, nStreams > 0, blockSize > 0, device >= 0 (or < 0: the current
+ * device).  K4LZ4_E_ARG for bad arguments, then K4LZ4_E_NODEVICE without a device, K4LZ4_E_NOMEM when the rings
+ * do not fit; *out is NULL unless K4LZ4_OK is returned.  Every stream starts new. */
+K4LZ4_API int32_t k4lz4_chain_group_create(int32_t kind, int32_t nStreams, int32_t blockSize, int32_t device,
+                                           k4lz4_chain_group **out);
+/* Frees the group after the device has finished its work (NULL is allowed). */
+K4LZ4_API int32_t k4lz4_chain_group_destroy(k4lz4_chain_group *g);
+/* Streams streams[0 .. n) become new (LZ4_createStream / a new LZ4ChainDecoder). */
+K4LZ4_API int32_t k4lz4_chain_group_reset(k4lz4_chain_group *g, const int32_t *streams, int32_t n,
+                                          int32_t memKind, void *cudaStream);
+K4LZ4_API int32_t k4lz4_chain_group_encode(k4lz4_chain_group *g, const int32_t *streams,
+                                           const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           int32_t *outLen, int32_t n, int32_t level,
+                                           int32_t memKind, void *cudaStream);
+K4LZ4_API int32_t k4lz4_chain_group_decode(k4lz4_chain_group *g, const int32_t *streams,
+                                           const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           int32_t *outLen, int32_t n, int32_t memKind, void *cudaStream);
+/* LZ4ChainDecoder.Inject (LZ4ChainDecoder.cs:64-93): srcBase[srcOff[i] .. +srcLen[i]) become the end of stream
+ * streams[i]'s history (a stored block of a linked frame).  Any length; only the last 65 536 bytes are kept. */
+K4LZ4_API int32_t k4lz4_chain_group_inject(k4lz4_chain_group *g, const int32_t *streams,
+                                           const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           int32_t n, int32_t memKind, void *cudaStream);
+/* Synchronous readers (they wait for the device).  _state: the encoder stream's K4LZ4_CHAIN_STATE_BYTES record
+ * into `out`.  Its dictSize may differ from a ring-buffer encoder's where both exceed 65 536: both mean a full
+ * window.  _history: copies the last min(history, cap) bytes of the stream's history (its last <= 65 536
+ * bytes) to `out` and returns how many, or K4LZ4_E_*. */
+K4LZ4_API int32_t k4lz4_chain_group_state(const k4lz4_chain_group *g, int32_t stream, uint8_t *out);
+K4LZ4_API int32_t k4lz4_chain_group_history(const k4lz4_chain_group *g, int32_t stream, uint8_t *out, int32_t cap);
+
 /* ---- XXH32: the checksum of the LZ4 Frame container (SURVEY 8f row 2) ------------------------ */
 
 /* XXH32 of one buffer on the host (frame header byte, serial content checksum) --

@@ -217,6 +217,67 @@ private:
     std::vector<uint8_t> out_;
 };
 
+// Chain groups (k4lz4_chain_group_*): S chained streams whose rings and encoder states stay on one GPU.  RAII owner
+// of the group; the calls take the C ABI's batch arrays (host or device memory) and throw NativeError on a
+// library-level failure.  Like the reference's encoder and decoder objects, not thread-safe.
+class ChainGroup {
+public:
+    ChainGroup(const ChainGroup&) = delete;
+    ChainGroup& operator=(const ChainGroup&) = delete;
+    ChainGroup(ChainGroup&& o) noexcept : g_(o.g_) { o.g_ = nullptr; }
+    ChainGroup& operator=(ChainGroup&& o) noexcept { if (this != &o) { k4lz4_chain_group_destroy(g_); g_ = o.g_; o.g_ = nullptr; } return *this; }
+    ~ChainGroup() { k4lz4_chain_group_destroy(g_); }
+    k4lz4_chain_group* handle() const { return g_; }
+    void Reset(const int32_t* streams, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_chain_group_reset(g_, streams, n, memKind, cudaStream));
+    }
+    // the stream's last <= 64 KiB (LZ4ChainDecoder.Peek / the encoder's dictionary)
+    std::vector<uint8_t> History(int stream) const {
+        std::vector<uint8_t> out(65536);
+        const int k = k4lz4_chain_group_history(g_, stream, out.data(), (int)out.size());
+        check(k < 0 ? k : K4LZ4_OK);
+        out.resize((size_t)k);
+        return out;
+    }
+
+protected:
+    ChainGroup(int kind, int nStreams, int blockSize, int device) { check(k4lz4_chain_group_create(kind, nStreams, blockSize, device, &g_)); }
+    static void check(int rc) { if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error()); }
+    k4lz4_chain_group* g_ = nullptr;
+};
+
+class ChainEncoderGroup : public ChainGroup {
+public:
+    ChainEncoderGroup(int nStreams, int blockSize, int device = 0) : ChainGroup(K4LZ4_CHAIN_ENCODER, nStreams, blockSize, device) {}
+    void Encode(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int n,
+                LZ4Level level = LZ4Level::L00_FAST, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_chain_group_encode(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
+                                       (int)level, memKind, cudaStream));
+    }
+    std::vector<uint8_t> State(int stream) const {
+        std::vector<uint8_t> out(K4LZ4_CHAIN_STATE_BYTES);
+        check(k4lz4_chain_group_state(g_, stream, out.data()));
+        return out;
+    }
+};
+
+class ChainDecoderGroup : public ChainGroup {
+public:
+    ChainDecoderGroup(int nStreams, int blockSize, int device = 0) : ChainGroup(K4LZ4_CHAIN_DECODER, nStreams, blockSize, device) {}
+    void Decode(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int n,
+                int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_chain_group_decode(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
+                                       memKind, cudaStream));
+    }
+    // LZ4ChainDecoder.Inject for every listed stream
+    void Inject(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen, int n,
+                int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_chain_group_inject(g_, streams, srcBase, srcOff, srcLen, n, memKind, cudaStream));
+    }
+};
+
 struct LZ4Pickler {
     // LZ4Pickler.Pickle(ReadOnlySpan<byte>, LZ4Level) -- LZ4Pickler.pickle.cs:51-74
     static std::vector<uint8_t> Pickle(const uint8_t* source, int length, LZ4Level level = LZ4Level::L00_FAST) {

@@ -14,6 +14,7 @@ R_CORRUPT = -1000
 MEM_HOST, MEM_DEVICE = 0, 1
 ALL_DEVICES = -1
 CHAIN_STATE_BYTES = 16400                 # K4LZ4_CHAIN_STATE_BYTES
+CHAIN_ENCODER, CHAIN_DECODER = 0, 1       # K4LZ4_CHAIN_ENCODER / K4LZ4_CHAIN_DECODER
 
 _vp, _i32, _i64, _u32, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64
 _BATCH = [_vp] * 7                        # srcBase srcOff srcLen dstBase dstOff dstCap outLen
@@ -52,6 +53,14 @@ SIGNATURES = {
     "k4lz4_copy_blocks_device": ([_vp] * 5 + [_i32, _vp, _i32], _i32),
     "k4lz4_decode_stats": ([_i32, _vp, _i32], _i32),
     "k4lz4_encode_stats": ([_i32, _vp, _i32], _i32),
+    "k4lz4_chain_group_create": ([_i32, _i32, _i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_destroy": ([_vp], _i32),
+    "k4lz4_chain_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_encode": ([_vp] * 9 + [_i32, _i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_decode": ([_vp] * 9 + [_i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_inject": ([_vp] * 5 + [_i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_state": ([_vp, _i32, _vp], _i32),
+    "k4lz4_chain_group_history": ([_vp, _i32, _vp, _i32], _i32),
 }
 SYMBOLS = list(SIGNATURES)
 

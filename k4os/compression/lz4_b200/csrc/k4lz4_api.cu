@@ -31,6 +31,7 @@
 #include "encode_generic.cuh"
 #include "encode_tile.cuh"
 #include "encode_chain.cuh"
+#include "chain_group.cuh"
 #include "pickle.cuh"
 #include "synth.cuh"
 #include "copy_blocks.cuh"
@@ -868,6 +869,220 @@ int read_stats(const void* sym, int32_t device, uint64_t* out4, int32_t reset) {
 
 }  // namespace
 
+// ---- chain groups -----------------------------------------------------------------------------------
+
+// S streams of one direction on one device (k4lz4.h, chain_group.cuh): rings, states and headers live there
+// between calls; the staging buffers of host-memory calls grow and never shrink.
+struct k4lz4_chain_group {
+    int kind = 0;
+    int32_t nStreams = 0, blockSize = 0;
+    int device = 0;
+    int64_t ring = 0, slot = 0;       // bytes per ring; the room a block or an injection may need at the write position
+    uint8_t* rings = nullptr;
+    uint8_t* states = nullptr;        // encoder groups: K4LZ4_CHAIN_STATE_BYTES per stream
+    k4::ChainGroupHdr* hdr = nullptr;
+    Buf dStage, dDown, hUp{true}, hDown{true};
+    std::vector<int64_t> compactOff;
+};
+
+namespace {
+
+void free_buf(Buf& b) {
+    if (b.p) { if (b.pinned) cudaFreeHost(b.p); else cudaFree(b.p); }
+    b.p = nullptr; b.cap = 0;
+}
+
+void group_free(k4lz4_chain_group* g) {
+    if (g->rings) cudaFree(g->rings);
+    if (g->states) cudaFree(g->states);
+    if (g->hdr) cudaFree(g->hdr);
+    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
+    delete g;
+}
+
+// The group's arguments, then the batch's, in k4lz4.h's order.  A group exists only on a device, so no check
+// here can meet "no device" before an argument error.
+int check_group(const k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int32_t* streams, int memKind) {
+    if (!g || g->kind != kind) return fail(K4LZ4_E_ARG, "null chain group or a group of the other kind");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
+    const bool io = cg != k4::CG_INJECT;
+    if (b.n > 0 && (!streams || !b.srcBase || !b.srcOff || !b.srcLen ||
+                    (io && (!b.dstBase || !b.dstOff || !b.dstCap || !b.outLen))))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
+        std::vector<uint8_t> seen((size_t)g->nStreams, 0);
+        for (int64_t i = 0; i < b.n; i++) {
+            const int32_t s = streams[i];
+            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at block %lld", s, (long long)i);
+            if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
+        }
+    }
+    if (cg == k4::CG_ENCODE && (b.level < 0 || b.level > 0xFF)) return fail(K4LZ4_E_ARG, "bad level %d", b.level);
+    return check_device(g->device, b.n);
+}
+
+// Table of n blocks (chain_group.cuh) carved from `p`: 40 bytes per block.
+k4::ChainGroupTable carve_table(uint8_t* p, int64_t n) {
+    k4::ChainGroupTable t;
+    t.ringOff = (int64_t*)p; t.stateOff = t.ringOff + n; t.copyOff = t.stateOff + n;
+    t.len = (int32_t*)(t.copyOff + n); t.prefix = t.len + n; t.stream = t.prefix + n; t.copyLen = t.stream + n;
+    return t;
+}
+constexpr int64_t TABLE_BYTES = 3 * 8 + 4 * 4;
+
+// The first half of a step on the device, current device = the group's: prepare, the copy into the rings, the
+// codec and, when `gather`, the copy of decoded bytes to the destination.  `b` holds device pointers; for
+// encoding its destination is where the codec writes.
+cudaError_t group_codec(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* streams, const k4::ChainGroupTable& t,
+                        bool gather, cudaStream_t st) {
+    const int n = (int)b.n, thr = 128, grid = (n + thr - 1) / thr;
+    k4::chain_group_prepare_kernel<<<grid, thr, 0, st>>>(cg, streams, cg == k4::CG_DECODE ? b.dstCap : b.srcLen,
+                                                         b.srcOff, n, g->nStreams, g->blockSize, g->ring, g->hdr, t);
+    g_launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && cg != k4::CG_DECODE)
+        e = launch_op(OP_COPY, Batch{b.srcBase, t.copyOff, t.copyLen, g->rings, t.ringOff, nullptr, nullptr, n}, st);
+    if (e == cudaSuccess && cg == k4::CG_ENCODE) {
+        Batch kb{g->rings, t.ringOff, t.len, b.dstBase, b.dstOff, b.dstCap, b.outLen, n, b.level};
+        kb.prefixLen = t.prefix; kb.stateBase = g->states; kb.stateOff = t.stateOff;
+        e = launch_op(OP_ENCCHAIN, kb, st);
+    }
+    if (e == cudaSuccess && cg == k4::CG_DECODE) {
+        Batch kb{b.srcBase, b.srcOff, b.srcLen, g->rings, t.ringOff, t.len, b.outLen, n};
+        kb.prefixLen = t.prefix;
+        e = launch_op(OP_CHAIN, kb, st);
+        if (e == cudaSuccess && gather)
+            e = launch_op(OP_COPY, Batch{g->rings, t.ringOff, b.outLen, b.dstBase, b.dstOff, nullptr, nullptr, n}, st);
+    }
+    return e;
+}
+
+// The second half, after every read of the block's slot: the commit and the slides (a slide may overwrite the
+// front of a block that started below 64 KiB).
+cudaError_t group_commit(k4lz4_chain_group* g, int cg, const int32_t* outLen, int64_t n64, const k4::ChainGroupTable& t,
+                         cudaStream_t st) {
+    const int n = (int)n64, thr = 128, grid = (n + thr - 1) / thr;
+    k4::chain_group_commit_kernel<<<grid, thr, 0, st>>>(cg, outLen, n, g->ring, g->slot, g->hdr, t);
+    g_launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess)
+        e = launch_op(OP_COPY, Batch{g->rings, t.copyOff, t.copyLen, g->rings, t.ringOff, nullptr, nullptr, n}, st);
+    return e;
+}
+
+// Device memory: the table comes from the device's stream-ordered pool, so nothing here waits for the device.
+int group_device(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* streams, cudaStream_t st) {
+    const Dev* D = dev_state(g->device);
+    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
+    uint8_t* tab = nullptr;
+    CU_TRY(cudaMallocFromPoolAsync((void**)&tab, (size_t)(b.n * TABLE_BYTES), D->pool, st));
+    const k4::ChainGroupTable t = carve_table(tab, b.n);
+    cudaError_t e = group_codec(g, cg, b, streams, t, cg == k4::CG_DECODE, st);
+    if (e == cudaSuccess) e = group_commit(g, cg, b.outLen, b.n, t, st);
+    cudaFreeAsync(tab, st);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain group step: %s", cudaGetErrorString(e)); }
+    return K4LZ4_OK;
+}
+
+// Host memory, synchronous.  Up, in one copy: source offsets, destination-slot offsets, streams, lengths,
+// capacities, then the sources packed (16-aligned; an injection sends only the bytes it keeps).  After the codec the
+// results come down; the produced bytes are gathered into one compact buffer (copy_blocks_kernel) and come down
+// in one copy, then exactly outLen[i] > 0 bytes of each block go to the caller.
+int group_host(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* streams, cudaStream_t st) {
+    const int64_t n = b.n;
+    const bool enc = cg == k4::CG_ENCODE, inj = cg == k4::CG_INJECT;
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    auto sendLen = [&](int64_t i) -> int64_t {     // the source bytes block i sends up
+        const int64_t L = b.srcLen[i];
+        if (L <= 0) return 0;
+        if (inj) return std::min<int64_t>(L, k4::CG_WINDOW);
+        return enc && L > g->blockSize ? 0 : L;
+    };
+    auto room = [&](int64_t i) -> int64_t {        // encoder: the device slot the codec writes
+        const int32_t L = b.srcLen[i];
+        if (!enc || L <= 0 || L > g->blockSize) return 0;
+        return std::min<int64_t>(std::max<int32_t>(b.dstCap[i], 0), k4::max_output_size(L));
+    };
+    const int64_t metaAt = 0, srcAt = a16(n * (4 * 3 + 8 * 2));
+    int64_t srcBytes = 0, scratch = 0;
+    for (int64_t i = 0; i < n; i++) { srcBytes = a16(srcBytes + sendLen(i)); scratch = a16(scratch + room(i)); }
+    const int64_t upBytes = srcAt + srcBytes;
+    const int64_t tabAt = a16(upBytes), outAt = tabAt + a16(n * TABLE_BYTES), coffAt = outAt + a16(n * 4);
+    const int64_t scratchAt = coffAt + a16(n * 8), stageBytes = scratchAt + scratch;
+    CU_TRY(g->hUp.ensure((size_t)upBytes + 16));
+    CU_TRY(g->dStage.ensure((size_t)stageBytes + 16));
+    uint8_t* H = (uint8_t*)g->hUp.p;             // srcOff dstOff (int64) | streams srcLen dstCap (int32)
+    int64_t* hso = (int64_t*)(H + metaAt); int64_t* hdo = hso + n;
+    int32_t* hs = (int32_t*)(hdo + n); int32_t* hl = hs + n; int32_t* hc = hl + n;
+    for (int64_t i = 0, sp = 0, dp = 0; i < n; i++) {
+        const int64_t k = sendLen(i);
+        hs[i] = streams[i];
+        hl[i] = inj ? (int32_t)k : b.srcLen[i];
+        hc[i] = inj ? 0 : b.dstCap[i];
+        hso[i] = sp; hdo[i] = dp;
+        sp = a16(sp + k); dp = a16(dp + room(i));
+    }
+    parallel_for_blocks(0, n, srcBytes, [&](int64_t lo, int64_t hi) {
+        for (int64_t i = lo; i < hi; i++) {
+            const int64_t k = sendLen(i);
+            if (k > 0) memcpy(H + srcAt + hso[i], b.srcBase + b.srcOff[i] + (b.srcLen[i] - k), (size_t)k);
+        }
+    });
+    uint8_t* D = (uint8_t*)g->dStage.p;
+    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
+    const int64_t* dso = (const int64_t*)(D + metaAt);
+    const int32_t* ds = (const int32_t*)(dso + 2 * n);
+    int32_t* dOut = (int32_t*)(D + outAt);
+    Batch kb = b;
+    kb.srcBase = D + srcAt; kb.srcOff = dso; kb.srcLen = ds + n;
+    kb.dstBase = D + scratchAt; kb.dstOff = dso + n; kb.dstCap = ds + 2 * n;
+    kb.outLen = dOut;
+    const k4::ChainGroupTable t = carve_table(D + tabAt, n);
+    cudaError_t e = group_codec(g, cg, kb, ds, t, false, st);
+    if (e == cudaSuccess && inj) e = group_commit(g, cg, dOut, n, t, st);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain group step: %s", cudaGetErrorString(e)); }
+    if (inj) { CU_TRY(cudaStreamSynchronize(st)); return K4LZ4_OK; }
+    CU_TRY(cudaMemcpyAsync(b.outLen, dOut, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    auto& co = g->compactOff;
+    co.resize((size_t)n);
+    int64_t total = 0;
+    for (int64_t i = 0; i < n; i++) { co[(size_t)i] = total; if (b.outLen[i] > 0) total = a16(total + b.outLen[i]); }
+    if (total == 0) {
+        CU_TRY(group_commit(g, cg, dOut, n, t, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        return K4LZ4_OK;
+    }
+    CU_TRY(g->dDown.ensure((size_t)total + 16));
+    CU_TRY(g->hDown.ensure((size_t)total + 16));
+    memcpy(H, co.data(), (size_t)n * 8);            // the upload buffer is free again
+    CU_TRY(cudaMemcpyAsync(D + coffAt, H, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    const Batch gb = enc ? Batch{kb.dstBase, kb.dstOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt), nullptr, nullptr, n}
+                         : Batch{g->rings, t.ringOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt), nullptr, nullptr, n};
+    CU_TRY(launch_op(OP_COPY, gb, st));
+    CU_TRY(group_commit(g, cg, dOut, n, t, st));
+    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    const uint8_t* stage = (const uint8_t*)g->hDown.p;
+    parallel_for_blocks(0, n, total, [&](int64_t lo, int64_t hi) {
+        for (int64_t i = lo; i < hi; i++)
+            if (b.outLen[i] > 0) memcpy(b.dstBase + b.dstOff[i], stage + co[(size_t)i], (size_t)b.outLen[i]);
+    });
+    return K4LZ4_OK;
+}
+
+int group_run(k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int32_t* streams, int memKind, void* stream) {
+    const int rc = check_group(g, kind, cg, b, streams, memKind);
+    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    return memKind == K4LZ4_MEM_HOST ? group_host(g, cg, b, streams, (cudaStream_t)stream)
+                                     : group_device(g, cg, b, streams, (cudaStream_t)stream);
+}
+
+}  // namespace
+
 // ---- exported C ABI ------------------------------------------------------------------------
 
 extern "C" {
@@ -948,6 +1163,122 @@ int32_t k4lz4_encode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, 
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level};
     b.prefixLen = prefixLen; b.stateBase = stateBase; b.stateOff = stateOff;
     return run(OP_ENCCHAIN, b, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_chain_group_create(int32_t kind, int32_t nStreams, int32_t blockSize, int32_t device,
+                                 k4lz4_chain_group** out) {
+    if (out) *out = nullptr;
+    if (!out || (kind != K4LZ4_CHAIN_ENCODER && kind != K4LZ4_CHAIN_DECODER) || nStreams <= 0 || blockSize <= 0)
+        return fail(K4LZ4_E_ARG, "bad chain group arguments (kind %d, %d streams, block size %d)", kind, nStreams, blockSize);
+    int rc = check_device(device, 1);
+    if (rc != K4LZ4_OK) return rc;
+    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    k4lz4_chain_group* g = new k4lz4_chain_group;
+    g->kind = kind; g->nStreams = nStreams; g->blockSize = blockSize; g->device = device;
+    g->slot = std::max<int64_t>((blockSize + 15) & ~int64_t(15), k4::CG_WINDOW);
+    g->ring = 2 * k4::CG_WINDOW + g->slot;
+    const size_t S = (size_t)nStreams;
+    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess && kind == K4LZ4_CHAIN_ENCODER) e = cudaMalloc((void**)&g->states, S * K4LZ4_CHAIN_STATE_BYTES);
+    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess && g->states) e = cudaMemset(g->states, 0, S * K4LZ4_CHAIN_STATE_BYTES);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        group_free(g);
+        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "chain group of %d x %lld bytes: %s",
+                    nStreams, (long long)(2 * k4::CG_WINDOW + std::max<int64_t>(blockSize, k4::CG_WINDOW)),
+                    cudaGetErrorString(e));
+    }
+    *out = g;
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_chain_group_destroy(k4lz4_chain_group* g) {
+    if (!g) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    cudaDeviceSynchronize();
+    group_free(g);
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_chain_group_reset(k4lz4_chain_group* g, const int32_t* streams, int32_t n, int32_t memKind,
+                                void* cudaStream) {
+    if (!g) return fail(K4LZ4_E_ARG, "null chain group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (n < 0) return fail(K4LZ4_E_ARG, "bad block count %d", n);
+    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST)
+        for (int32_t i = 0; i < n; i++)
+            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
+    if (n == 0) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    cudaStream_t st = (cudaStream_t)cudaStream;
+    const int32_t* ds = streams;
+    if (memKind == K4LZ4_MEM_HOST) {
+        CU_TRY(g->hUp.ensure((size_t)n * 4));
+        CU_TRY(g->dStage.ensure((size_t)n * 4));
+        memcpy(g->hUp.p, streams, (size_t)n * 4);
+        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        ds = (const int32_t*)g->dStage.p;
+    }
+    k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
+    g_launches++;
+    CU_TRY(cudaGetLastError());
+    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_chain_group_encode(k4lz4_chain_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                 const int64_t* srcOff, const int32_t* srcLen, uint8_t* dstBase, const int64_t* dstOff,
+                                 const int32_t* dstCap, int32_t* outLen, int32_t n, int32_t level, int32_t memKind,
+                                 void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n, level};
+    return group_run(g, K4LZ4_CHAIN_ENCODER, k4::CG_ENCODE, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_chain_group_decode(k4lz4_chain_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                 const int64_t* srcOff, const int32_t* srcLen, uint8_t* dstBase, const int64_t* dstOff,
+                                 const int32_t* dstCap, int32_t* outLen, int32_t n, int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
+    return group_run(g, K4LZ4_CHAIN_DECODER, k4::CG_DECODE, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_chain_group_inject(k4lz4_chain_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                 const int64_t* srcOff, const int32_t* srcLen, int32_t n, int32_t memKind,
+                                 void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, nullptr, n};
+    return group_run(g, K4LZ4_CHAIN_DECODER, k4::CG_INJECT, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_chain_group_state(const k4lz4_chain_group* g, int32_t stream, uint8_t* out) {
+    if (!g || g->kind != K4LZ4_CHAIN_ENCODER || !out || stream < 0 || stream >= g->nStreams)
+        return fail(K4LZ4_E_ARG, "bad chain group state arguments");
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    CU_TRY(cudaDeviceSynchronize());
+    CU_TRY(cudaMemcpy(out, g->states + (size_t)stream * K4LZ4_CHAIN_STATE_BYTES, K4LZ4_CHAIN_STATE_BYTES,
+                      cudaMemcpyDeviceToHost));
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_chain_group_history(const k4lz4_chain_group* g, int32_t stream, uint8_t* out, int32_t cap) {
+    if (!g || (!out && cap > 0) || cap < 0 || stream < 0 || stream >= g->nStreams)
+        return fail(K4LZ4_E_ARG, "bad chain group history arguments");
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    CU_TRY(cudaDeviceSynchronize());
+    k4::ChainGroupHdr h;
+    CU_TRY(cudaMemcpy(&h, g->hdr + stream, sizeof(h), cudaMemcpyDeviceToHost));
+    const int64_t k = std::min<int64_t>(std::min<int64_t>(h.pos, k4::CG_WINDOW), cap);
+    if (k > 0)
+        CU_TRY(cudaMemcpy(out, g->rings + (size_t)stream * (size_t)g->ring + (size_t)(h.pos - k), (size_t)k,
+                          cudaMemcpyDeviceToHost));
+    return (int32_t)k;
 }
 
 int32_t k4lz4_partial_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,

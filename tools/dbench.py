@@ -15,12 +15,19 @@ block k of every stream behind its history; GB/s of input over all B steps, next
 over the same raw bytes, with the encoder's path counters and a spot check against upstream's chained encoder.
 The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
 chained call also moves each block's history and its 16 400-byte state each way).
+Both chain arms also time a chain group (k4lz4_chain_group_*: rings and states resident on the GPU) and print
+per-step times (one block of every stream) through host memory -- LZ4FastChainEncoder.EncodeMany /
+LZ4ChainDecoder.DecodeMany (today's chained call with its ring staging), the group, one independent-block call
+over the same blocks -- and through device memory -- the chained batch call, the group, and the independent call
+over all steps divided by the step count.
 """
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 from k4os.compression.lz4_b200 import batch as B, _native as N
+import k4os.compression.lz4_b200 as K
+import time
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--blocks", type=int, default=32768)
@@ -34,6 +41,21 @@ ap.add_argument("--lib", default=None, help="alternative build of libk4lz4.so (e
 ap.add_argument("--streams", default="264,1024,4096", help="chain: stream counts")
 ap.add_argument("--chain-blocks", type=int, default=16, help="chain: linked blocks per stream")
 a = ap.parse_args()
+
+
+def host_ms(fn, reps):
+    """median wall time of fn() in ms after one warm-up call"""
+    fn()
+    t = []
+    for _ in range(reps):
+        t0 = time.perf_counter(); fn(); t.append((time.perf_counter() - t0) * 1e3)
+    return float(np.median(t))
+
+
+def report(kind, S, Bk, host, dev):
+    print(f"{kind}-group S={S} x {Bk} steps, ms per step | host memory: chained {host[0]:.2f}, group {host[1]:.2f}, "
+          f"independent {host[2]:.2f} | device memory: chained {dev[0]:.3f}, group {dev[1]:.3f}, "
+          f"independent {dev[2]:.3f}", flush=True)
 if a.what in ("chain", "chain-encode"):
     a.blocks = max(int(x) for x in a.streams.split(",")) * a.chain_blocks
 if a.lib:
@@ -180,6 +202,35 @@ if a.what == "chain":
         print(f"chain[{a.data}{a.mp}] S={S} B={Bk}: {ms:.3f} ms (median {med:.3f})  {n2*bs/ms/1e6:.1f} GB/s out  "
               f"ratio {cbytes/(n2*bs):.3f} ok={ok} stats {stats} | independent, one call: {ms2:.3f} ms "
               f"{n2*bs/ms2/1e6:.1f} GB/s ok={ok2}", flush=True)
+        # the group: device memory, one call per step into the same destination
+        gst = torch.arange(S, dtype=torch.int32, device=dev)
+        with K.ChainDecoderGroup(S, bs) as g:
+            def grp():
+                g.reset_device(gst.data_ptr(), S, st)
+                for t_src, t_so, t_ln, t_do, t_cap, t_pre in steps:
+                    g.decode_device(gst.data_ptr(), t_src.data_ptr(), t_so.data_ptr(), t_ln.data_ptr(), out.data_ptr(),
+                                    t_do.data_ptr(), t_cap.data_ptr(), olen.data_ptr(), S, st)
+            out.zero_()
+            grp(); torch.cuda.synchronize()
+            gok = bool(torch.equal(out, raw[:S * Bk * bs]))
+            gms, _ = timeit(grp, a.reps)
+            # host memory: every step through the group, LZ4ChainDecoder.DecodeMany and one independent call
+            hblocks = [[comp[s_][k] for s_ in range(S)] for k in range(Bk)]
+            def grp_host():
+                g.reset()
+                for blocks in hblocks:
+                    g.decode(blocks)
+            def today_host():
+                decs = [K.LZ4ChainDecoder(bs) for _ in range(S)]
+                for blocks in hblocks:
+                    K.LZ4ChainDecoder.DecodeMany(decs, blocks)
+            hpk = clen[:n2].cpu().numpy().reshape(S, Bk)
+            hsl = slots.cpu().numpy()
+            iblocks = [hsl[(s_ * Bk + 1) * bound:(s_ * Bk + 1) * bound + int(hpk[s_, 1])].tobytes() for s_ in range(S)]
+            host = [host_ms(today_host, 1) / Bk, host_ms(grp_host, max(a.reps // 2, 1)) / Bk,
+                    host_ms(lambda: B.decode_batch_host(iblocks, [bs] * S), a.reps)]
+        report("chain", S, Bk, host, [ms / Bk, gms / Bk, ms2 / Bk])
+        print(f"   group ok={gok}", flush=True)
 if a.what == "chain-encode":
     from tests import chain_ref as CR
     Bk, SB = a.chain_blocks, N.CHAIN_STATE_BYTES
@@ -246,3 +297,36 @@ if a.what == "chain-encode":
               f"ratio {cbytes/(n2*bs):.3f} ok={ok} stats {stats} | independent, one call: {ms2:.3f} ms "
               f"{n2*bs/ms2/1e6:.1f} GB/s stats {stats2} | host memory, one step: chained {th[0]:.2f} ms, "
               f"independent {th[1]:.2f} ms, state {2*S*SB/2**20:.1f} MiB moved", flush=True)
+        gst = torch.arange(S, dtype=torch.int32, device=dev)
+        gout = [torch.zeros(S, dtype=torch.int32, device=dev) for _ in range(Bk)]
+        gdst = torch.empty_like(dstc)
+        with K.ChainEncoderGroup(S, bs) as g:
+            def grp():
+                g.reset_device(gst.data_ptr(), S, st)
+                for (t_so, t_pre, t_do, t_out), t_g in zip(steps, gout):
+                    g.encode_device(gst.data_ptr(), raw.data_ptr(), t_so.data_ptr(), rl.data_ptr(), gdst.data_ptr(),
+                                    t_do.data_ptr(), cc.data_ptr(), t_g.data_ptr(), S, 0, st)
+            grp(); torch.cuda.synchronize()
+            gok = all(torch.equal(gout[k], steps[k][3]) for k in range(Bk))
+            gd = gdst.cpu().numpy()
+            for k in range(Bk):
+                for s_ in range(0, S, 61):
+                    o, r = (s_ * Bk + k) * bound, int(lens[k][s_])
+                    gok &= gd[o:o + r].tobytes() == hd[o:o + r].tobytes()
+            gms, _ = timeit(grp, a.reps)
+            hblocks = [[hraw[(s_ * Bk + k) * bs:(s_ * Bk + k + 1) * bs].tobytes() for s_ in range(S)] for k in range(Bk)]
+            def grp_host():
+                g.reset()
+                for blocks in hblocks:
+                    g.encode(blocks)
+            def today_host():
+                encs = [K.LZ4FastChainEncoder(bs) for _ in range(S)]
+                tg = [np.empty(bound, np.uint8) for _ in range(S)]
+                for blocks in hblocks:
+                    for e_, b_ in zip(encs, blocks):
+                        e_.Topup(b_)
+                    K.LZ4FastChainEncoder.EncodeMany(encs, tg)
+            host = [host_ms(today_host, 1) / Bk, host_ms(grp_host, max(a.reps // 2, 1)) / Bk,
+                    host_ms(lambda: B.encode_batch_host(hblocks[1]), a.reps)]
+        report("chain-encode", S, Bk, host, [ms / Bk, gms / Bk, ms2 / Bk])
+        print(f"   group ok={gok}", flush=True)
