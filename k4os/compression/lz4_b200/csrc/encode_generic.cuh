@@ -227,10 +227,10 @@ __device__ __forceinline__ int codec_encode_warp(const uint8_t* src, int n, uint
 constexpr int ENC_WARPS_PER_CTA = K4_ENC_TAGS ? 9 : 7;   // pickle_kernel: 2 CTAs x 7 warps x 16 KiB of tables fill the SM
 // encode_spec_kernel / encode_spec_gtab_kernel (one warp per CTA, see encode_tile.cuh): resident warps per SM
 #ifndef K4_ENC_SM_WARPS
-#define K4_ENC_SM_WARPS 8       // shared-memory tables: 8 x (16 KiB + 1 KiB the hardware reserves per CTA); the rest of the 256 KiB stays L1
+#define K4_ENC_SM_WARPS 10      // shared-memory tables: 10 x (16 KiB + 1 KiB the hardware reserves per CTA); the rest of the 256 KiB stays L1
 #endif
 #ifndef K4_ENC_GM_WARPS
-#define K4_ENC_GM_WARPS 22      // global-memory tables (H100 sweep in DESIGN.md 7.2)
+#define K4_ENC_GM_WARPS 20      // global-memory tables (H100 sweep in DESIGN.md 7.2)
 #endif
 constexpr int ENC_SM_WARPS = K4_ENC_SM_WARPS;
 constexpr int ENC_GM_WARPS = K4_ENC_GM_WARPS;

@@ -42,6 +42,19 @@ __device__ __forceinline__ uint32_t lds_u32u(const uint8_t* p) {
 #ifndef K4_ENC_PF
 #define K4_ENC_PF 0
 #endif
+//   K4_ENC_WIN  lanes of the FIRST batch of a search run in the persistent encoder (0 or 32: all 32).  Only lanes below it hash, load a slot and
+//               load candidate bytes; when none of them hits, their slot stores are committed and the run goes on
+//               32 lanes wide.  Most runs hit within a few probes, so the scattered loads of the lanes behind the
+//               hit (discarded anyway) are mostly not issued, at the price of one more batch for the longer runs.
+#ifndef K4_ENC_WIN
+#define K4_ENC_WIN 16
+#endif
+//   K4_ENC_SPEC global-table warps (TAGMODE 2): take the first lane whose tag agrees as the hit and check its candidate
+//               word in the same round of loads as the first catch-up and LZ4_count round (see encode_spec_warp)
+#ifndef K4_ENC_SPEC
+#define K4_ENC_SPEC 1
+#endif
+static_assert(K4_ENC_WIN >= 0 && K4_ENC_WIN <= 32, "K4_ENC_WIN: lanes of a run's first batch, 1..32 (0 = 32)");
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" :: "l"(p)); }
 
 __device__ __forceinline__ uint32_t probe_advance(uint32_t q) {
@@ -56,7 +69,8 @@ __device__ __forceinline__ uint32_t probe_advance(uint32_t q) {
 // Returns the engine's value: bytes written, 0 when the reference's limitedOutput checks fail.
 // TAGMODE: 0 = plain u16 slots; 1 = u16 slots + one filter byte per slot behind the table, both loaded per probe;
 // 2 = 32-bit slots (position | 16-bit tag << 16); 3 = as 1, but the position is loaded only when the tag agrees.
-template <bool STAGED, bool HARD = true, bool GTAB = false, int TAGMODE = (K4_ENC_TAGS ? 1 : 0)>
+// WIN: lanes of the first batch of every search run (32 = all; K4_ENC_WIN).
+template <bool STAGED, bool HARD = true, bool GTAB = false, int TAGMODE = (K4_ENC_TAGS ? 1 : 0), int WIN = 32>
 __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* sin, const uint32_t n,
                                 uint8_t* __restrict__ dst, const int cap, const int hardCap, uint16_t* table) {
     const int lane = lane_id();
@@ -118,6 +132,9 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
         bool post = false;              // lane 0 of the next batch is the post-match probe at ip
         uint32_t q0 = 0;                // first search-probe index of the next batch
         uint32_t base = 1;              // position of search probe 0 of the current run
+        constexpr uint32_t WIN0 = (WIN <= 0 || WIN > 32) ? 32u : (uint32_t)WIN;
+        constexpr bool NARROW = WIN0 < 32u;
+        uint32_t width = WIN0;          // lanes of the current batch: WIN0 for a run's first batch, then 32
         for (;;) {
             // ---- one batch of up to 32 probes (App. A step 3, and step 8 as lane 0) -----------------
             uint32_t h2 = 0xFFFFFFFFu, tag2 = 0;
@@ -125,8 +142,10 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
             const bool isPost = post && lane == 0;
             const uint32_t q = q0 + (uint32_t)lane - (post ? 1u : 0u);            // search-probe index (lanes >= 1 if post)
             const uint32_t pos = isPost ? ip : base + probe_advance(q);
-            // a search probe executes only if the NEXT probe position stays <= mflimitPlusOne (:172)
-            const bool valid = isPost || (base + probe_advance(q + 1) <= mfl1);
+            // a search probe executes only if the NEXT probe position stays <= mflimitPlusOne (:172); lanes beyond
+            // the batch's width are neither probes nor the end of the run
+            const bool inWin = !NARROW || (uint32_t)lane < width;
+            const bool valid = inWin && (isPost || (base + probe_advance(q + 1) <= mfl1));
             const uint32_t v = valid ? RD32(pos) : 0u;
             const uint32_t prod = v * 2654435761u;
             const uint32_t h = valid ? prod >> 19 : (0x10000u + (uint32_t)lane);
@@ -151,8 +170,15 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
             const uint32_t fwdPos = __shfl_sync(FULL, pos, fromLane);
             const uint32_t fwdTag = __shfl_sync(FULL, tg, fromLane);
             if (earlier) { cand = fwdPos; ctag = TAGS ? fwdTag : tg; lazyPos = false; }   // sees the nearest earlier store
+            // SPEC: equal 4-byte words have equal tags, so only a lane whose tag agrees can hit -- and with 16-bit
+            // tags nearly every such lane does.  So the first agreeing lane is taken as the hit, and the load that
+            // checks its candidate word (lane 8) goes out together with the first round of the catch-up and of
+            // LZ4_count (lanes 0..7), which only need the candidate's position: one memory round trip where
+            // checking first takes two.  A failed check moves on to the next agreeing lane, so `f` is exactly the
+            // first lane whose candidate word equals its own.
+            constexpr bool SPEC = K4_ENC_SPEC && TAGMODE == 2 && K4_ENC_OVL;
             bool hit = false;
-            if (valid && ctag == tg) {                                            // :228 (byU16: no distance test)
+            if (!SPEC && valid && ctag == tg) {                                            // :228 (byU16: no distance test)
                 if (TAGMODE == 3 && lazyPos) cand = TGET(h);
                 hit = RD32(cand) == v;
                 if (TAGS && !STAGED && (K4_ENC_PF & 1)) {                          // few lanes get here: the tag filter
@@ -161,10 +187,33 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
                 }
             }
             if (!STAGED && (K4_ENC_PF & 2) && lane == 0) prefetch_l1(src + (pos + 384u < n ? pos + 384u : n - 1u));
-            const unsigned hits = __ballot_sync(FULL, hit);
-            const unsigned ends = __ballot_sync(FULL, !valid);
-            const int f = hits ? __ffs(hits) - 1 : 32;
+            const unsigned ends = __ballot_sync(FULL, inWin && !valid);
             const int e = ends ? __ffs(ends) - 1 : 32;
+            int f = 32;
+            uint32_t sm = 0u, sip = 0u, sx1 = 0u;                                 // SPEC: the hit's candidate, position,
+            bool sok = true;                                                      // first count round and catch-up round
+            if (SPEC) {
+                for (unsigned agree = __ballot_sync(FULL, valid && ctag == tg); agree; agree &= agree - 1u) {
+                    const int c = __ffs(agree) - 1;
+                    if (e < c) break;
+                    sm = __shfl_sync(FULL, cand, c);
+                    sip = __shfl_sync(FULL, pos, c);
+                    const uint32_t vc = __shfl_sync(FULL, v, c);
+                    bool same = true;
+                    sx1 = 0u; sok = true;
+                    if (lane < 8) {
+                        const uint32_t a = sip + MINMATCH + 4u * lane;
+                        if ((int)mlim - (int)a > 0) sx1 = RD32(a) ^ RD32(sm + MINMATCH + 4u * lane);
+                        sok = (sip > anchor + lane) && (sm > (uint32_t)lane) && (RD8(sip - 1 - lane) == RD8(sm - 1 - lane));
+                    } else if (lane == 8) {
+                        same = RD32(sm) == vc;
+                    }
+                    if (__all_sync(FULL, same)) { f = c; break; }
+                }
+            } else {
+                const unsigned hits = __ballot_sync(FULL, hit);
+                f = hits ? __ffs(hits) - 1 : 32;
+            }
             if (e < f) break;                                                     // ran into the end: last literals
             // commit the slot stores of probes 0..f in serial order: last writer per hash wins
             {
@@ -180,20 +229,22 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
                 if (doStore) slotPut(h, pos, tg);
                 __syncwarp();
             }
-            if (f == 32) {                                                        // 32 misses: keep searching
-                if (post) { post = false; base = ip + 1; q0 = 31; }
-                else q0 += 32;
+            if (f == 32) {                                                        // no hit: keep searching
+                const uint32_t w = NARROW ? width : 32u;
+                if (post) { post = false; base = ip + 1; q0 = w - 1; }
+                else q0 += w;
+                width = 32;
                 continue;
             }
             const bool zeroLit = post && f == 0;                                  // :459-463
-            uint32_t m = __shfl_sync(FULL, cand, f);
-            ip = __shfl_sync(FULL, pos, f);
+            uint32_t m = SPEC ? sm : __shfl_sync(FULL, cand, f);
+            ip = SPEC ? sip : __shfl_sync(FULL, pos, f);
             // LZ4_count does not depend on the catch-up: [ip-c, ip+4) is known equal, so counting from the hit's
             // ip+4 and adding c gives the reference's value (ip+4 <= mflimit+4 < matchlimit).  Its first round of
             // loads is issued before the catch-up loop so that both wait for memory at the same time.
             const uint32_t a0h = ip + MINMATCH, b0h = m + MINMATCH;
-            uint32_t x1 = 0u;
-            if (K4_ENC_OVL) {
+            uint32_t x1 = sx1;
+            if (K4_ENC_OVL && !SPEC) {
                 const uint32_t a = a0h + 4u * lane;
                 if (lane < 8 && (int)mlim - (int)a > 0) x1 = RD32(a) ^ RD32(b0h + 4u * lane);
             }
@@ -202,8 +253,9 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
                 // eight lanes first: a catch-up is rarely longer, and lanes that do not take part issue no load
                 for (int width = 8;; width = 32) {
                     const bool part = lane < width;
-                    const bool ok = !part || ((ip > anchor + lane) && (m > (uint32_t)lane) &&
-                                              (RD8(ip - 1 - lane) == RD8(m - 1 - lane)));
+                    const bool ok = (SPEC && width == 8) ? sok
+                                  : (!part || ((ip > anchor + lane) && (m > (uint32_t)lane) &&
+                                               (RD8(ip - 1 - lane) == RD8(m - 1 - lane))));
                     const unsigned bad = __ballot_sync(FULL, !ok);
                     const int c = bad ? __ffs(bad) - 1 : width;
                     ip -= c; m -= c; caught += (uint32_t)c;
@@ -263,7 +315,7 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint8_t* 
             ip += mc + MINMATCH;
             anchor = ip;                                                          // :388
             if (ip >= mfl1) break;                                                // :391
-            post = true; q0 = 0; base = ip + 1;                                   // step 8 rides with the next batch
+            post = true; q0 = 0; base = ip + 1; width = WIN0;                     // step 8 rides with the next batch
         }
     }
     {   // ---- step 9: last literals, :469-503 -----------------------------------------------------------
@@ -319,7 +371,7 @@ __device__ __forceinline__ void encode_persistent_warp(
         if (level >= 3) { if (lane == 0) outLen[b] = -2; continue; }
         int r;
         if (n_ >= LIMIT_64K) r = encode_block_warp(src, n_, dst, cap, 0x7fffffff, table, enforce32);
-        else r = encode_spec_warp<false, false, GTAB, GTAB ? ENC_GTAG : (K4_ENC_TAGS ? 1 : 0)>(src, nullptr, (uint32_t)n_, dst, cap, 0x7fffffff, table);
+        else r = encode_spec_warp<false, false, GTAB, GTAB ? ENC_GTAG : (K4_ENC_TAGS ? 1 : 0), K4_ENC_WIN>(src, nullptr, (uint32_t)n_, dst, cap, 0x7fffffff, table);
         if (lane == 0) {
             outLen[b] = r <= 0 ? -1 : r;
             atomicAdd(&g_encode_stats[n_ >= LIMIT_64K ? 2 : (GTAB ? 1 : 0)], 1ull);
