@@ -87,6 +87,19 @@ namespace K4os.Compression.LZ4.Engine.Native
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
             int* outLen, int nMessages, int level, int memKind, void* cudaStream, int device);
 
+        // LZ4Frame.Encode / Decode over whole buffers, batched across frames (k4lz4.h "LZ4 Frame")
+        public const int FRAME_INDEPENDENT = 1, FRAME_BLOCK_CHECKSUM = 2, FRAME_CONTENT_CHECKSUM = 4;
+        public const int R_DST_SMALL = -1001;
+        [DllImport(Lib)] public static extern long k4lz4_frame_bound(long length, int blockSize, int flags);
+        [DllImport(Lib)] public static extern int k4lz4_frame_encode_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* outLen, int nFrames, int blockSize, int flags, int level, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_content_size_batch(
+            byte* srcBase, long* srcOff, int* srcLen, int* outSize, int nFrames, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_decode_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* outLen, int nFrames, int memKind, void* cudaStream, int device);
+
         public static string LastError() => new string(k4lz4_last_error());
     }
 }

@@ -275,6 +275,67 @@ K4LZ4_API int32_t k4lz4_xxh32_batch(const uint8_t *base, const int64_t *off, con
                                     uint32_t *out, int32_t nBlocks,
                                     int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- LZ4 Frame, whole buffers: LZ4Frame.Encode / LZ4Frame.Decode, batched across frames --------- */
+
+/*
+ * Frame i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]); frames and contents
+ * are at most 2^31 - 1 bytes.  Every array lives in one memory kind.  memKind == K4LZ4_MEM_DEVICE: every pointer is
+ * device memory of `device`, the work is enqueued on `cudaStream`, and the call synchronises the host ONCE, to read
+ * the number of blocks and steps (the largest block count of a linked frame) it has to launch for.
+ * memKind == K4LZ4_MEM_HOST: synchronous; chunks of whole frames go up and come down in one copy each way, and
+ * exactly outLen[i] > 0 bytes of each destination are written.  `device` >= 0 names the GPU (K4LZ4_ALL_DEVICES:
+ * GPU 0 with host memory, the current device with device memory), as for k4lz4_decode_chain_batch.  Every frame
+ * gets its own result; one bad frame does not affect the others.
+ */
+#define K4LZ4_FRAME_INDEPENDENT      1  /* LZ4EncoderSettings.ChainBlocks = false; linked blocks are the default */
+#define K4LZ4_FRAME_BLOCK_CHECKSUM   2  /* XXH32 of every stored block                                           */
+#define K4LZ4_FRAME_CONTENT_CHECKSUM 4  /* XXH32 of the content after the end mark                               */
+/* per-frame decode result: dstCap[i] is smaller than the frame's content (nothing of it is written) */
+#define K4LZ4_R_DST_SMALL  (-1001)
+
+/* The largest frame k4lz4_frame_encode_batch writes for `length` bytes: 7 header bytes, per block 4 bytes of
+ * length code + at most the raw length (+ 4 with block checksums), the 4-byte end mark (+ 4 with the content
+ * checksum).  blockSize is rounded as LZ4EncoderBase.cs:29 does (max(1024, rounded up to 1 KiB)) and must be
+ * 1 .. 4 MiB; a bad blockSize, a negative length or an unknown flag gives K4LZ4_E_ARG. */
+K4LZ4_API int64_t k4lz4_frame_bound(int64_t length, int32_t blockSize, int32_t flags);
+
+/* LZ4Frame.Encode(ReadOnlySpan<byte>, Span<byte>, LZ4EncoderSettings) per frame, L00_FAST
+ * (Streams/Frames/LZ4FrameWriter.cs:57-189): header (magic, FLG, BD for blockSize, HC), blocks of blockSize bytes
+ * (each encoded with capacity LZ4Codec.MaximumOutputSize(blockSize), linked unless K4LZ4_FRAME_INDEPENDENT, stored
+ * raw -- bit 31 of its length code -- when it does not shrink), the end mark and the checksums `flags` asks for.
+ * No content size and no dictionary id are written.  outLen[i] = the frame's length; -1 when it does not fit
+ * dstCap[i] (the frame may then have written anything inside [dstOff, dstOff + dstCap), as the reference's span
+ * writer does before it throws); K4LZ4_R_DELEGATE for level >= 3 (chained HC stays managed), nothing written.
+ * Nothing is ever written at or beyond dstCap[i].  Argument errors as k4lz4_encode_batch, then blockSize and flags
+ * as k4lz4_frame_bound. */
+K4LZ4_API int32_t k4lz4_frame_encode_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           int32_t *outLen, int32_t nFrames, int32_t blockSize, int32_t flags,
+                                           int32_t level, int32_t memKind, void *cudaStream, int32_t device);
+
+/* The decoded length of every frame, to size the buffers of k4lz4_frame_decode_batch (as k4lz4_unpickled_size_batch
+ * does for k4lz4_unpickle_batch).  outSize[i] = the content length from the blocks' length codes and token chains,
+ * or the structural verdict decode gives: K4LZ4_R_CORRUPT for a bad magic number, version or header checksum or a
+ * frame cut short, K4LZ4_R_DELEGATE for the dictionary-id flag; -1 for a token chain that does not parse.  Checksums
+ * and match offsets are not verified.  Wherever decode succeeds it returns exactly this length. */
+K4LZ4_API int32_t k4lz4_frame_content_size_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                 int32_t *outSize, int32_t nFrames,
+                                                 int32_t memKind, void *cudaStream, int32_t device);
+
+/* LZ4Frame.Decode(ReadOnlySpan<byte>, TBufferWriter) per frame (LZ4FrameReader.blocking.cs:57-144): linked and
+ * independent frames, every block size, stored blocks, both checksums; a content-size field is read and skipped.
+ * Each block decodes with the reference's capacity (blockSize + 8 independent, LZ4BlockDecoder.cs:26; blockSize
+ * linked, LZ4ChainDecoder.cs:45-53).  outLen[i] = the content length, written to exactly [dstOff, dstOff + outLen);
+ * else, for the first problem in stream order: K4LZ4_R_CORRUPT where the reader throws InvalidDataException (magic,
+ * version, header checksum, unexpected end, block or content checksum, a stored block larger than the decoder takes:
+ * blockSize + 8 independent, max(blockSize, 64 KiB) linked); -1 for a block the block decoder rejects;
+ * K4LZ4_R_DELEGATE for the dictionary-id flag (NotImplementedException); K4LZ4_R_DST_SMALL when the content does not
+ * fit dstCap[i].  A failed frame may have written inside [dstOff, dstOff + dstCap), never outside. */
+K4LZ4_API int32_t k4lz4_frame_decode_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                           int32_t *outLen, int32_t nFrames,
+                                           int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- LZ4Pickler, byte[] variant, batched ----------------------------------------------- */
 
 /* Upper bound of Pickle() output for an n-byte message: n + 1 (0 for n == 0). */

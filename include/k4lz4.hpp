@@ -312,4 +312,104 @@ struct LZ4Pickler {
     }
 };
 
+// LZ4Frame.Encode / Decode over whole buffers (k4lz4_frame_*): one frame, or many in one call (host memory).
+struct LZ4FrameSettings {      // LZ4EncoderSettings: the reference's defaults
+    int blockSize = 65536;
+    bool chainBlocks = true, blockChecksum = false, contentChecksum = false;
+    LZ4Level level = LZ4Level::L00_FAST;
+};
+
+struct LZ4Frame {
+    using Settings = LZ4FrameSettings;
+    static int flags(const Settings& s) {
+        return (s.chainBlocks ? 0 : K4LZ4_FRAME_INDEPENDENT) | (s.blockChecksum ? K4LZ4_FRAME_BLOCK_CHECKSUM : 0) |
+               (s.contentChecksum ? K4LZ4_FRAME_CONTENT_CHECKSUM : 0);
+    }
+    static int64_t Bound(int64_t length, const Settings& s = {}) {
+        const int64_t r = k4lz4_frame_bound(length, s.blockSize, flags(s));
+        if (r < 0) throw NativeError((int)r, k4lz4_last_error());
+        return r;
+    }
+    // frame i of the result holds sources[i]
+    static std::vector<std::vector<uint8_t>> EncodeMany(const std::vector<std::vector<uint8_t>>& sources,
+                                                        const Settings& s = {}, int device = 0) {
+        const size_t n = sources.size();
+        std::vector<int64_t> so(n), dofs(n);
+        std::vector<int32_t> sl(n), dc(n), out(n, -1);
+        std::vector<uint8_t> src, dst;
+        int64_t d = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)sources[i].size();
+            src.insert(src.end(), sources[i].begin(), sources[i].end());
+            dofs[i] = d; dc[i] = (int32_t)Bound(sl[i], s); d += dc[i];
+        }
+        src.resize(src.size() + 1); dst.resize((size_t)d + 1);
+        const int rc = k4lz4_frame_encode_batch(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
+                                                out.data(), (int32_t)n, s.blockSize, flags(s), (int)s.level,
+                                                K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        std::vector<std::vector<uint8_t>> frames(n);
+        for (size_t i = 0; i < n; i++) {
+            if (out[i] == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("chained HC levels stay managed");
+            if (out[i] < 0) throw std::runtime_error("Failed to encode chunk. Target buffer too small.");
+            frames[i].assign(dst.begin() + dofs[i], dst.begin() + dofs[i] + out[i]);
+        }
+        return frames;
+    }
+    static std::vector<uint8_t> Encode(const std::vector<uint8_t>& source, const Settings& s = {}, int device = 0) {
+        return EncodeMany({source}, s, device)[0];
+    }
+    static std::vector<int32_t> ContentSizes(const std::vector<std::vector<uint8_t>>& frames, int device = 0) {
+        const size_t n = frames.size();
+        std::vector<int64_t> so(n);
+        std::vector<int32_t> sl(n), out(n, -1);
+        std::vector<uint8_t> src;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)frames[i].size();
+            src.insert(src.end(), frames[i].begin(), frames[i].end());
+        }
+        src.resize(src.size() + 1);
+        const int rc = k4lz4_frame_content_size_batch(src.data(), so.data(), sl.data(), out.data(), (int32_t)n,
+                                                      K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        return out;
+    }
+    static int64_t ContentSize(const std::vector<uint8_t>& frame, int device = 0) {
+        const int32_t r = ContentSizes({frame}, device)[0];
+        raise_for(r);
+        return r;
+    }
+    static std::vector<std::vector<uint8_t>> DecodeMany(const std::vector<std::vector<uint8_t>>& frames, int device = 0) {
+        const size_t n = frames.size();
+        const std::vector<int32_t> sizes = ContentSizes(frames, device);
+        std::vector<int64_t> so(n), dofs(n);
+        std::vector<int32_t> sl(n), dc(n), out(n, -1);
+        std::vector<uint8_t> src, dst;
+        int64_t d = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)frames[i].size();
+            src.insert(src.end(), frames[i].begin(), frames[i].end());
+            dofs[i] = d; dc[i] = std::max<int32_t>(sizes[i], 0); d += dc[i];
+        }
+        src.resize(src.size() + 1); dst.resize((size_t)d + 1);
+        const int rc = k4lz4_frame_decode_batch(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
+                                                out.data(), (int32_t)n, K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        std::vector<std::vector<uint8_t>> contents(n);
+        for (size_t i = 0; i < n; i++) {
+            raise_for(out[i]);
+            contents[i].assign(dst.begin() + dofs[i], dst.begin() + dofs[i] + out[i]);
+        }
+        return contents;
+    }
+    static std::vector<uint8_t> Decode(const std::vector<uint8_t>& frame, int device = 0) {
+        return DecodeMany({frame}, device)[0];
+    }
+private:
+    static void raise_for(int32_t r) {
+        if (r == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("Predefined dictionaries feature is not implemented");
+        if (r < 0) throw InvalidDataException("Invalid LZ4 frame");
+    }
+};
+
 }  // namespace k4lz4

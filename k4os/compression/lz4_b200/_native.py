@@ -11,6 +11,8 @@ OK = 0
 E_NODEVICE, E_CUDA, E_ARG, E_NOMEM = -100, -101, -102, -103
 R_DELEGATE = -2
 R_CORRUPT = -1000
+R_DST_SMALL = -1001                       # K4LZ4_R_DST_SMALL (frame decode)
+FRAME_INDEPENDENT, FRAME_BLOCK_CHECKSUM, FRAME_CONTENT_CHECKSUM = 1, 2, 4
 MEM_HOST, MEM_DEVICE = 0, 1
 ALL_DEVICES = -1
 CHAIN_STATE_BYTES = 16400                 # K4LZ4_CHAIN_STATE_BYTES
@@ -61,6 +63,10 @@ SIGNATURES = {
     "k4lz4_chain_group_inject": ([_vp] * 5 + [_i32, _i32, _vp], _i32),
     "k4lz4_chain_group_state": ([_vp, _i32, _vp], _i32),
     "k4lz4_chain_group_history": ([_vp, _i32, _vp, _i32], _i32),
+    "k4lz4_frame_bound": ([_i64, _i32, _i32], _i64),
+    "k4lz4_frame_encode_batch": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
+    "k4lz4_frame_content_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
+    "k4lz4_frame_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
 }
 SYMBOLS = list(SIGNATURES)
 

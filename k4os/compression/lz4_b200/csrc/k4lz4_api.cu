@@ -36,6 +36,7 @@
 #include "synth.cuh"
 #include "copy_blocks.cuh"
 #include "xxh32.cuh"
+#include "frame.cuh"
 
 namespace {
 
@@ -867,6 +868,363 @@ int read_stats(const void* sym, int32_t device, uint64_t* out4, int32_t reset) {
     return K4LZ4_OK;
 }
 
+// ---- LZ4 frames (frame.cuh) ---------------------------------------------------------------------------------
+
+constexpr int FRAME_FLAGS = K4LZ4_FRAME_INDEPENDENT | K4LZ4_FRAME_BLOCK_CHECKSUM | K4LZ4_FRAME_CONTENT_CHECKSUM;
+static_assert(K4LZ4_FRAME_INDEPENDENT == k4::FR_INDEPENDENT && K4LZ4_FRAME_BLOCK_CHECKSUM == k4::FR_BLOCK_SUM &&
+              K4LZ4_FRAME_CONTENT_CHECKSUM == k4::FR_CONTENT_SUM && K4LZ4_R_CORRUPT == k4::FR_CORRUPT &&
+              K4LZ4_R_DELEGATE == k4::FR_DELEGATE && K4LZ4_R_DST_SMALL == k4::FR_DST_SMALL, "frame codes");
+constexpr int64_t FRAME_SCRATCH = 512ll << 20;   // encoder output slots per launch
+
+// LZ4EncoderBase.cs:29: max(1024, blockSize rounded up to 1 KiB); 0 for a block size a frame cannot declare.
+int32_t frame_block_size(int32_t blockSize) {
+    if (blockSize <= 0 || blockSize > (4 << 20)) return 0;
+    return std::max<int32_t>(1024, (blockSize + 1023) / 1024 * 1024);
+}
+
+int64_t frame_bound_of(int64_t length, int32_t bs, int flags) {
+    const int64_t nb = (length + bs - 1) / bs;
+    return 7 + nb * (4 + ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 4 : 0)) + length + 4 +
+           ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 4 : 0);
+}
+
+// Magic, FLG, BD (LZ4FrameWriter.cs:183-188: the code of the caller's block size) and HC, little-endian.
+uint64_t frame_header(int32_t blockSize, int flags) {
+    const int code = blockSize <= (1 << 16) ? 4 : blockSize <= (1 << 18) ? 5 : blockSize <= (1 << 20) ? 6 : 7;
+    const uint8_t fb[2] = {(uint8_t)((1 << 6) | ((flags & K4LZ4_FRAME_INDEPENDENT) ? 1 << 5 : 0) |
+                                     ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 1 << 4 : 0) |
+                                     ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 1 << 2 : 0)),
+                           (uint8_t)(code << 4)};
+    const uint8_t hc = (uint8_t)(k4::xxh32_host(fb, 2, 0) >> 8);
+    return (uint64_t)k4::FRAME_MAGIC | ((uint64_t)fb[0] << 32) | ((uint64_t)fb[1] << 40) | ((uint64_t)hc << 48);
+}
+
+// Stream-ordered allocations of one frame call, from the device's private pool; freed (in stream order) at the end.
+struct FramePool {
+    cudaMemPool_t pool; cudaStream_t st;
+    std::vector<void*> ps;
+    cudaError_t err = cudaSuccess;
+    FramePool(cudaMemPool_t p, cudaStream_t s) : pool(p), st(s) {}
+    ~FramePool() { for (void* p : ps) cudaFreeAsync(p, st); }
+    template <class T> T* get(int64_t count) {
+        void* p = nullptr;
+        if (err == cudaSuccess) err = cudaMallocFromPoolAsync(&p, (size_t)std::max<int64_t>(count, 1) * sizeof(T) + 16, pool, st);
+        if (err != cudaSuccess) return nullptr;
+        ps.push_back(p);
+        return (T*)p;
+    }
+};
+
+inline unsigned grid_of(int64_t n, int t = 128) { return (unsigned)std::max<int64_t>((n + t - 1) / t, 1); }
+
+#define FR_TRY(expr) do { const cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
+#define FR_LAUNCH() FR_TRY(cudaGetLastError())
+
+// Decode (or, with sizeOnly, only the content sizes of) b.n frames in device memory on `st`: parse, scan, one
+// host synchronisation for the block and step counts, then everything else enqueued.  b.dstCap may be null
+// (sizeOnly).
+cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const Dev* D = dev_state(dev);
+    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
+    const int n = (int)b.n;
+    FramePool P(D->pool, st);
+    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
+    k4::FrameTotals* tot = P.get<k4::FrameTotals>(1);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(k4::FrameTotals), st));
+    k4::frame_parse_kernel<<<grid_of(n), 128, 0, st>>>(0, b.srcBase, b.srcOff, b.srcLen, n, fr, k4::FrameTable{}, tot);
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, sizeOnly ? 0 : 1);
+    FR_LAUNCH();
+    g_launches += 2;
+    k4::FrameTotals h{};
+    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size and the number of steps
+    const int64_t nB = h.blocks;
+    uint8_t* rows = P.get<uint8_t>(nB * k4::FRAME_ROW_BYTES + 16 * 16);
+    FR_TRY(P.err);
+    k4::FrameTable t;
+    {
+        uint8_t* p = rows;
+        auto take = [&](int64_t bytes) { uint8_t* q = p; p += (bytes + 15) & ~int64_t(15); return q; };
+        t.srcOff = (int64_t*)take(nB * 8); t.fin = (int64_t*)take(nB * 8); t.dst = (int64_t*)take(nB * 8);
+        t.cpySrc = (int64_t*)take(nB * 8);
+        t.len = (int32_t*)take(nB * 4); t.kind = (int32_t*)take(nB * 4); t.sum = (uint32_t*)take(nB * 4);
+        t.frame = (int32_t*)take(nB * 4); t.idx = (int32_t*)take(nB * 4); t.size = (int32_t*)take(nB * 4);
+        t.cap = (int32_t*)take(nB * 4); t.ilen = (int32_t*)take(nB * 4); t.res = (int32_t*)take(nB * 4);
+        t.ckLen = (int32_t*)take(nB * 4); t.got = (uint32_t*)take(nB * 4); t.cpyLen = (int32_t*)take(nB * 4);
+    }
+    k4::frame_parse_kernel<<<grid_of(n), 128, 0, st>>>(1, b.srcBase, b.srcOff, b.srcLen, n, fr, t, nullptr);
+    FR_LAUNCH();
+    g_launches++;
+    if (nB > 0) {
+        k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, fr);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    const int64_t slotBytes = (k4::FR_HIST + std::max(h.maxCap, 0) + 15) & ~int64_t(15);
+    uint8_t* scratch = sizeOnly ? nullptr : P.get<uint8_t>(h.slots * slotBytes);
+    int32_t* ccLen = P.get<int32_t>(n);
+    uint32_t* ccGot = P.get<uint32_t>(n);
+    FR_TRY(P.err);
+    const int64_t scratchRel = sizeOnly ? 0 : (int64_t)((uintptr_t)scratch - (uintptr_t)b.dstBase);
+    k4::frame_layout_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, t, sizeOnly ? nullptr : b.dstOff,
+                                                       sizeOnly ? nullptr : b.dstCap, scratchRel, slotBytes, ccLen);
+    FR_LAUNCH();
+    g_launches++;
+    if (!sizeOnly && nB > 0) {
+        const int nb = (int)nB;
+        // stored blocks first: they are history for the linked blocks after them
+        FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
+        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
+        FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb}, st));
+        if (h.maxSteps > 0) {
+            k4::FrameStep s;
+            s.srcOff = P.get<int64_t>(n); s.dstOff = P.get<int64_t>(n); s.hSrc = P.get<int64_t>(n); s.hDst = P.get<int64_t>(n);
+            s.srcLen = P.get<int32_t>(n); s.cap = P.get<int32_t>(n); s.prefix = P.get<int32_t>(n); s.res = P.get<int32_t>(n);
+            s.hLen = P.get<int32_t>(n);
+            FR_TRY(P.err);
+            for (int k = 0; k < h.maxSteps; k++) {
+                k4::frame_step_prepare_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, n}, st));
+                Batch cb{b.srcBase, s.srcOff, s.srcLen, b.dstBase, s.dstOff, s.cap, s.res, n};
+                cb.prefixLen = s.prefix;
+                FR_TRY(launch_op(OP_CHAIN, cb, st));
+                k4::frame_step_commit_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, n}, st));
+            }
+        }
+        k4::frame_verdict_kernel<<<grid_of(nB), 128, 0, st>>>(fr, t, nB);
+        FR_LAUNCH();
+        g_launches++;
+        FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
+    }
+    if (!sizeOnly)
+        FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, b.dstOff, ccLen, nullptr, nullptr, nullptr, (int32_t*)ccGot, n}, st));
+    k4::frame_decode_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, sizeOnly ? nullptr : b.dstCap,
+                                                              sizeOnly ? nullptr : ccGot, ccLen, b.outLen);
+    FR_LAUNCH();
+    g_launches++;
+    return cudaSuccess;
+}
+
+// Encode b.n frames in device memory on `st` (level < 3): plan, scan, one host synchronisation for the block and
+// step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of at most
+// FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.
+cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const Dev* D = dev_state(dev);
+    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
+    const int n = (int)b.n;
+    const bool bc = flags & K4LZ4_FRAME_BLOCK_CHECKSUM, cc = flags & K4LZ4_FRAME_CONTENT_CHECKSUM;
+    FramePool P(D->pool, st);
+    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
+    k4::FrameTotals* tot = P.get<k4::FrameTotals>(1);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(k4::FrameTotals), st));
+    k4::FrameTable t{};
+    k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(0, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, 0);
+    FR_LAUNCH();
+    g_launches += 2;
+    k4::FrameTotals h{};
+    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size and the number of steps
+    const int64_t nB = h.blocks;
+    t.srcOff = P.get<int64_t>(nB);
+    t.len = P.get<int32_t>(nB);
+    uint32_t* csum = P.get<uint32_t>(n);
+    FR_TRY(P.err);
+    k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(1, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+    FR_LAUNCH();
+    g_launches++;
+    if (cc) FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, b.srcOff, b.srcLen, nullptr, nullptr, nullptr, (int32_t*)csum, n}, st));
+    const int32_t bound = k4::max_output_size(bs);
+    const bool linked = !(flags & K4LZ4_FRAME_INDEPENDENT);
+    const int64_t per = std::max<int64_t>(FRAME_SCRATCH / bound, 1);
+    const int64_t E = std::max<int64_t>(std::min<int64_t>(per, linked ? n : nB), 1);
+    if (nB > 0) {
+        uint8_t* scratch = P.get<uint8_t>(E * bound);
+        int64_t* eDst = P.get<int64_t>(E);
+        int32_t* eCap = P.get<int32_t>(E);
+        k4::FrameEnc e;
+        e.cSrc = P.get<int64_t>(E); e.cDst = P.get<int64_t>(E); e.rSrc = P.get<int64_t>(E); e.ckOff = P.get<int64_t>(E);
+        e.cLen = P.get<int32_t>(E); e.rLen = P.get<int32_t>(E); e.ckLen = P.get<int32_t>(E); e.ckSum = P.get<uint32_t>(E);
+        e.res = P.get<int32_t>(E);
+        FR_TRY(P.err);
+        k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(eDst, eCap, (int)E, bound, bound);
+        FR_LAUNCH();
+        g_launches++;
+        // the bodies into place, then the block checksums over them
+        auto place = [&](int k, int64_t b0, int64_t b1, int f0, int f1, int64_t m) -> cudaError_t {
+            k4::frame_enc_place_kernel<<<grid_of(f1 - f0), 128, 0, st>>>(k, b0, b1, f0, f1, fr, t, e, b.dstBase, b.dstOff,
+                                                                         b.dstCap, bound, bc ? 1 : 0);
+            FR_LAUNCH();
+            g_launches++;
+            const int mm = (int)m;
+            FR_TRY(launch_op(OP_COPY, Batch{scratch, e.cSrc, e.cLen, b.dstBase, e.cDst, nullptr, nullptr, mm}, st));
+            FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, e.rSrc, e.rLen, b.dstBase, e.cDst, nullptr, nullptr, mm}, st));
+            if (bc) {
+                FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, e.ckOff, e.ckLen, nullptr, nullptr, nullptr, (int32_t*)e.ckSum, mm}, st));
+                k4::frame_put_sum_kernel<<<grid_of(m), 128, 0, st>>>(b.dstBase, e, mm);
+                FR_LAUNCH();
+                g_launches++;
+            }
+            return cudaSuccess;
+        };
+        if (!linked) {
+            for (int64_t b0 = 0; b0 < nB; b0 += E) {
+                const int64_t m = std::min<int64_t>(E, nB - b0);
+                Batch kb{b.srcBase, t.srcOff + b0, t.len + b0, scratch, eDst, eCap, e.res, m, b.level};
+                FR_TRY(launch_op(OP_ENCODE, kb, st));
+                FR_TRY(place(-1, b0, b0 + m, 0, n, m));
+            }
+        } else {
+            uint8_t* state = P.get<uint8_t>(E * K4LZ4_CHAIN_STATE_BYTES);
+            int64_t* stOff = P.get<int64_t>(E);
+            int64_t* so = P.get<int64_t>(E);
+            int32_t* sl = P.get<int32_t>(E);
+            int32_t* pre = P.get<int32_t>(E);
+            FR_TRY(P.err);
+            k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(stOff, nullptr, (int)E, K4LZ4_CHAIN_STATE_BYTES, 0);
+            FR_LAUNCH();
+            g_launches++;
+            for (int f0 = 0; f0 < n; f0 += (int)E) {
+                const int m = (int)std::min<int64_t>(E, n - f0);
+                FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
+                for (int k = 0; k < h.maxSteps; k++) {
+                    k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fr, t, so, sl, pre, bs);
+                    FR_LAUNCH();
+                    g_launches++;
+                    Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level};
+                    kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
+                    FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
+                    FR_TRY(place(k, 0, 0, f0, f0 + m, m));
+                }
+            }
+        }
+    }
+    k4::frame_enc_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header, cc ? 1 : 0,
+                                                           csum, b.outLen);
+    FR_LAUNCH();
+    g_launches++;
+    return cudaSuccess;
+}
+
+enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE };
+
+cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st) {
+    if (fo == FO_ENCODE && b.level >= 3) {
+        k4::frame_fill_kernel<<<grid_of(b.n), 128, 0, st>>>(b.outLen, (int)b.n, K4LZ4_R_DELEGATE);
+        g_launches++;
+        return cudaGetLastError();
+    }
+    return fo == FO_ENCODE ? frame_encode_dev(b, bs, flags, header, st) : frame_decode_dev(b, fo == FO_SIZE, st);
+}
+
+// Host memory, one GPU, synchronous: chunks of whole frames (a frame is never split: its linked blocks and its
+// content checksum need all of it).  Per chunk, the offsets, lengths and packed frames go up in one copy; the
+// device path runs on them; the results come down, the produced bytes are gathered on the device and come down in
+// one copy, and exactly outLen[i] > 0 bytes of each frame go to the caller.  The device region of a frame is
+// min(dstCap, frame bound) when encoding (a frame never needs more) and dstCap when decoding.
+int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev) {
+    DeviceGuard guard(dev);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
+    if (fo == FO_ENCODE && b.level >= 3) {
+        for (int64_t i = 0; i < b.n; i++) b.outLen[i] = K4LZ4_R_DELEGATE;
+        return K4LZ4_OK;
+    }
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    auto room = [&](int64_t i) -> int64_t {
+        if (fo == FO_SIZE) return 0;
+        const int64_t c = std::max<int32_t>(b.dstCap[i], 0);
+        return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags)) : c;
+    };
+    std::vector<uint8_t> h;
+    std::vector<int64_t> pack;
+    DevMem d;
+    for (int64_t i = 0, j; i < b.n; i = j) {
+        int64_t bytes = 0;
+        for (j = i; j < b.n; j++) {
+            const int64_t add = a16(src_size(b, j)) + 2 * a16(room(j)) + 64;
+            if (j > i && bytes + add > STAGE_BYTES) break;
+            bytes += add;
+        }
+        const int64_t nb = j - i;
+        // up: srcOff dstOff packOff (int64) | srcLen dstCap outLen (int32) | frames; then the regions and the pack
+        const int64_t srcAt = a16(nb * (3 * 8 + 3 * 4));
+        int64_t sTot = 0, dTot = 0;
+        for (int64_t k = 0; k < nb; k++) { sTot += a16(src_size(b, i + k)); dTot += a16(room(i + k)); }
+        const int64_t dstAt = a16(srcAt + sTot), packAt = a16(dstAt + dTot), total = packAt + dTot;
+        if (h.size() < (size_t)srcAt + (size_t)sTot + 16) h.resize((size_t)srcAt + (size_t)sTot + 16);
+        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* po = doff + nb;
+        int32_t* sl = (int32_t*)(po + nb); int32_t* dc = sl + nb; int32_t* res = dc + nb;
+        for (int64_t k = 0, sp = 0, dp = 0; k < nb; k++) {
+            const int64_t x = i + k, s = src_size(b, x), r = room(x);
+            so[k] = sp; doff[k] = dp; sl[k] = (int32_t)s; dc[k] = (int32_t)r; po[k] = 0;
+            sp += a16(s); dp += a16(r);
+        }
+        parallel_for_blocks(0, nb, sTot, [&](int64_t lo, int64_t hi) {
+            for (int64_t k = lo; k < hi; k++)
+                if (sl[k] > 0) memcpy(h.data() + srcAt + so[k], b.srcBase + b.srcOff[i + k], (size_t)sl[k]);
+        });
+        CU_TRY(d.ensure((size_t)total + 16));
+        uint8_t* Dp = (uint8_t*)d.p;
+        CU_TRY(cudaMemcpy(Dp, h.data(), (size_t)(srcAt + sTot), cudaMemcpyHostToDevice));
+        Batch kb = b;
+        kb.srcBase = Dp + srcAt; kb.srcOff = (int64_t*)Dp; kb.srcLen = (int32_t*)(Dp + ((uint8_t*)sl - h.data()));
+        kb.dstBase = Dp + dstAt; kb.dstOff = kb.srcOff + nb; kb.dstCap = fo == FO_SIZE ? nullptr : kb.srcLen + nb;
+        kb.outLen = (int32_t*)(Dp + ((uint8_t*)res - h.data())); kb.n = nb;
+        const cudaError_t e = frame_dev(fo, kb, bs, flags, header, nullptr);
+        if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
+        CU_TRY(cudaMemcpy(b.outLen + i, kb.outLen, (size_t)nb * 4, cudaMemcpyDeviceToHost));
+        if (fo == FO_SIZE) continue;
+        pack.resize((size_t)nb);
+        int64_t got = 0;
+        for (int64_t k = 0; k < nb; k++) { pack[(size_t)k] = got; if (b.outLen[i + k] > 0) got = a16(got + b.outLen[i + k]); }
+        if (got == 0) continue;
+        CU_TRY(cudaMemcpy(Dp + ((uint8_t*)po - h.data()), pack.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
+        CU_TRY(launch_op(OP_COPY, Batch{kb.dstBase, kb.dstOff, kb.outLen, Dp + packAt, (int64_t*)(Dp + ((uint8_t*)po - h.data())),
+                                        nullptr, nullptr, nb}, nullptr));
+        if (h.size() < (size_t)got + 16) { h.resize((size_t)got + 16); }
+        CU_TRY(cudaMemcpy(h.data(), Dp + packAt, (size_t)got, cudaMemcpyDeviceToHost));
+        parallel_for_blocks(0, nb, got, [&](int64_t lo, int64_t hi) {
+            for (int64_t k = lo; k < hi; k++) {
+                const int32_t r = b.outLen[i + k];
+                if (r > 0) memcpy(b.dstBase + b.dstOff[i + k], h.data() + pack[(size_t)k], (size_t)r);
+            }
+        });
+    }
+    return K4LZ4_OK;
+}
+
+// Every frame export: its own arguments, then the batch's (check()), then host or device.
+int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memKind, void* stream, int device) {
+    int32_t bs = 0;
+    if (fo == FO_ENCODE) {
+        bs = frame_block_size(blockSize);
+        if (!bs) return fail(K4LZ4_E_ARG, "bad frame block size %d (1 .. 4 MiB)", blockSize);
+        if (flags & ~FRAME_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
+    }
+    const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device);
+    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    const uint64_t header = fo == FO_ENCODE ? frame_header(blockSize, flags) : 0;
+    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, bs, flags, header, device < 0 ? 0 : device);
+    DeviceGuard g(device);
+    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    const cudaError_t e = frame_dev(fo, b, bs, flags, header, (cudaStream_t)stream);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
+    return K4LZ4_OK;
+}
+
 }  // namespace
 
 // ---- chain groups -----------------------------------------------------------------------------------
@@ -1402,6 +1760,34 @@ int32_t k4lz4_copy_blocks_device(const uint8_t* srcBase, const int64_t* srcOff, 
     CU_TRY(launch_op(OP_COPY, Batch{srcBase, srcOff, len, dstBase, dstOff, nullptr, nullptr, nBlocks},
                      (cudaStream_t)cudaStream));
     return K4LZ4_OK;
+}
+
+int64_t k4lz4_frame_bound(int64_t length, int32_t blockSize, int32_t flags) {
+    const int32_t bs = frame_block_size(blockSize);
+    if (!bs || length < 0 || (flags & ~FRAME_FLAGS)) return fail(K4LZ4_E_ARG, "bad frame bound arguments");
+    return frame_bound_of(length, bs, flags);
+}
+
+int32_t k4lz4_frame_encode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                                 int32_t nFrames, int32_t blockSize, int32_t flags, int32_t level, int32_t memKind,
+                                 void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level};
+    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_frame_content_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                       int32_t* outSize, int32_t nFrames, int32_t memKind, void* cudaStream,
+                                       int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
+    return frame_run(FO_SIZE, b, 0, 0, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_frame_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                                 int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
+    return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device);
 }
 
 }  // extern "C"
