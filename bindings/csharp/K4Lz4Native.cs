@@ -99,6 +99,20 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_frame_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* outLen, int nFrames, int memKind, void* cudaStream, int device);
+        // LZ4EncoderStream / LZ4FrameWriter written incrementally, batched across streams (k4lz4.h "frame writer group")
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_create(
+            int nStreams, int blockSize, int flags, int level, int device, void** group);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_destroy(void* group);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_reset(
+            void* group, int* streams, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_write(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* dstCap, int* outLen, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_close(
+            void* group, int* streams, byte* dstBase, long* dstOff, int* dstCap, int* outLen, int n, int memKind,
+            void* cudaStream);
+        [DllImport(Lib)] public static extern long k4lz4_frame_writer_bound(void* group, long length);
+        [DllImport(Lib)] public static extern long k4lz4_frame_writer_close_bound(void* group);
 
         public static string LastError() => new string(k4lz4_last_error());
     }

@@ -336,6 +336,70 @@ K4LZ4_API int32_t k4lz4_frame_decode_batch(const uint8_t *srcBase, const int64_t
                                            int32_t *outLen, int32_t nFrames,
                                            int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- LZ4 Frame, written incrementally: LZ4EncoderStream / LZ4FrameWriter, batched across streams ------ */
+
+/*
+ * A frame writer group holds S frame writers at L00_FAST on one device (Streams/Frames/LZ4FrameWriter.cs and
+ * LZ4FrameWriter.blocking.cs): per stream a ring with the chain-group layout (128 KiB + max(B, 64 KiB) bytes for
+ * linked frames, B for independent ones, B = blockSize rounded as LZ4EncoderBase.cs:29 does), the partial block,
+ * the 16 400-byte chain state (linked frames) and the running XXH32 of the content (content checksum).  Each call
+ * takes one write (or one close) for any subset of the streams.
+ *
+ * Write: the first write of a frame (even of 0 bytes) emits the header k4lz4_frame_encode_batch writes; every block
+ * the write completes is emitted in the same call, encoded with capacity MaximumOutputSize(B) and stored raw when
+ * it does not shrink, with its XXH32 when K4LZ4_FRAME_BLOCK_CHECKSUM is set; the rest (< B bytes) waits for the
+ * next write.  There is no flush: the reference's Flush emits nothing between full blocks.  Close: the partial
+ * block, the end mark and, with K4LZ4_FRAME_CONTENT_CHECKSUM, the XXH32 of all the frame's content; a stream that
+ * was not written since it was created, reset or closed emits nothing.  After a close the stream is new.  For
+ * every way of cutting a stream's content into writes, the bytes it emits equal k4lz4_frame_encode_batch of the
+ * whole content with the same blockSize and flags.
+ *
+ * streams[i] names the stream entry i writes or closes; entry i appends to dstBase[dstOff[i] .. +dstCap[i]) and
+ * outLen[i] is the number of bytes appended.  outLen[i] = -1 when dstCap[i] is below the call's bound
+ * (k4lz4_frame_writer_bound of srcLen[i], or k4lz4_frame_writer_close_bound); nothing is then consumed or written
+ * and the stream is as it was.  With device memory -1 is also the result of a stream index out of range and of a
+ * write whose bound exceeds 2^31 - 1.
+ *
+ * Host memory: synchronous; sources go up packed (in sub-writes of at most 256 MiB of source), produced bytes come
+ * down compacted, and exactly outLen[i] > 0 bytes of each destination are written.  Device memory: every array
+ * (streams included) lives on the group's device and the work is enqueued on `cudaStream`; a write synchronises the
+ * host ONCE, to read the call's number of steps (the most blocks one entry completes), a close never does.
+ *
+ * Arguments, in this order, give K4LZ4_E_ARG: a null group; an unknown memKind; a negative count; a required
+ * pointer that is NULL while n > 0; with host memory a stream index out of range or listed twice in one call, and
+ * a write whose bound exceeds 2^31 - 1.  A group is not thread-safe, and device-memory calls on different CUDA
+ * streams must be ordered by the caller; with device memory, listing a stream twice in one call is undefined.
+ * Blocks are counted in k4lz4_encode_stats like the calls whose codec they use: out4[3] for linked frames, out4[0..2]
+ * for independent ones.
+ */
+typedef struct k4lz4_frame_writer_group k4lz4_frame_writer_group;
+
+/* nStreams > 0; blockSize 1 .. 4 MiB and flags as k4lz4_frame_bound takes them; level 0..255; device >= 0 (or < 0:
+ * the current device).  K4LZ4_E_ARG for bad arguments, K4LZ4_R_DELEGATE for level >= 3 (no group: chained HC stays
+ * managed), then K4LZ4_E_NODEVICE without a device, K4LZ4_E_NOMEM when the rings do not fit; *out is NULL unless
+ * K4LZ4_OK is returned.  Every stream starts new. */
+K4LZ4_API int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int32_t flags, int32_t level,
+                                                  int32_t device, k4lz4_frame_writer_group **out);
+/* Frees the group after the device has finished its work (NULL is allowed). */
+K4LZ4_API int32_t k4lz4_frame_writer_group_destroy(k4lz4_frame_writer_group *g);
+/* Streams streams[0 .. n) are abandoned: they emit nothing and become new. */
+K4LZ4_API int32_t k4lz4_frame_writer_group_reset(k4lz4_frame_writer_group *g, const int32_t *streams, int32_t n,
+                                                 int32_t memKind, void *cudaStream);
+/* Entry i writes srcBase[srcOff[i] .. +srcLen[i]) to stream streams[i]. */
+K4LZ4_API int32_t k4lz4_frame_writer_group_write(k4lz4_frame_writer_group *g, const int32_t *streams,
+                                                 const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                 uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                                 int32_t *outLen, int32_t n, int32_t memKind, void *cudaStream);
+/* Entry i closes stream streams[i]. */
+K4LZ4_API int32_t k4lz4_frame_writer_group_close(k4lz4_frame_writer_group *g, const int32_t *streams,
+                                                 uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                                 int32_t *outLen, int32_t n, int32_t memKind, void *cudaStream);
+/* The most one write of `length` bytes appends: 7 + floor((B - 1 + length) / B) * (4 + B + 4 with block
+ * checksums).  K4LZ4_E_ARG for a null group or a negative length. */
+K4LZ4_API int64_t k4lz4_frame_writer_bound(const k4lz4_frame_writer_group *g, int64_t length);
+/* The most one close appends: 4 + B (+ 4 with block checksums), the end mark (4), the content checksum (4). */
+K4LZ4_API int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group *g);
+
 /* ---- LZ4Pickler, byte[] variant, batched ----------------------------------------------- */
 
 /* Upper bound of Pickle() output for an n-byte message: n + 1 (0 for n == 0). */

@@ -278,6 +278,48 @@ public:
     }
 };
 
+// Frame writer groups (k4lz4_frame_writer_group_*): S LZ4EncoderStream / LZ4FrameWriter streams written
+// incrementally, their partial blocks, chain states and content checksums on one GPU.  RAII owner of the group;
+// Write and Close take the C ABI's arrays (host or device memory) and append to each entry's destination.
+// flags: K4LZ4_FRAME_*.  A level >= 3 throws DelegateToManagedEngine.  Not thread-safe.
+class FrameWriterGroup {
+public:
+    FrameWriterGroup(int nStreams, int blockSize = 65536, int flags = 0, LZ4Level level = LZ4Level::L00_FAST,
+                     int device = 0) {
+        const int rc = k4lz4_frame_writer_group_create(nStreams, blockSize, flags, (int)level, device, &g_);
+        if (rc == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("chained HC levels stay with the managed engine");
+        check(rc);
+    }
+    FrameWriterGroup(const FrameWriterGroup&) = delete;
+    FrameWriterGroup& operator=(const FrameWriterGroup&) = delete;
+    FrameWriterGroup(FrameWriterGroup&& o) noexcept : g_(o.g_) { o.g_ = nullptr; }
+    FrameWriterGroup& operator=(FrameWriterGroup&& o) noexcept {
+        if (this != &o) { k4lz4_frame_writer_group_destroy(g_); g_ = o.g_; o.g_ = nullptr; }
+        return *this;
+    }
+    ~FrameWriterGroup() { k4lz4_frame_writer_group_destroy(g_); }
+    k4lz4_frame_writer_group* handle() const { return g_; }
+    int64_t Bound(int64_t length) const { return k4lz4_frame_writer_bound(g_, length); }
+    int64_t CloseBound() const { return k4lz4_frame_writer_close_bound(g_); }
+    void Write(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+               uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int n,
+               int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_writer_group_write(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
+                                             memKind, cudaStream));
+    }
+    void Close(const int32_t* streams, uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+               int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_writer_group_close(g_, streams, dstBase, dstOff, dstCap, outLen, n, memKind, cudaStream));
+    }
+    void Reset(const int32_t* streams, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_writer_group_reset(g_, streams, n, memKind, cudaStream));
+    }
+
+private:
+    static void check(int rc) { if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error()); }
+    k4lz4_frame_writer_group* g_ = nullptr;
+};
+
 struct LZ4Pickler {
     // LZ4Pickler.Pickle(ReadOnlySpan<byte>, LZ4Level) -- LZ4Pickler.pickle.cs:51-74
     static std::vector<uint8_t> Pickle(const uint8_t* source, int length, LZ4Level level = LZ4Level::L00_FAST) {

@@ -67,6 +67,13 @@ SIGNATURES = {
     "k4lz4_frame_encode_batch": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
     "k4lz4_frame_content_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_frame_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
+    "k4lz4_frame_writer_group_create": ([_i32, _i32, _i32, _i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_group_destroy": ([_vp], _i32),
+    "k4lz4_frame_writer_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_group_write": ([_vp] * 9 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_group_close": ([_vp] * 6 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_bound": ([_vp, _i64], _i64),
+    "k4lz4_frame_writer_close_bound": ([_vp], _i64),
 }
 SYMBOLS = list(SIGNATURES)
 

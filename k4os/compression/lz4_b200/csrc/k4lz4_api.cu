@@ -37,6 +37,7 @@
 #include "copy_blocks.cuh"
 #include "xxh32.cuh"
 #include "frame.cuh"
+#include "frame_writer.cuh"
 
 namespace {
 
@@ -1441,6 +1442,281 @@ int group_run(k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int3
 
 }  // namespace
 
+// ---- frame writer groups ----------------------------------------------------------------------------
+
+// S incrementally written LZ4 frames on one device (k4lz4.h, frame_writer.cuh): rings, chain states, stream
+// headers and checksum states live there between calls; the staging buffers of host-memory calls grow and never
+// shrink.
+struct k4lz4_frame_writer_group {
+    int32_t nStreams = 0, blockSize = 0, B = 0;   // the caller's block size (BD) and the encoder's (blocks)
+    int flags = 0, level = 0, device = 0;
+    uint64_t header = 0;
+    int64_t ring = 0, slot = 0;
+    uint8_t* rings = nullptr;
+    uint8_t* states = nullptr;        // linked frames: K4LZ4_CHAIN_STATE_BYTES per stream
+    k4::ChainGroupHdr* hdr = nullptr;
+    k4::FwState* fw = nullptr;
+    Buf dStage, dDown, hUp{true}, hDown{true};
+    bool linked() const { return !(flags & K4LZ4_FRAME_INDEPENDENT); }
+    bool bc() const { return flags & K4LZ4_FRAME_BLOCK_CHECKSUM; }
+    bool cc() const { return flags & K4LZ4_FRAME_CONTENT_CHECKSUM; }
+};
+
+namespace {
+
+constexpr int64_t FW_STAGE_BYTES = 256ll << 20;   // source bytes of one host-memory sub-write
+
+void fw_free(k4lz4_frame_writer_group* g) {
+    if (g->rings) cudaFree(g->rings);
+    if (g->states) cudaFree(g->states);
+    if (g->hdr) cudaFree(g->hdr);
+    if (g->fw) cudaFree(g->fw);
+    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
+    delete g;
+}
+
+// The chain groups' order: the group, memKind, the count, the pointers, then (host memory) the stream indices and
+// the bounds of the writes.
+int check_fw(const k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, int memKind) {
+    if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)b.n);
+    if (b.n > 0 && (!streams || !b.dstBase || !b.dstOff || !b.dstCap || !b.outLen ||
+                    (!closing && (!b.srcBase || !b.srcOff || !b.srcLen))))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
+        std::vector<uint8_t> seen((size_t)g->nStreams, 0);
+        for (int64_t i = 0; i < b.n; i++) {
+            const int32_t s = streams[i];
+            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at entry %lld", s, (long long)i);
+            if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
+            if (!closing && k4::fw_write_bound(src_size(b, i), g->B, g->bc()) > INT32_MAX)
+                return fail(K4LZ4_E_ARG, "write of %d bytes at entry %lld: its bound exceeds 2^31 - 1", b.srcLen[i], (long long)i);
+        }
+    }
+    return check_device(g->device, b.n);
+}
+
+// One write (or close) of b.n entries in device memory on `st`: plan, the content checksum, one host
+// synchronisation for the number of steps (a close has at most one and does not wait), the steps over chunks of at
+// most FRAME_SCRATCH bytes of encoder output, then the rest of each source into its ring (or the end marks).
+cudaError_t fw_device(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, cudaStream_t st) {
+    const Dev* D = dev_state(g->device);
+    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
+    const int n = (int)b.n;
+    const bool linked = g->linked(), bc = g->bc(), cc = g->cc();
+    FramePool P(D->pool, st);
+    k4::FwEntry* ent = P.get<k4::FwEntry>(n);
+    int32_t* mx = P.get<int32_t>(1);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(mx, 0, 4, st));
+    k4::frame_writer_plan_kernel<<<grid_of(n), 128, 0, st>>>(streams, b.srcOff, closing ? nullptr : b.srcLen, b.dstOff,
+                                                            b.dstCap, n, g->nStreams, g->B, g->flags, g->header,
+                                                            b.dstBase, g->fw, ent, b.outLen, mx);
+    FR_LAUNCH();
+    g_launches++;
+    int32_t steps = 1;
+    if (!closing) {
+        if (cc) {
+            k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, ent, n, g->fw);
+            FR_LAUNCH();
+            g_launches++;
+        }
+        FR_TRY(cudaMemcpyAsync(&steps, mx, 4, cudaMemcpyDeviceToHost, st));
+        FR_TRY(cudaStreamSynchronize(st));             // the one wait: the number of steps
+    }
+    if (steps > 0) {
+        const int32_t bound = k4::max_output_size(g->B);
+        const int E = (int)std::max<int64_t>(std::min<int64_t>(FRAME_SCRATCH / bound, n), 1);
+        uint8_t* scratch = P.get<uint8_t>((int64_t)E * bound);
+        uint8_t* tab = P.get<uint8_t>((int64_t)E * TABLE_BYTES);
+        int64_t* copyDst = P.get<int64_t>(E);
+        int64_t* eDst = P.get<int64_t>(E);
+        int32_t* eCap = P.get<int32_t>(E);
+        k4::FrameEnc e;
+        e.cSrc = P.get<int64_t>(E); e.cDst = P.get<int64_t>(E); e.rSrc = P.get<int64_t>(E); e.ckOff = P.get<int64_t>(E);
+        e.cLen = P.get<int32_t>(E); e.rLen = P.get<int32_t>(E); e.ckLen = P.get<int32_t>(E); e.ckSum = P.get<uint32_t>(E);
+        e.res = P.get<int32_t>(E);
+        FR_TRY(P.err);
+        const k4::ChainGroupTable t = carve_table(tab, E);
+        k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(eDst, eCap, E, bound, bound);
+        FR_LAUNCH();
+        g_launches++;
+        for (int k = 0; k < steps; k++) {
+            for (int e0 = 0; e0 < n; e0 += E) {
+                const int m = std::min(E, n - e0);
+                k4::frame_writer_step_kernel<<<grid_of(m), 128, 0, st>>>(k, e0, m, closing ? 1 : 0, ent, g->fw, g->hdr,
+                                                                        g->B, g->ring, linked ? 1 : 0, t, copyDst);
+                FR_LAUNCH();
+                g_launches++;
+                if (!closing)
+                    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.copyOff, t.copyLen, g->rings, copyDst, nullptr, nullptr, m}, st));
+                Batch kb{g->rings, t.ringOff, t.len, scratch, eDst, eCap, e.res, m, g->level};
+                if (linked) { kb.prefixLen = t.prefix; kb.stateBase = g->states; kb.stateOff = t.stateOff; }
+                FR_TRY(launch_op(linked ? OP_ENCCHAIN : OP_ENCODE, kb, st));
+                k4::frame_writer_place_kernel<<<grid_of(m), 128, 0, st>>>(e0, m, ent, g->fw, t, e, b.dstBase, bound,
+                                                                         bc ? 1 : 0);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{scratch, e.cSrc, e.cLen, b.dstBase, e.cDst, nullptr, nullptr, m}, st));
+                FR_TRY(launch_op(OP_COPY, Batch{g->rings, e.rSrc, e.rLen, b.dstBase, e.cDst, nullptr, nullptr, m}, st));
+                if (bc) {
+                    FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, e.ckOff, e.ckLen, nullptr, nullptr, nullptr, (int32_t*)e.ckSum, m}, st));
+                    k4::frame_put_sum_kernel<<<grid_of(m), 128, 0, st>>>(b.dstBase, e, m);
+                    FR_LAUNCH();
+                    g_launches++;
+                }
+                if (linked) {        // pos += B and the slide, after every read of the slot
+                    k4::chain_group_commit_kernel<<<grid_of(m), 128, 0, st>>>(k4::CG_ENCODE, e.res, m, g->ring, g->slot,
+                                                                              g->hdr, t);
+                    FR_LAUNCH();
+                    g_launches++;
+                    FR_TRY(launch_op(OP_COPY, Batch{g->rings, t.copyOff, t.copyLen, g->rings, t.ringOff, nullptr, nullptr, m}, st));
+                }
+            }
+        }
+    }
+    int64_t* rOff = closing ? nullptr : P.get<int64_t>(n);
+    int64_t* rDst = closing ? nullptr : P.get<int64_t>(n);
+    int32_t* rLen = closing ? nullptr : P.get<int32_t>(n);
+    int32_t* reset = closing ? P.get<int32_t>(n) : nullptr;
+    FR_TRY(P.err);
+    k4::frame_writer_finish_kernel<<<grid_of(n), 128, 0, st>>>(closing ? 1 : 0, ent, n, g->fw, g->hdr, g->ring,
+                                                              linked ? 1 : 0, cc ? 1 : 0, b.dstBase, rOff, rDst, rLen,
+                                                              reset, b.outLen);
+    FR_LAUNCH();
+    g_launches++;
+    if (!closing) {
+        FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, rOff, rLen, g->rings, rDst, nullptr, nullptr, n}, st));
+    } else {
+        k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(reset, n, g->nStreams, g->hdr, linked ? g->states : nullptr);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    return cudaSuccess;
+}
+
+// Host memory, synchronous.  One sub-write (or the close) of entries idx[k] with piece[k] source bytes starting
+// at srcAt[k] of theirs: offsets, lengths and packed sources go up in one copy, the device path runs on them with
+// a destination slot of the piece's bound per entry, the produced bytes are gathered on the device and come down
+// in one copy, and exactly res[k] > 0 bytes go to the caller at dstOff + wrote[k].
+int fw_host_part(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams,
+                 const std::vector<int64_t>& idx, const std::vector<int64_t>& srcAt, const std::vector<int64_t>& piece,
+                 std::vector<int64_t>& wrote, std::vector<int32_t>& res, cudaStream_t st) {
+    const int64_t m = (int64_t)idx.size();
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    const int64_t cb = k4::fw_close_bound(g->B, g->bc(), g->cc());
+    auto room = [&](int64_t k) -> int64_t {
+        return closing ? std::min<int64_t>(std::max<int32_t>(b.dstCap[idx[k]], 0), cb)
+                       : k4::fw_write_bound(piece[k], g->B, g->bc());
+    };
+    const int64_t srcOffAt = 0, sendAt = a16(m * (8 * 2 + 4 * 3));
+    int64_t srcBytes = 0, dstBytes = 0;
+    for (int64_t k = 0; k < m; k++) { srcBytes += a16(piece[k]); dstBytes += a16(room(k)); }
+    const int64_t upBytes = sendAt + srcBytes;
+    const int64_t outAt = a16(upBytes), coffAt = outAt + a16(m * 4), dstAt = coffAt + a16(m * 8);
+    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 8) + 16));
+    CU_TRY(g->dStage.ensure((size_t)(dstAt + dstBytes) + 16));
+    uint8_t* H = (uint8_t*)g->hUp.p;             // srcOff dstOff (int64) | streams srcLen dstCap (int32) | sources
+    int64_t* hso = (int64_t*)(H + srcOffAt); int64_t* hdo = hso + m;
+    int32_t* hs = (int32_t*)(hdo + m); int32_t* hl = hs + m; int32_t* hc = hl + m;
+    for (int64_t k = 0, sp = 0, dp = 0; k < m; k++) {
+        hs[k] = streams[idx[k]];
+        hl[k] = (int32_t)piece[k];
+        hc[k] = (int32_t)room(k);
+        hso[k] = sp; hdo[k] = dp;
+        sp += a16(piece[k]); dp += a16(room(k));
+    }
+    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (piece[k] > 0) memcpy(H + sendAt + hso[k], b.srcBase + b.srcOff[idx[k]] + srcAt[k], (size_t)piece[k]);
+    });
+    uint8_t* D = (uint8_t*)g->dStage.p;
+    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
+    const int64_t* dso = (const int64_t*)(D + srcOffAt);
+    const int32_t* ds = (const int32_t*)(dso + 2 * m);
+    int32_t* dOut = (int32_t*)(D + outAt);
+    Batch kb{D + sendAt, dso, ds + m, D + dstAt, dso + m, ds + 2 * m, dOut, m, g->level};
+    const cudaError_t e = fw_device(g, closing, kb, ds, st);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame writer step: %s", cudaGetErrorString(e)); }
+    res.resize((size_t)m);
+    CU_TRY(cudaMemcpyAsync(res.data(), dOut, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    std::vector<int64_t> co((size_t)m);
+    int64_t total = 0;
+    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (res[(size_t)k] > 0) total = a16(total + res[(size_t)k]); }
+    if (total > 0) {
+        CU_TRY(g->dDown.ensure((size_t)total + 16));
+        CU_TRY(g->hDown.ensure((size_t)total + 16));
+        memcpy(H, co.data(), (size_t)m * 8);        // the upload buffer is free again
+        CU_TRY(cudaMemcpyAsync(D + coffAt, H, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+        CU_TRY(launch_op(OP_COPY, Batch{kb.dstBase, kb.dstOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt),
+                                        nullptr, nullptr, m}, st));
+        CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaStreamSynchronize(st));
+        const uint8_t* stage = (const uint8_t*)g->hDown.p;
+        parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
+            for (int64_t k = lo; k < hi; k++)
+                if (res[(size_t)k] > 0)
+                    memcpy(b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k], stage + co[(size_t)k], (size_t)res[(size_t)k]);
+        });
+    }
+    for (int64_t k = 0; k < m; k++) if (res[(size_t)k] > 0) wrote[(size_t)k] += res[(size_t)k];
+    return K4LZ4_OK;
+}
+
+// Host memory: entries whose capacity is below their bound get -1 and are left out; the others are written in
+// sub-writes of at most FW_STAGE_BYTES source bytes, in entry order (cutting a write in two changes nothing of what
+// a stream emits).  The first sub-write lists every such entry, so that a 0-byte write still opens its frame.
+int fw_host(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, cudaStream_t st) {
+    std::vector<int32_t> res;
+    if (closing) {                   // the device checks the capacities
+        std::vector<int64_t> idx((size_t)b.n), zero((size_t)b.n, 0), wrote((size_t)b.n, 0);
+        for (int64_t i = 0; i < b.n; i++) idx[(size_t)i] = i;
+        const int rc = fw_host_part(g, true, b, streams, idx, zero, zero, wrote, res, st);
+        if (rc != K4LZ4_OK) return rc;
+        for (int64_t i = 0; i < b.n; i++) b.outLen[i] = res[(size_t)i];
+        return K4LZ4_OK;
+    }
+    std::vector<int64_t> all;
+    for (int64_t i = 0; i < b.n; i++) {
+        if (b.dstCap[i] < k4::fw_write_bound(src_size(b, i), g->B, g->bc())) b.outLen[i] = -1;
+        else all.push_back(i);
+    }
+    std::vector<int64_t> used(all.size(), 0), total(all.size(), 0);
+    for (bool first = true;; first = false) {
+        std::vector<int64_t> idx, at, piece, wrote, which;
+        int64_t budget = FW_STAGE_BYTES;
+        for (size_t k = 0; k < all.size(); k++) {
+            const int64_t take = std::min(src_size(b, all[k]) - used[k], budget);
+            if (!first && take == 0) continue;
+            idx.push_back(all[k]); at.push_back(used[k]); piece.push_back(take); wrote.push_back(total[k]);
+            which.push_back((int64_t)k);
+            used[k] += take;
+            budget -= take;
+        }
+        if (idx.empty()) break;
+        const int rc = fw_host_part(g, false, b, streams, idx, at, piece, wrote, res, st);
+        if (rc != K4LZ4_OK) return rc;
+        for (size_t k = 0; k < idx.size(); k++) total[(size_t)which[k]] = wrote[k];
+    }
+    for (size_t k = 0; k < all.size(); k++) b.outLen[all[k]] = (int32_t)total[k];
+    return K4LZ4_OK;
+}
+
+int fw_run(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, int memKind, void* stream) {
+    const int rc = check_fw(g, closing, b, streams, memKind);
+    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    if (memKind == K4LZ4_MEM_HOST) return fw_host(g, closing, b, streams, (cudaStream_t)stream);
+    const cudaError_t e = fw_device(g, closing, b, streams, (cudaStream_t)stream);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame writer step: %s", cudaGetErrorString(e)); }
+    return K4LZ4_OK;
+}
+
+}  // namespace
+
 // ---- exported C ABI ------------------------------------------------------------------------
 
 extern "C" {
@@ -1788,6 +2064,106 @@ int32_t k4lz4_frame_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, 
                                  int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
     return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int32_t flags, int32_t level,
+                                        int32_t device, k4lz4_frame_writer_group** out) {
+    if (out) *out = nullptr;
+    const int32_t B = frame_block_size(blockSize);
+    if (!out || nStreams <= 0 || !B || (flags & ~FRAME_FLAGS) || level < 0 || level > 0xFF)
+        return fail(K4LZ4_E_ARG, "bad frame writer group arguments (%d streams, block size %d, flags 0x%x, level %d)",
+                    nStreams, blockSize, flags, level);
+    if (level >= 3) return K4LZ4_R_DELEGATE;
+    int rc = check_device(device, 1);
+    if (rc != K4LZ4_OK) return rc;
+    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    k4lz4_frame_writer_group* g = new k4lz4_frame_writer_group;
+    g->nStreams = nStreams; g->blockSize = blockSize; g->B = B; g->flags = flags; g->level = level; g->device = device;
+    g->header = frame_header(blockSize, flags);
+    g->slot = g->linked() ? std::max<int64_t>(B, k4::CG_WINDOW) : B;
+    g->ring = g->linked() ? 2 * k4::CG_WINDOW + g->slot : g->slot;
+    const size_t S = (size_t)nStreams;
+    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->fw, S * sizeof(k4::FwState));
+    if (e == cudaSuccess && g->linked()) e = cudaMalloc((void**)&g->states, S * K4LZ4_CHAIN_STATE_BYTES);
+    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess) e = cudaMemset(g->fw, 0, S * sizeof(k4::FwState));
+    if (e == cudaSuccess && g->states) e = cudaMemset(g->states, 0, S * K4LZ4_CHAIN_STATE_BYTES);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        const long long ring = g->ring;
+        fw_free(g);
+        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "frame writer group of %d x %lld bytes: %s",
+                    nStreams, ring, cudaGetErrorString(e));
+    }
+    *out = g;
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_writer_group_destroy(k4lz4_frame_writer_group* g) {
+    if (!g) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    cudaDeviceSynchronize();
+    fw_free(g);
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_writer_group_reset(k4lz4_frame_writer_group* g, const int32_t* streams, int32_t n, int32_t memKind,
+                                       void* cudaStream) {
+    if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (n < 0) return fail(K4LZ4_E_ARG, "bad stream count %d", n);
+    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST)
+        for (int32_t i = 0; i < n; i++)
+            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
+    if (n == 0) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    cudaStream_t st = (cudaStream_t)cudaStream;
+    const int32_t* ds = streams;
+    if (memKind == K4LZ4_MEM_HOST) {
+        CU_TRY(g->hUp.ensure((size_t)n * 4));
+        CU_TRY(g->dStage.ensure((size_t)n * 4));
+        memcpy(g->hUp.p, streams, (size_t)n * 4);
+        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        ds = (const int32_t*)g->dStage.p;
+    }
+    k4::frame_writer_reset_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->fw);
+    k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
+    g_launches += 2;
+    CU_TRY(cudaGetLastError());
+    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_writer_group_write(k4lz4_frame_writer_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                       const int64_t* srcOff, const int32_t* srcLen, uint8_t* dstBase,
+                                       const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int32_t n,
+                                       int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
+    return fw_run(g, false, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_frame_writer_group_close(k4lz4_frame_writer_group* g, const int32_t* streams, uint8_t* dstBase,
+                                       const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int32_t n,
+                                       int32_t memKind, void* cudaStream) {
+    Batch b{nullptr, nullptr, nullptr, dstBase, dstOff, dstCap, outLen, n};
+    return fw_run(g, true, b, streams, memKind, cudaStream);
+}
+
+int64_t k4lz4_frame_writer_bound(const k4lz4_frame_writer_group* g, int64_t length) {
+    if (!g || length < 0) return fail(K4LZ4_E_ARG, "bad frame writer bound arguments");
+    return k4::fw_write_bound(length, g->B, g->bc());
+}
+
+int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group* g) {
+    if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
+    return k4::fw_close_bound(g->B, g->bc(), g->cc());
 }
 
 }  // extern "C"

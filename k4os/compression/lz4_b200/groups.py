@@ -141,3 +141,97 @@ class ChainDecoderGroup(_ChainGroup):
                       stream: int = 0) -> None:
         N.check(N.lib().k4lz4_chain_group_inject(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr, int(n),
                                                  N.MEM_DEVICE, stream or None))
+
+
+class FrameWriterGroup:
+    """S LZ4EncoderStream / LZ4FrameWriter streams at L00_FAST (k4lz4_frame_writer_group_*) whose partial blocks,
+    chain states and content checksums live on the GPU.  Each call writes one chunk of any size to (or closes) any
+    subset of the streams and returns the frame bytes it produced; for every stream the concatenation of what its
+    writes and its close returned is the LZ4 frame of everything written to it.  ``close(streams)`` ends frames;
+    ``free()`` (or ``with``) frees the group's device memory."""
+
+    def __init__(self, n_streams: int, block_size: int = 65536, chaining: bool = True, block_checksum: bool = False,
+                 content_checksum: bool = False, level: int = 0, device: int = 0):
+        self.flags = (0 if chaining else N.FRAME_INDEPENDENT) | (N.FRAME_BLOCK_CHECKSUM if block_checksum else 0) | \
+            (N.FRAME_CONTENT_CHECKSUM if content_checksum else 0)
+        h = C.c_void_p()
+        rc = N.lib().k4lz4_frame_writer_group_create(int(n_streams), int(block_size), self.flags, int(level),
+                                                     int(device), C.byref(h))
+        if rc == N.R_DELEGATE:
+            raise NotImplementedError("LZ4HighChainEncoder (chained HC levels) stays with the managed engine")
+        N.check(rc)
+        self._h = h.value
+        self.n_streams, self.block_size = int(n_streams), int(block_size)
+
+    handle = _ChainGroup.handle
+    _streams = _ChainGroup._streams
+
+    def free(self) -> None:
+        """Frees the group's device memory; frames not closed are abandoned."""
+        if getattr(self, "_h", None):
+            N.lib().k4lz4_frame_writer_group_destroy(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+    def reset(self, streams: Sequence[int] | None = None) -> None:
+        """Streams (default: all) are abandoned: they emit nothing and become new."""
+        s = self._streams(streams, self.n_streams)
+        N.check(N.lib().k4lz4_frame_writer_group_reset(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
+
+    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
+        N.check(N.lib().k4lz4_frame_writer_group_reset(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+
+    def bound(self, length: int) -> int:
+        """The most one write of `length` bytes appends."""
+        return int(N.lib().k4lz4_frame_writer_bound(self.handle, int(length)))
+
+    def close_bound(self) -> int:
+        """The most one close appends."""
+        return int(N.lib().k4lz4_frame_writer_close_bound(self.handle))
+
+    def write(self, chunks: Sequence, streams: Sequence[int] | None = None, caps: Sequence[int] | None = None):
+        """chunks[i] is written to stream streams[i] (default: stream i), into caps[i] bytes (default: the bound).
+        -> (list of frame bytes each write produced, int32 results: bytes appended, or -1 where caps[i] is below
+        the bound)."""
+        src, so, sl = _pack(chunks)
+        s = self._streams(streams, len(sl))
+        dst, do, dc = _slots([self.bound(int(x)) for x in sl] if caps is None else caps)
+        out = np.full(len(sl), -1, dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_writer_group_write(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
+                                                       sl.ctypes.data, dst.ctypes.data, do.ctypes.data,
+                                                       dc.ctypes.data, out.ctypes.data, len(sl), N.MEM_HOST, None))
+        return _slices(dst, do, out), out
+
+    def close(self, streams: Sequence[int] | None = None, caps: Sequence[int] | None = None):
+        """Closes streams (default: all): their pending block, end mark and content checksum.  -> (list of frame
+        bytes, int32 results; 0 and no bytes for a stream that was not written since it was new)."""
+        s = self._streams(streams, self.n_streams)
+        dst, do, dc = _slots([self.close_bound()] * len(s) if caps is None else caps)
+        out = np.full(len(s), -1, dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_writer_group_close(self.handle, s.ctypes.data, dst.ctypes.data, do.ctypes.data,
+                                                       dc.ctypes.data, out.ctypes.data, len(s), N.MEM_HOST, None))
+        return _slices(dst, do, out), out
+
+    def write_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int,
+                     dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int, n: int, stream: int = 0) -> None:
+        """Device-pointer form of write: enqueues work on `stream` (and waits once for the number of steps)."""
+        N.check(N.lib().k4lz4_frame_writer_group_write(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
+                                                       dst_ptr, dst_off_ptr, dst_cap_ptr, out_len_ptr, int(n),
+                                                       N.MEM_DEVICE, stream or None))
+
+    def close_device(self, streams_ptr: int, dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int,
+                     n: int, stream: int = 0) -> None:
+        """Device-pointer form of close: only enqueues work on `stream`."""
+        N.check(N.lib().k4lz4_frame_writer_group_close(self.handle, streams_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
+                                                       out_len_ptr, int(n), N.MEM_DEVICE, stream or None))
