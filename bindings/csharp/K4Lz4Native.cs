@@ -113,6 +113,17 @@ namespace K4os.Compression.LZ4.Engine.Native
             void* cudaStream);
         [DllImport(Lib)] public static extern long k4lz4_frame_writer_bound(void* group, long length);
         [DllImport(Lib)] public static extern long k4lz4_frame_writer_close_bound(void* group);
+        // LZ4DecoderStream / LZ4FrameReader read incrementally, batched across streams (k4lz4.h "frame reader group")
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_create(
+            int nStreams, int maxBlockSize, int device, void** group);
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_destroy(void* group);
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_reset(
+            void* group, int* streams, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_read(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, int* srcUsed, byte* dstBase,
+            long* dstOff, int* dstCap, int* outLen, int* frameEnded, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_end(
+            void* group, int* streams, int* status, int n, int memKind, void* cudaStream);
 
         public static string LastError() => new string(k4lz4_last_error());
     }

@@ -400,6 +400,73 @@ K4LZ4_API int64_t k4lz4_frame_writer_bound(const k4lz4_frame_writer_group *g, in
 /* The most one close appends: 4 + B (+ 4 with block checksums), the end mark (4), the content checksum (4). */
 K4LZ4_API int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group *g);
 
+/* ---- LZ4 Frame, read incrementally: LZ4DecoderStream / LZ4FrameReader, batched across streams --------- */
+
+/*
+ * A frame reader group holds S frame readers on one device (Streams/Frames/LZ4FrameReader.async.cs): per stream a
+ * ring with the chain-group layout (128 KiB + SLOT bytes, SLOT = max(maxBlockSize + 8, 64 KiB)), a stash for a block
+ * cut by the end of a chunk (length code, body, checksum), a stash for a cut header or content checksum, the open
+ * frame's flags and BD, the running XXH32 of its content, a phase and a sticky error: about 256 KiB per stream at
+ * maxBlockSize 64 KiB, 8.3 MB at 4 MiB.  Each call feeds one chunk of compressed bytes (of any size, cut anywhere)
+ * to any subset of the streams.  Frames written at any level read alike: the reader has no level.
+ *
+ * Read: entry i consumes the first srcUsed[i] <= srcLen[i] bytes of srcBase[srcOff[i] ..), in stream order, and
+ * appends the content of every block it decodes to dstBase[dstOff[i] ..); outLen[i] is the number of bytes
+ * appended.  A call consumes bytes of at most one frame: it stops after the byte that ends a frame (the end mark, or
+ * the content checksum when the frame has one), and then frameEnded[i] = 1; the next call starts the next frame, so
+ * concatenated frames are read one after another.
+ *
+ * Room: blockCap is the frame's BD maximum for a linked frame and that maximum + 8 for an independent one (the
+ * reference decoder's capacity).  A call decodes at most floor(dstCap[i] / blockCap) blocks, each counted as
+ * blockCap whatever it decodes to (decoded bytes are still appended densely).  Once that budget is spent the call
+ * stops before the next length code, except that a complete end mark and the content checksum behind it are still
+ * consumed.  Header bytes need no room.  A block is never drained across calls: dstCap[i] >= blockCap always makes
+ * progress.
+ *
+ * Errors: the first problem in stream order decides, and outLen[i] is then the code k4lz4_frame_decode_batch gives
+ * for that frame: K4LZ4_R_CORRUPT for a bad magic (skippable and legacy frames included), version, header checksum,
+ * block or content checksum, or a stored block larger than blockCap; -1 for a block the decoder rejects;
+ * K4LZ4_R_DELEGATE for the dictionary flag and for a BD above the group's maxBlockSize.  A header is judged when its
+ * magic (4 bytes) or all of it (7 or 15 bytes) has arrived.  A compressed block too long for any block the decoder
+ * accepts is not stashed but skipped (its body hashed as it passes): its checksum mismatch gives K4LZ4_R_CORRUPT,
+ * its truncation K4LZ4_R_CORRUPT from _end, and otherwise -1 once its last byte has arrived.  srcUsed[i] and dstBase[dstOff[i] .. +dstCap[i]) are then unspecified,
+ * and the stream has failed: every later read returns the same code and consumes nothing until it is reset or ended.
+ *
+ * Host memory: synchronous; chunks go up packed, in sub-reads of at most 256 MiB (cutting a read in two changes
+ * nothing), decoded bytes come down compacted, and exactly outLen[i] > 0 bytes of each destination are written.
+ * Device memory: every array (streams included) lives on the group's device and the work is enqueued on
+ * `cudaStream`; a read synchronises the host ONCE, to read the call's row and step counts, an end or reset never
+ * does.  A stream index out of range gives outLen[i] (or status[i]) = K4LZ4_E_ARG and consumes nothing.
+ *
+ * Arguments, in this order, give K4LZ4_E_ARG: a null group; an unknown memKind; a negative count; a required pointer
+ * that is NULL while n > 0; with host memory a stream index out of range or listed twice in one call.  A group is not
+ * thread-safe; with device memory, listing a stream twice in one call is undefined.  Blocks are counted in
+ * k4lz4_decode_stats like the decode calls whose engine they use.
+ */
+typedef struct k4lz4_frame_reader_group k4lz4_frame_reader_group;
+
+/* nStreams > 0; maxBlockSize 65 536, 262 144, 1 048 576 or 4 194 304; device >= 0 (or < 0: the current device).
+ * K4LZ4_E_ARG for bad arguments, then K4LZ4_E_NODEVICE without a device, K4LZ4_E_NOMEM when the rings do not fit;
+ * *out is NULL unless K4LZ4_OK is returned.  Every stream starts new. */
+K4LZ4_API int32_t k4lz4_frame_reader_group_create(int32_t nStreams, int32_t maxBlockSize, int32_t device,
+                                                  k4lz4_frame_reader_group **out);
+/* Frees the group after the device has finished its work (NULL is allowed). */
+K4LZ4_API int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group *g);
+/* Streams streams[0 .. n) become new (their input so far is dropped). */
+K4LZ4_API int32_t k4lz4_frame_reader_group_reset(k4lz4_frame_reader_group *g, const int32_t *streams, int32_t n,
+                                                 int32_t memKind, void *cudaStream);
+/* Entry i feeds srcBase[srcOff[i] .. +srcLen[i]) to stream streams[i]. */
+K4LZ4_API int32_t k4lz4_frame_reader_group_read(k4lz4_frame_reader_group *g, const int32_t *streams,
+                                                const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                int32_t *srcUsed, uint8_t *dstBase, const int64_t *dstOff,
+                                                const int32_t *dstCap, int32_t *outLen, int32_t *frameEnded,
+                                                int32_t n, int32_t memKind, void *cudaStream);
+/* The input of streams[i] has ended: status[i] = 0 between frames (never fed, or its last read ended a frame),
+ * K4LZ4_R_CORRUPT inside a frame (the reference's EndOfStreamException; 1-3 bytes of a magic included), the failed
+ * stream's code.  Every stream named becomes new. */
+K4LZ4_API int32_t k4lz4_frame_reader_group_end(k4lz4_frame_reader_group *g, const int32_t *streams, int32_t *status,
+                                               int32_t n, int32_t memKind, void *cudaStream);
+
 /* ---- LZ4Pickler, byte[] variant, batched ----------------------------------------------- */
 
 /* Upper bound of Pickle() output for an n-byte message: n + 1 (0 for n == 0). */

@@ -320,6 +320,39 @@ private:
     k4lz4_frame_writer_group* g_ = nullptr;
 };
 
+// LZ4DecoderStream / LZ4FrameReader for many streams (k4lz4.h "frame reader group"); move-only.
+class FrameReaderGroup {
+public:
+    explicit FrameReaderGroup(int nStreams, int maxBlockSize = 65536, int device = 0) {
+        check(k4lz4_frame_reader_group_create(nStreams, maxBlockSize, device, &g_));
+    }
+    FrameReaderGroup(const FrameReaderGroup&) = delete;
+    FrameReaderGroup& operator=(const FrameReaderGroup&) = delete;
+    FrameReaderGroup(FrameReaderGroup&& o) noexcept : g_(o.g_) { o.g_ = nullptr; }
+    FrameReaderGroup& operator=(FrameReaderGroup&& o) noexcept {
+        if (this != &o) { k4lz4_frame_reader_group_destroy(g_); g_ = o.g_; o.g_ = nullptr; }
+        return *this;
+    }
+    ~FrameReaderGroup() { k4lz4_frame_reader_group_destroy(g_); }
+    k4lz4_frame_reader_group* handle() const { return g_; }
+    void Read(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+              int32_t* srcUsed, uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+              int32_t* frameEnded, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_reader_group_read(g_, streams, srcBase, srcOff, srcLen, srcUsed, dstBase, dstOff, dstCap,
+                                            outLen, frameEnded, n, memKind, cudaStream));
+    }
+    void End(const int32_t* streams, int32_t* status, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_reader_group_end(g_, streams, status, n, memKind, cudaStream));
+    }
+    void Reset(const int32_t* streams, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
+        check(k4lz4_frame_reader_group_reset(g_, streams, n, memKind, cudaStream));
+    }
+
+private:
+    static void check(int rc) { if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error()); }
+    k4lz4_frame_reader_group* g_ = nullptr;
+};
+
 struct LZ4Pickler {
     // LZ4Pickler.Pickle(ReadOnlySpan<byte>, LZ4Level) -- LZ4Pickler.pickle.cs:51-74
     static std::vector<uint8_t> Pickle(const uint8_t* source, int length, LZ4Level level = LZ4Level::L00_FAST) {

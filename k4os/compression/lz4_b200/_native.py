@@ -74,6 +74,11 @@ SIGNATURES = {
     "k4lz4_frame_writer_group_close": ([_vp] * 6 + [_i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_bound": ([_vp, _i64], _i64),
     "k4lz4_frame_writer_close_bound": ([_vp], _i64),
+    "k4lz4_frame_reader_group_create": ([_i32, _i32, _i32, _vp], _i32),
+    "k4lz4_frame_reader_group_destroy": ([_vp], _i32),
+    "k4lz4_frame_reader_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
+    "k4lz4_frame_reader_group_read": ([_vp] * 11 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_reader_group_end": ([_vp] * 3 + [_i32, _i32, _vp], _i32),
 }
 SYMBOLS = list(SIGNATURES)
 

@@ -82,6 +82,32 @@ __device__ __forceinline__ int64_t frame_lb(int64_t L, bool raw) {
 
 // ---- decode ---------------------------------------------------------------------------------------------------
 
+// The header checks on the first L bytes of a frame, in frame.py's _Frame order: magic, version with the
+// reference's 0x11 mask, dictionary flag, HC.  -> 0 or the verdict (R_CORRUPT / R_DELEGATE); *p = the offset of the
+// HC byte (6 or 14); *flg, *bd = the FLG and BD bytes (0 when L < 7).
+__device__ __forceinline__ int frame_header_check(const uint8_t* f, int64_t L, int64_t* p, int* flg, int* bd) {
+    int status = 0;
+    if (L < 7 || fr_rd32(f) != FRAME_MAGIC) status = FR_CORRUPT;
+    *flg = L >= 7 ? f[4] : 0;
+    *bd = L >= 7 ? f[5] : 0;
+    if (!status && ((*flg >> 6) & 0x11) != 1) status = FR_CORRUPT;
+    if (!status && (*flg & 1)) status = FR_DELEGATE;
+    const bool hasSize = (*flg >> 3) & 1;
+    *p = 6 + (hasSize ? 8 : 0);
+    if (!status) {
+        if (L < *p + 1) status = FR_CORRUPT;
+        else {
+            const uint32_t h = xx_finish(XXP5 + (uint32_t)(*p - 4), f + 4, (size_t)(*p - 4));
+            if (((h >> 8) & 0xFF) != f[*p]) status = FR_CORRUPT;
+        }
+    }
+    return status;
+}
+__device__ __forceinline__ int frame_flags_of(int flg) {
+    return (((flg >> 5) & 1) ? FR_INDEPENDENT : 0) | (((flg >> 4) & 1) ? FR_BLOCK_SUM : 0) |
+           (((flg >> 2) & 1) ? FR_CONTENT_SUM : 0);
+}
+
 // One thread per frame.  Pass 0: header (frame.py's _Frame order: magic, version with the reference's 0x11 mask,
 // dictionary flag, HC), the block length codes, the first block that may need a scratch slot, and the frame's
 // counts.  Pass 1: the table rows.
@@ -98,22 +124,10 @@ __global__ void frame_parse_kernel(int pass, const uint8_t* __restrict__ srcBase
     if (pass == 0) {
         r.status = 0; r.err = FK_NONE; r.nb = 0; r.nslot = 0; r.flags = 0; r.maxBlock = 1 << 16; r.k0 = 0; r.expect = 0;
         r.pos = 0;
-        if (L < 7 || fr_rd32(f) != FRAME_MAGIC) r.status = FR_CORRUPT;
-        const int flg = L >= 7 ? f[4] : 0, bd = L >= 7 ? f[5] : 0;
-        if (!r.status && ((flg >> 6) & 0x11) != 1) r.status = FR_CORRUPT;
-        if (!r.status && (flg & 1)) r.status = FR_DELEGATE;
-        const bool hasSize = (flg >> 3) & 1;
-        p = 6 + (hasSize ? 8 : 0);
-        if (!r.status) {
-            if (L < p + 1) r.status = FR_CORRUPT;
-            else {
-                const uint32_t h = xx_finish(XXP5 + (uint32_t)(p - 4), f + 4, (size_t)(p - 4));
-                if (((h >> 8) & 0xFF) != f[p]) r.status = FR_CORRUPT;
-            }
-        }
+        int flg, bd;
+        r.status = frame_header_check(f, L, &p, &flg, &bd);
         if (r.status) { r.nb = 0; fr[i] = r; return; }
-        r.flags = (((flg >> 5) & 1) ? FR_INDEPENDENT : 0) | (((flg >> 4) & 1) ? FR_BLOCK_SUM : 0) |
-                  (((flg >> 2) & 1) ? FR_CONTENT_SUM : 0);
+        r.flags = frame_flags_of(flg);
         r.maxBlock = frame_max_block((bd >> 4) & 7);
         p += 1;
         r.pos = p;               // where the first length code is, for pass 1

@@ -38,6 +38,7 @@
 #include "xxh32.cuh"
 #include "frame.cuh"
 #include "frame_writer.cuh"
+#include "frame_reader.cuh"
 
 namespace {
 
@@ -1717,6 +1718,322 @@ int fw_run(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int3
 
 }  // namespace
 
+// ---- frame reader groups ----------------------------------------------------------------------------
+
+// S incrementally read LZ4 frame streams on one device (k4lz4.h, frame_reader.cuh): rings, stashes, stream states
+// and content checksum states live there between calls; the staging buffers of host-memory calls grow and never
+// shrink.
+struct k4lz4_frame_reader_group {
+    int32_t nStreams = 0, maxBlockSize = 0, stashBody = 0;
+    int device = 0;
+    int64_t ring = 0, slot = 0, stashStride = 0;
+    uint8_t* rings = nullptr;
+    uint8_t* stash = nullptr;
+    k4::ChainGroupHdr* hdr = nullptr;
+    k4::FwState* xs = nullptr;
+    k4::FwState* bxs = nullptr;       // the XXH32 of a block being skipped
+    k4::FrState* st = nullptr;
+    Buf dStage, dDown, hUp{true}, hDown{true};
+};
+
+namespace {
+
+void fr_free(k4lz4_frame_reader_group* g) {
+    if (g->rings) cudaFree(g->rings);
+    if (g->stash) cudaFree(g->stash);
+    if (g->hdr) cudaFree(g->hdr);
+    if (g->xs) cudaFree(g->xs);
+    if (g->bxs) cudaFree(g->bxs);
+    if (g->st) cudaFree(g->st);
+    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
+    delete g;
+}
+
+// check_fw's order: the group, memKind, the count, the pointers, then (host memory) the stream indices.
+int check_fr(const k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int32_t* streams,
+             const void* srcUsed, const void* frameEnded, int memKind) {
+    if (!g) return fail(K4LZ4_E_ARG, "null frame reader group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)b.n);
+    if (b.n > 0 && (!streams || !b.outLen || (reading && (!b.srcBase || !b.srcOff || !b.srcLen || !srcUsed || !b.dstBase ||
+                                                             !b.dstOff || !b.dstCap || !frameEnded))))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
+        std::vector<uint8_t> seen((size_t)g->nStreams, 0);
+        for (int64_t i = 0; i < b.n; i++) {
+            const int32_t s = streams[i];
+            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at entry %lld", s, (long long)i);
+            if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
+        }
+    }
+    return check_device(g->device, b.n);
+}
+
+// One read of b.n entries on `st` with every array on the device: plan (count, scan, one host synchronisation for
+// the row and step counts, fill), the top-up copies into the stashes, the block checksums, the steps, the finish,
+// the tail copies.  Host staging (stageOff non-null): the output goes densely to a pool buffer (*stage, FrameRec.slot
+// * stageSlot per entry), b.dstOff is ignored, spent / rowsOut carry the room rule across sub-reads.
+cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* used,
+                      int32_t* ended, const int32_t* spent, int32_t* rowsOut, int64_t* stageOff, uint8_t** stage,
+                      FramePool& P, cudaStream_t st) {
+    const int n = (int)b.n;
+    const int64_t stageSlot = (int64_t)g->maxBlockSize + 8;
+    struct Tot { k4::FrameTotals t; int32_t kinds; };
+    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
+    k4::FrEntry* ent = P.get<k4::FrEntry>(n);
+    k4::FwEntry* skipEnt = P.get<k4::FwEntry>(n);
+    Tot* tot = P.get<Tot>(1);
+    k4::FrCopies c;
+    c.upOff = P.get<int64_t>(n); c.upDst = P.get<int64_t>(n); c.upLen = P.get<int32_t>(n);
+    c.tailOff = P.get<int64_t>(n); c.tailDst = P.get<int64_t>(n); c.tailLen = P.get<int32_t>(n);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(Tot), st));
+    FR_TRY(cudaMemsetAsync(c.upLen, 0, (size_t)n * 4, st));
+    const int64_t stashRel = (int64_t)((uintptr_t)g->stash - (uintptr_t)b.srcBase);
+    auto plan = [&](int pass, const k4::FrameTable& t) {
+        k4::frame_reader_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, streams, b.srcBase, b.srcOff, b.srcLen, b.dstOff,
+                                                                b.dstCap, spent, n, g->nStreams, g->maxBlockSize,
+                                                                g->stashBody, g->stashStride, stashRel, g->stash, g->st,
+                                                                g->xs, g->bxs, skipEnt, fr, ent, t, c, stageOff,
+                                                                stageSlot, &tot->t,
+                                                                &tot->kinds);
+        g_launches++;
+    };
+    plan(0, k4::FrameTable{});
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, &tot->t, stageOff ? 1 : 0);
+    FR_LAUNCH();
+    g_launches++;
+    Tot h{};
+    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the rows, the steps, the staged output
+    const int64_t nB = h.t.blocks;
+    k4::FrameTable t{};
+    t.srcOff = P.get<int64_t>(nB); t.len = P.get<int32_t>(nB); t.kind = P.get<int32_t>(nB);
+    t.sum = P.get<uint32_t>(nB); t.ckLen = P.get<int32_t>(nB); t.got = P.get<uint32_t>(nB);
+    uint8_t* dstBase = b.dstBase;
+    if (stageOff) *stage = dstBase = P.get<uint8_t>(h.t.slots * stageSlot);
+    FR_TRY(P.err);
+    plan(1, t);
+    FR_LAUNCH();
+    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.upOff, c.upLen, g->stash, c.upDst, nullptr, nullptr, n}, st));
+    if (h.kinds & k4::FRK_SKIP) {
+        k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, skipEnt, n, g->bxs);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    if (nB > 0 && (h.kinds & k4::FRK_BLOCK_SUM))
+        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nB}, st));
+    if (h.t.maxSteps > 0) {
+        uint8_t* tab = P.get<uint8_t>((int64_t)n * TABLE_BYTES);
+        k4::FrStep s;
+        s.srcOff = P.get<int64_t>(n); s.gDst = P.get<int64_t>(n);
+        s.lenC = P.get<int32_t>(n); s.lenD = P.get<int32_t>(n); s.resC = P.get<int32_t>(n); s.resD = P.get<int32_t>(n);
+        s.kind = P.get<int32_t>(n); s.res = P.get<int32_t>(n); s.gLen = P.get<int32_t>(n);
+        s.xe = P.get<k4::FwEntry>(n);
+        FR_TRY(P.err);
+        const k4::ChainGroupTable ct = carve_table(tab, n);
+        const bool linked = h.kinds & k4::FRK_LINKED, indep = h.kinds & k4::FRK_INDEP;
+        for (int k = 0; k < h.t.maxSteps; k++) {
+            k4::frame_reader_step_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, t, g->hdr, g->ring, ct, s);
+            FR_LAUNCH();
+            g_launches++;
+            FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
+            if (linked) {
+                Batch kb{b.srcBase, s.srcOff, s.lenC, g->rings, ct.ringOff, ct.len, s.resC, n};
+                kb.prefixLen = ct.prefix;
+                FR_TRY(launch_op(OP_CHAIN, kb, st));
+            }
+            if (indep) FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, s.srcOff, s.lenD, g->rings, ct.ringOff, ct.len, s.resD, n}, st));
+            k4::frame_reader_post_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, ct, s);
+            FR_LAUNCH();
+            g_launches++;
+            FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.ringOff, s.gLen, dstBase, s.gDst, nullptr, nullptr, n}, st));
+            if (h.kinds & k4::FRK_CONTENT_SUM) {
+                k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(g->rings, s.xe, n, g->xs);
+                FR_LAUNCH();
+                g_launches++;
+            }
+            if (linked) {        // pos += the block and the slide, after every read of the slot
+                k4::chain_group_commit_kernel<<<grid_of(n), 128, 0, st>>>(k4::CG_DECODE, s.res, n, g->ring, g->slot,
+                                                                          g->hdr, ct);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
+            }
+        }
+    }
+    k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen, used,
+                                                              ended,
+                                                              rowsOut);
+    FR_LAUNCH();
+    g_launches++;
+    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.tailOff, c.tailLen, g->stash, c.tailDst, nullptr, nullptr, n}, st));
+    return cudaSuccess;
+}
+
+// Host memory, synchronous.  One sub-read of entries idx[k], piece[k] chunk bytes from at[k] of theirs, spent[k]
+// blocks already decoded: streams, lengths, capacities and packed chunks go up in one copy, the device path stages
+// the output densely, the results come down, the produced bytes are gathered on the device and come down in one
+// copy, and res[k] > 0 bytes go to the caller at dstOff + wrote[k].
+int fr_host_part(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, const std::vector<int64_t>& idx,
+                 const std::vector<int64_t>& at, const std::vector<int64_t>& piece, const std::vector<int32_t>& spent,
+                 const std::vector<int64_t>& wrote, std::vector<int32_t>& res, std::vector<int32_t>& used,
+                 std::vector<int32_t>& ended, std::vector<int32_t>& rows, cudaStream_t st) {
+    const Dev* D = dev_state(g->device);
+    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
+    const int64_t m = (int64_t)idx.size();
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    // up: srcOff (int64) | streams srcLen dstCap spent (int32) | chunks;  down: outLen used ended rows (int32)
+    const int64_t sendAt = a16(m * (8 + 4 * 4));
+    int64_t srcBytes = 0;
+    for (int64_t k = 0; k < m; k++) srcBytes += a16(piece[k]);
+    const int64_t upBytes = sendAt + srcBytes, resAt = a16(upBytes), offAt = resAt + a16(m * 16), coffAt = offAt + a16(m * 8);
+    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 16) + 16));
+    CU_TRY(g->dStage.ensure((size_t)(coffAt + m * 8) + 16));
+    uint8_t* H = (uint8_t*)g->hUp.p;
+    int64_t* hso = (int64_t*)H;
+    int32_t* hs = (int32_t*)(hso + m); int32_t* hl = hs + m; int32_t* hc = hl + m; int32_t* hp = hc + m;
+    for (int64_t k = 0, sp = 0; k < m; k++) {
+        hs[k] = streams[idx[k]];
+        hl[k] = (int32_t)piece[k];
+        hc[k] = b.dstCap[idx[k]];
+        hp[k] = spent[(size_t)k];
+        hso[k] = sp;
+        sp += a16(piece[k]);
+    }
+    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (piece[k] > 0) memcpy(H + sendAt + hso[k], b.srcBase + b.srcOff[idx[k]] + at[k], (size_t)piece[k]);
+    });
+    uint8_t* Dp = (uint8_t*)g->dStage.p;
+    CU_TRY(cudaMemcpyAsync(Dp, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
+    const int32_t* ds = (const int32_t*)(Dp + m * 8);
+    int32_t* dRes = (int32_t*)(Dp + resAt);
+    int64_t* dOff = (int64_t*)(Dp + offAt);
+    uint8_t* stage = nullptr;
+    FramePool P(D->pool, st);
+    Batch kb{Dp + sendAt, (const int64_t*)Dp, ds + m, nullptr, nullptr, ds + 2 * m, dRes, m};
+    const cudaError_t e = fr_device(g, kb, ds, dRes + m, dRes + 2 * m, ds + 3 * m, dRes + 3 * m, dOff, &stage, P, st);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
+    std::vector<int32_t> down((size_t)m * 4);
+    CU_TRY(cudaMemcpyAsync(down.data(), dRes, (size_t)m * 16, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    res.assign(down.begin(), down.begin() + m);
+    used.assign(down.begin() + m, down.begin() + 2 * m);
+    ended.assign(down.begin() + 2 * m, down.begin() + 3 * m);
+    rows.assign(down.begin() + 3 * m, down.end());
+    std::vector<int64_t> co((size_t)m);
+    int64_t total = 0;
+    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (res[(size_t)k] > 0) total = a16(total + res[(size_t)k]); }
+    if (total == 0) return K4LZ4_OK;
+    CU_TRY(g->dDown.ensure((size_t)total + 16));
+    CU_TRY(g->hDown.ensure((size_t)total + 16));
+    memcpy(H, co.data(), (size_t)m * 8);            // the upload buffer is free again
+    CU_TRY(cudaMemcpyAsync(Dp + coffAt, H, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+    CU_TRY(launch_op(OP_COPY, Batch{stage, dOff, dRes, (uint8_t*)g->dDown.p, (const int64_t*)(Dp + coffAt), nullptr,
+                                    nullptr, m}, st));
+    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    const uint8_t* src = (const uint8_t*)g->hDown.p;
+    parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (res[(size_t)k] > 0)
+                memcpy(b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k], src + co[(size_t)k], (size_t)res[(size_t)k]);
+    });
+    return K4LZ4_OK;
+}
+
+// Host memory: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order.  An entry goes on from where it
+// stopped while it consumed something, ended no frame, failed nothing and has bytes left; the blocks it decoded
+// count against its room in the next sub-read.  So cutting a read in two changes nothing: a sub-read that stopped
+// at a length code cut by its piece sees the whole code in the next one.  The first sub-read lists every entry.
+int fr_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* srcUsed, int32_t* frameEnded,
+            cudaStream_t st) {
+    const int64_t n = b.n;
+    std::vector<int64_t> usedTot((size_t)n, 0), outTot((size_t)n, 0);
+    std::vector<int32_t> spentTot((size_t)n, 0);
+    std::vector<uint8_t> active((size_t)n, 1);
+    for (int64_t i = 0; i < n; i++) { b.outLen[i] = 0; srcUsed[i] = 0; frameEnded[i] = 0; }
+    for (bool first = true;; first = false) {
+        std::vector<int64_t> idx, at, piece, wrote;
+        std::vector<int32_t> spent;
+        int64_t budget = FW_STAGE_BYTES;
+        for (int64_t i = 0; i < n; i++) {
+            if (!active[(size_t)i]) continue;
+            if (!first && budget == 0) break;
+            const int64_t take = std::min(src_size(b, i) - usedTot[(size_t)i], budget);
+            if (!first && take <= 0) { active[(size_t)i] = 0; continue; }
+            idx.push_back(i); at.push_back(usedTot[(size_t)i]); piece.push_back(take);
+            spent.push_back(spentTot[(size_t)i]); wrote.push_back(outTot[(size_t)i]);
+            budget -= take;
+        }
+        if (idx.empty()) break;
+        std::vector<int32_t> res, used, ended, rows;
+        const int rc = fr_host_part(g, b, streams, idx, at, piece, spent, wrote, res, used, ended, rows, st);
+        if (rc != K4LZ4_OK) return rc;
+        for (size_t k = 0; k < idx.size(); k++) {
+            const int64_t i = idx[k];
+            if (res[k] < 0) { b.outLen[i] = res[k]; active[(size_t)i] = 0; continue; }
+            outTot[(size_t)i] += res[k];
+            usedTot[(size_t)i] += used[k];
+            spentTot[(size_t)i] += rows[k];
+            b.outLen[i] = (int32_t)outTot[(size_t)i];
+            srcUsed[i] = (int32_t)usedTot[(size_t)i];
+            frameEnded[i] = ended[k];
+            // a sub-read that stopped short of its piece stopped at the room rule; only a length code cut by the
+            // piece may still be an end mark
+            const int64_t end = at[k] + piece[k];
+            const bool more = used[k] == piece[k] || (end < src_size(b, i) && end - usedTot[(size_t)i] < 4);
+            if (ended[k] || usedTot[(size_t)i] >= src_size(b, i) || !more) active[(size_t)i] = 0;
+        }
+    }
+    return K4LZ4_OK;
+}
+
+// A read, or an end (b.outLen = the statuses).  Device memory: enqueued on `stream`; a read waits once.
+int fr_run(k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int32_t* streams, int32_t* srcUsed,
+           int32_t* frameEnded, int memKind, void* stream) {
+    const int rc = check_fr(g, reading, b, streams, srcUsed, frameEnded, memKind);
+    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n = (int)b.n;
+    if (!reading) {
+        const int32_t* ds = streams;
+        int32_t* dStatus = b.outLen;
+        if (memKind == K4LZ4_MEM_HOST) {
+            CU_TRY(g->hUp.ensure((size_t)n * 4));
+            CU_TRY(g->dStage.ensure((size_t)n * 8));
+            memcpy(g->hUp.p, streams, (size_t)n * 4);
+            CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+            ds = (const int32_t*)g->dStage.p;
+            dStatus = (int32_t*)g->dStage.p + n;
+        }
+        k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, dStatus);
+        g_launches++;
+        CU_TRY(cudaGetLastError());
+        if (memKind == K4LZ4_MEM_HOST) {
+            CU_TRY(cudaMemcpyAsync(b.outLen, dStatus, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaStreamSynchronize(st));
+        }
+        return K4LZ4_OK;
+    }
+    if (memKind == K4LZ4_MEM_HOST) return fr_host(g, b, streams, srcUsed, frameEnded, st);
+    const Dev* D = dev_state(g->device);
+    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
+    cudaError_t e;
+    {
+        FramePool P(D->pool, st);
+        e = fr_device(g, b, streams, srcUsed, frameEnded, nullptr, nullptr, nullptr, nullptr, P, st);
+    }
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
+    return K4LZ4_OK;
+}
+
+}  // namespace
+
 // ---- exported C ABI ------------------------------------------------------------------------
 
 extern "C" {
@@ -2164,6 +2481,100 @@ int64_t k4lz4_frame_writer_bound(const k4lz4_frame_writer_group* g, int64_t leng
 int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group* g) {
     if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
     return k4::fw_close_bound(g->B, g->bc(), g->cc());
+}
+
+int32_t k4lz4_frame_reader_group_create(int32_t nStreams, int32_t maxBlockSize, int32_t device,
+                                        k4lz4_frame_reader_group** out) {
+    if (out) *out = nullptr;
+    const bool bd = maxBlockSize == (1 << 16) || maxBlockSize == (1 << 18) || maxBlockSize == (1 << 20) ||
+                    maxBlockSize == (1 << 22);
+    if (!out || nStreams <= 0 || !bd)
+        return fail(K4LZ4_E_ARG, "bad frame reader group arguments (%d streams, max block size %d)", nStreams,
+                    maxBlockSize);
+    int rc = check_device(device, 1);
+    if (rc != K4LZ4_OK) return rc;
+    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    k4lz4_frame_reader_group* g = new k4lz4_frame_reader_group;
+    g->nStreams = nStreams; g->maxBlockSize = maxBlockSize; g->device = device;
+    g->slot = std::max<int64_t>((int64_t)maxBlockSize + 8, k4::CG_WINDOW);
+    g->ring = 2 * k4::CG_WINDOW + g->slot;
+    // a compressed block longer than this decodes to more than maxBlockSize + 8 bytes (frame_lb), so every block
+    // a reader can accept fits: [length code | body | checksum]; a longer one is skipped (frame_reader.cuh)
+    const int32_t M = maxBlockSize + 8;
+    g->stashBody = M + M / 255 + 4;
+    g->stashStride = (4 + (int64_t)g->stashBody + 4 + 15) & ~int64_t(15);
+    const size_t S = (size_t)nStreams;
+    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->stash, S * (size_t)g->stashStride);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->xs, S * sizeof(k4::FwState));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->bxs, S * sizeof(k4::FwState));
+    if (e == cudaSuccess) e = cudaMalloc((void**)&g->st, S * sizeof(k4::FrState));
+    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
+    if (e == cudaSuccess) e = cudaMemset(g->xs, 0, S * sizeof(k4::FwState));
+    if (e == cudaSuccess) e = cudaMemset(g->st, 0, S * sizeof(k4::FrState));
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        const long long per = g->ring + g->stashStride;
+        fr_free(g);
+        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "frame reader group of %d x %lld bytes: %s",
+                    nStreams, per, cudaGetErrorString(e));
+    }
+    *out = g;
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group* g) {
+    if (!g) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    cudaDeviceSynchronize();
+    fr_free(g);
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_reader_group_reset(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t n, int32_t memKind,
+                                       void* cudaStream) {
+    if (!g) return fail(K4LZ4_E_ARG, "null frame reader group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (n < 0) return fail(K4LZ4_E_ARG, "bad stream count %d", n);
+    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST)
+        for (int32_t i = 0; i < n; i++)
+            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
+    if (n == 0) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    cudaStream_t st = (cudaStream_t)cudaStream;
+    const int32_t* ds = streams;
+    if (memKind == K4LZ4_MEM_HOST) {
+        CU_TRY(g->hUp.ensure((size_t)n * 4));
+        CU_TRY(g->dStage.ensure((size_t)n * 4));
+        memcpy(g->hUp.p, streams, (size_t)n * 4);
+        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        ds = (const int32_t*)g->dStage.p;
+    }
+    k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, nullptr);
+    g_launches++;
+    CU_TRY(cudaGetLastError());
+    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return K4LZ4_OK;
+}
+
+int32_t k4lz4_frame_reader_group_read(k4lz4_frame_reader_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                      const int64_t* srcOff, const int32_t* srcLen, int32_t* srcUsed, uint8_t* dstBase,
+                                      const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                                      int32_t* frameEnded, int32_t n, int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
+    return fr_run(g, true, b, streams, srcUsed, frameEnded, memKind, cudaStream);
+}
+
+int32_t k4lz4_frame_reader_group_end(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t* status, int32_t n,
+                                     int32_t memKind, void* cudaStream) {
+    Batch b{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, status, n};
+    return fr_run(g, false, b, streams, nullptr, nullptr, memKind, cudaStream);
 }
 
 }  // extern "C"

@@ -235,3 +235,119 @@ class FrameWriterGroup:
         """Device-pointer form of close: only enqueues work on `stream`."""
         N.check(N.lib().k4lz4_frame_writer_group_close(self.handle, streams_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
                                                        out_len_ptr, int(n), N.MEM_DEVICE, stream or None))
+
+
+class FrameReaderGroup:
+    """S LZ4DecoderStream / LZ4FrameReader streams (k4lz4_frame_reader_group_*) whose partial headers and blocks,
+    histories and content checksums live on the GPU.  Each call feeds one chunk of compressed bytes, cut anywhere,
+    to any subset of the streams and returns the content it decoded; a call consumes bytes of at most one frame and
+    decodes at most floor(cap / blockCap) blocks (blockCap: the frame's BD maximum, + 8 for independent blocks), so
+    a caller re-feeds what was not consumed.  ``end(streams)`` reports whether each input stopped between frames;
+    ``free()`` (or ``with``) frees the group's device memory."""
+
+    def __init__(self, n_streams: int, max_block_size: int = 65536, device: int = 0):
+        h = C.c_void_p()
+        N.check(N.lib().k4lz4_frame_reader_group_create(int(n_streams), int(max_block_size), int(device), C.byref(h)))
+        self._h = h.value
+        self.n_streams, self.max_block_size = int(n_streams), int(max_block_size)
+
+    handle = _ChainGroup.handle
+    _streams = _ChainGroup._streams
+
+    def free(self) -> None:
+        """Frees the group's device memory."""
+        if getattr(self, "_h", None):
+            N.lib().k4lz4_frame_reader_group_destroy(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+    def reset(self, streams: Sequence[int] | None = None) -> None:
+        """Streams (default: all) become new; their input so far is dropped."""
+        s = self._streams(streams, self.n_streams)
+        N.check(N.lib().k4lz4_frame_reader_group_reset(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
+
+    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
+        N.check(N.lib().k4lz4_frame_reader_group_reset(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+
+    def read(self, chunks: Sequence, caps: Sequence[int], streams: Sequence[int] | None = None):
+        """chunks[i] is fed to stream streams[i] (default: stream i) with caps[i] bytes of room.  -> (list of
+        content each entry decoded, int32 results: bytes appended or the verdict, int32 bytes consumed, int32 1
+        where the entry ended a frame)."""
+        src, so, sl = _pack(chunks)
+        s = self._streams(streams, len(sl))
+        dst, do, dc = _slots(caps)
+        out = np.full(len(sl), -1, dtype=np.int32)
+        used = np.zeros(len(sl), dtype=np.int32)
+        ended = np.zeros(len(sl), dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_reader_group_read(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
+                                                      sl.ctypes.data, used.ctypes.data, dst.ctypes.data,
+                                                      do.ctypes.data, dc.ctypes.data, out.ctypes.data,
+                                                      ended.ctypes.data, len(sl), N.MEM_HOST, None))
+        return _slices(dst, do, out), out, used, ended
+
+    def read_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int, src_used_ptr: int,
+                    dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int, frame_ended_ptr: int, n: int,
+                    stream: int = 0) -> None:
+        """Device-pointer form of read: enqueues work on `stream` (and waits once for the row and step counts)."""
+        N.check(N.lib().k4lz4_frame_reader_group_read(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
+                                                      src_used_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr, out_len_ptr,
+                                                      frame_ended_ptr, int(n), N.MEM_DEVICE, stream or None))
+
+    def end(self, streams: Sequence[int] | None = None) -> np.ndarray:
+        """The input of streams (default: all) has ended.  -> int32 statuses: 0 between frames, R_CORRUPT inside a
+        frame, a failed stream's verdict.  The streams become new."""
+        s = self._streams(streams, self.n_streams)
+        out = np.zeros(len(s), dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_reader_group_end(self.handle, s.ctypes.data, out.ctypes.data, len(s), N.MEM_HOST,
+                                                     None))
+        return out
+
+    def end_device(self, streams_ptr: int, status_ptr: int, n: int, stream: int = 0) -> None:
+        N.check(N.lib().k4lz4_frame_reader_group_end(self.handle, streams_ptr, status_ptr, int(n), N.MEM_DEVICE,
+                                                     stream or None))
+
+    def read_all(self, chunks: Sequence, cap: int, streams: Sequence[int] | None = None):
+        """Feeds chunks[i] to stream streams[i] (default: stream i) whole, re-feeding what each call leaves, across
+        frame ends, until every chunk is consumed or its stream fails, then ends the streams (they become new).
+        -> (list of content, int32 results: total bytes, or the verdict -- R_CORRUPT where a chunk stops inside
+        a frame).  Each call is fed at most what it can consume: its blocks at `cap`, a header and an end mark."""
+        s = [int(x) for x in self._streams(streams, len(chunks))]
+        data = [memoryview(bytes(c)) for c in chunks]
+        # a block's stored bytes never exceed max_block_size + 8 + (max_block_size + 8) // 255 + 16 (longer
+        # compressed blocks are skipped in pieces), so a window this long holds everything one call consumes
+        m = self.max_block_size + 8
+        window = (max(int(cap), 0) // 65536 + 1) * (m + m // 255 + 16) + 64
+        at = [0] * len(data)
+        got = [[] for _ in data]
+        res = np.zeros(len(data), dtype=np.int32)
+        todo = [i for i in range(len(data)) if len(data[i])]
+        while todo:
+            outs, r, used, _ = self.read([data[i][at[i]:at[i] + window] for i in todo], [cap] * len(todo),
+                                         [s[i] for i in todo])
+            nxt = []
+            for k, i in enumerate(todo):
+                if r[k] < 0:
+                    res[i] = r[k]
+                    continue
+                got[i].append(outs[k])
+                res[i] += r[k]
+                at[i] += int(used[k])
+                if at[i] < len(data[i]):
+                    if used[k] == 0 and r[k] == 0:
+                        raise ValueError(f"stream {s[i]}: cap {cap} leaves no room for a block")
+                    nxt.append(i)
+            todo = nxt
+        st = self.end(s)
+        res = np.where(res < 0, res, np.where(st < 0, st, res)).astype(np.int32)
+        return [b"".join(g) for g in got], res
