@@ -214,7 +214,8 @@ __device__ __forceinline__ void seq_header(const uint32_t sStg, const int p, con
     if (mm2 && m2 == 255u && !last) {                           // rare: match of >= 529 bytes, byte loop
         while (q2 < n) { const uint32_t s = lds8_ro(sStg + q2); q2++; mlen += (int)s; if (s != 255u) break; }
     }
-    if (EXACT && m15 && q2 >= n - 4) flags |= SQ_EDGE;           // any overrun is fatal in the reference (:326-334)
+    // any overrun is fatal in the reference (:326-334); the terminal sequence's match nibble is never read (:247-294)
+    if (EXACT && m15 && !last && q2 >= n - 4) flags |= SQ_EDGE;
     off = last ? 0 : (int)(w2 & 0xFFFFu);
     ml = last ? 0 : mlen + MINMATCH;
     next = last ? n : (q2 < n ? q2 : n);
