@@ -171,6 +171,10 @@ struct Buf {           // grows, never shrinks: device memory, or pinned host me
         if (e == cudaSuccess) cap = want; else p = nullptr;
         return e;
     }
+    void release() {
+        if (p) { if (pinned) cudaFreeHost(p); else cudaFree(p); }
+        p = nullptr; cap = 0;
+    }
 };
 
 struct Slot {          // one in-flight chunk of the pipelined host path
@@ -1227,60 +1231,233 @@ int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memK
     return K4LZ4_OK;
 }
 
-}  // namespace
+// ---- resident groups: what chain, frame writer and frame reader groups share ---------------------------------
 
-// ---- chain groups -----------------------------------------------------------------------------------
-
-// S streams of one direction on one device (k4lz4.h, chain_group.cuh): rings, states and headers live there
-// between calls; the staging buffers of host-memory calls grow and never shrink.
-struct k4lz4_chain_group {
-    int kind = 0;
-    int32_t nStreams = 0, blockSize = 0;
+// S streams on one device, each with a ring in the chain-group layout (chain_group.cuh) and its header; the kind's
+// own per-stream arrays; the staging buffers of host-memory calls, which grow and never shrink.  Every device array
+// comes from alloc() and is freed with the group.
+struct GroupCore {
+    int32_t nStreams = 0;
     int device = 0;
     int64_t ring = 0, slot = 0;       // bytes per ring; the room a block or an injection may need at the write position
     uint8_t* rings = nullptr;
-    uint8_t* states = nullptr;        // encoder groups: K4LZ4_CHAIN_STATE_BYTES per stream
     k4::ChainGroupHdr* hdr = nullptr;
     Buf dStage, dDown, hUp{true}, hDown{true};
-    std::vector<int64_t> compactOff;
+    std::vector<void*> owned;
+    cudaError_t allocErr = cudaSuccess;   // the first failure of alloc(), after which it allocates nothing
+
+    // nStreams * per bytes on the current device, zeroed when `zero`
+    template <class T> T* alloc(size_t per, bool zero) {
+        void* p = nullptr;
+        if (allocErr == cudaSuccess) allocErr = cudaMalloc(&p, (size_t)nStreams * per);
+        if (allocErr != cudaSuccess) return nullptr;
+        owned.push_back(p);
+        if (zero) allocErr = cudaMemset(p, 0, (size_t)nStreams * per);
+        return (T*)p;
+    }
+    ~GroupCore() {
+        for (void* p : owned) cudaFree(p);
+        for (Buf* b : {&dStage, &dDown, &hUp, &hDown}) b->release();
+    }
+};
+
+}  // namespace
+
+// S streams of one direction (k4lz4.h, chain_group.cuh): encoder groups also keep each stream's state record.
+struct k4lz4_chain_group : GroupCore {
+    int kind = 0;
+    int32_t blockSize = 0;
+    uint8_t* states = nullptr;        // encoder groups: K4LZ4_CHAIN_STATE_BYTES per stream
 };
 
 namespace {
 
-void free_buf(Buf& b) {
-    if (b.p) { if (b.pinned) cudaFreeHost(b.p); else cudaFree(b.p); }
-    b.p = nullptr; b.cap = 0;
+// The chain-group ring layout: 128 KiB of history in front of a slot of max(x, 64 KiB) bytes.
+void chain_layout(GroupCore& g, int64_t x) {
+    g.slot = std::max<int64_t>(x, k4::CG_WINDOW);
+    g.ring = 2 * k4::CG_WINDOW + g.slot;
 }
 
-void group_free(k4lz4_chain_group* g) {
-    if (g->rings) cudaFree(g->rings);
-    if (g->states) cudaFree(g->states);
-    if (g->hdr) cudaFree(g->hdr);
-    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
+// Every group's create after the kind's own argument check: the device (the current one when negative), then on
+// it a new group of nStreams streams that `setup` sizes (ring, slot) and gives its kind's arrays through alloc(),
+// and a ring and a zeroed header per stream.  On failure everything is freed again and *out stays null.
+template <class G, class Setup>
+int group_create(int32_t nStreams, int device, const char* what, G** out, Setup setup) {
+    const int rc = check_device(device, 1);
+    if (rc != K4LZ4_OK) return rc;
+    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
+    DeviceGuard guard(device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    G* g = new G;
+    g->nStreams = nStreams; g->device = device;
+    setup(*g);
+    g->rings = g->template alloc<uint8_t>((size_t)g->ring, false);
+    g->hdr = g->template alloc<k4::ChainGroupHdr>(sizeof(k4::ChainGroupHdr), true);
+    cudaError_t e = g->allocErr;
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        const long long ring = g->ring;
+        delete g;
+        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "%s of %d streams x %lld-byte rings: %s",
+                    what, nStreams, ring, cudaGetErrorString(e));
+    }
+    *out = g;
+    return K4LZ4_OK;
+}
+
+// Every group's destroy, after the device has finished its work.
+template <class G>
+int32_t group_destroy(G* g) {
+    if (!g) return K4LZ4_OK;
+    DeviceGuard guard(g->device);
+    cudaDeviceSynchronize();
     delete g;
+    return K4LZ4_OK;
 }
 
-// The group's arguments, then the batch's, in k4lz4.h's order.  A group exists only on a device, so no check
-// here can meet "no device" before an argument error.
-int check_group(const k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int32_t* streams, int memKind) {
-    if (!g || g->kind != kind) return fail(K4LZ4_E_ARG, "null chain group or a group of the other kind");
+// The work of a reset or an end on the group's device: with host memory the stream list goes up through the staging
+// buffers first (dStage has room for an int32 result per stream behind it), and the call waits for the device after
+// `enqueue(ds, st)` has launched the kind's kernels over the list `ds`.
+template <class Enqueue>
+int group_streams_run(GroupCore* g, const int32_t* streams, int32_t n, int memKind, void* stream, Enqueue enqueue) {
+    DeviceGuard guard(g->device);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int32_t* ds = streams;
+    if (memKind == K4LZ4_MEM_HOST) {
+        CU_TRY(g->hUp.ensure((size_t)n * 4));
+        CU_TRY(g->dStage.ensure((size_t)n * 8));
+        memcpy(g->hUp.p, streams, (size_t)n * 4);
+        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        ds = (const int32_t*)g->dStage.p;
+    }
+    CU_TRY(enqueue(ds, st));
+    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return K4LZ4_OK;
+}
+
+// Every group's reset, in k4lz4.h's order: the group, memKind, the count, the pointer, with host memory the stream
+// range (a stream listed twice is reset twice, and no device is needed to get here), then n == 0 is done.
+template <class Enqueue>
+int group_reset(GroupCore* g, const int32_t* streams, int32_t n, int32_t memKind, void* stream, Enqueue enqueue) {
+    if (!g) return fail(K4LZ4_E_ARG, "null group");
     if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
-    const bool io = cg != k4::CG_INJECT;
-    if (b.n > 0 && (!streams || !b.srcBase || !b.srcOff || !b.srcLen ||
-                    (io && (!b.dstBase || !b.dstOff || !b.dstCap || !b.outLen))))
-        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (n < 0) return fail(K4LZ4_E_ARG, "bad stream count %d", n);
+    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (memKind == K4LZ4_MEM_HOST)
+        for (int32_t i = 0; i < n; i++)
+            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
+    if (n == 0) return K4LZ4_OK;
+    return group_streams_run(g, streams, n, memKind, stream, enqueue);
+}
+
+// Every group's step-call check, in k4lz4.h's order: the group, memKind, the count, the pointers (`pointers`: the
+// call's required ones besides `streams` are set), with host memory each entry's stream (in range, listed once) and
+// then `entry(i)`, the level (b.level is 0 but in a chain encoder's calls), then the machine.  A group exists only on
+// a device, so no check here meets "no device" before an argument error.
+template <class Entry>
+int check_step(const GroupCore* g, const Batch& b, const int32_t* streams, bool pointers, int memKind, Entry entry) {
+    if (!g) return fail(K4LZ4_E_ARG, "null group");
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)b.n);
+    if (b.n > 0 && (!streams || !pointers)) return fail(K4LZ4_E_ARG, "null pointer argument");
     if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
         std::vector<uint8_t> seen((size_t)g->nStreams, 0);
         for (int64_t i = 0; i < b.n; i++) {
             const int32_t s = streams[i];
-            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at block %lld", s, (long long)i);
+            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at entry %lld", s, (long long)i);
             if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
+            const int rc = entry(i);
+            if (rc != K4LZ4_OK) return rc;
         }
     }
-    if (cg == k4::CG_ENCODE && (b.level < 0 || b.level > 0xFF)) return fail(K4LZ4_E_ARG, "bad level %d", b.level);
+    if (b.level < 0 || b.level > 0xFF) return fail(K4LZ4_E_ARG, "bad level %d", b.level);
     return check_device(g->device, b.n);
 }
+
+const auto no_entry_check = [](int64_t) { return K4LZ4_OK; };
+
+// One host-memory step's upload, in one copy into dStage: the table srcOff dstOff (int64) | stream len cap aux
+// (int32) of the m entries row(k) describes, then their `send` source bytes packed 16-aligned.  Behind it in dStage:
+// resInts * m int32 results, m compact offsets (stage_down), `extra` bytes for the caller, and the entries'
+// destination slots, `room` bytes each at dstOff (16-aligned).
+struct UpRow { const uint8_t* src; int64_t send, room; int32_t stream, len, cap, aux; };
+struct StageUp {                      // device pointers into dStage
+    const uint8_t* src; const int64_t* srcOff; const int64_t* dstOff;
+    const int32_t* stream; const int32_t* len; const int32_t* cap; const int32_t* aux;
+    int32_t* res; int64_t* coff; uint8_t* extra; uint8_t* dst;
+};
+
+template <class Row>
+int stage_up(GroupCore* g, int64_t m, int64_t resInts, int64_t extra, Row row, StageUp& up, cudaStream_t st) {
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    std::vector<UpRow> r((size_t)m);
+    int64_t srcBytes = 0, dstBytes = 0;
+    for (int64_t k = 0; k < m; k++) {
+        r[(size_t)k] = row(k);
+        srcBytes += a16(r[(size_t)k].send); dstBytes += a16(r[(size_t)k].room);
+    }
+    const int64_t sendAt = a16(m * (8 * 2 + 4 * 4)), upBytes = sendAt + srcBytes;
+    const int64_t resAt = a16(upBytes), coffAt = resAt + a16(m * 4 * resInts), extraAt = coffAt + a16(m * 8);
+    const int64_t dstAt = extraAt + a16(extra);
+    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 8) + 16));   // stage_down sends the compact offsets through it
+    CU_TRY(g->dStage.ensure((size_t)(dstAt + dstBytes) + 16));
+    uint8_t* H = (uint8_t*)g->hUp.p;
+    int64_t* hso = (int64_t*)H; int64_t* hdo = hso + m;
+    int32_t* hs = (int32_t*)(hdo + m); int32_t* hl = hs + m; int32_t* hc = hl + m; int32_t* ha = hc + m;
+    for (int64_t k = 0, sp = 0, dp = 0; k < m; k++) {
+        const UpRow& x = r[(size_t)k];
+        hs[k] = x.stream; hl[k] = x.len; hc[k] = x.cap; ha[k] = x.aux;
+        hso[k] = sp; hdo[k] = dp;
+        sp += a16(x.send); dp += a16(x.room);
+    }
+    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (r[(size_t)k].send > 0) memcpy(H + sendAt + hso[k], r[(size_t)k].src, (size_t)r[(size_t)k].send);
+    });
+    uint8_t* D = (uint8_t*)g->dStage.p;
+    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
+    const int32_t* ds = (const int32_t*)(D + m * 16);
+    up = StageUp{D + sendAt, (const int64_t*)D, (const int64_t*)D + m, ds, ds + m, ds + 2 * m, ds + 3 * m,
+                 (int32_t*)(D + resAt), (int64_t*)(D + coffAt), D + extraAt, D + dstAt};
+    return K4LZ4_OK;
+}
+
+// One host-memory step's download, behind the device work on `st`: the resInts * m results come back into hRes (the
+// first m are the entries' lengths) and, where any is positive, entry k's hRes[k] bytes at from + fromOff[k] on the
+// device are gathered into dDown and come down in one copy, then go to to(k), exactly hRes[k] > 0 bytes each.
+// `after` (may be empty) is enqueued behind the gather, or alone when nothing was produced, and the call waits for it.
+template <class To>
+int stage_down(GroupCore* g, const StageUp& up, int64_t m, int32_t* hRes, int64_t resInts, const uint8_t* from,
+               const int64_t* fromOff, const std::function<cudaError_t()>& after, To to, cudaStream_t st) {
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    CU_TRY(cudaMemcpyAsync(hRes, up.res, (size_t)(m * 4 * resInts), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    std::vector<int64_t> co((size_t)m);
+    int64_t total = 0;
+    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (hRes[k] > 0) total = a16(total + hRes[k]); }
+    if (total == 0) {
+        if (after) { CU_TRY(after()); CU_TRY(cudaStreamSynchronize(st)); }
+        return K4LZ4_OK;
+    }
+    CU_TRY(g->dDown.ensure((size_t)total + 16));
+    CU_TRY(g->hDown.ensure((size_t)total + 16));
+    memcpy(g->hUp.p, co.data(), (size_t)m * 8);     // the upload buffer is free again
+    CU_TRY(cudaMemcpyAsync(up.coff, g->hUp.p, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+    CU_TRY(launch_op(OP_COPY, Batch{from, fromOff, up.res, (uint8_t*)g->dDown.p, up.coff, nullptr, nullptr, m}, st));
+    if (after) CU_TRY(after());
+    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    const uint8_t* stage = (const uint8_t*)g->hDown.p;
+    parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (hRes[k] > 0) memcpy(to(k), stage + co[(size_t)k], (size_t)hRes[k]);
+    });
+    return K4LZ4_OK;
+}
+
+// ---- chain groups -----------------------------------------------------------------------------------
 
 // Table of n blocks (chain_group.cuh) carved from `p`: 40 bytes per block.
 k4::ChainGroupTable carve_table(uint8_t* p, int64_t n) {
@@ -1320,7 +1497,7 @@ cudaError_t group_codec(k4lz4_chain_group* g, int cg, const Batch& b, const int3
 
 // The second half, after every read of the block's slot: the commit and the slides (a slide may overwrite the
 // front of a block that started below 64 KiB).
-cudaError_t group_commit(k4lz4_chain_group* g, int cg, const int32_t* outLen, int64_t n64, const k4::ChainGroupTable& t,
+cudaError_t group_commit(const GroupCore* g, int cg, const int32_t* outLen, int64_t n64, const k4::ChainGroupTable& t,
                          cudaStream_t st) {
     const int n = (int)n64, thr = 128, grid = (n + thr - 1) / thr;
     k4::chain_group_commit_kernel<<<grid, thr, 0, st>>>(cg, outLen, n, g->ring, g->slot, g->hdr, t);
@@ -1335,105 +1512,54 @@ cudaError_t group_commit(k4lz4_chain_group* g, int cg, const int32_t* outLen, in
 int group_device(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* streams, cudaStream_t st) {
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
-    uint8_t* tab = nullptr;
-    CU_TRY(cudaMallocFromPoolAsync((void**)&tab, (size_t)(b.n * TABLE_BYTES), D->pool, st));
-    const k4::ChainGroupTable t = carve_table(tab, b.n);
-    cudaError_t e = group_codec(g, cg, b, streams, t, cg == k4::CG_DECODE, st);
-    if (e == cudaSuccess) e = group_commit(g, cg, b.outLen, b.n, t, st);
-    cudaFreeAsync(tab, st);
+    FramePool P(D->pool, st);
+    uint8_t* tab = P.get<uint8_t>(b.n * TABLE_BYTES);
+    cudaError_t e = P.err;
+    if (e == cudaSuccess) {
+        const k4::ChainGroupTable t = carve_table(tab, b.n);
+        e = group_codec(g, cg, b, streams, t, cg == k4::CG_DECODE, st);
+        if (e == cudaSuccess) e = group_commit(g, cg, b.outLen, b.n, t, st);
+    }
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain group step: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
 }
 
-// Host memory, synchronous.  Up, in one copy: source offsets, destination-slot offsets, streams, lengths,
-// capacities, then the sources packed (16-aligned; an injection sends only the bytes it keeps).  After the codec the
-// results come down; the produced bytes are gathered into one compact buffer (copy_blocks_kernel) and come down
-// in one copy, then exactly outLen[i] > 0 bytes of each block go to the caller.
+// Host memory, synchronous: stage_up (an injection sends only the bytes it keeps; an encoder's destination slot is
+// where the codec writes), the codec, stage_down with the commit and the slides behind the gather.  An injection
+// commits right after the codec and brings nothing down.
 int group_host(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* streams, cudaStream_t st) {
     const int64_t n = b.n;
     const bool enc = cg == k4::CG_ENCODE, inj = cg == k4::CG_INJECT;
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
-    auto sendLen = [&](int64_t i) -> int64_t {     // the source bytes block i sends up
-        const int64_t L = b.srcLen[i];
-        if (L <= 0) return 0;
-        if (inj) return std::min<int64_t>(L, k4::CG_WINDOW);
-        return enc && L > g->blockSize ? 0 : L;
-    };
-    auto room = [&](int64_t i) -> int64_t {        // encoder: the device slot the codec writes
+    StageUp up;
+    const int rc = stage_up(g, n, 1, n * TABLE_BYTES, [&](int64_t i) {
         const int32_t L = b.srcLen[i];
-        if (!enc || L <= 0 || L > g->blockSize) return 0;
-        return std::min<int64_t>(std::max<int32_t>(b.dstCap[i], 0), k4::max_output_size(L));
-    };
-    const int64_t metaAt = 0, srcAt = a16(n * (4 * 3 + 8 * 2));
-    int64_t srcBytes = 0, scratch = 0;
-    for (int64_t i = 0; i < n; i++) { srcBytes = a16(srcBytes + sendLen(i)); scratch = a16(scratch + room(i)); }
-    const int64_t upBytes = srcAt + srcBytes;
-    const int64_t tabAt = a16(upBytes), outAt = tabAt + a16(n * TABLE_BYTES), coffAt = outAt + a16(n * 4);
-    const int64_t scratchAt = coffAt + a16(n * 8), stageBytes = scratchAt + scratch;
-    CU_TRY(g->hUp.ensure((size_t)upBytes + 16));
-    CU_TRY(g->dStage.ensure((size_t)stageBytes + 16));
-    uint8_t* H = (uint8_t*)g->hUp.p;             // srcOff dstOff (int64) | streams srcLen dstCap (int32)
-    int64_t* hso = (int64_t*)(H + metaAt); int64_t* hdo = hso + n;
-    int32_t* hs = (int32_t*)(hdo + n); int32_t* hl = hs + n; int32_t* hc = hl + n;
-    for (int64_t i = 0, sp = 0, dp = 0; i < n; i++) {
-        const int64_t k = sendLen(i);
-        hs[i] = streams[i];
-        hl[i] = inj ? (int32_t)k : b.srcLen[i];
-        hc[i] = inj ? 0 : b.dstCap[i];
-        hso[i] = sp; hdo[i] = dp;
-        sp = a16(sp + k); dp = a16(dp + room(i));
-    }
-    parallel_for_blocks(0, n, srcBytes, [&](int64_t lo, int64_t hi) {
-        for (int64_t i = lo; i < hi; i++) {
-            const int64_t k = sendLen(i);
-            if (k > 0) memcpy(H + srcAt + hso[i], b.srcBase + b.srcOff[i] + (b.srcLen[i] - k), (size_t)k);
-        }
-    });
-    uint8_t* D = (uint8_t*)g->dStage.p;
-    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
-    const int64_t* dso = (const int64_t*)(D + metaAt);
-    const int32_t* ds = (const int32_t*)(dso + 2 * n);
-    int32_t* dOut = (int32_t*)(D + outAt);
+        const bool fits = L > 0 && L <= g->blockSize;
+        const int64_t send = L <= 0 ? 0 : inj ? std::min<int64_t>(L, k4::CG_WINDOW) : enc && !fits ? 0 : L;
+        const int64_t room = enc && fits ? std::min<int64_t>(std::max<int32_t>(b.dstCap[i], 0), k4::max_output_size(L)) : 0;
+        return UpRow{send > 0 ? b.srcBase + b.srcOff[i] + (L - send) : nullptr, send, room, streams[i],
+                     inj ? (int32_t)send : L, inj ? 0 : b.dstCap[i], 0};
+    }, up, st);
+    if (rc != K4LZ4_OK) return rc;
     Batch kb = b;
-    kb.srcBase = D + srcAt; kb.srcOff = dso; kb.srcLen = ds + n;
-    kb.dstBase = D + scratchAt; kb.dstOff = dso + n; kb.dstCap = ds + 2 * n;
-    kb.outLen = dOut;
-    const k4::ChainGroupTable t = carve_table(D + tabAt, n);
-    cudaError_t e = group_codec(g, cg, kb, ds, t, false, st);
-    if (e == cudaSuccess && inj) e = group_commit(g, cg, dOut, n, t, st);
+    kb.srcBase = up.src; kb.srcOff = up.srcOff; kb.srcLen = up.len;
+    kb.dstBase = up.dst; kb.dstOff = up.dstOff; kb.dstCap = up.cap;
+    kb.outLen = up.res;
+    const k4::ChainGroupTable t = carve_table(up.extra, n);
+    auto commit = [&] { return group_commit(g, cg, up.res, n, t, st); };
+    cudaError_t e = group_codec(g, cg, kb, up.stream, t, false, st);
+    if (e == cudaSuccess && inj) e = commit();
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain group step: %s", cudaGetErrorString(e)); }
     if (inj) { CU_TRY(cudaStreamSynchronize(st)); return K4LZ4_OK; }
-    CU_TRY(cudaMemcpyAsync(b.outLen, dOut, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    auto& co = g->compactOff;
-    co.resize((size_t)n);
-    int64_t total = 0;
-    for (int64_t i = 0; i < n; i++) { co[(size_t)i] = total; if (b.outLen[i] > 0) total = a16(total + b.outLen[i]); }
-    if (total == 0) {
-        CU_TRY(group_commit(g, cg, dOut, n, t, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        return K4LZ4_OK;
-    }
-    CU_TRY(g->dDown.ensure((size_t)total + 16));
-    CU_TRY(g->hDown.ensure((size_t)total + 16));
-    memcpy(H, co.data(), (size_t)n * 8);            // the upload buffer is free again
-    CU_TRY(cudaMemcpyAsync(D + coffAt, H, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    const Batch gb = enc ? Batch{kb.dstBase, kb.dstOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt), nullptr, nullptr, n}
-                         : Batch{g->rings, t.ringOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt), nullptr, nullptr, n};
-    CU_TRY(launch_op(OP_COPY, gb, st));
-    CU_TRY(group_commit(g, cg, dOut, n, t, st));
-    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    const uint8_t* stage = (const uint8_t*)g->hDown.p;
-    parallel_for_blocks(0, n, total, [&](int64_t lo, int64_t hi) {
-        for (int64_t i = lo; i < hi; i++)
-            if (b.outLen[i] > 0) memcpy(b.dstBase + b.dstOff[i], stage + co[(size_t)i], (size_t)b.outLen[i]);
-    });
-    return K4LZ4_OK;
+    return stage_down(g, up, n, b.outLen, 1, enc ? up.dst : g->rings, enc ? up.dstOff : t.ringOff, commit,
+                      [&](int64_t i) { return b.dstBase + b.dstOff[i]; }, st);
 }
 
 int group_run(k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int32_t* streams, int memKind, void* stream) {
-    const int rc = check_group(g, kind, cg, b, streams, memKind);
+    if (g && g->kind != kind) return fail(K4LZ4_E_ARG, "chain group of the other kind");
+    const bool io = cg != k4::CG_INJECT;
+    const int rc = check_step(g, b, streams, b.srcBase && b.srcOff && b.srcLen &&
+                                                 (!io || (b.dstBase && b.dstOff && b.dstCap && b.outLen)),
+                              memKind, no_entry_check);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     DeviceGuard guard(g->device);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
@@ -1445,19 +1571,14 @@ int group_run(k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int3
 
 // ---- frame writer groups ----------------------------------------------------------------------------
 
-// S incrementally written LZ4 frames on one device (k4lz4.h, frame_writer.cuh): rings, chain states, stream
-// headers and checksum states live there between calls; the staging buffers of host-memory calls grow and never
-// shrink.
-struct k4lz4_frame_writer_group {
-    int32_t nStreams = 0, blockSize = 0, B = 0;   // the caller's block size (BD) and the encoder's (blocks)
-    int flags = 0, level = 0, device = 0;
+// S incrementally written LZ4 frames (k4lz4.h, frame_writer.cuh): each stream also keeps its FwState (partial block,
+// content checksum) and, in linked frames, its chain state.
+struct k4lz4_frame_writer_group : GroupCore {
+    int32_t blockSize = 0, B = 0;     // the caller's block size (BD) and the encoder's (blocks)
+    int flags = 0, level = 0;
     uint64_t header = 0;
-    int64_t ring = 0, slot = 0;
-    uint8_t* rings = nullptr;
     uint8_t* states = nullptr;        // linked frames: K4LZ4_CHAIN_STATE_BYTES per stream
-    k4::ChainGroupHdr* hdr = nullptr;
     k4::FwState* fw = nullptr;
-    Buf dStage, dDown, hUp{true}, hDown{true};
     bool linked() const { return !(flags & K4LZ4_FRAME_INDEPENDENT); }
     bool bc() const { return flags & K4LZ4_FRAME_BLOCK_CHECKSUM; }
     bool cc() const { return flags & K4LZ4_FRAME_CONTENT_CHECKSUM; }
@@ -1466,37 +1587,6 @@ struct k4lz4_frame_writer_group {
 namespace {
 
 constexpr int64_t FW_STAGE_BYTES = 256ll << 20;   // source bytes of one host-memory sub-write
-
-void fw_free(k4lz4_frame_writer_group* g) {
-    if (g->rings) cudaFree(g->rings);
-    if (g->states) cudaFree(g->states);
-    if (g->hdr) cudaFree(g->hdr);
-    if (g->fw) cudaFree(g->fw);
-    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
-    delete g;
-}
-
-// The chain groups' order: the group, memKind, the count, the pointers, then (host memory) the stream indices and
-// the bounds of the writes.
-int check_fw(const k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, int memKind) {
-    if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)b.n);
-    if (b.n > 0 && (!streams || !b.dstBase || !b.dstOff || !b.dstCap || !b.outLen ||
-                    (!closing && (!b.srcBase || !b.srcOff || !b.srcLen))))
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
-        std::vector<uint8_t> seen((size_t)g->nStreams, 0);
-        for (int64_t i = 0; i < b.n; i++) {
-            const int32_t s = streams[i];
-            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at entry %lld", s, (long long)i);
-            if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
-            if (!closing && k4::fw_write_bound(src_size(b, i), g->B, g->bc()) > INT32_MAX)
-                return fail(K4LZ4_E_ARG, "write of %d bytes at entry %lld: its bound exceeds 2^31 - 1", b.srcLen[i], (long long)i);
-        }
-    }
-    return check_device(g->device, b.n);
-}
 
 // One write (or close) of b.n entries in device memory on `st`: plan, the content checksum, one host
 // synchronisation for the number of steps (a close has at most one and does not wait), the steps over chunks of at
@@ -1567,13 +1657,7 @@ cudaError_t fw_device(k4lz4_frame_writer_group* g, bool closing, const Batch& b,
                     FR_LAUNCH();
                     g_launches++;
                 }
-                if (linked) {        // pos += B and the slide, after every read of the slot
-                    k4::chain_group_commit_kernel<<<grid_of(m), 128, 0, st>>>(k4::CG_ENCODE, e.res, m, g->ring, g->slot,
-                                                                              g->hdr, t);
-                    FR_LAUNCH();
-                    g_launches++;
-                    FR_TRY(launch_op(OP_COPY, Batch{g->rings, t.copyOff, t.copyLen, g->rings, t.ringOff, nullptr, nullptr, m}, st));
-                }
+                if (linked) FR_TRY(group_commit(g, k4::CG_ENCODE, e.res, m, t, st));   // pos += B and the slide
             }
         }
     }
@@ -1598,70 +1682,28 @@ cudaError_t fw_device(k4lz4_frame_writer_group* g, bool closing, const Batch& b,
 }
 
 // Host memory, synchronous.  One sub-write (or the close) of entries idx[k] with piece[k] source bytes starting
-// at srcAt[k] of theirs: offsets, lengths and packed sources go up in one copy, the device path runs on them with
-// a destination slot of the piece's bound per entry, the produced bytes are gathered on the device and come down
-// in one copy, and exactly res[k] > 0 bytes go to the caller at dstOff + wrote[k].
+// at srcAt[k] of theirs: stage_up with a destination slot of the piece's bound per entry, the device path, and
+// stage_down to the caller at dstOff + wrote[k].
 int fw_host_part(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams,
                  const std::vector<int64_t>& idx, const std::vector<int64_t>& srcAt, const std::vector<int64_t>& piece,
                  std::vector<int64_t>& wrote, std::vector<int32_t>& res, cudaStream_t st) {
     const int64_t m = (int64_t)idx.size();
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
     const int64_t cb = k4::fw_close_bound(g->B, g->bc(), g->cc());
-    auto room = [&](int64_t k) -> int64_t {
-        return closing ? std::min<int64_t>(std::max<int32_t>(b.dstCap[idx[k]], 0), cb)
-                       : k4::fw_write_bound(piece[k], g->B, g->bc());
-    };
-    const int64_t srcOffAt = 0, sendAt = a16(m * (8 * 2 + 4 * 3));
-    int64_t srcBytes = 0, dstBytes = 0;
-    for (int64_t k = 0; k < m; k++) { srcBytes += a16(piece[k]); dstBytes += a16(room(k)); }
-    const int64_t upBytes = sendAt + srcBytes;
-    const int64_t outAt = a16(upBytes), coffAt = outAt + a16(m * 4), dstAt = coffAt + a16(m * 8);
-    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 8) + 16));
-    CU_TRY(g->dStage.ensure((size_t)(dstAt + dstBytes) + 16));
-    uint8_t* H = (uint8_t*)g->hUp.p;             // srcOff dstOff (int64) | streams srcLen dstCap (int32) | sources
-    int64_t* hso = (int64_t*)(H + srcOffAt); int64_t* hdo = hso + m;
-    int32_t* hs = (int32_t*)(hdo + m); int32_t* hl = hs + m; int32_t* hc = hl + m;
-    for (int64_t k = 0, sp = 0, dp = 0; k < m; k++) {
-        hs[k] = streams[idx[k]];
-        hl[k] = (int32_t)piece[k];
-        hc[k] = (int32_t)room(k);
-        hso[k] = sp; hdo[k] = dp;
-        sp += a16(piece[k]); dp += a16(room(k));
-    }
-    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
-        for (int64_t k = lo; k < hi; k++)
-            if (piece[k] > 0) memcpy(H + sendAt + hso[k], b.srcBase + b.srcOff[idx[k]] + srcAt[k], (size_t)piece[k]);
-    });
-    uint8_t* D = (uint8_t*)g->dStage.p;
-    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
-    const int64_t* dso = (const int64_t*)(D + srcOffAt);
-    const int32_t* ds = (const int32_t*)(dso + 2 * m);
-    int32_t* dOut = (int32_t*)(D + outAt);
-    Batch kb{D + sendAt, dso, ds + m, D + dstAt, dso + m, ds + 2 * m, dOut, m, g->level};
-    const cudaError_t e = fw_device(g, closing, kb, ds, st);
+    StageUp up;
+    const int rc = stage_up(g, m, 1, 0, [&](int64_t k) {
+        const int64_t room = closing ? std::min<int64_t>(std::max<int32_t>(b.dstCap[idx[k]], 0), cb)
+                                     : k4::fw_write_bound(piece[k], g->B, g->bc());
+        return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[idx[k]] + srcAt[k] : nullptr, piece[k], room,
+                     streams[idx[k]], (int32_t)piece[k], (int32_t)room, 0};
+    }, up, st);
+    if (rc != K4LZ4_OK) return rc;
+    const Batch kb{up.src, up.srcOff, up.len, up.dst, up.dstOff, up.cap, up.res, m, g->level};
+    const cudaError_t e = fw_device(g, closing, kb, up.stream, st);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame writer step: %s", cudaGetErrorString(e)); }
     res.resize((size_t)m);
-    CU_TRY(cudaMemcpyAsync(res.data(), dOut, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    std::vector<int64_t> co((size_t)m);
-    int64_t total = 0;
-    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (res[(size_t)k] > 0) total = a16(total + res[(size_t)k]); }
-    if (total > 0) {
-        CU_TRY(g->dDown.ensure((size_t)total + 16));
-        CU_TRY(g->hDown.ensure((size_t)total + 16));
-        memcpy(H, co.data(), (size_t)m * 8);        // the upload buffer is free again
-        CU_TRY(cudaMemcpyAsync(D + coffAt, H, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-        CU_TRY(launch_op(OP_COPY, Batch{kb.dstBase, kb.dstOff, dOut, (uint8_t*)g->dDown.p, (const int64_t*)(D + coffAt),
-                                        nullptr, nullptr, m}, st));
-        CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        const uint8_t* stage = (const uint8_t*)g->hDown.p;
-        parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
-            for (int64_t k = lo; k < hi; k++)
-                if (res[(size_t)k] > 0)
-                    memcpy(b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k], stage + co[(size_t)k], (size_t)res[(size_t)k]);
-        });
-    }
+    const int rd = stage_down(g, up, m, res.data(), 1, up.dst, up.dstOff, nullptr,
+                              [&](int64_t k) { return b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k]; }, st);
+    if (rd != K4LZ4_OK) return rd;
     for (int64_t k = 0; k < m; k++) if (res[(size_t)k] > 0) wrote[(size_t)k] += res[(size_t)k];
     return K4LZ4_OK;
 }
@@ -1706,7 +1748,12 @@ int fw_host(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int
 }
 
 int fw_run(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, int memKind, void* stream) {
-    const int rc = check_fw(g, closing, b, streams, memKind);
+    const int rc = check_step(g, b, streams, b.dstBase && b.dstOff && b.dstCap && b.outLen &&
+                                                 (closing || (b.srcBase && b.srcOff && b.srcLen)),
+                              memKind, [&](int64_t i) {
+        if (closing || k4::fw_write_bound(src_size(b, i), g->B, g->bc()) <= INT32_MAX) return K4LZ4_OK;
+        return fail(K4LZ4_E_ARG, "write of %d bytes at entry %lld: its bound exceeds 2^31 - 1", b.srcLen[i], (long long)i);
+    });
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     DeviceGuard guard(g->device);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
@@ -1720,54 +1767,18 @@ int fw_run(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int3
 
 // ---- frame reader groups ----------------------------------------------------------------------------
 
-// S incrementally read LZ4 frame streams on one device (k4lz4.h, frame_reader.cuh): rings, stashes, stream states
-// and content checksum states live there between calls; the staging buffers of host-memory calls grow and never
-// shrink.
-struct k4lz4_frame_reader_group {
-    int32_t nStreams = 0, maxBlockSize = 0, stashBody = 0;
-    int device = 0;
-    int64_t ring = 0, slot = 0, stashStride = 0;
-    uint8_t* rings = nullptr;
+// S incrementally read LZ4 frame streams (k4lz4.h, frame_reader.cuh): each stream also keeps a stash for a cut
+// block, its FrState and the checksum states of its content and of a block being skipped.
+struct k4lz4_frame_reader_group : GroupCore {
+    int32_t maxBlockSize = 0, stashBody = 0;
+    int64_t stashStride = 0;
     uint8_t* stash = nullptr;
-    k4::ChainGroupHdr* hdr = nullptr;
     k4::FwState* xs = nullptr;
     k4::FwState* bxs = nullptr;       // the XXH32 of a block being skipped
     k4::FrState* st = nullptr;
-    Buf dStage, dDown, hUp{true}, hDown{true};
 };
 
 namespace {
-
-void fr_free(k4lz4_frame_reader_group* g) {
-    if (g->rings) cudaFree(g->rings);
-    if (g->stash) cudaFree(g->stash);
-    if (g->hdr) cudaFree(g->hdr);
-    if (g->xs) cudaFree(g->xs);
-    if (g->bxs) cudaFree(g->bxs);
-    if (g->st) cudaFree(g->st);
-    free_buf(g->dStage); free_buf(g->dDown); free_buf(g->hUp); free_buf(g->hDown);
-    delete g;
-}
-
-// check_fw's order: the group, memKind, the count, the pointers, then (host memory) the stream indices.
-int check_fr(const k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int32_t* streams,
-             const void* srcUsed, const void* frameEnded, int memKind) {
-    if (!g) return fail(K4LZ4_E_ARG, "null frame reader group");
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)b.n);
-    if (b.n > 0 && (!streams || !b.outLen || (reading && (!b.srcBase || !b.srcOff || !b.srcLen || !srcUsed || !b.dstBase ||
-                                                             !b.dstOff || !b.dstCap || !frameEnded))))
-        return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST && b.n > 0) {
-        std::vector<uint8_t> seen((size_t)g->nStreams, 0);
-        for (int64_t i = 0; i < b.n; i++) {
-            const int32_t s = streams[i];
-            if (s < 0 || s >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range at entry %lld", s, (long long)i);
-            if (seen[(size_t)s]++) return fail(K4LZ4_E_ARG, "stream %d listed twice", s);
-        }
-    }
-    return check_device(g->device, b.n);
-}
 
 // One read of b.n entries on `st` with every array on the device: plan (count, scan, one host synchronisation for
 // the row and step counts, fill), the top-up copies into the stashes, the block checksums, the steps, the finish,
@@ -1854,13 +1865,7 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t
                 FR_LAUNCH();
                 g_launches++;
             }
-            if (linked) {        // pos += the block and the slide, after every read of the slot
-                k4::chain_group_commit_kernel<<<grid_of(n), 128, 0, st>>>(k4::CG_DECODE, s.res, n, g->ring, g->slot,
-                                                                          g->hdr, ct);
-                FR_LAUNCH();
-                g_launches++;
-                FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
-            }
+            if (linked) FR_TRY(group_commit(g, k4::CG_DECODE, s.res, n, ct, st));   // pos += the block and the slide
         }
     }
     k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen, used,
@@ -1873,9 +1878,8 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t
 }
 
 // Host memory, synchronous.  One sub-read of entries idx[k], piece[k] chunk bytes from at[k] of theirs, spent[k]
-// blocks already decoded: streams, lengths, capacities and packed chunks go up in one copy, the device path stages
-// the output densely, the results come down, the produced bytes are gathered on the device and come down in one
-// copy, and res[k] > 0 bytes go to the caller at dstOff + wrote[k].
+// blocks already decoded (the table's aux): stage_up, the device path staging the output densely in a pool buffer
+// (alive until the gather is enqueued), and stage_down of outLen used ended rows to the caller at dstOff + wrote[k].
 int fr_host_part(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, const std::vector<int64_t>& idx,
                  const std::vector<int64_t>& at, const std::vector<int64_t>& piece, const std::vector<int32_t>& spent,
                  const std::vector<int64_t>& wrote, std::vector<int32_t>& res, std::vector<int32_t>& used,
@@ -1883,64 +1887,27 @@ int fr_host_part(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* str
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
     const int64_t m = (int64_t)idx.size();
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
-    // up: srcOff (int64) | streams srcLen dstCap spent (int32) | chunks;  down: outLen used ended rows (int32)
-    const int64_t sendAt = a16(m * (8 + 4 * 4));
-    int64_t srcBytes = 0;
-    for (int64_t k = 0; k < m; k++) srcBytes += a16(piece[k]);
-    const int64_t upBytes = sendAt + srcBytes, resAt = a16(upBytes), offAt = resAt + a16(m * 16), coffAt = offAt + a16(m * 8);
-    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 16) + 16));
-    CU_TRY(g->dStage.ensure((size_t)(coffAt + m * 8) + 16));
-    uint8_t* H = (uint8_t*)g->hUp.p;
-    int64_t* hso = (int64_t*)H;
-    int32_t* hs = (int32_t*)(hso + m); int32_t* hl = hs + m; int32_t* hc = hl + m; int32_t* hp = hc + m;
-    for (int64_t k = 0, sp = 0; k < m; k++) {
-        hs[k] = streams[idx[k]];
-        hl[k] = (int32_t)piece[k];
-        hc[k] = b.dstCap[idx[k]];
-        hp[k] = spent[(size_t)k];
-        hso[k] = sp;
-        sp += a16(piece[k]);
-    }
-    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
-        for (int64_t k = lo; k < hi; k++)
-            if (piece[k] > 0) memcpy(H + sendAt + hso[k], b.srcBase + b.srcOff[idx[k]] + at[k], (size_t)piece[k]);
-    });
-    uint8_t* Dp = (uint8_t*)g->dStage.p;
-    CU_TRY(cudaMemcpyAsync(Dp, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
-    const int32_t* ds = (const int32_t*)(Dp + m * 8);
-    int32_t* dRes = (int32_t*)(Dp + resAt);
-    int64_t* dOff = (int64_t*)(Dp + offAt);
+    StageUp up;
+    const int rc = stage_up(g, m, 4, m * 8, [&](int64_t k) {
+        return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[idx[k]] + at[k] : nullptr, piece[k], 0, streams[idx[k]],
+                     (int32_t)piece[k], b.dstCap[idx[k]], spent[(size_t)k]};
+    }, up, st);
+    if (rc != K4LZ4_OK) return rc;
+    int64_t* dOff = (int64_t*)up.extra;
     uint8_t* stage = nullptr;
     FramePool P(D->pool, st);
-    Batch kb{Dp + sendAt, (const int64_t*)Dp, ds + m, nullptr, nullptr, ds + 2 * m, dRes, m};
-    const cudaError_t e = fr_device(g, kb, ds, dRes + m, dRes + 2 * m, ds + 3 * m, dRes + 3 * m, dOff, &stage, P, st);
+    const Batch kb{up.src, up.srcOff, up.len, nullptr, nullptr, up.cap, up.res, m};
+    const cudaError_t e = fr_device(g, kb, up.stream, up.res + m, up.res + 2 * m, up.aux, up.res + 3 * m, dOff, &stage,
+                                    P, st);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
     std::vector<int32_t> down((size_t)m * 4);
-    CU_TRY(cudaMemcpyAsync(down.data(), dRes, (size_t)m * 16, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
+    const int rd = stage_down(g, up, m, down.data(), 4, stage, dOff, nullptr,
+                              [&](int64_t k) { return b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k]; }, st);
+    if (rd != K4LZ4_OK) return rd;
     res.assign(down.begin(), down.begin() + m);
     used.assign(down.begin() + m, down.begin() + 2 * m);
     ended.assign(down.begin() + 2 * m, down.begin() + 3 * m);
     rows.assign(down.begin() + 3 * m, down.end());
-    std::vector<int64_t> co((size_t)m);
-    int64_t total = 0;
-    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (res[(size_t)k] > 0) total = a16(total + res[(size_t)k]); }
-    if (total == 0) return K4LZ4_OK;
-    CU_TRY(g->dDown.ensure((size_t)total + 16));
-    CU_TRY(g->hDown.ensure((size_t)total + 16));
-    memcpy(H, co.data(), (size_t)m * 8);            // the upload buffer is free again
-    CU_TRY(cudaMemcpyAsync(Dp + coffAt, H, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(launch_op(OP_COPY, Batch{stage, dOff, dRes, (uint8_t*)g->dDown.p, (const int64_t*)(Dp + coffAt), nullptr,
-                                    nullptr, m}, st));
-    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    const uint8_t* src = (const uint8_t*)g->hDown.p;
-    parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
-        for (int64_t k = lo; k < hi; k++)
-            if (res[(size_t)k] > 0)
-                memcpy(b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k], src + co[(size_t)k], (size_t)res[(size_t)k]);
-    });
     return K4LZ4_OK;
 }
 
@@ -1994,32 +1961,24 @@ int fr_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams,
 // A read, or an end (b.outLen = the statuses).  Device memory: enqueued on `stream`; a read waits once.
 int fr_run(k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int32_t* streams, int32_t* srcUsed,
            int32_t* frameEnded, int memKind, void* stream) {
-    const int rc = check_fr(g, reading, b, streams, srcUsed, frameEnded, memKind);
+    const int rc = check_step(g, b, streams, b.outLen && (!reading || (b.srcBase && b.srcOff && b.srcLen && srcUsed &&
+                                                                        b.dstBase && b.dstOff && b.dstCap && frameEnded)),
+                              memKind, no_entry_check);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
+    const int n = (int)b.n;
+    if (!reading)             // with host memory the statuses come back from behind the stream list in dStage
+        return group_streams_run(g, streams, n, memKind, stream, [&](const int32_t* ds, cudaStream_t st) {
+            const bool host = memKind == K4LZ4_MEM_HOST;
+            int32_t* dStatus = host ? (int32_t*)g->dStage.p + n : b.outLen;
+            k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, dStatus);
+            g_launches++;
+            cudaError_t e = cudaGetLastError();
+            if (e == cudaSuccess && host) e = cudaMemcpyAsync(b.outLen, dStatus, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
+            return e;
+        });
     DeviceGuard guard(g->device);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
     cudaStream_t st = (cudaStream_t)stream;
-    const int n = (int)b.n;
-    if (!reading) {
-        const int32_t* ds = streams;
-        int32_t* dStatus = b.outLen;
-        if (memKind == K4LZ4_MEM_HOST) {
-            CU_TRY(g->hUp.ensure((size_t)n * 4));
-            CU_TRY(g->dStage.ensure((size_t)n * 8));
-            memcpy(g->hUp.p, streams, (size_t)n * 4);
-            CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-            ds = (const int32_t*)g->dStage.p;
-            dStatus = (int32_t*)g->dStage.p + n;
-        }
-        k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, dStatus);
-        g_launches++;
-        CU_TRY(cudaGetLastError());
-        if (memKind == K4LZ4_MEM_HOST) {
-            CU_TRY(cudaMemcpyAsync(b.outLen, dStatus, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-            CU_TRY(cudaStreamSynchronize(st));
-        }
-        return K4LZ4_OK;
-    }
     if (memKind == K4LZ4_MEM_HOST) return fr_host(g, b, streams, srcUsed, frameEnded, st);
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
@@ -2121,67 +2080,22 @@ int32_t k4lz4_chain_group_create(int32_t kind, int32_t nStreams, int32_t blockSi
     if (out) *out = nullptr;
     if (!out || (kind != K4LZ4_CHAIN_ENCODER && kind != K4LZ4_CHAIN_DECODER) || nStreams <= 0 || blockSize <= 0)
         return fail(K4LZ4_E_ARG, "bad chain group arguments (kind %d, %d streams, block size %d)", kind, nStreams, blockSize);
-    int rc = check_device(device, 1);
-    if (rc != K4LZ4_OK) return rc;
-    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    k4lz4_chain_group* g = new k4lz4_chain_group;
-    g->kind = kind; g->nStreams = nStreams; g->blockSize = blockSize; g->device = device;
-    g->slot = std::max<int64_t>((blockSize + 15) & ~int64_t(15), k4::CG_WINDOW);
-    g->ring = 2 * k4::CG_WINDOW + g->slot;
-    const size_t S = (size_t)nStreams;
-    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess && kind == K4LZ4_CHAIN_ENCODER) e = cudaMalloc((void**)&g->states, S * K4LZ4_CHAIN_STATE_BYTES);
-    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess && g->states) e = cudaMemset(g->states, 0, S * K4LZ4_CHAIN_STATE_BYTES);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        (void)cudaGetLastError();
-        group_free(g);
-        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "chain group of %d x %lld bytes: %s",
-                    nStreams, (long long)(2 * k4::CG_WINDOW + std::max<int64_t>(blockSize, k4::CG_WINDOW)),
-                    cudaGetErrorString(e));
-    }
-    *out = g;
-    return K4LZ4_OK;
+    return group_create(nStreams, device, "chain group", out, [&](k4lz4_chain_group& g) {
+        g.kind = kind; g.blockSize = blockSize;
+        chain_layout(g, (blockSize + 15) & ~int64_t(15));
+        if (kind == K4LZ4_CHAIN_ENCODER) g.states = g.alloc<uint8_t>(K4LZ4_CHAIN_STATE_BYTES, true);
+    });
 }
 
-int32_t k4lz4_chain_group_destroy(k4lz4_chain_group* g) {
-    if (!g) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    cudaDeviceSynchronize();
-    group_free(g);
-    return K4LZ4_OK;
-}
+int32_t k4lz4_chain_group_destroy(k4lz4_chain_group* g) { return group_destroy(g); }
 
 int32_t k4lz4_chain_group_reset(k4lz4_chain_group* g, const int32_t* streams, int32_t n, int32_t memKind,
                                 void* cudaStream) {
-    if (!g) return fail(K4LZ4_E_ARG, "null chain group");
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (n < 0) return fail(K4LZ4_E_ARG, "bad block count %d", n);
-    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST)
-        for (int32_t i = 0; i < n; i++)
-            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
-    if (n == 0) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
-    cudaStream_t st = (cudaStream_t)cudaStream;
-    const int32_t* ds = streams;
-    if (memKind == K4LZ4_MEM_HOST) {
-        CU_TRY(g->hUp.ensure((size_t)n * 4));
-        CU_TRY(g->dStage.ensure((size_t)n * 4));
-        memcpy(g->hUp.p, streams, (size_t)n * 4);
-        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        ds = (const int32_t*)g->dStage.p;
-    }
-    k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
-    g_launches++;
-    CU_TRY(cudaGetLastError());
-    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
-    return K4LZ4_OK;
+    return group_reset(g, streams, n, memKind, cudaStream, [&](const int32_t* ds, cudaStream_t st) {
+        k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
+        g_launches++;
+        return cudaGetLastError();
+    });
 }
 
 int32_t k4lz4_chain_group_encode(k4lz4_chain_group* g, const int32_t* streams, const uint8_t* srcBase,
@@ -2391,71 +2305,26 @@ int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int
         return fail(K4LZ4_E_ARG, "bad frame writer group arguments (%d streams, block size %d, flags 0x%x, level %d)",
                     nStreams, blockSize, flags, level);
     if (level >= 3) return K4LZ4_R_DELEGATE;
-    int rc = check_device(device, 1);
-    if (rc != K4LZ4_OK) return rc;
-    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    k4lz4_frame_writer_group* g = new k4lz4_frame_writer_group;
-    g->nStreams = nStreams; g->blockSize = blockSize; g->B = B; g->flags = flags; g->level = level; g->device = device;
-    g->header = frame_header(blockSize, flags);
-    g->slot = g->linked() ? std::max<int64_t>(B, k4::CG_WINDOW) : B;
-    g->ring = g->linked() ? 2 * k4::CG_WINDOW + g->slot : g->slot;
-    const size_t S = (size_t)nStreams;
-    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->fw, S * sizeof(k4::FwState));
-    if (e == cudaSuccess && g->linked()) e = cudaMalloc((void**)&g->states, S * K4LZ4_CHAIN_STATE_BYTES);
-    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess) e = cudaMemset(g->fw, 0, S * sizeof(k4::FwState));
-    if (e == cudaSuccess && g->states) e = cudaMemset(g->states, 0, S * K4LZ4_CHAIN_STATE_BYTES);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        (void)cudaGetLastError();
-        const long long ring = g->ring;
-        fw_free(g);
-        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "frame writer group of %d x %lld bytes: %s",
-                    nStreams, ring, cudaGetErrorString(e));
-    }
-    *out = g;
-    return K4LZ4_OK;
+    return group_create(nStreams, device, "frame writer group", out, [&](k4lz4_frame_writer_group& g) {
+        g.blockSize = blockSize; g.B = B; g.flags = flags; g.level = level;
+        g.header = frame_header(blockSize, flags);
+        if (g.linked()) chain_layout(g, B);
+        else g.ring = g.slot = B;     // independent blocks: the slot alone, pos stays 0
+        g.fw = g.alloc<k4::FwState>(sizeof(k4::FwState), true);
+        if (g.linked()) g.states = g.alloc<uint8_t>(K4LZ4_CHAIN_STATE_BYTES, true);
+    });
 }
 
-int32_t k4lz4_frame_writer_group_destroy(k4lz4_frame_writer_group* g) {
-    if (!g) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    cudaDeviceSynchronize();
-    fw_free(g);
-    return K4LZ4_OK;
-}
+int32_t k4lz4_frame_writer_group_destroy(k4lz4_frame_writer_group* g) { return group_destroy(g); }
 
 int32_t k4lz4_frame_writer_group_reset(k4lz4_frame_writer_group* g, const int32_t* streams, int32_t n, int32_t memKind,
                                        void* cudaStream) {
-    if (!g) return fail(K4LZ4_E_ARG, "null frame writer group");
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (n < 0) return fail(K4LZ4_E_ARG, "bad stream count %d", n);
-    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST)
-        for (int32_t i = 0; i < n; i++)
-            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
-    if (n == 0) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
-    cudaStream_t st = (cudaStream_t)cudaStream;
-    const int32_t* ds = streams;
-    if (memKind == K4LZ4_MEM_HOST) {
-        CU_TRY(g->hUp.ensure((size_t)n * 4));
-        CU_TRY(g->dStage.ensure((size_t)n * 4));
-        memcpy(g->hUp.p, streams, (size_t)n * 4);
-        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        ds = (const int32_t*)g->dStage.p;
-    }
-    k4::frame_writer_reset_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->fw);
-    k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
-    g_launches += 2;
-    CU_TRY(cudaGetLastError());
-    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
-    return K4LZ4_OK;
+    return group_reset(g, streams, n, memKind, cudaStream, [&](const int32_t* ds, cudaStream_t st) {
+        k4::frame_writer_reset_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->fw);
+        k4::chain_group_reset_kernel<<<n, 256, 0, st>>>(ds, n, g->nStreams, g->hdr, g->states);
+        g_launches += 2;
+        return cudaGetLastError();
+    });
 }
 
 int32_t k4lz4_frame_writer_group_write(k4lz4_frame_writer_group* g, const int32_t* streams, const uint8_t* srcBase,
@@ -2491,76 +2360,30 @@ int32_t k4lz4_frame_reader_group_create(int32_t nStreams, int32_t maxBlockSize, 
     if (!out || nStreams <= 0 || !bd)
         return fail(K4LZ4_E_ARG, "bad frame reader group arguments (%d streams, max block size %d)", nStreams,
                     maxBlockSize);
-    int rc = check_device(device, 1);
-    if (rc != K4LZ4_OK) return rc;
-    if (device < 0 && cudaGetDevice(&device) != cudaSuccess) return fail(K4LZ4_E_CUDA, "cudaGetDevice failed");
-    DeviceGuard guard(device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    k4lz4_frame_reader_group* g = new k4lz4_frame_reader_group;
-    g->nStreams = nStreams; g->maxBlockSize = maxBlockSize; g->device = device;
-    g->slot = std::max<int64_t>((int64_t)maxBlockSize + 8, k4::CG_WINDOW);
-    g->ring = 2 * k4::CG_WINDOW + g->slot;
-    // a compressed block longer than this decodes to more than maxBlockSize + 8 bytes (frame_lb), so every block
-    // a reader can accept fits: [length code | body | checksum]; a longer one is skipped (frame_reader.cuh)
-    const int32_t M = maxBlockSize + 8;
-    g->stashBody = M + M / 255 + 4;
-    g->stashStride = (4 + (int64_t)g->stashBody + 4 + 15) & ~int64_t(15);
-    const size_t S = (size_t)nStreams;
-    cudaError_t e = cudaMalloc((void**)&g->rings, S * (size_t)g->ring);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->stash, S * (size_t)g->stashStride);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->hdr, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->xs, S * sizeof(k4::FwState));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->bxs, S * sizeof(k4::FwState));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&g->st, S * sizeof(k4::FrState));
-    if (e == cudaSuccess) e = cudaMemset(g->hdr, 0, S * sizeof(k4::ChainGroupHdr));
-    if (e == cudaSuccess) e = cudaMemset(g->xs, 0, S * sizeof(k4::FwState));
-    if (e == cudaSuccess) e = cudaMemset(g->st, 0, S * sizeof(k4::FrState));
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        (void)cudaGetLastError();
-        const long long per = g->ring + g->stashStride;
-        fr_free(g);
-        return fail(e == cudaErrorMemoryAllocation ? K4LZ4_E_NOMEM : K4LZ4_E_CUDA, "frame reader group of %d x %lld bytes: %s",
-                    nStreams, per, cudaGetErrorString(e));
-    }
-    *out = g;
-    return K4LZ4_OK;
+    return group_create(nStreams, device, "frame reader group", out, [&](k4lz4_frame_reader_group& g) {
+        g.maxBlockSize = maxBlockSize;
+        chain_layout(g, (int64_t)maxBlockSize + 8);
+        // a compressed block longer than this decodes to more than maxBlockSize + 8 bytes (frame_lb), so every block
+        // a reader can accept fits: [length code | body | checksum]; a longer one is skipped (frame_reader.cuh)
+        const int32_t M = maxBlockSize + 8;
+        g.stashBody = M + M / 255 + 4;
+        g.stashStride = (4 + (int64_t)g.stashBody + 4 + 15) & ~int64_t(15);
+        g.stash = g.alloc<uint8_t>((size_t)g.stashStride, false);
+        g.xs = g.alloc<k4::FwState>(sizeof(k4::FwState), true);
+        g.bxs = g.alloc<k4::FwState>(sizeof(k4::FwState), false);
+        g.st = g.alloc<k4::FrState>(sizeof(k4::FrState), true);
+    });
 }
 
-int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group* g) {
-    if (!g) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    cudaDeviceSynchronize();
-    fr_free(g);
-    return K4LZ4_OK;
-}
+int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group* g) { return group_destroy(g); }
 
 int32_t k4lz4_frame_reader_group_reset(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t n, int32_t memKind,
                                        void* cudaStream) {
-    if (!g) return fail(K4LZ4_E_ARG, "null frame reader group");
-    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
-    if (n < 0) return fail(K4LZ4_E_ARG, "bad stream count %d", n);
-    if (n > 0 && !streams) return fail(K4LZ4_E_ARG, "null pointer argument");
-    if (memKind == K4LZ4_MEM_HOST)
-        for (int32_t i = 0; i < n; i++)
-            if (streams[i] < 0 || streams[i] >= g->nStreams) return fail(K4LZ4_E_ARG, "stream %d out of range", streams[i]);
-    if (n == 0) return K4LZ4_OK;
-    DeviceGuard guard(g->device);
-    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
-    cudaStream_t st = (cudaStream_t)cudaStream;
-    const int32_t* ds = streams;
-    if (memKind == K4LZ4_MEM_HOST) {
-        CU_TRY(g->hUp.ensure((size_t)n * 4));
-        CU_TRY(g->dStage.ensure((size_t)n * 4));
-        memcpy(g->hUp.p, streams, (size_t)n * 4);
-        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        ds = (const int32_t*)g->dStage.p;
-    }
-    k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, nullptr);
-    g_launches++;
-    CU_TRY(cudaGetLastError());
-    if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
-    return K4LZ4_OK;
+    return group_reset(g, streams, n, memKind, cudaStream, [&](const int32_t* ds, cudaStream_t st) {
+        k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, nullptr);
+        g_launches++;
+        return cudaGetLastError();
+    });
 }
 
 int32_t k4lz4_frame_reader_group_read(k4lz4_frame_reader_group* g, const int32_t* streams, const uint8_t* srcBase,

@@ -20,8 +20,48 @@ from . import _native as N
 from .batch import _i32, _pack, _slices, _slots
 
 
-class _ChainGroup:
+class _Group:
+    """What every resident group's mirror shares: the handle, with-blocks, and the kind's destroy and reset."""
+    _destroy = _reset = ""            # names of the kind's k4lz4_*_destroy / k4lz4_*_reset
+
+    @property
+    def handle(self) -> int:
+        if not self._h:
+            raise RuntimeError("ObjectDisposedException")
+        return self._h
+
+    def _free(self) -> None:
+        if getattr(self, "_h", None):
+            getattr(N.lib(), self._destroy)(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self._free()
+
+    def __del__(self):
+        try:
+            self._free()
+        except Exception:
+            pass
+
+    def _streams(self, streams, n: int) -> np.ndarray:
+        return _i32(np.arange(n) if streams is None else streams)
+
+    def reset(self, streams: Sequence[int] | None = None) -> None:
+        """Streams (default: all) become new; what they held is dropped (a writer's open frames emit nothing)."""
+        s = self._streams(streams, self.n_streams)
+        N.check(getattr(N.lib(), self._reset)(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
+
+    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
+        N.check(getattr(N.lib(), self._reset)(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+
+
+class _ChainGroup(_Group):
     _kind = -1
+    _destroy, _reset = "k4lz4_chain_group_destroy", "k4lz4_chain_group_reset"
 
     def __init__(self, n_streams: int, block_size: int, device: int = 0):
         h = C.c_void_p()
@@ -30,39 +70,7 @@ class _ChainGroup:
         self._h = h.value
         self.n_streams, self.block_size = int(n_streams), int(block_size)
 
-    @property
-    def handle(self) -> int:
-        if not self._h:
-            raise RuntimeError("ObjectDisposedException")
-        return self._h
-
-    def close(self) -> None:
-        if getattr(self, "_h", None):
-            N.lib().k4lz4_chain_group_destroy(self._h)
-            self._h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _streams(self, streams, n: int) -> np.ndarray:
-        return _i32(np.arange(n) if streams is None else streams)
-
-    def reset(self, streams: Sequence[int] | None = None) -> None:
-        """Streams (default: all) become new."""
-        s = self._streams(streams, self.n_streams)
-        N.check(N.lib().k4lz4_chain_group_reset(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
-
-    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
-        N.check(N.lib().k4lz4_chain_group_reset(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+    close = _Group._free
 
     def history(self, i: int) -> bytes:
         """The stream's history: its last <= 65 536 bytes (waits for the device)."""
@@ -143,12 +151,13 @@ class ChainDecoderGroup(_ChainGroup):
                                                  N.MEM_DEVICE, stream or None))
 
 
-class FrameWriterGroup:
+class FrameWriterGroup(_Group):
     """S LZ4EncoderStream / LZ4FrameWriter streams at L00_FAST (k4lz4_frame_writer_group_*) whose partial blocks,
     chain states and content checksums live on the GPU.  Each call writes one chunk of any size to (or closes) any
     subset of the streams and returns the frame bytes it produced; for every stream the concatenation of what its
     writes and its close returned is the LZ4 frame of everything written to it.  ``close(streams)`` ends frames;
-    ``free()`` (or ``with``) frees the group's device memory."""
+    ``free()`` (or ``with``) frees the group's device memory, abandoning frames not closed."""
+    _destroy, _reset = "k4lz4_frame_writer_group_destroy", "k4lz4_frame_writer_group_reset"
 
     def __init__(self, n_streams: int, block_size: int = 65536, chaining: bool = True, block_checksum: bool = False,
                  content_checksum: bool = False, level: int = 0, device: int = 0):
@@ -163,34 +172,7 @@ class FrameWriterGroup:
         self._h = h.value
         self.n_streams, self.block_size = int(n_streams), int(block_size)
 
-    handle = _ChainGroup.handle
-    _streams = _ChainGroup._streams
-
-    def free(self) -> None:
-        """Frees the group's device memory; frames not closed are abandoned."""
-        if getattr(self, "_h", None):
-            N.lib().k4lz4_frame_writer_group_destroy(self._h)
-            self._h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.free()
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
-
-    def reset(self, streams: Sequence[int] | None = None) -> None:
-        """Streams (default: all) are abandoned: they emit nothing and become new."""
-        s = self._streams(streams, self.n_streams)
-        N.check(N.lib().k4lz4_frame_writer_group_reset(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
-
-    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
-        N.check(N.lib().k4lz4_frame_writer_group_reset(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+    free = _Group._free
 
     def bound(self, length: int) -> int:
         """The most one write of `length` bytes appends."""
@@ -237,13 +219,14 @@ class FrameWriterGroup:
                                                        out_len_ptr, int(n), N.MEM_DEVICE, stream or None))
 
 
-class FrameReaderGroup:
+class FrameReaderGroup(_Group):
     """S LZ4DecoderStream / LZ4FrameReader streams (k4lz4_frame_reader_group_*) whose partial headers and blocks,
     histories and content checksums live on the GPU.  Each call feeds one chunk of compressed bytes, cut anywhere,
     to any subset of the streams and returns the content it decoded; a call consumes bytes of at most one frame and
     decodes at most floor(cap / blockCap) blocks (blockCap: the frame's BD maximum, + 8 for independent blocks), so
     a caller re-feeds what was not consumed.  ``end(streams)`` reports whether each input stopped between frames;
     ``free()`` (or ``with``) frees the group's device memory."""
+    _destroy, _reset = "k4lz4_frame_reader_group_destroy", "k4lz4_frame_reader_group_reset"
 
     def __init__(self, n_streams: int, max_block_size: int = 65536, device: int = 0):
         h = C.c_void_p()
@@ -251,34 +234,7 @@ class FrameReaderGroup:
         self._h = h.value
         self.n_streams, self.max_block_size = int(n_streams), int(max_block_size)
 
-    handle = _ChainGroup.handle
-    _streams = _ChainGroup._streams
-
-    def free(self) -> None:
-        """Frees the group's device memory."""
-        if getattr(self, "_h", None):
-            N.lib().k4lz4_frame_reader_group_destroy(self._h)
-            self._h = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.free()
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
-
-    def reset(self, streams: Sequence[int] | None = None) -> None:
-        """Streams (default: all) become new; their input so far is dropped."""
-        s = self._streams(streams, self.n_streams)
-        N.check(N.lib().k4lz4_frame_reader_group_reset(self.handle, s.ctypes.data, len(s), N.MEM_HOST, None))
-
-    def reset_device(self, streams_ptr: int, n: int, stream: int = 0) -> None:
-        N.check(N.lib().k4lz4_frame_reader_group_reset(self.handle, streams_ptr, int(n), N.MEM_DEVICE, stream or None))
+    free = _Group._free
 
     def read(self, chunks: Sequence, caps: Sequence[int], streams: Sequence[int] | None = None):
         """chunks[i] is fed to stream streams[i] (default: stream i) with caps[i] bytes of room.  -> (list of
