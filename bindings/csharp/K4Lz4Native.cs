@@ -122,6 +122,10 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_read(
             void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, int* srcUsed, byte* dstBase,
             long* dstOff, int* dstCap, int* outLen, int* frameEnded, int n, int memKind, void* cudaStream);
+        // LZ4DecoderStream.Read(buffer, offset, count): dstCap = count (any size); flags = 1 for interactive reads
+        [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_read_bytes(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, int* srcUsed, byte* dstBase,
+            long* dstOff, int* dstCap, int* outLen, int* frameEnded, int n, int flags, int memKind, void* cudaStream);
         [DllImport(Lib)] public static extern int k4lz4_frame_reader_group_end(
             void* group, int* streams, int* status, int n, int memKind, void* cudaStream);
 

@@ -420,8 +420,8 @@ K4LZ4_API int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group 
  * reference decoder's capacity).  A call decodes at most floor(dstCap[i] / blockCap) blocks, each counted as
  * blockCap whatever it decodes to (decoded bytes are still appended densely).  Once that budget is spent the call
  * stops before the next length code, except that a complete end mark and the content checksum behind it are still
- * consumed.  Header bytes need no room.  A block is never drained across calls: dstCap[i] >= blockCap always makes
- * progress.
+ * consumed.  Header bytes need no room.  A _read block is never drained across calls: dstCap[i] >= blockCap always
+ * makes progress.  For destinations of any size, use k4lz4_frame_reader_group_read_bytes.
  *
  * Errors: the first problem in stream order decides, and outLen[i] is then the code k4lz4_frame_decode_batch gives
  * for that frame: K4LZ4_R_CORRUPT for a bad magic (skippable and legacy frames included), version, header checksum,
@@ -461,6 +461,37 @@ K4LZ4_API int32_t k4lz4_frame_reader_group_read(k4lz4_frame_reader_group *g, con
                                                 int32_t *srcUsed, uint8_t *dstBase, const int64_t *dstOff,
                                                 const int32_t *dstCap, int32_t *outLen, int32_t *frameEnded,
                                                 int32_t n, int32_t memKind, void *cudaStream);
+
+/*
+ * Byte reads: entry i is one ReadManyBytes(buffer[dstCap[i]], interactive) of the reference
+ * (Streams/Frames/LZ4FrameReader.blocking.cs), fed srcBase[srcOff[i] .. +srcLen[i]) instead of pulling.  dstCap[i]
+ * may be anything >= 0 and outLen[i] <= dstCap[i].
+ *
+ * The call first appends min(dstCap[i], undrained) bytes of the stream's current decoded block.  While room is left
+ * it then decodes the next complete block of the chunk (or the stashed one) and appends as much of it as fits; the
+ * rest stays undrained, on the device, for the next call.  It stops when the destination is full, when the chunk
+ * holds no further complete block, at the frame's end, or after a block that decodes to 0 bytes (a raw block
+ * 0x80000000, say; the frame stays open).  With K4LZ4_READ_INTERACTIVE it stops after the first drain that appended
+ * anything: the leftover of the current block, or else the first new block.  The end mark is consumed only when the
+ * call reaches it (nothing undrained and room left), so a call that exactly fills the destination leaves it to the
+ * next call, which returns 0 with frameEnded[i] = 1.  Header bytes need no room, as with _read.
+ *
+ * Otherwise as _read: cut headers and blocks are stashed, at most one frame is consumed per call, and the codes,
+ * their order, the sticky failure and the skipped blocks are the same.  A block the call does not reach is neither
+ * checksummed nor decoded; the content checksum covers each block as it is decoded.  Host memory: synchronous, and
+ * cutting a read into sub-reads changes nothing; device memory: the host waits once per call.
+ *
+ * Mixing: a _read entry on a stream that holds undrained bytes gives outLen[i] = K4LZ4_E_ARG, consumes nothing and
+ * does not fail the stream.  _end and _reset discard undrained bytes; _end then reports K4LZ4_R_CORRUPT, since the
+ * frame is still open.  Arguments: _read's, in its order, then flags other than 0 or K4LZ4_READ_INTERACTIVE.
+ */
+#define K4LZ4_READ_INTERACTIVE 1
+K4LZ4_API int32_t k4lz4_frame_reader_group_read_bytes(k4lz4_frame_reader_group *g, const int32_t *streams,
+                                                      const uint8_t *srcBase, const int64_t *srcOff,
+                                                      const int32_t *srcLen, int32_t *srcUsed, uint8_t *dstBase,
+                                                      const int64_t *dstOff, const int32_t *dstCap, int32_t *outLen,
+                                                      int32_t *frameEnded, int32_t n, int32_t flags, int32_t memKind,
+                                                      void *cudaStream);
 /* The input of streams[i] has ended: status[i] = 0 between frames (never fed, or its last read ended a frame),
  * K4LZ4_R_CORRUPT inside a frame (the reference's EndOfStreamException; 1-3 bytes of a magic included), the failed
  * stream's code.  Every stream named becomes new. */

@@ -341,6 +341,15 @@ public:
         check(k4lz4_frame_reader_group_read(g_, streams, srcBase, srcOff, srcLen, srcUsed, dstBase, dstOff, dstCap,
                                             outLen, frameEnded, n, memKind, cudaStream));
     }
+    // Destinations of any size: drains the current block first, keeps what does not fit for the next call.
+    void ReadBytes(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                   int32_t* srcUsed, uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                   int32_t* frameEnded, int n, bool interactive = false, int memKind = K4LZ4_MEM_HOST,
+                   void* cudaStream = nullptr) {
+        check(k4lz4_frame_reader_group_read_bytes(g_, streams, srcBase, srcOff, srcLen, srcUsed, dstBase, dstOff,
+                                                  dstCap, outLen, frameEnded, n,
+                                                  interactive ? K4LZ4_READ_INTERACTIVE : 0, memKind, cudaStream));
+    }
     void End(const int32_t* streams, int32_t* status, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
         check(k4lz4_frame_reader_group_end(g_, streams, status, n, memKind, cudaStream));
     }

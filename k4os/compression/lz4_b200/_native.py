@@ -17,6 +17,7 @@ MEM_HOST, MEM_DEVICE = 0, 1
 ALL_DEVICES = -1
 CHAIN_STATE_BYTES = 16400                 # K4LZ4_CHAIN_STATE_BYTES
 CHAIN_ENCODER, CHAIN_DECODER = 0, 1       # K4LZ4_CHAIN_ENCODER / K4LZ4_CHAIN_DECODER
+READ_INTERACTIVE = 1                      # K4LZ4_READ_INTERACTIVE
 
 _vp, _i32, _i64, _u32, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64
 _BATCH = [_vp] * 7                        # srcBase srcOff srcLen dstBase dstOff dstCap outLen
@@ -78,6 +79,7 @@ SIGNATURES = {
     "k4lz4_frame_reader_group_destroy": ([_vp], _i32),
     "k4lz4_frame_reader_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
     "k4lz4_frame_reader_group_read": ([_vp] * 11 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_reader_group_read_bytes": ([_vp] * 11 + [_i32, _i32, _i32, _vp], _i32),
     "k4lz4_frame_reader_group_end": ([_vp] * 3 + [_i32, _i32, _vp], _i32),
 }
 SYMBOLS = list(SIGNATURES)

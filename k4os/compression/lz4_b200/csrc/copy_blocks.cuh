@@ -23,7 +23,9 @@ copy_blocks_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
         const uint4* s4 = reinterpret_cast<const uint4*>(s + head);
         uint4* d4 = reinterpret_cast<uint4*>(d + head);
         for (int i = threadIdx.x; i < body; i += blockDim.x) d4[i] = __ldg(s4 + i);
-        for (int i = head + (body << 4) + threadIdx.x; i < L; i += blockDim.x) d[i] = s[i];
+        // the tails count in 64 bits: head + body * 16 + threadIdx.x passes INT32_MAX when L is near it
+#pragma unroll 1
+        for (int64_t i = head + ((int64_t)body << 4) + threadIdx.x; i < L; i += blockDim.x) d[i] = s[i];
     } else {
         // mutually misaligned: 4-byte destination words assembled from two source words
         int head = (int)((4 - (da & 3)) & 3);
@@ -32,7 +34,8 @@ copy_blocks_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
         const int body = (L - head) >> 2;
         uint32_t* d4 = reinterpret_cast<uint32_t*>(d + head);
         for (int i = threadIdx.x; i < body; i += blockDim.x) d4[i] = ldg_u32u(s + head + 4 * i);
-        for (int i = head + (body << 2) + threadIdx.x; i < L; i += blockDim.x) d[i] = s[i];
+#pragma unroll 1
+        for (int64_t i = head + ((int64_t)body << 2) + threadIdx.x; i < L; i += blockDim.x) d[i] = s[i];
     }
 }
 

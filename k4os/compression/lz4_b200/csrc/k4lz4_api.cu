@@ -1776,6 +1776,7 @@ struct k4lz4_frame_reader_group : GroupCore {
     k4::FwState* xs = nullptr;
     k4::FwState* bxs = nullptr;       // the XXH32 of a block being skipped
     k4::FrState* st = nullptr;
+    k4::FrDrain* drain = nullptr;     // the undrained rest of each stream's current block (byte reads)
 };
 
 namespace {
@@ -1958,20 +1959,228 @@ int fr_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams,
     return K4LZ4_OK;
 }
 
-// A read, or an end (b.outLen = the statuses).  Device memory: enqueued on `stream`; a read waits once.
-int fr_run(k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int32_t* streams, int32_t* srcUsed,
+// One byte read (k4lz4_frame_reader_group_read_bytes, frame_reader.cuh) of b.n entries on `st` with every array
+// on the device: plan (count, scan, the one host synchronisation, fill), the stash top-ups, the walk of the
+// candidate rows, the cut, the drain and pending slides, the checksums, the steps (each: step, copy, codec, post,
+// gather, content checksum, commit, slide), the finish, the tail copies.  Host staging (stageOff non-null): once
+// the cut knows each entry's output size, a second wait sizes a pool buffer (*stage) by the bytes the read
+// appends, the entries are placed in it densely (16-aligned, offsets in stageOff) and b.dstOff is ignored.
+// stopped: per entry, 1 when the read stopped on room, interactive mode or an empty block (for the next sub-read).
+cudaError_t frb_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* used,
+                       int32_t* ended, int interactive, int32_t* stopped, int64_t* stageOff, uint8_t** stage,
+                       FramePool& P, cudaStream_t st) {
+    const int n = (int)b.n;
+    struct Tot { k4::FrameTotals t; int32_t kinds; };
+    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
+    k4::FrameRec* walkFr = P.get<k4::FrameRec>(n);     // the walk's error keys: the cut and the decoder decide
+    k4::FrEntry* ent = P.get<k4::FrEntry>(n);
+    k4::FrCut* cut = P.get<k4::FrCut>(n);
+    k4::FwEntry* skipEnt = P.get<k4::FwEntry>(n);
+    Tot* tot = P.get<Tot>(1);
+    k4::FrCopies c;
+    c.upOff = P.get<int64_t>(n); c.upDst = P.get<int64_t>(n); c.upLen = P.get<int32_t>(n);
+    c.tailOff = P.get<int64_t>(n); c.tailDst = P.get<int64_t>(n); c.tailLen = P.get<int32_t>(n);
+    k4::FrPre pre;
+    pre.dOff = P.get<int64_t>(n); pre.dDst = P.get<int64_t>(n); pre.dLen = P.get<int32_t>(n);
+    pre.sOff = P.get<int64_t>(n); pre.sDst = P.get<int64_t>(n); pre.sLen = P.get<int32_t>(n);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(Tot), st));
+    FR_TRY(cudaMemsetAsync(c.upLen, 0, (size_t)n * 4, st));
+    const int64_t stashRel = (int64_t)((uintptr_t)g->stash - (uintptr_t)b.srcBase);
+    auto plan = [&](int pass, const k4::FrameTable& t, int64_t* rowEnd) {
+        k4::frame_reader_bytes_plan_kernel<<<grid_of(n), 128, 0, st>>>(
+            pass, interactive, streams, b.srcBase, b.srcOff, b.srcLen, b.dstOff, b.dstCap, n, g->nStreams,
+            g->maxBlockSize, g->stashBody, g->stashStride, stashRel, g->stash, g->st, g->drain, g->xs, fr, ent, cut, t,
+            rowEnd, c, stageOff ? 1 : 0, &tot->t, &tot->kinds);
+        g_launches++;
+    };
+    plan(0, k4::FrameTable{}, nullptr);
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, &tot->t, 0);
+    FR_LAUNCH();
+    g_launches++;
+    Tot h{};
+    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the candidate rows and the steps
+    const int64_t nB = h.t.blocks;
+    k4::FrameTable t{};
+    t.srcOff = P.get<int64_t>(nB); t.len = P.get<int32_t>(nB); t.kind = P.get<int32_t>(nB);
+    t.sum = P.get<uint32_t>(nB); t.ckLen = P.get<int32_t>(nB); t.got = P.get<uint32_t>(nB);
+    t.frame = P.get<int32_t>(nB); t.idx = P.get<int32_t>(nB); t.size = P.get<int32_t>(nB);
+    int64_t* rowEnd = P.get<int64_t>(nB);
+    k4::FrameRec* place = stageOff ? P.get<k4::FrameRec>(n) : nullptr;
+    k4::FrameTotals* placeTot = stageOff ? P.get<k4::FrameTotals>(1) : nullptr;
+    uint8_t* dstBase = b.dstBase;
+    FR_TRY(P.err);
+    plan(1, t, rowEnd);
+    FR_LAUNCH();
+    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.upOff, c.upLen, g->stash, c.upDst, nullptr, nullptr, n}, st));
+    if (nB > 0) {
+        k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, walkFr);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    k4::frame_reader_bytes_cut_kernel<<<grid_of(n), 128, 0, st>>>(interactive, fr, ent, cut, n, t, rowEnd, g->st,
+                                                                   g->bxs, skipEnt, g->drain, g->hdr, g->ring, g->slot,
+                                                                   g->stashStride, c, pre, stopped, place);
+    FR_LAUNCH();
+    g_launches++;
+    if (stageOff) {              // host staging only: a second wait, for the bytes the read appends
+        k4::frame_scan_kernel<<<1, 1024, 0, st>>>(place, n, placeTot, 1);
+        FR_LAUNCH();
+        k4::FrameTotals pt{};
+        FR_TRY(cudaMemcpyAsync(&pt, placeTot, sizeof(pt), cudaMemcpyDeviceToHost, st));
+        FR_TRY(cudaStreamSynchronize(st));
+        *stage = dstBase = P.get<uint8_t>(pt.slots * 16);
+        FR_TRY(P.err);
+        k4::frame_reader_bytes_place_kernel<<<grid_of(n), 128, 0, st>>>(place, fr, ent, pre, stageOff, n);
+        FR_LAUNCH();
+        g_launches += 2;
+    }
+    FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.dOff, pre.dLen, dstBase, pre.dDst, nullptr, nullptr, n}, st));
+    FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.sOff, pre.sLen, g->rings, pre.sDst, nullptr, nullptr, n}, st));
+    if (h.kinds & k4::FRK_SKIP) {
+        k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, skipEnt, n, g->bxs);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    if (nB > 0 && (h.kinds & k4::FRK_BLOCK_SUM))
+        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nB}, st));
+    if (h.t.maxSteps > 0) {
+        uint8_t* tab = P.get<uint8_t>((int64_t)n * TABLE_BYTES);
+        k4::FrStep s;
+        s.srcOff = P.get<int64_t>(n); s.gDst = P.get<int64_t>(n);
+        s.lenC = P.get<int32_t>(n); s.lenD = P.get<int32_t>(n); s.resC = P.get<int32_t>(n); s.resD = P.get<int32_t>(n);
+        s.kind = P.get<int32_t>(n); s.res = P.get<int32_t>(n); s.gLen = P.get<int32_t>(n);
+        s.xe = P.get<k4::FwEntry>(n);
+        FR_TRY(P.err);
+        const k4::ChainGroupTable ct = carve_table(tab, n);
+        const bool linked = h.kinds & k4::FRK_LINKED, indep = h.kinds & k4::FRK_INDEP;
+        for (int k = 0; k < h.t.maxSteps; k++) {
+            k4::frame_reader_step_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, t, g->hdr, g->ring, ct, s);
+            FR_LAUNCH();
+            g_launches++;
+            FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
+            if (linked) {
+                Batch kb{b.srcBase, s.srcOff, s.lenC, g->rings, ct.ringOff, ct.len, s.resC, n};
+                kb.prefixLen = ct.prefix;
+                FR_TRY(launch_op(OP_CHAIN, kb, st));
+            }
+            if (indep) FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, s.srcOff, s.lenD, g->rings, ct.ringOff, ct.len, s.resD, n}, st));
+            k4::frame_reader_bytes_post_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, b.dstCap, n, ct, s);
+            FR_LAUNCH();
+            g_launches++;
+            FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.ringOff, s.gLen, dstBase, s.gDst, nullptr, nullptr, n}, st));
+            if (h.kinds & k4::FRK_CONTENT_SUM) {
+                k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(g->rings, s.xe, n, g->xs);
+                FR_LAUNCH();
+                g_launches++;
+            }
+            k4::frame_reader_bytes_commit_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, g->ring, g->slot, g->hdr, g->drain,
+                                                                             ct, s);
+            FR_LAUNCH();
+            g_launches++;
+            if (linked)
+                FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
+        }
+    }
+    k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen, used,
+                                                              ended, nullptr);
+    FR_LAUNCH();
+    g_launches++;
+    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.tailOff, c.tailLen, g->stash, c.tailDst, nullptr, nullptr, n}, st));
+    return cudaSuccess;
+}
+
+// Host memory, synchronous: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order, as fr_host.  Each
+// sub-read gets the room the earlier ones left (dstCap minus the bytes they appended) and its output comes down
+// behind it, exactly outLen bytes per entry.  An entry goes on while its sub-read ran to the end of its piece
+// (it did not stop on room, interactive mode or an empty block), ended no frame, failed nothing and has bytes
+// left -- and, interactively, appended nothing yet.  The first sub-read lists every entry, so that a read of an
+// empty chunk still drains.
+int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* srcUsed,
+             int32_t* frameEnded, int interactive, cudaStream_t st) {
+    const Dev* D = dev_state(g->device);
+    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
+    const int64_t n = b.n;
+    std::vector<int64_t> usedTot((size_t)n, 0), outTot((size_t)n, 0);
+    std::vector<uint8_t> active((size_t)n, 1);
+    for (int64_t i = 0; i < n; i++) { b.outLen[i] = 0; srcUsed[i] = 0; frameEnded[i] = 0; }
+    for (bool first = true;; first = false) {
+        std::vector<int64_t> idx, at, piece;
+        int64_t budget = FW_STAGE_BYTES;
+        for (int64_t i = 0; i < n; i++) {
+            if (!active[(size_t)i]) continue;
+            if (!first && budget == 0) break;
+            const int64_t take = std::min(src_size(b, i) - usedTot[(size_t)i], budget);
+            if (!first && take <= 0) { active[(size_t)i] = 0; continue; }
+            idx.push_back(i); at.push_back(usedTot[(size_t)i]); piece.push_back(take);
+            budget -= take;
+        }
+        if (idx.empty()) break;
+        const int64_t m = (int64_t)idx.size();
+        StageUp up;
+        const int rc = stage_up(g, m, 4, m * 8, [&](int64_t k) {
+            const int64_t i = idx[(size_t)k];
+            const int64_t room = std::max<int64_t>(b.dstCap[i], 0) - outTot[(size_t)i];
+            return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[i] + at[k] : nullptr, piece[k], 0, streams[i],
+                         (int32_t)piece[k], (int32_t)room, 0};
+        }, up, st);
+        if (rc != K4LZ4_OK) return rc;
+        int64_t* dOff = (int64_t*)up.extra;
+        uint8_t* stage = nullptr;
+        cudaError_t e;
+        {
+            FramePool P(D->pool, st);
+            const Batch kb{up.src, up.srcOff, up.len, nullptr, nullptr, up.cap, up.res, m};
+            e = frb_device(g, kb, up.stream, up.res + m, up.res + 2 * m, interactive, up.res + 3 * m, dOff, &stage, P, st);
+            if (e == cudaSuccess) {
+                std::vector<int32_t> down((size_t)m * 4);
+                const int rd = stage_down(g, up, m, down.data(), 4, stage, dOff, nullptr, [&](int64_t k) {
+                    return b.dstBase + b.dstOff[idx[(size_t)k]] + outTot[(size_t)idx[(size_t)k]];
+                }, st);
+                if (rd != K4LZ4_OK) return rd;
+                for (int64_t k = 0; k < m; k++) {
+                    const int64_t i = idx[(size_t)k];
+                    const int32_t res = down[(size_t)k], used = down[(size_t)(m + k)];
+                    const int32_t ended = down[(size_t)(2 * m + k)], stopped = down[(size_t)(3 * m + k)];
+                    if (res < 0) { b.outLen[i] = res; active[(size_t)i] = 0; continue; }
+                    outTot[(size_t)i] += res;
+                    usedTot[(size_t)i] += used;
+                    b.outLen[i] = (int32_t)outTot[(size_t)i];
+                    srcUsed[i] = (int32_t)usedTot[(size_t)i];
+                    frameEnded[i] = ended;
+                    if (stopped || ended || usedTot[(size_t)i] >= src_size(b, i) || (interactive && outTot[(size_t)i] > 0))
+                        active[(size_t)i] = 0;
+                }
+            }
+        }
+        if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
+    }
+    return K4LZ4_OK;
+}
+
+enum FrMode { FR_END = 0, FR_READ = 1, FR_BYTES = 2, FR_BYTES_INTERACTIVE = 3 };
+
+// A read, a byte read, or an end (b.outLen = the statuses).  Device memory: enqueued on `stream`; a read waits
+// once.  mode -1: a byte read with unknown flags (K4LZ4_E_ARG after the pointer and stream checks).
+int fr_run(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t* streams, int32_t* srcUsed,
            int32_t* frameEnded, int memKind, void* stream) {
+    const bool reading = mode != FR_END;
     const int rc = check_step(g, b, streams, b.outLen && (!reading || (b.srcBase && b.srcOff && b.srcLen && srcUsed &&
                                                                         b.dstBase && b.dstOff && b.dstCap && frameEnded)),
                               memKind, no_entry_check);
-    if (rc != K4LZ4_OK || b.n == 0) return rc;
+    if (rc != K4LZ4_OK) return rc;
+    if (mode < 0) return fail(K4LZ4_E_ARG, "unknown read flags");
+    if (b.n == 0) return rc;
     const int n = (int)b.n;
     if (!reading)             // with host memory the statuses come back from behind the stream list in dStage
         return group_streams_run(g, streams, n, memKind, stream, [&](const int32_t* ds, cudaStream_t st) {
             const bool host = memKind == K4LZ4_MEM_HOST;
             int32_t* dStatus = host ? (int32_t*)g->dStage.p + n : b.outLen;
+            k4::frame_reader_bytes_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->drain);
             k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, dStatus);
-            g_launches++;
+            g_launches += 2;
             cudaError_t e = cudaGetLastError();
             if (e == cudaSuccess && host) e = cudaMemcpyAsync(b.outLen, dStatus, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
             return e;
@@ -1979,13 +2188,23 @@ int fr_run(k4lz4_frame_reader_group* g, bool reading, const Batch& b, const int3
     DeviceGuard guard(g->device);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
     cudaStream_t st = (cudaStream_t)stream;
-    if (memKind == K4LZ4_MEM_HOST) return fr_host(g, b, streams, srcUsed, frameEnded, st);
+    const bool bytes = mode != FR_READ;
+    const int interactive = mode == FR_BYTES_INTERACTIVE;
+    if (memKind == K4LZ4_MEM_HOST)
+        return bytes ? frb_host(g, b, streams, srcUsed, frameEnded, interactive, st)
+                     : fr_host(g, b, streams, srcUsed, frameEnded, st);
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
     cudaError_t e;
     {
         FramePool P(D->pool, st);
-        e = fr_device(g, b, streams, srcUsed, frameEnded, nullptr, nullptr, nullptr, nullptr, P, st);
+        if (bytes) {
+            int32_t* stopped = P.get<int32_t>(n);
+            e = P.err;
+            if (e == cudaSuccess) e = frb_device(g, b, streams, srcUsed, frameEnded, interactive, stopped, nullptr, nullptr, P, st);
+        } else {
+            e = fr_device(g, b, streams, srcUsed, frameEnded, nullptr, nullptr, nullptr, nullptr, P, st);
+        }
     }
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
@@ -2372,6 +2591,7 @@ int32_t k4lz4_frame_reader_group_create(int32_t nStreams, int32_t maxBlockSize, 
         g.xs = g.alloc<k4::FwState>(sizeof(k4::FwState), true);
         g.bxs = g.alloc<k4::FwState>(sizeof(k4::FwState), false);
         g.st = g.alloc<k4::FrState>(sizeof(k4::FrState), true);
+        g.drain = g.alloc<k4::FrDrain>(sizeof(k4::FrDrain), true);
     });
 }
 
@@ -2380,8 +2600,9 @@ int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group* g) { return g
 int32_t k4lz4_frame_reader_group_reset(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t n, int32_t memKind,
                                        void* cudaStream) {
     return group_reset(g, streams, n, memKind, cudaStream, [&](const int32_t* ds, cudaStream_t st) {
+        k4::frame_reader_bytes_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->drain);
         k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, nullptr);
-        g_launches++;
+        g_launches += 2;
         return cudaGetLastError();
     });
 }
@@ -2391,13 +2612,23 @@ int32_t k4lz4_frame_reader_group_read(k4lz4_frame_reader_group* g, const int32_t
                                       const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
                                       int32_t* frameEnded, int32_t n, int32_t memKind, void* cudaStream) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
-    return fr_run(g, true, b, streams, srcUsed, frameEnded, memKind, cudaStream);
+    return fr_run(g, FR_READ, b, streams, srcUsed, frameEnded, memKind, cudaStream);
+}
+
+int32_t k4lz4_frame_reader_group_read_bytes(k4lz4_frame_reader_group* g, const int32_t* streams,
+                                            const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                            int32_t* srcUsed, uint8_t* dstBase, const int64_t* dstOff,
+                                            const int32_t* dstCap, int32_t* outLen, int32_t* frameEnded, int32_t n,
+                                            int32_t flags, int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
+    return fr_run(g, flags == 0 ? FR_BYTES : flags == K4LZ4_READ_INTERACTIVE ? FR_BYTES_INTERACTIVE : -1, b, streams,
+                  srcUsed, frameEnded, memKind, cudaStream);
 }
 
 int32_t k4lz4_frame_reader_group_end(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t* status, int32_t n,
                                      int32_t memKind, void* cudaStream) {
     Batch b{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, status, n};
-    return fr_run(g, false, b, streams, nullptr, nullptr, memKind, cudaStream);
+    return fr_run(g, FR_END, b, streams, nullptr, nullptr, memKind, cudaStream);
 }
 
 }  // extern "C"
