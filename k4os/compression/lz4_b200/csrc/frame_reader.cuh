@@ -12,13 +12,34 @@
 // keeps the whole-frame order -- truncated (end) or a block checksum mismatch: R_CORRUPT; otherwise -1.
 //
 // A read plans every entry first (one thread per entry, a count pass, frame_scan_kernel, a fill pass): it
-// continues the stream's phase over the chunk, hops over the length codes under the room rule (at most
-// floor(dstCap / blockCap) blocks per call, blockCap = the reference decoder's capacity) and writes one row per
-// block it completes -- stored bytes in the chunk, or in the stash for the one block a previous chunk began.  The
-// rows' checksums are verified by xxh32_batch_kernel before anything decodes; then step k decodes block k of every
-// entry into its slot, gathers it to the entry's cursor, advances the content XXH32 and commits the ring
-// (chain_group_commit_kernel).  The finish kernel gives the verdicts, and the unconsumed tail of a cut block is
-// copied into the stash last.
+// continues the stream's phase over the chunk, hops over the length codes under the read's room rule and writes
+// one row per block it completes -- stored bytes in the chunk, or in the stash for the one block a previous chunk
+// began.  The rows' checksums are verified by xxh32_batch_kernel before anything decodes; then step k decodes
+// block k of every entry into its slot, gathers it to the entry's cursor, advances the content XXH32 and commits
+// the ring.  The finish kernel gives the verdicts, and the unconsumed tail of a cut block is copied into the stash
+// last.
+//
+// Two kinds of reads share all of this and differ in their room rule:
+//
+// * A plain read (k4lz4_frame_reader_group_read) decodes whole blocks only, at most floor(dstCap / blockCap) of
+//   them per call (blockCap = the reference decoder's capacity).
+// * A byte read (k4lz4_frame_reader_group_read_bytes) is ReadManyBytes (Streams/Frames/LZ4FrameReader.blocking.cs:
+//   157-179) for the push contract: it first drains the rest of the stream's current decoded block, then decodes
+//   blocks while room is left, appending as much of each as fits; what does not fit stays undrained in the ring
+//   for the next read.  The room a block takes is its decoded size, so its plan takes candidate rows until the
+//   lower bounds frame_lb of their sizes cover the room left after the drain (one row in interactive mode); its
+//   stops and the stream's state at the first length code of the call go to an FrCut, and the stream's state
+//   itself is not written.  block_size_walk_kernel then gives each candidate's exact size (the lower bound for a
+//   chain that does not parse: the decoder rejects that block wherever the cut falls), and the cut kernel replays
+//   the reference's loop over the sizes: the rows that decode, whether the plan's last step (end mark, cut block,
+//   skipped block, raw block above its limit) is reached, the stream's new phase, `have`, stash tail and
+//   undrained length.  Rows it does not reach are neither checksummed nor decoded.
+//
+// The undrained bytes are the last FrDrain.len bytes in front of FrDrain.end in the stream's ring.  While a stream
+// holds any, its FrState.err is FR_ARG: a plain read then gets K4LZ4_E_ARG and consumes nothing, and only byte
+// reads, end and reset clear it.  Slides: a linked block that leaves at most 64 KiB undrained slides at once (its
+// undrained bytes stay the last ones in front of pos); one that leaves more keeps pos beyond RING - SLOT and slides
+// when a later read has drained it, before anything else decodes.
 #pragma once
 #include "common.cuh"
 #include "chain_group.cuh"
@@ -52,375 +73,6 @@ struct FrEntry {             // per entry of one read; the rest is in its FrameR
     int32_t reserved;
 };
 
-// Copies the plan orders from the chunk into the stash: the rest of a block a previous chunk began (before the
-// checksums) and the tail of the chunk when it ends inside a block (after every decode).
-struct FrCopies { int64_t* upOff; int64_t* upDst; int32_t* upLen; int64_t* tailOff; int64_t* tailDst; int32_t* tailLen; };
-
-// Byte j of the current item: the `have` stashed bytes, then the chunk from q on.
-__device__ __forceinline__ uint32_t fr_vbyte(const uint8_t* stash, int have, const uint8_t* p, int64_t q, int64_t j) {
-    return j < have ? stash[j] : p[q + j - have];
-}
-// xxhash.c's XXH32_digest of a streaming state (seed 0).
-__device__ __forceinline__ uint32_t fr_digest(const FwState& f) {
-    uint32_t h = f.total >= 16 ? xx_rotl(f.v[0], 1) + xx_rotl(f.v[1], 7) + xx_rotl(f.v[2], 12) + xx_rotl(f.v[3], 18)
-                               : f.v[2] + XXP5;
-    h += (uint32_t)f.total;
-    return xx_finish(h, f.carry, (size_t)f.carryLen);
-}
-__device__ __forceinline__ void fr_xxh_reset(FwState& x) {
-    x.v[0] = XXP1 + XXP2; x.v[1] = XXP2; x.v[2] = 0; x.v[3] = 0u - XXP1;
-    x.total = 0; x.carryLen = 0;
-}
-__device__ __forceinline__ uint32_t fr_vrd32(const uint8_t* stash, int have, const uint8_t* p, int64_t q, int64_t j) {
-    return fr_vbyte(stash, have, p, q, j) | (fr_vbyte(stash, have, p, q, j + 1) << 8) |
-           (fr_vbyte(stash, have, p, q, j + 2) << 16) | (fr_vbyte(stash, have, p, q, j + 3) << 24);
-}
-
-// One thread per entry.  Pass 0 counts the rows (FrameRec.nb; nslot = nb when the output is staged densely);
-// pass 1, after frame_scan_kernel, walks again and writes the rows, the copies, the stream's new phase and, for a
-// frame it opens, a fresh content checksum state.  spent (nullable): blocks earlier sub-reads of the same read
-// decoded.  stageOff (nullable): the output goes to stageOff[i] = FrameRec.slot * stageSlot instead of dstOff[i].
-// A verdict before any row is FrameRec.status (header, sticky error, stream out of range); one at row k is the
-// error key (k << 4) | kind in FrameRec.err, as frame.cuh keeps it.  skipEnt[i]: the skipped block's bytes in the
-// chunk, for frame_writer_xxh_kernel over bxs (stream -1: none).
-__global__ void frame_reader_plan_kernel(int pass, const int32_t* __restrict__ streams, const uint8_t* __restrict__ srcBase,
-                                         const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
-                                         const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                                         const int32_t* __restrict__ spent, int n, int nStreams, int32_t maxBlockSize,
-                                         int32_t stashBody, int64_t stashStride, int64_t stashRel,
-                                         const uint8_t* __restrict__ stash, FrState* __restrict__ st,
-                                         FwState* __restrict__ xs, FwState* __restrict__ bxs, FwEntry* __restrict__ skipEnt,
-                                         FrameRec* __restrict__ fr, FrEntry* __restrict__ ent,
-                                         FrameTable t, FrCopies c, int64_t* __restrict__ stageOff, int64_t stageSlot,
-                                         FrameTotals* __restrict__ tot, int32_t* __restrict__ kinds) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int s = streams[i];
-    FrameRec r = {};
-    r.err = FK_NONE;
-    if (pass == 1) { r.first = fr[i].first; r.slot = fr[i].slot; }
-    FrEntry e = {};
-    e.stream = s >= 0 && s < nStreams ? s : -1;
-    e.start = stageOff ? r.slot * stageSlot : dstOff[i];
-    int64_t q = 0, tailFrom = -1, tailAt = 0;
-    int rows = 0;
-    bool opened = false, skipStart = false;
-    FwEntry sk = {};
-    sk.stream = -1;
-    FrState S = {};
-    if (e.stream < 0) r.status = FR_ARG;
-    else {
-        S = st[s];
-        r.status = S.err;
-    }
-    if (!r.status) {
-        const uint8_t* p = srcBase + srcOff[i];
-        const uint8_t* sp = stash + (int64_t)s * stashStride;
-        const int64_t L = srcLen[i] > 0 ? srcLen[i] : 0;
-        int64_t budget = -1;
-        for (;;) {
-            if (S.phase == FP_IDLE) {
-                if (q >= L) break;
-                S.phase = FP_HEADER;
-                S.have = 0;
-            }
-            if (S.phase == FP_HEADER) {
-                // the magic is judged at 4 bytes, the rest once the header (7 or 15 bytes) is complete
-                int v = 0;
-                bool done = false;
-                for (;;) {
-                    const int need = S.have < 4 ? 4 : S.have < 7 ? 7 : (S.hbuf[4] & 8) ? 15 : 7;
-                    while (S.have < need && q < L) S.hbuf[S.have++] = p[q++];
-                    if (S.have < need) break;
-                    if (need == 4) {
-                        if (fr_rd32(S.hbuf) != FRAME_MAGIC) { v = FR_CORRUPT; break; }
-                        continue;
-                    }
-                    int64_t hp;
-                    int flg, bd;
-                    v = frame_header_check(S.hbuf, S.have, &hp, &flg, &bd);
-                    if (v == FR_CORRUPT && hp + 1 > S.have) { v = 0; continue; }
-                    if (!v && frame_max_block((bd >> 4) & 7) > maxBlockSize) v = FR_DELEGATE;
-                    if (!v) { S.flags = frame_flags_of(flg); S.maxBlock = frame_max_block((bd >> 4) & 7); done = true; }
-                    break;
-                }
-                if (v) { r.status = v; break; }
-                if (!done) break;
-                S.phase = FP_BLOCK;
-                S.have = 0;
-                opened = true;
-            }
-            if (S.phase == FP_BLOCK) {
-                const bool linked = !(S.flags & FR_INDEPENDENT), bc = S.flags & FR_BLOCK_SUM;
-                const int64_t cap = linked ? S.maxBlock : (int64_t)S.maxBlock + 8;
-                if (budget < 0) budget = (dstCap[i] > 0 ? dstCap[i] : 0) / cap - (spent ? spent[i] : 0);
-                const int64_t avail = S.have + (L - q);
-                if (avail < 4) {
-                    if (rows >= budget) break;          // stops before the length code
-                    tailFrom = q; tailAt = S.have; S.have = (int32_t)avail; q = L;
-                    break;
-                }
-                const uint32_t code = fr_vrd32(sp, S.have, p, q, 0);
-                if (code == 0) {                        // the end mark: consumed whatever the budget
-                    q += 4 - S.have;
-                    S.have = 0;
-                    if (!(S.flags & FR_CONTENT_SUM)) { S.phase = FP_IDLE; e.ended = 1; break; }
-                    S.phase = FP_TAIL;
-                } else {
-                    if (rows >= budget) break;
-                    const int64_t blen = code & 0x7FFFFFFFu;
-                    const bool raw = code >> 31;
-                    // a stored block larger than the decoder takes: R_CORRUPT whatever follows (a truncation or a
-                    // checksum mismatch in it is R_CORRUPT too)
-                    if (raw && blen > cap) {
-                        r.err = ((unsigned long long)rows << 4) | FK_RAW;
-                        break;
-                    }
-                    // a compressed block too long to decode within blockCap (frame_lb(stashBody + 1) >
-                    // maxBlockSize + 8): its body is skipped and hashed, its checksum then decides
-                    if (!raw && blen > stashBody) {
-                        q += 4 - S.have;
-                        S.have = 0;
-                        S.skip = (int32_t)blen;
-                        S.phase = FP_SKIP;
-                        skipStart = true;
-                        continue;
-                    }
-                    const int64_t total = 4 + blen + (bc ? 4 : 0);
-                    if (avail < total) {
-                        tailFrom = q; tailAt = S.have; S.have = (int32_t)avail; q = L;
-                        break;
-                    }
-                    if (pass == 1) {
-                        const int64_t b = r.first + rows;
-                        t.srcOff[b] = S.have ? stashRel + (int64_t)s * stashStride + 4 : srcOff[i] + q + 4;
-                        t.len[b] = (int32_t)blen;
-                        t.kind[b] = raw ? RK_RAW : 0;
-                        t.sum[b] = bc ? fr_vrd32(sp, S.have, p, q, 4 + blen) : 0;
-                        t.ckLen[b] = bc ? (int32_t)blen : 0;
-                        if (S.have) {
-                            c.upOff[i] = srcOff[i] + q;
-                            c.upDst[i] = (int64_t)s * stashStride + S.have;
-                            c.upLen[i] = (int32_t)(total - S.have);
-                        }
-                    }
-                    q += total - S.have;
-                    S.have = 0;
-                    rows++;
-                    continue;
-                }
-            }
-            if (S.phase == FP_SKIP) {
-                const bool bc = S.flags & FR_BLOCK_SUM;
-                const int64_t take = S.skip < L - q ? S.skip : L - q;
-                if (bc && take > 0) { sk.srcOff = srcOff[i] + q; sk.len = (int32_t)take; sk.stream = s; }
-                q += take;
-                S.skip -= (int32_t)take;
-                if (S.skip > 0) break;
-                if (!bc) { r.err = ((unsigned long long)rows << 4) | FK_BLOCK; break; }
-                while (S.have < 4 && q < L) S.hbuf[S.have++] = p[q++];
-                if (S.have < 4) break;
-                r.expect = fr_rd32(S.hbuf);
-                e.check = 2;
-                break;
-            }
-            if (S.phase == FP_TAIL) {
-                while (S.have < 4 && q < L) S.hbuf[S.have++] = p[q++];
-                if (S.have < 4) break;
-                r.expect = fr_rd32(S.hbuf);
-                e.check = 1; e.ended = 1;
-                S.phase = FP_IDLE; S.have = 0;
-                break;
-            }
-        }
-    }
-    r.nb = rows;
-    r.flags = S.flags;
-    r.maxBlock = S.maxBlock;
-    e.used = r.status ? 0 : q;
-    if (pass == 0) {
-        r.nslot = stageOff ? rows : 0;
-        fr[i] = r;
-        if (sk.stream >= 0) atomicOr(kinds, FRK_SKIP);
-        if (rows > 0) {
-            atomicMax(&tot->maxSteps, rows);
-            atomicOr(kinds, ((S.flags & FR_INDEPENDENT) ? FRK_INDEP : FRK_LINKED) |
-                                ((S.flags & FR_BLOCK_SUM) ? FRK_BLOCK_SUM : 0) |
-                                ((S.flags & FR_CONTENT_SUM) ? FRK_CONTENT_SUM : 0));
-        }
-        return;
-    }
-    r.pos = e.start;
-    fr[i] = r;
-    ent[i] = e;
-    if (stageOff) stageOff[i] = e.start;
-    const bool tail = !r.status && tailFrom >= 0;
-    c.tailOff[i] = tail ? srcOff[i] + tailFrom : 0;
-    c.tailDst[i] = tail ? (int64_t)s * stashStride + tailAt : 0;
-    c.tailLen[i] = tail ? (int32_t)(q - tailFrom) : 0;
-    skipEnt[i] = sk;
-    if (e.stream < 0 || S.err) return;
-    st[s] = S;
-    if (opened) fr_xxh_reset(xs[s]);
-    if (skipStart) fr_xxh_reset(bxs[s]);
-}
-
-// The arrays of one step, n entries each.
-struct FrStep {
-    int64_t* srcOff;         // the stored bytes, relative to the chunks' base
-    int32_t* lenC; int32_t* lenD;   // compressed length for OP_CHAIN (linked) / OP_DECODE (independent), else 0
-    int32_t* resC; int32_t* resD;   // their results
-    int32_t* kind;           // 0: no block; 1: raw; 2: compressed
-    int32_t* res;            // the bytes the block added (the commit's outLen)
-    int64_t* gDst; int32_t* gLen;   // gather: slot -> cursor
-    FwEntry* xe;             // content checksum: the slot's bytes (frame_writer_xxh_kernel)
-};
-
-// Step k, before the codec: block k of every entry that has one and no verdict at or before it.  Its checksum
-// (verified by xxh32_batch_kernel over all rows) is checked first, then the block goes to the codec table -- the
-// slot at ring + pos (pos 0 for independent frames), the reference's capacity, the history min(pos, 64 KiB) --
-// or, raw, to the copy into the slot (t.copyOff / copyLen).
-__global__ void frame_reader_step_kernel(int k, FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent, int n,
-                                         FrameTable rows, const ChainGroupHdr* __restrict__ hdr, int64_t ring,
-                                         ChainGroupTable t, FrStep s) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const FrameRec& r = fr[i];
-    int32_t kind = 0, len = 0, cap = 0, pre = 0;
-    int64_t at = 0, src = 0;
-    const bool linked = !(r.flags & FR_INDEPENDENT);
-    if (k < r.nb && !r.status && (r.err >> 4) > (unsigned long long)k) {
-        const int64_t b = r.first + k;
-        if (rows.ckLen[b] > 0 && rows.got[b] != rows.sum[b]) {
-            fr[i].err = ((unsigned long long)k << 4) | FK_SUM;
-        } else {
-            const int sm = ent[i].stream;
-            const int64_t pos = linked ? hdr[sm].pos : 0;
-            at = (int64_t)sm * ring + pos;
-            src = rows.srcOff[b];
-            len = rows.len[b];
-            kind = (rows.kind[b] & RK_RAW) ? 1 : 2;
-            cap = linked ? r.maxBlock : r.maxBlock + 8;
-            pre = (int32_t)(pos < CG_WINDOW ? pos : CG_WINDOW);
-        }
-    }
-    s.srcOff[i] = src;
-    s.kind[i] = kind;
-    s.lenC[i] = kind == 2 && linked ? len : 0;
-    s.lenD[i] = kind == 2 && !linked ? len : 0;
-    t.ringOff[i] = at;
-    t.len[i] = kind == 2 ? cap : 0;
-    t.prefix[i] = kind == 2 && linked ? pre : 0;
-    t.copyOff[i] = src;
-    t.copyLen[i] = kind == 1 ? len : 0;
-}
-
-// Step k, after the codec: a rejected block is the verdict -1 at row k; an accepted one is gathered to the cursor,
-// hashed into the content checksum and, in a linked frame, committed to the ring.
-__global__ void frame_reader_post_kernel(int k, FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent, int n,
-                                         ChainGroupTable t, FrStep s) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int kind = s.kind[i];
-    const int flags = fr[i].flags;
-    int32_t res = 0;
-    if (kind == 1) res = t.copyLen[i];
-    else if (kind == 2) res = (flags & FR_INDEPENDENT) ? s.resD[i] : s.resC[i];
-    const bool ok = kind != 0 && res >= 0;
-    if (kind == 2 && res < 0) fr[i].err = ((unsigned long long)k << 4) | FK_BLOCK;
-    int64_t cur = fr[i].pos;
-    s.gDst[i] = cur;
-    s.gLen[i] = ok ? res : 0;
-    if (ok) fr[i].pos = cur + res;
-    s.res[i] = ok ? res : 0;
-    t.stream[i] = ok && !(flags & FR_INDEPENDENT) ? ent[i].stream : -1;
-    FwEntry x = {};
-    x.srcOff = t.ringOff[i];
-    x.len = ok ? res : 0;
-    x.stream = ok && (flags & FR_CONTENT_SUM) ? ent[i].stream : -1;
-    s.xe[i] = x;
-}
-
-// The end of a read: the content checksum of a frame it ended, the verdict (the smallest key; frame.cuh's codes),
-// outLen = the bytes appended or the verdict, srcUsed, frameEnded, and the stream's state: failed (sticky), or,
-// after a frame's end, an empty ring.  rowsOut (nullable): the blocks decoded, for the next sub-read.
-__global__ void frame_reader_finish_kernel(const FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent, int n,
-                                           FrState* __restrict__ st, const FwState* __restrict__ xs,
-                                           const FwState* __restrict__ bxs,
-                                           ChainGroupHdr* __restrict__ hdr, int32_t* __restrict__ outLen,
-                                           int32_t* __restrict__ srcUsed, int32_t* __restrict__ frameEnded,
-                                           int32_t* __restrict__ rowsOut) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const FrameRec r = fr[i];
-    const FrEntry e = ent[i];
-    const int s = e.stream;
-    int32_t out;
-    if (r.status) out = r.status;
-    else {
-        unsigned long long key = r.err;
-        const unsigned long long at = (unsigned long long)r.nb << 4;
-        if (e.check == 1 && fr_digest(xs[s]) != r.expect && (at | FK_SUM) < key) key = at | FK_SUM;
-        if (e.check == 2) {              // the skipped block: its checksum, else the decoder's verdict
-            const unsigned long long k2 = at | (fr_digest(bxs[s]) != r.expect ? FK_SUM : FK_BLOCK);
-            if (k2 < key) key = k2;
-        }
-        if (key != FK_NONE) out = (key & 15) == FK_BLOCK ? -1 : FR_CORRUPT;
-        else out = (int32_t)(r.pos - e.start);
-    }
-    if (s >= 0) {
-        if (out < 0) st[s].err = out;
-        else if (e.ended) hdr[s].pos = 0;
-    }
-    outLen[i] = out;
-    srcUsed[i] = out < 0 ? 0 : (int32_t)e.used;
-    frameEnded[i] = out < 0 ? 0 : e.ended;
-    if (rowsOut) rowsOut[i] = r.nb;
-}
-
-// End (status non-null) or reset: the stream's verdict -- 0 between frames, R_CORRUPT inside one, its sticky
-// error when failed, K4LZ4_E_ARG for an index out of range -- and it becomes new.
-__global__ void frame_reader_end_kernel(const int32_t* __restrict__ streams, int n, int nStreams,
-                                        FrState* __restrict__ st, ChainGroupHdr* __restrict__ hdr,
-                                        int32_t* __restrict__ status) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int s = streams[i];
-    if (s < 0 || s >= nStreams) {
-        if (status) status[i] = FR_ARG;
-        return;
-    }
-    FrState& S = st[s];
-    if (status) status[i] = S.err ? S.err : S.phase == FP_IDLE ? 0 : FR_CORRUPT;
-    S.phase = FP_IDLE;
-    S.have = 0;
-    S.err = 0;
-    hdr[s].pos = 0;
-}
-
-// ---- byte-granular reads (k4lz4_frame_reader_group_read_bytes) -------------------------------------------------
-//
-// ReadManyBytes (Streams/Frames/LZ4FrameReader.blocking.cs:157-179) for the push contract: a read first drains the
-// rest of the stream's current decoded block, then decodes blocks while room is left, appending as much of each as
-// fits; what does not fit stays undrained in the ring for the next read.  The room a block takes is its decoded
-// size, so a read plans in two steps, both before anything decodes:
-//
-// * The plan (one thread per entry, count and fill passes around frame_scan_kernel) continues the stream's phase
-//   like frame_reader_plan_kernel, but takes candidate rows until the lower bounds frame_lb of their sizes cover
-//   the room left after the drain (one row in interactive mode).  Its stops and the stream's state at the first
-//   length code of the call go to an FrCut; the stream's state itself is not written.
-// * block_size_walk_kernel gives each candidate's exact size (the lower bound for a chain that does not parse: the
-//   decoder rejects that block wherever the cut falls), and the cut kernel replays the reference's loop over the
-//   sizes: the rows that decode, whether the plan's last step (end mark, cut block, skipped block, raw block above
-//   its limit) is reached, the stream's new phase, `have`, stash tail and undrained length.  Rows it does not reach
-//   are neither checksummed nor decoded.
-//
-// The undrained bytes are the last FrDrain.len bytes in front of FrDrain.end in the stream's ring.  While a stream
-// holds any, its FrState.err is FR_ARG: frame_reader_plan_kernel then answers a plain read K4LZ4_E_ARG and consumes
-// nothing, and only byte reads, end and reset clear it.  Slides: a linked block that leaves at most 64 KiB
-// undrained slides at once (its undrained bytes stay the last ones in front of pos); one that leaves more keeps
-// pos beyond RING - SLOT and slides when a later read has drained it, before anything else decodes.
-
 struct FrDrain {             // per stream: the undrained rest of its current block, ring[end - len, end)
     int64_t end;
     int32_t len;
@@ -442,59 +94,115 @@ struct FrCut {               // per entry of a byte read: what its plan found, f
     int32_t opened, skipStart, check, ended;
 };
 
+// Copies the plan orders from the chunk into the stash: the rest of a block a previous chunk began (before the
+// checksums) and the tail of the chunk when it ends inside a block (after every decode).
+struct FrCopies { int64_t* upOff; int64_t* upDst; int32_t* upLen; int64_t* tailOff; int64_t* tailDst; int32_t* tailLen; };
+
 // The copies a byte read makes before its first step: the drain (ring -> the entry's output) and a pending slide.
 struct FrPre { int64_t* dOff; int64_t* dDst; int32_t* dLen; int64_t* sOff; int64_t* sDst; int32_t* sLen; };
 
-// One thread per entry; pass 0 counts candidate rows (FrameRec.nb); pass 1 writes the rows (t.frame / t.idx for
-// the walk, rowEnd = chunk bytes consumed up to the end of each), the stash top-up, the FrCut and, for a frame it
-// opens, a fresh content checksum.  staged: the output is placed in a staging buffer once the cut knows its size
-// (frame_reader_bytes_place_kernel), so it starts at 0 here instead of dstOff[i].
-__global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const int32_t* __restrict__ streams,
-                                               const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
-                                               const int32_t* __restrict__ srcLen, const int64_t* __restrict__ dstOff,
-                                               const int32_t* __restrict__ dstCap, int n, int nStreams,
-                                               int32_t maxBlockSize, int32_t stashBody, int64_t stashStride,
-                                               int64_t stashRel, const uint8_t* __restrict__ stash,
-                                               const FrState* __restrict__ st, const FrDrain* __restrict__ drain,
-                                               FwState* __restrict__ xs, FrameRec* __restrict__ fr,
-                                               FrEntry* __restrict__ ent, FrCut* __restrict__ cut, FrameTable t,
-                                               int64_t* __restrict__ rowEnd, FrCopies c, int staged,
-                                               FrameTotals* __restrict__ tot, int32_t* __restrict__ kinds) {
+// Byte j of the current item: the `have` stashed bytes, then the chunk from q on.
+__device__ __forceinline__ uint32_t fr_vbyte(const uint8_t* stash, int have, const uint8_t* p, int64_t q, int64_t j) {
+    return j < have ? stash[j] : p[q + j - have];
+}
+// xxhash.c's XXH32_digest of a streaming state (seed 0).
+__device__ __forceinline__ uint32_t fr_digest(const FwState& f) {
+    uint32_t h = f.total >= 16 ? xx_rotl(f.v[0], 1) + xx_rotl(f.v[1], 7) + xx_rotl(f.v[2], 12) + xx_rotl(f.v[3], 18)
+                               : f.v[2] + XXP5;
+    h += (uint32_t)f.total;
+    return xx_finish(h, f.carry, (size_t)f.carryLen);
+}
+__device__ __forceinline__ void fr_xxh_reset(FwState& x) {
+    x.v[0] = XXP1 + XXP2; x.v[1] = XXP2; x.v[2] = 0; x.v[3] = 0u - XXP1;
+    x.total = 0; x.carryLen = 0;
+}
+__device__ __forceinline__ uint32_t fr_vrd32(const uint8_t* stash, int have, const uint8_t* p, int64_t q, int64_t j) {
+    return fr_vbyte(stash, have, p, q, j) | (fr_vbyte(stash, have, p, q, j + 1) << 8) |
+           (fr_vbyte(stash, have, p, q, j + 2) << 16) | (fr_vbyte(stash, have, p, q, j + 3) << 24);
+}
+
+// The arguments of both plan passes.  t is empty in pass 0.
+struct FrPlan {
+    const int32_t* streams; const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen;
+    const int64_t* dstOff; const int32_t* dstCap;
+    int n, nStreams;
+    int32_t maxBlockSize, stashBody;
+    int64_t stashStride, stashRel;   // stash s is at stash + s * stashStride = srcBase + stashRel + s * stashStride
+    const uint8_t* stash;
+    FrState* st; FwState* xs; FwState* bxs;
+    FrameRec* fr; FrEntry* ent; FrameTable t; FrCopies c;
+    FrameTotals* tot; int32_t* kinds;
+    int64_t* stageOff;       // nullable: the output is staged (host memory), b.dstOff is not used
+    // plain reads
+    const int32_t* spent;    // nullable: blocks earlier sub-reads of the same read decoded
+    int64_t stageSlot;       // staged: entry i's output at FrameRec.slot * stageSlot
+    FwEntry* skipEnt;        // the skipped block's bytes in the chunk, for frame_writer_xxh_kernel over bxs
+    // byte reads
+    int interactive;
+    const FrDrain* drain;
+    FrCut* cut;
+    int64_t* rowEnd;         // per row: chunk bytes consumed up to its end
+};
+
+// One thread per entry.  Pass 0 counts the rows (FrameRec.nb; for a staged plain read nslot = nb, the output
+// placed densely by rows); pass 1, after frame_scan_kernel, walks again and writes the rows, the stash top-up and,
+// for a frame it opens, a fresh content checksum state.  A verdict before any row is FrameRec.status (header,
+// sticky error, stream out of range); one at row k is the error key (k << 4) | kind in FrameRec.err, as frame.cuh
+// keeps it.  The room rule and what the walk leaves behind depend on the read:
+//
+// * Plain (Bytes = false): the room is a budget of floor(dstCap / blockCap) - spent rows, checked before a
+//   non-zero length code and before stashing a partial one; an end mark is consumed whatever the budget.  Pass 1
+//   writes the stream's new state, the tail copy and skipEnt itself.  A stream with undrained bytes (FR_ARG) gets
+//   K4LZ4_E_ARG.
+// * Bytes: the room left after the drain gates every length code, the end mark included; rows are taken while
+//   their lower bounds are below it.  The rows also carry t.frame / t.idx (for block_size_walk_kernel) and rowEnd;
+//   pass 1 writes an FrCut and leaves the stream to the cut kernel.  A staged byte read is placed once the cut
+//   knows its size (frame_reader_place_kernel), so its output starts at 0 here.
+template <bool Bytes>
+__global__ void frame_reader_plan_kernel(int pass, FrPlan a) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int s = streams[i];
+    if (i >= a.n) return;
+    const int s = a.streams[i];
     FrameRec r = {};
     r.err = FK_NONE;
-    if (pass == 1) { r.first = fr[i].first; r.slot = fr[i].slot; }
+    if (pass == 1) { r.first = a.fr[i].first; r.slot = a.fr[i].slot; }
     FrEntry e = {};
-    e.stream = s >= 0 && s < nStreams ? s : -1;
-    e.start = staged ? 0 : dstOff[i];
-    FrCut u = {};
-    u.tailFrom = -1;
-    u.sk.stream = -1;
-    int64_t q = 0, lbSum = 0;
-    int rows = 0;
+    e.stream = s >= 0 && s < a.nStreams ? s : -1;
+    if (Bytes) e.start = a.stageOff ? 0 : a.dstOff[i];
+    else e.start = a.stageOff ? r.slot * a.stageSlot : a.dstOff[i];
     FrState S = {};
     if (e.stream < 0) r.status = FR_ARG;
     else {
-        S = st[s];
-        r.status = S.err == FR_ARG ? 0 : S.err;
+        S = a.st[s];
+        r.status = Bytes && S.err == FR_ARG ? 0 : S.err;
     }
-    const int64_t cap0 = dstCap[i] > 0 ? dstCap[i] : 0;
-    u.drain = !r.status && S.err == FR_ARG ? drain[s].len : 0;
-    u.take = (int32_t)(cap0 < u.drain ? cap0 : u.drain);
-    const int64_t room = cap0 - u.take;
+    const int64_t cap0 = a.dstCap[i] > 0 ? a.dstCap[i] : 0;
+    FrCut u = {};
+    int64_t room = 0, lbSum = 0, budget = -1;
+    if (Bytes) {
+        u.drain = !r.status && S.err == FR_ARG ? a.drain[s].len : 0;
+        u.take = (int32_t)(cap0 < u.drain ? cap0 : u.drain);
+        room = cap0 - u.take;
+    }
+    int64_t q = 0, tailFrom = -1;
+    int32_t tailAt = 0, check = 0, ended = 0;
+    int rows = 0;
+    bool opened = false, skipStart = false;
+    FwEntry sk = {};
+    sk.stream = -1;
     if (!r.status) {
-        const uint8_t* p = srcBase + srcOff[i];
-        const uint8_t* sp = stash + (int64_t)s * stashStride;
-        const int64_t L = srcLen[i] > 0 ? srcLen[i] : 0;
+        const uint8_t* p = a.srcBase + a.srcOff[i];
+        const uint8_t* sp = a.stash + (int64_t)s * a.stashStride;
+        const int64_t L = a.srcLen[i] > 0 ? a.srcLen[i] : 0;
         for (;;) {
             if (S.phase == FP_IDLE) {
                 if (q >= L) break;
                 S.phase = FP_HEADER;
                 S.have = 0;
             }
-            if (S.phase == FP_HEADER) {             // EnsureHeader: before the loop, whatever the room
+            if (S.phase == FP_HEADER) {
+                // the magic is judged at 4 bytes, the rest once the header (7 or 15 bytes) is complete; a byte read
+                // (EnsureHeader) reads it before its loop, whatever the room
                 int v = 0;
                 bool done = false;
                 for (;;) {
@@ -509,7 +217,7 @@ __global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const 
                     int flg, bd;
                     v = frame_header_check(S.hbuf, S.have, &hp, &flg, &bd);
                     if (v == FR_CORRUPT && hp + 1 > S.have) { v = 0; continue; }
-                    if (!v && frame_max_block((bd >> 4) & 7) > maxBlockSize) v = FR_DELEGATE;
+                    if (!v && frame_max_block((bd >> 4) & 7) > a.maxBlockSize) v = FR_DELEGATE;
                     if (!v) { S.flags = frame_flags_of(flg); S.maxBlock = frame_max_block((bd >> 4) & 7); done = true; }
                     break;
                 }
@@ -517,67 +225,81 @@ __global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const 
                 if (!done) break;
                 S.phase = FP_BLOCK;
                 S.have = 0;
-                u.opened = 1;
+                opened = true;
             }
             if (S.phase == FP_BLOCK) {
-                if (!u.gated) {
-                    u.gated = 1;
-                    u.at = S;
-                    u.q0 = q;
-                    u.go = room > 0 && !(interactive && u.take > 0);
-                }
-                // the candidates: the loop can reach this length code only if the rows before it may leave room
-                if (rows == 0 ? !u.go : (interactive || lbSum >= room)) break;
                 const bool bc = S.flags & FR_BLOCK_SUM;
                 const int64_t cap = (S.flags & FR_INDEPENDENT) ? (int64_t)S.maxBlock + 8 : S.maxBlock;
+                bool full = false;
+                if (Bytes) {
+                    if (!u.gated) {
+                        u.gated = 1;
+                        u.at = S;
+                        u.q0 = q;
+                        u.go = room > 0 && !(a.interactive && u.take > 0);
+                    }
+                    // the candidates: the loop can reach this length code only if the rows before it may leave room
+                    if (rows == 0 ? !u.go : (a.interactive || lbSum >= room)) break;
+                } else {
+                    if (budget < 0) budget = cap0 / cap - (a.spent ? a.spent[i] : 0);
+                    full = rows >= budget;
+                }
                 const int64_t avail = S.have + (L - q);
                 if (avail < 4) {
-                    u.tailFrom = q; u.tailAt = S.have; S.have = (int32_t)avail; q = L;
+                    if (full) break;                    // stops before the length code
+                    tailFrom = q; tailAt = S.have; S.have = (int32_t)avail; q = L;
                     break;
                 }
                 const uint32_t code = fr_vrd32(sp, S.have, p, q, 0);
-                if (code == 0) {
+                if (code == 0) {                        // the end mark: a plain read consumes it whatever the budget
                     q += 4 - S.have;
                     S.have = 0;
-                    if (!(S.flags & FR_CONTENT_SUM)) { S.phase = FP_IDLE; u.ended = 1; break; }
+                    if (!(S.flags & FR_CONTENT_SUM)) { S.phase = FP_IDLE; ended = 1; break; }
                     S.phase = FP_TAIL;
                 } else {
+                    if (full) break;
                     const int64_t blen = code & 0x7FFFFFFFu;
                     const bool raw = code >> 31;
+                    // a stored block larger than the decoder takes: R_CORRUPT whatever follows (a truncation or a
+                    // checksum mismatch in it is R_CORRUPT too)
                     if (raw && blen > cap) {
                         r.err = ((unsigned long long)rows << 4) | FK_RAW;
                         break;
                     }
-                    if (!raw && blen > stashBody) {
+                    // a compressed block too long to decode within blockCap (frame_lb(stashBody + 1) >
+                    // maxBlockSize + 8): its body is skipped and hashed, its checksum then decides
+                    if (!raw && blen > a.stashBody) {
                         q += 4 - S.have;
                         S.have = 0;
                         S.skip = (int32_t)blen;
                         S.phase = FP_SKIP;
-                        u.skipStart = 1;
+                        skipStart = true;
                         continue;
                     }
                     const int64_t total = 4 + blen + (bc ? 4 : 0);
                     if (avail < total) {
-                        u.tailFrom = q; u.tailAt = S.have; S.have = (int32_t)avail; q = L;
+                        tailFrom = q; tailAt = S.have; S.have = (int32_t)avail; q = L;
                         break;
                     }
                     if (pass == 1) {
                         const int64_t b = r.first + rows;
-                        t.srcOff[b] = S.have ? stashRel + (int64_t)s * stashStride + 4 : srcOff[i] + q + 4;
-                        t.len[b] = (int32_t)blen;
-                        t.kind[b] = raw ? RK_RAW : 0;
-                        t.sum[b] = bc ? fr_vrd32(sp, S.have, p, q, 4 + blen) : 0;
-                        t.ckLen[b] = bc ? (int32_t)blen : 0;
-                        t.frame[b] = i;
-                        t.idx[b] = rows;
-                        rowEnd[b] = q + total - S.have;
+                        a.t.srcOff[b] = S.have ? a.stashRel + (int64_t)s * a.stashStride + 4 : a.srcOff[i] + q + 4;
+                        a.t.len[b] = (int32_t)blen;
+                        a.t.kind[b] = raw ? RK_RAW : 0;
+                        a.t.sum[b] = bc ? fr_vrd32(sp, S.have, p, q, 4 + blen) : 0;
+                        a.t.ckLen[b] = bc ? (int32_t)blen : 0;
+                        if (Bytes) {
+                            a.t.frame[b] = i;
+                            a.t.idx[b] = rows;
+                            a.rowEnd[b] = q + total - S.have;
+                        }
                         if (S.have) {
-                            c.upOff[i] = srcOff[i] + q;
-                            c.upDst[i] = (int64_t)s * stashStride + S.have;
-                            c.upLen[i] = (int32_t)(total - S.have);
+                            a.c.upOff[i] = a.srcOff[i] + q;
+                            a.c.upDst[i] = (int64_t)s * a.stashStride + S.have;
+                            a.c.upLen[i] = (int32_t)(total - S.have);
                         }
                     }
-                    lbSum += frame_lb(blen, raw);
+                    if (Bytes) lbSum += frame_lb(blen, raw);
                     q += total - S.have;
                     S.have = 0;
                     rows++;
@@ -587,7 +309,7 @@ __global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const 
             if (S.phase == FP_SKIP) {
                 const bool bc = S.flags & FR_BLOCK_SUM;
                 const int64_t take = S.skip < L - q ? S.skip : L - q;
-                if (bc && take > 0) { u.sk.srcOff = srcOff[i] + q; u.sk.len = (int32_t)take; u.sk.stream = s; }
+                if (bc && take > 0) { sk.srcOff = a.srcOff[i] + q; sk.len = (int32_t)take; sk.stream = s; }
                 q += take;
                 S.skip -= (int32_t)take;
                 if (S.skip > 0) break;
@@ -595,14 +317,14 @@ __global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const 
                 while (S.have < 4 && q < L) S.hbuf[S.have++] = p[q++];
                 if (S.have < 4) break;
                 r.expect = fr_rd32(S.hbuf);
-                u.check = 2;
+                check = 2;
                 break;
             }
             if (S.phase == FP_TAIL) {
                 while (S.have < 4 && q < L) S.hbuf[S.have++] = p[q++];
                 if (S.have < 4) break;
                 r.expect = fr_rd32(S.hbuf);
-                u.check = 1; u.ended = 1;
+                check = 1; ended = 1;
                 S.phase = FP_IDLE; S.have = 0;
                 break;
             }
@@ -612,36 +334,57 @@ __global__ void frame_reader_bytes_plan_kernel(int pass, int interactive, const 
     r.flags = S.flags;
     r.maxBlock = S.maxBlock;
     if (pass == 0) {
-        fr[i] = r;
-        if (u.sk.stream >= 0) atomicOr(kinds, FRK_SKIP);
+        if (!Bytes) r.nslot = a.stageOff ? rows : 0;
+        a.fr[i] = r;
+        if (sk.stream >= 0) atomicOr(a.kinds, FRK_SKIP);
         if (rows > 0) {
-            atomicMax(&tot->maxSteps, rows);
-            atomicOr(kinds, ((S.flags & FR_INDEPENDENT) ? FRK_INDEP : FRK_LINKED) |
-                                ((S.flags & FR_BLOCK_SUM) ? FRK_BLOCK_SUM : 0) |
-                                ((S.flags & FR_CONTENT_SUM) ? FRK_CONTENT_SUM : 0));
+            atomicMax(&a.tot->maxSteps, rows);
+            atomicOr(a.kinds, ((S.flags & FR_INDEPENDENT) ? FRK_INDEP : FRK_LINKED) |
+                                  ((S.flags & FR_BLOCK_SUM) ? FRK_BLOCK_SUM : 0) |
+                                  ((S.flags & FR_CONTENT_SUM) ? FRK_CONTENT_SUM : 0));
         }
         return;
     }
     r.pos = e.start;
-    u.fin = S;
-    u.qFin = q;
-    u.err = r.err;
-    u.room = (int32_t)room;
-    if (u.tailFrom >= 0) { u.tailLen = (int32_t)(q - u.tailFrom); u.tailFrom += srcOff[i]; }
-    if (!u.gated) u.at = S;
-    fr[i] = r;
-    ent[i] = e;
-    cut[i] = u;
-    if (u.opened && !r.status) fr_xxh_reset(xs[s]);
+    a.fr[i] = r;
+    if (Bytes) {
+        u.fin = S;
+        u.qFin = q;
+        u.err = r.err;
+        u.room = (int32_t)room;
+        u.sk = sk;
+        u.opened = opened; u.skipStart = skipStart; u.check = check; u.ended = ended;
+        u.tailFrom = tailFrom; u.tailAt = tailAt;
+        if (tailFrom >= 0) { u.tailLen = (int32_t)(q - tailFrom); u.tailFrom += a.srcOff[i]; }
+        if (!u.gated) u.at = S;
+        a.ent[i] = e;
+        a.cut[i] = u;
+        if (opened && !r.status) fr_xxh_reset(a.xs[s]);
+        return;
+    }
+    e.used = r.status ? 0 : q;
+    e.check = check;
+    e.ended = ended;
+    a.ent[i] = e;
+    if (a.stageOff) a.stageOff[i] = e.start;
+    const bool tail = !r.status && tailFrom >= 0;
+    a.c.tailOff[i] = tail ? a.srcOff[i] + tailFrom : 0;
+    a.c.tailDst[i] = tail ? (int64_t)s * a.stashStride + tailAt : 0;
+    a.c.tailLen[i] = tail ? (int32_t)(q - tailFrom) : 0;
+    a.skipEnt[i] = sk;
+    if (e.stream < 0 || S.err) return;
+    a.st[s] = S;
+    if (opened) fr_xxh_reset(a.xs[s]);
+    if (skipStart) fr_xxh_reset(a.bxs[s]);
 }
 
-// One thread per entry, after the walk: the reference's loop over the candidates' sizes -- a row decodes while
-// the rows before it left room (and, interactively, appended nothing), and none of them decoded to 0 bytes.  The
-// plan's last step counts only when the loop reaches it (always, when the call met no length code).  Writes the
-// rows to decode (FrameRec.nb), srcUsed, the stream's state, the tail copy, the skipped bytes to hash, the drain
-// copy, a pending slide, `stopped` (the loop stopped on room, interactive mode or an empty block) and zeroes the
-// checksum lengths of the rows left over.  place (nullable, staged output): FrameRec.nslot = the bytes the entry
-// appends (the rows' walked sizes; a row the decoder rejects appends less) in 16-byte units, nb = 0, for
+// One thread per entry of a byte read, after the walk: the reference's loop over the candidates' sizes -- a row
+// decodes while the rows before it left room (and, interactively, appended nothing), and none of them decoded to
+// 0 bytes.  The plan's last step counts only when the loop reaches it (always, when the call met no length code).
+// Writes the rows to decode (FrameRec.nb), srcUsed, the stream's state, the tail copy, the skipped bytes to hash,
+// the drain copy, a pending slide, `stopped` (the loop stopped on room, interactive mode or an empty block) and
+// zeroes the checksum lengths of the rows left over.  place (nullable, staged output): FrameRec.nslot = the bytes
+// the entry appends (the rows' walked sizes; a row the decoder rejects appends less) in 16-byte units, nb = 0, for
 // frame_scan_kernel.
 __global__ void frame_reader_bytes_cut_kernel(int interactive, FrameRec* __restrict__ fr, FrEntry* __restrict__ ent,
                                               const FrCut* __restrict__ cut, int n, FrameTable t,
@@ -729,8 +472,8 @@ __global__ void frame_reader_bytes_cut_kernel(int interactive, FrameRec* __restr
     ent[i] = e;
 }
 
-// Staged output, after frame_scan_kernel over `place`: entry i's output starts at byte 16 * place[i].slot of the
-// staging buffer; its cursor, its drain copy's destination and stageOff[i] move there.
+// Staged byte read, after frame_scan_kernel over `place`: entry i's output starts at byte 16 * place[i].slot of
+// the staging buffer; its cursor, its drain copy's destination and stageOff[i] move there.
 __global__ void frame_reader_bytes_place_kernel(const FrameRec* __restrict__ place, FrameRec* __restrict__ fr,
                                                 FrEntry* __restrict__ ent, FrPre pre, int64_t* __restrict__ stageOff,
                                                 int n) {
@@ -743,10 +486,61 @@ __global__ void frame_reader_bytes_place_kernel(const FrameRec* __restrict__ pla
     stageOff[i] = at;
 }
 
-// Step k of a byte read, after the codec: as frame_reader_post_kernel, but the gather takes only what fits in the
-// room left (dstCap here is the entry's), and every accepted block -- linked or independent -- goes to the commit.
-__global__ void frame_reader_bytes_post_kernel(int k, FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent,
-                                               const int32_t* __restrict__ dstCap, int n, ChainGroupTable t, FrStep s) {
+// The arrays of one step, n entries each.
+struct FrStep {
+    int64_t* srcOff;         // the stored bytes, relative to the chunks' base
+    int32_t* lenC; int32_t* lenD;   // compressed length for OP_CHAIN (linked) / OP_DECODE (independent), else 0
+    int32_t* resC; int32_t* resD;   // their results
+    int32_t* kind;           // 0: no block; 1: raw; 2: compressed
+    int32_t* res;            // the bytes the block added (the commit's outLen)
+    int64_t* gDst; int32_t* gLen;   // gather: slot -> cursor
+    FwEntry* xe;             // content checksum: the slot's bytes (frame_writer_xxh_kernel)
+};
+
+// Step k, before the codec: block k of every entry that has one and no verdict at or before it.  Its checksum
+// (verified by xxh32_batch_kernel over all rows) is checked first, then the block goes to the codec table -- the
+// slot at ring + pos (pos 0 for independent frames), the reference's capacity, the history min(pos, 64 KiB) --
+// or, raw, to the copy into the slot (t.copyOff / copyLen).
+__global__ void frame_reader_step_kernel(int k, FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent, int n,
+                                         FrameTable rows, const ChainGroupHdr* __restrict__ hdr, int64_t ring,
+                                         ChainGroupTable t, FrStep s) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec& r = fr[i];
+    int32_t kind = 0, len = 0, cap = 0, pre = 0;
+    int64_t at = 0, src = 0;
+    const bool linked = !(r.flags & FR_INDEPENDENT);
+    if (k < r.nb && !r.status && (r.err >> 4) > (unsigned long long)k) {
+        const int64_t b = r.first + k;
+        if (rows.ckLen[b] > 0 && rows.got[b] != rows.sum[b]) {
+            fr[i].err = ((unsigned long long)k << 4) | FK_SUM;
+        } else {
+            const int sm = ent[i].stream;
+            const int64_t pos = linked ? hdr[sm].pos : 0;
+            at = (int64_t)sm * ring + pos;
+            src = rows.srcOff[b];
+            len = rows.len[b];
+            kind = (rows.kind[b] & RK_RAW) ? 1 : 2;
+            cap = linked ? r.maxBlock : r.maxBlock + 8;
+            pre = (int32_t)(pos < CG_WINDOW ? pos : CG_WINDOW);
+        }
+    }
+    s.srcOff[i] = src;
+    s.kind[i] = kind;
+    s.lenC[i] = kind == 2 && linked ? len : 0;
+    s.lenD[i] = kind == 2 && !linked ? len : 0;
+    t.ringOff[i] = at;
+    t.len[i] = kind == 2 ? cap : 0;
+    t.prefix[i] = kind == 2 && linked ? pre : 0;
+    t.copyOff[i] = src;
+    t.copyLen[i] = kind == 1 ? len : 0;
+}
+
+// Step k, after the codec: a rejected block is the verdict -1 at row k; an accepted one is gathered to the cursor
+// -- only what fits in the room left (dstCap here is the entry's); in a plain read the room rule leaves room for
+// every accepted block -- hashed into the content checksum and goes to the commit.
+__global__ void frame_reader_post_kernel(int k, FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent,
+                                         const int32_t* __restrict__ dstCap, int n, ChainGroupTable t, FrStep s) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int kind = s.kind[i];
@@ -771,12 +565,18 @@ __global__ void frame_reader_bytes_post_kernel(int k, FrameRec* __restrict__ fr,
     s.xe[i] = x;
 }
 
-// Step k of a byte read, after the gather and the content checksum: the stream's undrained rest of the block
-// and, in a linked frame, pos += the block and the slide -- unless more than 64 KiB stay undrained, whose slide
-// the cut kernel makes once they are drained.  t.copyOff / ringOff / copyLen: the slide, for copy_blocks_kernel.
-__global__ void frame_reader_bytes_commit_kernel(const FrameRec* __restrict__ fr, int n, int64_t ring, int64_t slot,
-                                                 ChainGroupHdr* __restrict__ hdr, FrDrain* __restrict__ drain,
-                                                 ChainGroupTable t, FrStep s) {
+// Step k, after the gather and the content checksum: the stream's undrained rest of the block and, in a linked
+// frame, pos += the block and the slide -- unless more than 64 KiB stay undrained, whose slide the cut kernel
+// makes once they are drained.  t.copyOff / ringOff / copyLen: the slide, for copy_blocks_kernel.
+//
+// A plain read commits here too, by chain_group_commit_kernel's decode rule: it leaves nothing undrained (left =
+// 0), so a linked block slides when pos + res + SLOT > RING.  The one difference, a block of 0 bytes that slides
+// where the chain kernel would leave pos alone, cannot arise: a plain read always starts with pos + SLOT <= RING,
+// because every commit that leaves pos beyond RING - SLOT leaves undrained bytes, a stream holding them refuses
+// plain reads (FR_ARG), and the cut kernel makes the deferred slide before anything else decodes.
+__global__ void frame_reader_commit_kernel(const FrameRec* __restrict__ fr, int n, int64_t ring, int64_t slot,
+                                           ChainGroupHdr* __restrict__ hdr, FrDrain* __restrict__ drain,
+                                           ChainGroupTable t, FrStep s) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int sm = t.stream[i];
@@ -801,15 +601,63 @@ __global__ void frame_reader_bytes_commit_kernel(const FrameRec* __restrict__ fr
     t.copyLen[i] = slide;
 }
 
-// Before frame_reader_end_kernel in an end or reset: the stream's undrained bytes go, and with them the FR_ARG
-// mark, so that an end inside a frame reports R_CORRUPT.
-__global__ void frame_reader_bytes_end_kernel(const int32_t* __restrict__ streams, int n, int nStreams,
-                                              FrState* __restrict__ st, FrDrain* __restrict__ drain) {
+// The end of a read: the content checksum of a frame it ended, the verdict (the smallest key; frame.cuh's codes),
+// outLen = the bytes appended or the verdict, srcUsed, frameEnded, and the stream's state: failed (sticky), or,
+// after a frame's end, an empty ring.  rowsOut (nullable): the blocks decoded, for the next sub-read.
+__global__ void frame_reader_finish_kernel(const FrameRec* __restrict__ fr, const FrEntry* __restrict__ ent, int n,
+                                           FrState* __restrict__ st, const FwState* __restrict__ xs,
+                                           const FwState* __restrict__ bxs,
+                                           ChainGroupHdr* __restrict__ hdr, int32_t* __restrict__ outLen,
+                                           int32_t* __restrict__ srcUsed, int32_t* __restrict__ frameEnded,
+                                           int32_t* __restrict__ rowsOut) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec r = fr[i];
+    const FrEntry e = ent[i];
+    const int s = e.stream;
+    int32_t out;
+    if (r.status) out = r.status;
+    else {
+        unsigned long long key = r.err;
+        const unsigned long long at = (unsigned long long)r.nb << 4;
+        if (e.check == 1 && fr_digest(xs[s]) != r.expect && (at | FK_SUM) < key) key = at | FK_SUM;
+        if (e.check == 2) {              // the skipped block: its checksum, else the decoder's verdict
+            const unsigned long long k2 = at | (fr_digest(bxs[s]) != r.expect ? FK_SUM : FK_BLOCK);
+            if (k2 < key) key = k2;
+        }
+        if (key != FK_NONE) out = (key & 15) == FK_BLOCK ? -1 : FR_CORRUPT;
+        else out = (int32_t)(r.pos - e.start);
+    }
+    if (s >= 0) {
+        if (out < 0) st[s].err = out;
+        else if (e.ended) hdr[s].pos = 0;
+    }
+    outLen[i] = out;
+    srcUsed[i] = out < 0 ? 0 : (int32_t)e.used;
+    frameEnded[i] = out < 0 ? 0 : e.ended;
+    if (rowsOut) rowsOut[i] = r.nb;
+}
+
+// End (status non-null) or reset: the stream's undrained bytes go, and with them the FR_ARG mark; then its verdict
+// -- 0 between frames, R_CORRUPT inside one, its sticky error when failed, K4LZ4_E_ARG for an index out of range
+// -- and it becomes new.
+__global__ void frame_reader_end_kernel(const int32_t* __restrict__ streams, int n, int nStreams,
+                                        FrState* __restrict__ st, ChainGroupHdr* __restrict__ hdr,
+                                        FrDrain* __restrict__ drain, int32_t* __restrict__ status) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int s = streams[i];
-    if (s < 0 || s >= nStreams) return;
-    if (st[s].err == FR_ARG) st[s].err = 0;
+    if (s < 0 || s >= nStreams) {
+        if (status) status[i] = FR_ARG;
+        return;
+    }
+    FrState& S = st[s];
+    const int32_t err = S.err == FR_ARG ? 0 : S.err;
+    if (status) status[i] = err ? err : S.phase == FP_IDLE ? 0 : FR_CORRUPT;
+    S.phase = FP_IDLE;
+    S.have = 0;
+    S.err = 0;
+    hdr[s].pos = 0;
     drain[s].len = 0;
 }
 

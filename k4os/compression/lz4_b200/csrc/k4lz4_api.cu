@@ -1781,56 +1781,111 @@ struct k4lz4_frame_reader_group : GroupCore {
 
 namespace {
 
-// One read of b.n entries on `st` with every array on the device: plan (count, scan, one host synchronisation for
-// the row and step counts, fill), the top-up copies into the stashes, the block checksums, the steps, the finish,
-// the tail copies.  Host staging (stageOff non-null): the output goes densely to a pool buffer (*stage, FrameRec.slot
-// * stageSlot per entry), b.dstOff is ignored, spent / rowsOut carry the room rule across sub-reads.
-cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* used,
-                      int32_t* ended, const int32_t* spent, int32_t* rowsOut, int64_t* stageOff, uint8_t** stage,
+enum FrMode { FR_END = 0, FR_READ = 1, FR_BYTES = 2, FR_BYTES_INTERACTIVE = 3 };
+
+// One read (FR_READ) or byte read (FR_BYTES*) of b.n entries on `st` with every array on the device: the plan
+// (count, scan, the one host synchronisation for the rows and steps, fill), the top-up copies into the stashes;
+// for a byte read the walk of the candidate rows, the cut, the drain and pending slides; the skipped blocks' and
+// the block checksums, the steps (each: step, copy, codec, post, gather, content checksum, commit, slide), the
+// finish, the tail copies.  Host staging (stageOff non-null; b.dstOff is ignored): a plain read places its output
+// densely in a pool buffer (*stage) by rows x (maxBlockSize + 8); a byte read waits a second time, once the cut
+// knows each entry's output size, and places it 16-aligned in a buffer of the bytes the read appends.  spent (plain
+// reads, nullable): the blocks earlier sub-reads decoded.  more (nullable): per entry, for the next sub-read --
+// plain: the blocks decoded; byte read: 1 when it stopped on room, interactive mode or an empty block.
+cudaError_t fr_device(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t* streams, int32_t* used,
+                      int32_t* ended, const int32_t* spent, int32_t* more, int64_t* stageOff, uint8_t** stage,
                       FramePool& P, cudaStream_t st) {
     const int n = (int)b.n;
-    const int64_t stageSlot = (int64_t)g->maxBlockSize + 8;
+    const bool bytes = mode != FR_READ;
+    const int interactive = mode == FR_BYTES_INTERACTIVE;
     struct Tot { k4::FrameTotals t; int32_t kinds; };
-    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
-    k4::FrEntry* ent = P.get<k4::FrEntry>(n);
-    k4::FwEntry* skipEnt = P.get<k4::FwEntry>(n);
+    k4::FrPlan a{};
+    a.streams = streams; a.srcBase = b.srcBase; a.srcOff = b.srcOff; a.srcLen = b.srcLen;
+    a.dstOff = b.dstOff; a.dstCap = b.dstCap; a.n = n; a.nStreams = g->nStreams;
+    a.maxBlockSize = g->maxBlockSize; a.stashBody = g->stashBody; a.stashStride = g->stashStride;
+    a.stashRel = (int64_t)((uintptr_t)g->stash - (uintptr_t)b.srcBase);
+    a.stash = g->stash; a.st = g->st; a.xs = g->xs; a.bxs = g->bxs; a.stageOff = stageOff;
+    a.spent = spent; a.stageSlot = (int64_t)g->maxBlockSize + 8;
+    a.interactive = interactive; a.drain = g->drain;
+    a.fr = P.get<k4::FrameRec>(n);
+    a.ent = P.get<k4::FrEntry>(n);
+    a.skipEnt = P.get<k4::FwEntry>(n);
     Tot* tot = P.get<Tot>(1);
-    k4::FrCopies c;
+    a.tot = &tot->t; a.kinds = &tot->kinds;
+    k4::FrCopies& c = a.c;
     c.upOff = P.get<int64_t>(n); c.upDst = P.get<int64_t>(n); c.upLen = P.get<int32_t>(n);
     c.tailOff = P.get<int64_t>(n); c.tailDst = P.get<int64_t>(n); c.tailLen = P.get<int32_t>(n);
+    k4::FrameRec* walkFr = nullptr;                    // the walk's error keys: the cut and the decoder decide
+    k4::FrPre pre{};
+    if (bytes) {
+        walkFr = P.get<k4::FrameRec>(n);
+        a.cut = P.get<k4::FrCut>(n);
+        pre.dOff = P.get<int64_t>(n); pre.dDst = P.get<int64_t>(n); pre.dLen = P.get<int32_t>(n);
+        pre.sOff = P.get<int64_t>(n); pre.sDst = P.get<int64_t>(n); pre.sLen = P.get<int32_t>(n);
+        if (!more) more = P.get<int32_t>(n);
+    }
     FR_TRY(P.err);
     FR_TRY(cudaMemsetAsync(tot, 0, sizeof(Tot), st));
     FR_TRY(cudaMemsetAsync(c.upLen, 0, (size_t)n * 4, st));
-    const int64_t stashRel = (int64_t)((uintptr_t)g->stash - (uintptr_t)b.srcBase);
-    auto plan = [&](int pass, const k4::FrameTable& t) {
-        k4::frame_reader_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, streams, b.srcBase, b.srcOff, b.srcLen, b.dstOff,
-                                                                b.dstCap, spent, n, g->nStreams, g->maxBlockSize,
-                                                                g->stashBody, g->stashStride, stashRel, g->stash, g->st,
-                                                                g->xs, g->bxs, skipEnt, fr, ent, t, c, stageOff,
-                                                                stageSlot, &tot->t,
-                                                                &tot->kinds);
+    auto plan = [&](int pass) {
+        if (bytes) k4::frame_reader_plan_kernel<true><<<grid_of(n), 128, 0, st>>>(pass, a);
+        else k4::frame_reader_plan_kernel<false><<<grid_of(n), 128, 0, st>>>(pass, a);
         g_launches++;
     };
-    plan(0, k4::FrameTable{});
+    plan(0);
     FR_LAUNCH();
-    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, &tot->t, stageOff ? 1 : 0);
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(a.fr, n, &tot->t, !bytes && stageOff ? 1 : 0);
     FR_LAUNCH();
     g_launches++;
     Tot h{};
     FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
-    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the rows, the steps, the staged output
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the rows, the steps, a plain read's staging
     const int64_t nB = h.t.blocks;
-    k4::FrameTable t{};
+    k4::FrameTable& t = a.t;
     t.srcOff = P.get<int64_t>(nB); t.len = P.get<int32_t>(nB); t.kind = P.get<int32_t>(nB);
     t.sum = P.get<uint32_t>(nB); t.ckLen = P.get<int32_t>(nB); t.got = P.get<uint32_t>(nB);
+    k4::FrameRec* place = nullptr;
+    k4::FrameTotals* placeTot = nullptr;
+    if (bytes) {
+        t.frame = P.get<int32_t>(nB); t.idx = P.get<int32_t>(nB); t.size = P.get<int32_t>(nB);
+        a.rowEnd = P.get<int64_t>(nB);
+        if (stageOff) { place = P.get<k4::FrameRec>(n); placeTot = P.get<k4::FrameTotals>(1); }
+    }
     uint8_t* dstBase = b.dstBase;
-    if (stageOff) *stage = dstBase = P.get<uint8_t>(h.t.slots * stageSlot);
+    if (stageOff && !bytes) *stage = dstBase = P.get<uint8_t>(h.t.slots * a.stageSlot);
     FR_TRY(P.err);
-    plan(1, t);
+    plan(1);
     FR_LAUNCH();
     FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.upOff, c.upLen, g->stash, c.upDst, nullptr, nullptr, n}, st));
+    if (bytes) {
+        if (nB > 0) {
+            k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, walkFr);
+            FR_LAUNCH();
+            g_launches++;
+        }
+        k4::frame_reader_bytes_cut_kernel<<<grid_of(n), 128, 0, st>>>(interactive, a.fr, a.ent, a.cut, n, t, a.rowEnd,
+                                                                       g->st, g->bxs, a.skipEnt, g->drain, g->hdr,
+                                                                       g->ring, g->slot, g->stashStride, c, pre, more,
+                                                                       place);
+        FR_LAUNCH();
+        g_launches++;
+        if (stageOff) {          // host staging only: a second wait, for the bytes the read appends
+            k4::frame_scan_kernel<<<1, 1024, 0, st>>>(place, n, placeTot, 1);
+            FR_LAUNCH();
+            k4::FrameTotals pt{};
+            FR_TRY(cudaMemcpyAsync(&pt, placeTot, sizeof(pt), cudaMemcpyDeviceToHost, st));
+            FR_TRY(cudaStreamSynchronize(st));
+            *stage = dstBase = P.get<uint8_t>(pt.slots * 16);
+            FR_TRY(P.err);
+            k4::frame_reader_bytes_place_kernel<<<grid_of(n), 128, 0, st>>>(place, a.fr, a.ent, pre, stageOff, n);
+            FR_LAUNCH();
+            g_launches += 2;
+        }
+        FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.dOff, pre.dLen, dstBase, pre.dDst, nullptr, nullptr, n}, st));
+        FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.sOff, pre.sLen, g->rings, pre.sDst, nullptr, nullptr, n}, st));
+    }
     if (h.kinds & k4::FRK_SKIP) {
-        k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, skipEnt, n, g->bxs);
+        k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, a.skipEnt, n, g->bxs);
         FR_LAUNCH();
         g_launches++;
     }
@@ -1847,7 +1902,7 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t
         const k4::ChainGroupTable ct = carve_table(tab, n);
         const bool linked = h.kinds & k4::FRK_LINKED, indep = h.kinds & k4::FRK_INDEP;
         for (int k = 0; k < h.t.maxSteps; k++) {
-            k4::frame_reader_step_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, t, g->hdr, g->ring, ct, s);
+            k4::frame_reader_step_kernel<<<grid_of(n), 128, 0, st>>>(k, a.fr, a.ent, n, t, g->hdr, g->ring, ct, s);
             FR_LAUNCH();
             g_launches++;
             FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
@@ -1857,7 +1912,7 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t
                 FR_TRY(launch_op(OP_CHAIN, kb, st));
             }
             if (indep) FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, s.srcOff, s.lenD, g->rings, ct.ringOff, ct.len, s.resD, n}, st));
-            k4::frame_reader_post_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, ct, s);
+            k4::frame_reader_post_kernel<<<grid_of(n), 128, 0, st>>>(k, a.fr, a.ent, b.dstCap, n, ct, s);
             FR_LAUNCH();
             g_launches++;
             FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.ringOff, s.gLen, dstBase, s.gDst, nullptr, nullptr, n}, st));
@@ -1866,244 +1921,46 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t
                 FR_LAUNCH();
                 g_launches++;
             }
-            if (linked) FR_TRY(group_commit(g, k4::CG_DECODE, s.res, n, ct, st));   // pos += the block and the slide
-        }
-    }
-    k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen, used,
-                                                              ended,
-                                                              rowsOut);
-    FR_LAUNCH();
-    g_launches++;
-    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.tailOff, c.tailLen, g->stash, c.tailDst, nullptr, nullptr, n}, st));
-    return cudaSuccess;
-}
-
-// Host memory, synchronous.  One sub-read of entries idx[k], piece[k] chunk bytes from at[k] of theirs, spent[k]
-// blocks already decoded (the table's aux): stage_up, the device path staging the output densely in a pool buffer
-// (alive until the gather is enqueued), and stage_down of outLen used ended rows to the caller at dstOff + wrote[k].
-int fr_host_part(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, const std::vector<int64_t>& idx,
-                 const std::vector<int64_t>& at, const std::vector<int64_t>& piece, const std::vector<int32_t>& spent,
-                 const std::vector<int64_t>& wrote, std::vector<int32_t>& res, std::vector<int32_t>& used,
-                 std::vector<int32_t>& ended, std::vector<int32_t>& rows, cudaStream_t st) {
-    const Dev* D = dev_state(g->device);
-    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
-    const int64_t m = (int64_t)idx.size();
-    StageUp up;
-    const int rc = stage_up(g, m, 4, m * 8, [&](int64_t k) {
-        return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[idx[k]] + at[k] : nullptr, piece[k], 0, streams[idx[k]],
-                     (int32_t)piece[k], b.dstCap[idx[k]], spent[(size_t)k]};
-    }, up, st);
-    if (rc != K4LZ4_OK) return rc;
-    int64_t* dOff = (int64_t*)up.extra;
-    uint8_t* stage = nullptr;
-    FramePool P(D->pool, st);
-    const Batch kb{up.src, up.srcOff, up.len, nullptr, nullptr, up.cap, up.res, m};
-    const cudaError_t e = fr_device(g, kb, up.stream, up.res + m, up.res + 2 * m, up.aux, up.res + 3 * m, dOff, &stage,
-                                    P, st);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
-    std::vector<int32_t> down((size_t)m * 4);
-    const int rd = stage_down(g, up, m, down.data(), 4, stage, dOff, nullptr,
-                              [&](int64_t k) { return b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k]; }, st);
-    if (rd != K4LZ4_OK) return rd;
-    res.assign(down.begin(), down.begin() + m);
-    used.assign(down.begin() + m, down.begin() + 2 * m);
-    ended.assign(down.begin() + 2 * m, down.begin() + 3 * m);
-    rows.assign(down.begin() + 3 * m, down.end());
-    return K4LZ4_OK;
-}
-
-// Host memory: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order.  An entry goes on from where it
-// stopped while it consumed something, ended no frame, failed nothing and has bytes left; the blocks it decoded
-// count against its room in the next sub-read.  So cutting a read in two changes nothing: a sub-read that stopped
-// at a length code cut by its piece sees the whole code in the next one.  The first sub-read lists every entry.
-int fr_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* srcUsed, int32_t* frameEnded,
-            cudaStream_t st) {
-    const int64_t n = b.n;
-    std::vector<int64_t> usedTot((size_t)n, 0), outTot((size_t)n, 0);
-    std::vector<int32_t> spentTot((size_t)n, 0);
-    std::vector<uint8_t> active((size_t)n, 1);
-    for (int64_t i = 0; i < n; i++) { b.outLen[i] = 0; srcUsed[i] = 0; frameEnded[i] = 0; }
-    for (bool first = true;; first = false) {
-        std::vector<int64_t> idx, at, piece, wrote;
-        std::vector<int32_t> spent;
-        int64_t budget = FW_STAGE_BYTES;
-        for (int64_t i = 0; i < n; i++) {
-            if (!active[(size_t)i]) continue;
-            if (!first && budget == 0) break;
-            const int64_t take = std::min(src_size(b, i) - usedTot[(size_t)i], budget);
-            if (!first && take <= 0) { active[(size_t)i] = 0; continue; }
-            idx.push_back(i); at.push_back(usedTot[(size_t)i]); piece.push_back(take);
-            spent.push_back(spentTot[(size_t)i]); wrote.push_back(outTot[(size_t)i]);
-            budget -= take;
-        }
-        if (idx.empty()) break;
-        std::vector<int32_t> res, used, ended, rows;
-        const int rc = fr_host_part(g, b, streams, idx, at, piece, spent, wrote, res, used, ended, rows, st);
-        if (rc != K4LZ4_OK) return rc;
-        for (size_t k = 0; k < idx.size(); k++) {
-            const int64_t i = idx[k];
-            if (res[k] < 0) { b.outLen[i] = res[k]; active[(size_t)i] = 0; continue; }
-            outTot[(size_t)i] += res[k];
-            usedTot[(size_t)i] += used[k];
-            spentTot[(size_t)i] += rows[k];
-            b.outLen[i] = (int32_t)outTot[(size_t)i];
-            srcUsed[i] = (int32_t)usedTot[(size_t)i];
-            frameEnded[i] = ended[k];
-            // a sub-read that stopped short of its piece stopped at the room rule; only a length code cut by the
-            // piece may still be an end mark
-            const int64_t end = at[k] + piece[k];
-            const bool more = used[k] == piece[k] || (end < src_size(b, i) && end - usedTot[(size_t)i] < 4);
-            if (ended[k] || usedTot[(size_t)i] >= src_size(b, i) || !more) active[(size_t)i] = 0;
-        }
-    }
-    return K4LZ4_OK;
-}
-
-// One byte read (k4lz4_frame_reader_group_read_bytes, frame_reader.cuh) of b.n entries on `st` with every array
-// on the device: plan (count, scan, the one host synchronisation, fill), the stash top-ups, the walk of the
-// candidate rows, the cut, the drain and pending slides, the checksums, the steps (each: step, copy, codec, post,
-// gather, content checksum, commit, slide), the finish, the tail copies.  Host staging (stageOff non-null): once
-// the cut knows each entry's output size, a second wait sizes a pool buffer (*stage) by the bytes the read
-// appends, the entries are placed in it densely (16-aligned, offsets in stageOff) and b.dstOff is ignored.
-// stopped: per entry, 1 when the read stopped on room, interactive mode or an empty block (for the next sub-read).
-cudaError_t frb_device(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* used,
-                       int32_t* ended, int interactive, int32_t* stopped, int64_t* stageOff, uint8_t** stage,
-                       FramePool& P, cudaStream_t st) {
-    const int n = (int)b.n;
-    struct Tot { k4::FrameTotals t; int32_t kinds; };
-    k4::FrameRec* fr = P.get<k4::FrameRec>(n);
-    k4::FrameRec* walkFr = P.get<k4::FrameRec>(n);     // the walk's error keys: the cut and the decoder decide
-    k4::FrEntry* ent = P.get<k4::FrEntry>(n);
-    k4::FrCut* cut = P.get<k4::FrCut>(n);
-    k4::FwEntry* skipEnt = P.get<k4::FwEntry>(n);
-    Tot* tot = P.get<Tot>(1);
-    k4::FrCopies c;
-    c.upOff = P.get<int64_t>(n); c.upDst = P.get<int64_t>(n); c.upLen = P.get<int32_t>(n);
-    c.tailOff = P.get<int64_t>(n); c.tailDst = P.get<int64_t>(n); c.tailLen = P.get<int32_t>(n);
-    k4::FrPre pre;
-    pre.dOff = P.get<int64_t>(n); pre.dDst = P.get<int64_t>(n); pre.dLen = P.get<int32_t>(n);
-    pre.sOff = P.get<int64_t>(n); pre.sDst = P.get<int64_t>(n); pre.sLen = P.get<int32_t>(n);
-    FR_TRY(P.err);
-    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(Tot), st));
-    FR_TRY(cudaMemsetAsync(c.upLen, 0, (size_t)n * 4, st));
-    const int64_t stashRel = (int64_t)((uintptr_t)g->stash - (uintptr_t)b.srcBase);
-    auto plan = [&](int pass, const k4::FrameTable& t, int64_t* rowEnd) {
-        k4::frame_reader_bytes_plan_kernel<<<grid_of(n), 128, 0, st>>>(
-            pass, interactive, streams, b.srcBase, b.srcOff, b.srcLen, b.dstOff, b.dstCap, n, g->nStreams,
-            g->maxBlockSize, g->stashBody, g->stashStride, stashRel, g->stash, g->st, g->drain, g->xs, fr, ent, cut, t,
-            rowEnd, c, stageOff ? 1 : 0, &tot->t, &tot->kinds);
-        g_launches++;
-    };
-    plan(0, k4::FrameTable{}, nullptr);
-    FR_LAUNCH();
-    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, &tot->t, 0);
-    FR_LAUNCH();
-    g_launches++;
-    Tot h{};
-    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
-    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the candidate rows and the steps
-    const int64_t nB = h.t.blocks;
-    k4::FrameTable t{};
-    t.srcOff = P.get<int64_t>(nB); t.len = P.get<int32_t>(nB); t.kind = P.get<int32_t>(nB);
-    t.sum = P.get<uint32_t>(nB); t.ckLen = P.get<int32_t>(nB); t.got = P.get<uint32_t>(nB);
-    t.frame = P.get<int32_t>(nB); t.idx = P.get<int32_t>(nB); t.size = P.get<int32_t>(nB);
-    int64_t* rowEnd = P.get<int64_t>(nB);
-    k4::FrameRec* place = stageOff ? P.get<k4::FrameRec>(n) : nullptr;
-    k4::FrameTotals* placeTot = stageOff ? P.get<k4::FrameTotals>(1) : nullptr;
-    uint8_t* dstBase = b.dstBase;
-    FR_TRY(P.err);
-    plan(1, t, rowEnd);
-    FR_LAUNCH();
-    FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.upOff, c.upLen, g->stash, c.upDst, nullptr, nullptr, n}, st));
-    if (nB > 0) {
-        k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, walkFr);
-        FR_LAUNCH();
-        g_launches++;
-    }
-    k4::frame_reader_bytes_cut_kernel<<<grid_of(n), 128, 0, st>>>(interactive, fr, ent, cut, n, t, rowEnd, g->st,
-                                                                   g->bxs, skipEnt, g->drain, g->hdr, g->ring, g->slot,
-                                                                   g->stashStride, c, pre, stopped, place);
-    FR_LAUNCH();
-    g_launches++;
-    if (stageOff) {              // host staging only: a second wait, for the bytes the read appends
-        k4::frame_scan_kernel<<<1, 1024, 0, st>>>(place, n, placeTot, 1);
-        FR_LAUNCH();
-        k4::FrameTotals pt{};
-        FR_TRY(cudaMemcpyAsync(&pt, placeTot, sizeof(pt), cudaMemcpyDeviceToHost, st));
-        FR_TRY(cudaStreamSynchronize(st));
-        *stage = dstBase = P.get<uint8_t>(pt.slots * 16);
-        FR_TRY(P.err);
-        k4::frame_reader_bytes_place_kernel<<<grid_of(n), 128, 0, st>>>(place, fr, ent, pre, stageOff, n);
-        FR_LAUNCH();
-        g_launches += 2;
-    }
-    FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.dOff, pre.dLen, dstBase, pre.dDst, nullptr, nullptr, n}, st));
-    FR_TRY(launch_op(OP_COPY, Batch{g->rings, pre.sOff, pre.sLen, g->rings, pre.sDst, nullptr, nullptr, n}, st));
-    if (h.kinds & k4::FRK_SKIP) {
-        k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(b.srcBase, skipEnt, n, g->bxs);
-        FR_LAUNCH();
-        g_launches++;
-    }
-    if (nB > 0 && (h.kinds & k4::FRK_BLOCK_SUM))
-        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nB}, st));
-    if (h.t.maxSteps > 0) {
-        uint8_t* tab = P.get<uint8_t>((int64_t)n * TABLE_BYTES);
-        k4::FrStep s;
-        s.srcOff = P.get<int64_t>(n); s.gDst = P.get<int64_t>(n);
-        s.lenC = P.get<int32_t>(n); s.lenD = P.get<int32_t>(n); s.resC = P.get<int32_t>(n); s.resD = P.get<int32_t>(n);
-        s.kind = P.get<int32_t>(n); s.res = P.get<int32_t>(n); s.gLen = P.get<int32_t>(n);
-        s.xe = P.get<k4::FwEntry>(n);
-        FR_TRY(P.err);
-        const k4::ChainGroupTable ct = carve_table(tab, n);
-        const bool linked = h.kinds & k4::FRK_LINKED, indep = h.kinds & k4::FRK_INDEP;
-        for (int k = 0; k < h.t.maxSteps; k++) {
-            k4::frame_reader_step_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, n, t, g->hdr, g->ring, ct, s);
-            FR_LAUNCH();
-            g_launches++;
-            FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
-            if (linked) {
-                Batch kb{b.srcBase, s.srcOff, s.lenC, g->rings, ct.ringOff, ct.len, s.resC, n};
-                kb.prefixLen = ct.prefix;
-                FR_TRY(launch_op(OP_CHAIN, kb, st));
-            }
-            if (indep) FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, s.srcOff, s.lenD, g->rings, ct.ringOff, ct.len, s.resD, n}, st));
-            k4::frame_reader_bytes_post_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, ent, b.dstCap, n, ct, s);
-            FR_LAUNCH();
-            g_launches++;
-            FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.ringOff, s.gLen, dstBase, s.gDst, nullptr, nullptr, n}, st));
-            if (h.kinds & k4::FRK_CONTENT_SUM) {
-                k4::frame_writer_xxh_kernel<<<grid_of((int64_t)n * 4), 128, 0, st>>>(g->rings, s.xe, n, g->xs);
+            // a plain read of independent blocks only has nothing to commit: it leaves neither history nor
+            // undrained bytes
+            if (bytes || linked) {
+                k4::frame_reader_commit_kernel<<<grid_of(n), 128, 0, st>>>(a.fr, n, g->ring, g->slot, g->hdr, g->drain,
+                                                                           ct, s);
                 FR_LAUNCH();
                 g_launches++;
             }
-            k4::frame_reader_bytes_commit_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, g->ring, g->slot, g->hdr, g->drain,
-                                                                             ct, s);
-            FR_LAUNCH();
-            g_launches++;
             if (linked)
                 FR_TRY(launch_op(OP_COPY, Batch{g->rings, ct.copyOff, ct.copyLen, g->rings, ct.ringOff, nullptr, nullptr, n}, st));
         }
     }
-    k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen, used,
-                                                              ended, nullptr);
+    k4::frame_reader_finish_kernel<<<grid_of(n), 128, 0, st>>>(a.fr, a.ent, n, g->st, g->xs, g->bxs, g->hdr, b.outLen,
+                                                              used, ended, bytes ? nullptr : more);
     FR_LAUNCH();
     g_launches++;
     FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.tailOff, c.tailLen, g->stash, c.tailDst, nullptr, nullptr, n}, st));
     return cudaSuccess;
 }
 
-// Host memory, synchronous: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order, as fr_host.  Each
-// sub-read gets the room the earlier ones left (dstCap minus the bytes they appended) and its output comes down
-// behind it, exactly outLen bytes per entry.  An entry goes on while its sub-read ran to the end of its piece
-// (it did not stop on room, interactive mode or an empty block), ended no frame, failed nothing and has bytes
-// left -- and, interactively, appended nothing yet.  The first sub-read lists every entry, so that a read of an
-// empty chunk still drains.
-int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams, int32_t* srcUsed,
-             int32_t* frameEnded, int interactive, cudaStream_t st) {
+// Host memory, synchronous: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order.  Each sub-read is
+// one fr_device call on stage_up's table -- cap / aux: a plain read's dstCap and the blocks earlier sub-reads
+// decoded, or the room a byte read has left (dstCap minus the bytes earlier sub-reads appended) -- and its output
+// comes down behind it, exactly outLen bytes per entry.  The first sub-read lists every entry, so that a byte read
+// of an empty chunk still drains.  An entry goes on from where it stopped while it ended no frame, failed nothing
+// and has bytes left, and:
+// * plain: it consumed its whole piece, or stopped less than 4 bytes before the piece's end inside its chunk.  A
+//   sub-read that stopped short of its piece stopped at the room rule, but it consumes an end mark without room, so
+//   a length code cut by the piece must be seen whole in the next sub-read.
+// * bytes: it did not stop on room, interactive mode or an empty block (a byte read never reads a code once it is
+//   out of room) and, interactively, appended nothing yet.
+// So cutting a read in two changes nothing.
+int fr_host(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t* streams, int32_t* srcUsed,
+            int32_t* frameEnded, cudaStream_t st) {
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
+    const bool bytes = mode != FR_READ;
     const int64_t n = b.n;
     std::vector<int64_t> usedTot((size_t)n, 0), outTot((size_t)n, 0);
+    std::vector<int32_t> spentTot((size_t)n, 0);
     std::vector<uint8_t> active((size_t)n, 1);
     for (int64_t i = 0; i < n; i++) { b.outLen[i] = 0; srcUsed[i] = 0; frameEnded[i] = 0; }
     for (bool first = true;; first = false) {
@@ -2124,7 +1981,7 @@ int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams
             const int64_t i = idx[(size_t)k];
             const int64_t room = std::max<int64_t>(b.dstCap[i], 0) - outTot[(size_t)i];
             return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[i] + at[k] : nullptr, piece[k], 0, streams[i],
-                         (int32_t)piece[k], (int32_t)room, 0};
+                         (int32_t)piece[k], bytes ? (int32_t)room : b.dstCap[i], bytes ? 0 : spentTot[(size_t)i]};
         }, up, st);
         if (rc != K4LZ4_OK) return rc;
         int64_t* dOff = (int64_t*)up.extra;
@@ -2133,7 +1990,7 @@ int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams
         {
             FramePool P(D->pool, st);
             const Batch kb{up.src, up.srcOff, up.len, nullptr, nullptr, up.cap, up.res, m};
-            e = frb_device(g, kb, up.stream, up.res + m, up.res + 2 * m, interactive, up.res + 3 * m, dOff, &stage, P, st);
+            e = fr_device(g, mode, kb, up.stream, up.res + m, up.res + 2 * m, up.aux, up.res + 3 * m, dOff, &stage, P, st);
             if (e == cudaSuccess) {
                 std::vector<int32_t> down((size_t)m * 4);
                 const int rd = stage_down(g, up, m, down.data(), 4, stage, dOff, nullptr, [&](int64_t k) {
@@ -2143,15 +2000,22 @@ int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams
                 for (int64_t k = 0; k < m; k++) {
                     const int64_t i = idx[(size_t)k];
                     const int32_t res = down[(size_t)k], used = down[(size_t)(m + k)];
-                    const int32_t ended = down[(size_t)(2 * m + k)], stopped = down[(size_t)(3 * m + k)];
+                    const int32_t ended = down[(size_t)(2 * m + k)], more = down[(size_t)(3 * m + k)];
                     if (res < 0) { b.outLen[i] = res; active[(size_t)i] = 0; continue; }
                     outTot[(size_t)i] += res;
                     usedTot[(size_t)i] += used;
                     b.outLen[i] = (int32_t)outTot[(size_t)i];
                     srcUsed[i] = (int32_t)usedTot[(size_t)i];
                     frameEnded[i] = ended;
-                    if (stopped || ended || usedTot[(size_t)i] >= src_size(b, i) || (interactive && outTot[(size_t)i] > 0))
-                        active[(size_t)i] = 0;
+                    bool stop;
+                    if (bytes) {
+                        stop = more || (mode == FR_BYTES_INTERACTIVE && outTot[(size_t)i] > 0);
+                    } else {
+                        spentTot[(size_t)i] += more;
+                        const int64_t end = at[(size_t)k] + piece[(size_t)k];
+                        stop = used != piece[(size_t)k] && (end >= src_size(b, i) || end - usedTot[(size_t)i] >= 4);
+                    }
+                    if (stop || ended || usedTot[(size_t)i] >= src_size(b, i)) active[(size_t)i] = 0;
                 }
             }
         }
@@ -2159,8 +2023,6 @@ int frb_host(k4lz4_frame_reader_group* g, const Batch& b, const int32_t* streams
     }
     return K4LZ4_OK;
 }
-
-enum FrMode { FR_END = 0, FR_READ = 1, FR_BYTES = 2, FR_BYTES_INTERACTIVE = 3 };
 
 // A read, a byte read, or an end (b.outLen = the statuses).  Device memory: enqueued on `stream`; a read waits
 // once.  mode -1: a byte read with unknown flags (K4LZ4_E_ARG after the pointer and stream checks).
@@ -2178,9 +2040,8 @@ int fr_run(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t*
         return group_streams_run(g, streams, n, memKind, stream, [&](const int32_t* ds, cudaStream_t st) {
             const bool host = memKind == K4LZ4_MEM_HOST;
             int32_t* dStatus = host ? (int32_t*)g->dStage.p + n : b.outLen;
-            k4::frame_reader_bytes_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->drain);
-            k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, dStatus);
-            g_launches += 2;
+            k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, g->drain, dStatus);
+            g_launches++;
             cudaError_t e = cudaGetLastError();
             if (e == cudaSuccess && host) e = cudaMemcpyAsync(b.outLen, dStatus, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
             return e;
@@ -2188,23 +2049,13 @@ int fr_run(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t*
     DeviceGuard guard(g->device);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", g->device);
     cudaStream_t st = (cudaStream_t)stream;
-    const bool bytes = mode != FR_READ;
-    const int interactive = mode == FR_BYTES_INTERACTIVE;
-    if (memKind == K4LZ4_MEM_HOST)
-        return bytes ? frb_host(g, b, streams, srcUsed, frameEnded, interactive, st)
-                     : fr_host(g, b, streams, srcUsed, frameEnded, st);
+    if (memKind == K4LZ4_MEM_HOST) return fr_host(g, mode, b, streams, srcUsed, frameEnded, st);
     const Dev* D = dev_state(g->device);
     if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d setup failed", g->device);
     cudaError_t e;
     {
         FramePool P(D->pool, st);
-        if (bytes) {
-            int32_t* stopped = P.get<int32_t>(n);
-            e = P.err;
-            if (e == cudaSuccess) e = frb_device(g, b, streams, srcUsed, frameEnded, interactive, stopped, nullptr, nullptr, P, st);
-        } else {
-            e = fr_device(g, b, streams, srcUsed, frameEnded, nullptr, nullptr, nullptr, nullptr, P, st);
-        }
+        e = fr_device(g, mode, b, streams, srcUsed, frameEnded, nullptr, nullptr, nullptr, nullptr, P, st);
     }
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame reader step: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
@@ -2600,9 +2451,8 @@ int32_t k4lz4_frame_reader_group_destroy(k4lz4_frame_reader_group* g) { return g
 int32_t k4lz4_frame_reader_group_reset(k4lz4_frame_reader_group* g, const int32_t* streams, int32_t n, int32_t memKind,
                                        void* cudaStream) {
     return group_reset(g, streams, n, memKind, cudaStream, [&](const int32_t* ds, cudaStream_t st) {
-        k4::frame_reader_bytes_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->drain);
-        k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, nullptr);
-        g_launches += 2;
+        k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, g->drain, nullptr);
+        g_launches++;
         return cudaGetLastError();
     });
 }

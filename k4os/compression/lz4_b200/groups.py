@@ -240,25 +240,14 @@ class FrameReaderGroup(_Group):
         """chunks[i] is fed to stream streams[i] (default: stream i) with caps[i] bytes of room.  -> (list of
         content each entry decoded, int32 results: bytes appended or the verdict, int32 bytes consumed, int32 1
         where the entry ended a frame)."""
-        src, so, sl = _pack(chunks)
-        s = self._streams(streams, len(sl))
-        dst, do, dc = _slots(caps)
-        out = np.full(len(sl), -1, dtype=np.int32)
-        used = np.zeros(len(sl), dtype=np.int32)
-        ended = np.zeros(len(sl), dtype=np.int32)
-        N.check(N.lib().k4lz4_frame_reader_group_read(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
-                                                      sl.ctypes.data, used.ctypes.data, dst.ctypes.data,
-                                                      do.ctypes.data, dc.ctypes.data, out.ctypes.data,
-                                                      ended.ctypes.data, len(sl), N.MEM_HOST, None))
-        return _slices(dst, do, out), out, used, ended
+        return self._read(chunks, caps, streams, None)
 
     def read_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int, src_used_ptr: int,
                     dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int, frame_ended_ptr: int, n: int,
                     stream: int = 0) -> None:
         """Device-pointer form of read: enqueues work on `stream` (and waits once for the row and step counts)."""
-        N.check(N.lib().k4lz4_frame_reader_group_read(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
-                                                      src_used_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr, out_len_ptr,
-                                                      frame_ended_ptr, int(n), N.MEM_DEVICE, stream or None))
+        self._call(None, streams_ptr, src_ptr, src_off_ptr, src_len_ptr, src_used_ptr, dst_ptr, dst_off_ptr,
+                   dst_cap_ptr, out_len_ptr, frame_ended_ptr, int(n), mem=N.MEM_DEVICE, stream=stream or None)
 
     def read_bytes(self, chunks: Sequence, caps: Sequence[int], streams: Sequence[int] | None = None,
                    interactive: bool = False):
@@ -266,26 +255,34 @@ class FrameReaderGroup(_Group):
         current block, then decodes blocks while room is left; what does not fit stays on the device for the next
         call (k4lz4_frame_reader_group_read_bytes).  interactive: stop after the first drain that appended
         anything.  -> as read."""
+        return self._read(chunks, caps, streams, N.READ_INTERACTIVE if interactive else 0)
+
+    def read_bytes_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int,
+                          src_used_ptr: int, dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int,
+                          frame_ended_ptr: int, n: int, interactive: bool = False, stream: int = 0) -> None:
+        """Device-pointer form of read_bytes: enqueues work on `stream` (and waits once for the candidate rows)."""
+        self._call(N.READ_INTERACTIVE if interactive else 0, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
+                   src_used_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr, out_len_ptr, frame_ended_ptr, int(n),
+                   mem=N.MEM_DEVICE, stream=stream or None)
+
+    def _call(self, flags, *args, mem, stream):
+        """k4lz4_frame_reader_group_read (flags None) or _read_bytes with these flags."""
+        if flags is None:
+            N.check(N.lib().k4lz4_frame_reader_group_read(self.handle, *args, mem, stream))
+        else:
+            N.check(N.lib().k4lz4_frame_reader_group_read_bytes(self.handle, *args, flags, mem, stream))
+
+    def _read(self, chunks, caps, streams, flags):
         src, so, sl = _pack(chunks)
         s = self._streams(streams, len(sl))
         dst, do, dc = _slots(caps)
         out = np.full(len(sl), -1, dtype=np.int32)
         used = np.zeros(len(sl), dtype=np.int32)
         ended = np.zeros(len(sl), dtype=np.int32)
-        N.check(N.lib().k4lz4_frame_reader_group_read_bytes(
-            self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data, sl.ctypes.data, used.ctypes.data,
-            dst.ctypes.data, do.ctypes.data, dc.ctypes.data, out.ctypes.data, ended.ctypes.data, len(sl),
-            N.READ_INTERACTIVE if interactive else 0, N.MEM_HOST, None))
+        self._call(flags, s.ctypes.data, src.ctypes.data, so.ctypes.data, sl.ctypes.data, used.ctypes.data,
+                   dst.ctypes.data, do.ctypes.data, dc.ctypes.data, out.ctypes.data, ended.ctypes.data, len(sl),
+                   mem=N.MEM_HOST, stream=None)
         return _slices(dst, do, out), out, used, ended
-
-    def read_bytes_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int,
-                          src_used_ptr: int, dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int,
-                          frame_ended_ptr: int, n: int, interactive: bool = False, stream: int = 0) -> None:
-        """Device-pointer form of read_bytes: enqueues work on `stream` (and waits once for the candidate rows)."""
-        N.check(N.lib().k4lz4_frame_reader_group_read_bytes(
-            self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr, src_used_ptr, dst_ptr, dst_off_ptr,
-            dst_cap_ptr, out_len_ptr, frame_ended_ptr, int(n), N.READ_INTERACTIVE if interactive else 0,
-            N.MEM_DEVICE, stream or None))
 
     def end(self, streams: Sequence[int] | None = None) -> np.ndarray:
         """The input of streams (default: all) has ended.  -> int32 statuses: 0 between frames, R_CORRUPT inside a

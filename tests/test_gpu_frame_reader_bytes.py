@@ -244,7 +244,7 @@ def test_int32_max_cap_through_host_staging(k4, eng):
 def test_host_read_over_256_mib_in_sub_reads(k4, eng, interactive):
     """One host read whose chunks total more than 256 MiB, so that it runs as several sub-reads, at small and large
     caps and a second read from where the first stopped: every entry equals the push model and the same reads
-    through device memory."""
+    through device memory.  Plain reads too, whose room in blocks carries over from one sub-read to the next."""
     up, ref, _, dec = eng
     rng = np.random.default_rng(23)
     noise = rng.integers(0, 256, 24 << 20, dtype=np.uint8).tobytes()
@@ -257,19 +257,26 @@ def test_host_read_over_256_mib_in_sub_reads(k4, eng, interactive):
         fr, _ = k4.LZ4Frame.EncodeMany([d], 65536, not s & 1, bool(s & 2), bool(s & 4))
         blobs.append(fr[0])
     assert sum(len(b) for b in blobs) > 300 << 20
-    for cap in (4096, 16 << 20):
+    arms = [(cap, False) for cap in (4096, 16 << 20)]
+    if not interactive:
+        arms += [(cap, True) for cap in (1 << 20, 16 << 20)]
+    for cap, plain in arms:
         models = [RB.BytesReader(65536, dec, ref.xxh32) for _ in range(S)]
         at = [0] * S
         streams = list(range(S))[::-1]
         with k4.FrameReaderGroup(S, 65536) as gh, k4.FrameReaderGroup(S, 65536) as gd:
             for rnd in range(2):
                 chunks = [blobs[s][at[s]:] for s in streams]
-                got, out, used, ended = gh.read_bytes(chunks, [cap] * S, streams, interactive=interactive)
-                dout, dused, dended, dgot = call(k4, gd, "device", streams, chunks, [cap] * S, interactive)
+                if plain:
+                    got, out, used, ended = gh.read(chunks, [cap] * S, streams)
+                else:
+                    got, out, used, ended = gh.read_bytes(chunks, [cap] * S, streams, interactive=interactive)
+                dout, dused, dended, dgot = call(k4, gd, "device", streams, chunks, [cap] * S, interactive, plain)
                 assert out.tolist() == dout.tolist() and used.tolist() == dused.tolist()
                 assert ended.tolist() == dended.tolist() and got == dgot
                 for k, s in enumerate(streams):
-                    want = models[s].read_bytes(chunks[k], cap, interactive)
-                    assert (out[k], used[k], ended[k]) == want[:3], (cap, rnd, s, want[:3])
-                    assert got[k] == want[3], (cap, rnd, s)
+                    m = models[s]
+                    want = m.read(chunks[k], cap) if plain else m.read_bytes(chunks[k], cap, interactive)
+                    assert (out[k], used[k], ended[k]) == want[:3], (cap, plain, rnd, s, want[:3])
+                    assert got[k] == want[3], (cap, plain, rnd, s)
                     at[s] += int(used[k])
