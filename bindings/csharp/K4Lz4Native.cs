@@ -86,6 +86,29 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_pickle_writer_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
             int* outLen, int nMessages, int level, int memKind, void* cudaStream, int device);
+        // the other encoders' twins under LZ4Codec.Enforce32: pick the export from LL.Algorithm at each call
+        [DllImport(Lib)] public static extern int k4lz4_encode_chain_batch_x32(
+            byte* srcBase, long* srcOff, int* srcLen, int* prefixLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* stateBase, long* stateOff, int* outLen, int nBlocks, int level, int memKind, void* cudaStream,
+            int device);
+        [DllImport(Lib)] public static extern int k4lz4_chain_group_encode_x32(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* dstCap, int* outLen, int n, int level, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_pickle_batch_x32(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* outLen, int nMessages, int level, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_pickle_writer_batch_x32(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* outLen, int nMessages, int level, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_encode_batch_x32(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* outLen, int nFrames, int blockSize, int flags, int level, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_write_x32(
+            void* group, int* streams, byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
+            int* dstCap, int* outLen, int n, int memKind, void* cudaStream);
+        [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_close_x32(
+            void* group, int* streams, byte* dstBase, long* dstOff, int* dstCap, int* outLen, int n, int memKind,
+            void* cudaStream);
 
         // LZ4Frame.Encode / Decode over whole buffers, batched across frames (k4lz4.h "LZ4 Frame")
         public const int FRAME_INDEPENDENT = 1, FRAME_BLOCK_CHECKSUM = 2, FRAME_CONTENT_CHECKSUM = 4;

@@ -110,7 +110,10 @@ K4LZ4_API int32_t k4lz4_encode_batch(const uint8_t *srcBase, const int64_t *srcO
 /* The same two calls with the reference's global LL.Enforce32 switch set (Engine/LL.tools.cs:29-36,
  * LZ4Codec.cs:21-25): the 32-bit engine LL32.  Its output differs from LL64's only for inputs of
  * >= 65 547 bytes (4 096-entry u32 table with hash4 instead of hash5, LL64.tools.cs:135-143 vs
- * LL32); below that both engines emit identical bytes and these calls equal the plain ones. */
+ * LL32); below that both engines emit identical bytes and these calls equal the plain ones.
+ * Every encoder call has such an _x32 twin: the same arguments, checks in the same order and result codes;
+ * only the engine differs.  The reference reads the switch at every encode call (Engine/LLxx.cs:65-91), so a
+ * caller picks the export per call.  Decoders need no twin: both engines decode alike. */
 K4LZ4_API int32_t k4lz4_encode_x32(const uint8_t *src, int32_t srcLen, uint8_t *dst, int32_t dstCap, int32_t level);
 K4LZ4_API int32_t k4lz4_encode_batch_x32(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
                                          uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
@@ -176,7 +179,8 @@ K4LZ4_API int32_t k4lz4_decode_chain_batch(const uint8_t *srcBase, const int64_t
  * stateBase + stateOff[i] (K4LZ4_CHAIN_STATE_BYTES, 16-aligned) is read and advanced.  The dictionary the
  * block sees is min(state.dictSize, prefixLen[i]) bytes, which is LZ4_saveDict's clamp: a caller that moves
  * its history (a ring buffer) passes the bytes it kept and never writes the state.  At most 65 535 history
- * bytes are read, never written.  Every block size up to 2 GiB uses the same u32 table (hash5).
+ * bytes are read, never written.  Every block size up to 2 GiB uses the same u32 table (hash5; hash4 in the
+ * _x32 twin below).
  * outLen[i] = bytes written; 0 for srcLen <= 0 and K4LZ4_R_DELEGATE for level >= 3, both with the state
  * untouched; -1 where LZ4FastChainEncoder.Encode would throw (the engine returned 0: the block does not fit
  * dstCap), with the state advanced exactly as the reference's is.
@@ -194,6 +198,14 @@ K4LZ4_API int32_t k4lz4_encode_chain_batch(const uint8_t *srcBase, const int64_t
                                            uint8_t *stateBase, const int64_t *stateOff,
                                            int32_t *outLen, int32_t nBlocks, int32_t level,
                                            int32_t memKind, void *cudaStream, int32_t device);
+/* The same under LL.Enforce32 (LL32.LZ4_compress_fast_continue): hash4 over 4 bytes for the u32 table, for every
+ * block size.  The state record is the same, so one stream may alternate between the two calls. */
+K4LZ4_API int32_t k4lz4_encode_chain_batch_x32(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                               const int32_t *prefixLen,
+                                               uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                               uint8_t *stateBase, const int64_t *stateOff,
+                                               int32_t *outLen, int32_t nBlocks, int32_t level,
+                                               int32_t memKind, void *cudaStream, int32_t device);
 
 /* ---- chain groups: chained streams whose context stays on the GPU ---------------------------- */
 
@@ -248,6 +260,12 @@ K4LZ4_API int32_t k4lz4_chain_group_encode(k4lz4_chain_group *g, const int32_t *
                                            uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
                                            int32_t *outLen, int32_t n, int32_t level,
                                            int32_t memKind, void *cudaStream);
+/* The same with the 32-bit engine (k4lz4_encode_chain_batch_x32).  The engine is chosen per call, not per group. */
+K4LZ4_API int32_t k4lz4_chain_group_encode_x32(k4lz4_chain_group *g, const int32_t *streams,
+                                               const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                               uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                               int32_t *outLen, int32_t n, int32_t level,
+                                               int32_t memKind, void *cudaStream);
 K4LZ4_API int32_t k4lz4_chain_group_decode(k4lz4_chain_group *g, const int32_t *streams,
                                            const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
                                            uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
@@ -312,6 +330,12 @@ K4LZ4_API int32_t k4lz4_frame_encode_batch(const uint8_t *srcBase, const int64_t
                                            uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
                                            int32_t *outLen, int32_t nFrames, int32_t blockSize, int32_t flags,
                                            int32_t level, int32_t memKind, void *cudaStream, int32_t device);
+/* The same with the 32-bit engine: linked blocks as k4lz4_encode_chain_batch_x32, independent blocks as
+ * k4lz4_encode_batch_x32 (identical to the plain call below 65 547-byte blocks). */
+K4LZ4_API int32_t k4lz4_frame_encode_batch_x32(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                               uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                               int32_t *outLen, int32_t nFrames, int32_t blockSize, int32_t flags,
+                                               int32_t level, int32_t memKind, void *cudaStream, int32_t device);
 
 /* The decoded length of every frame, to size the buffers of k4lz4_frame_decode_batch (as k4lz4_unpickled_size_batch
  * does for k4lz4_unpickle_batch).  outSize[i] = the content length from the blocks' length codes and token chains,
@@ -394,6 +418,16 @@ K4LZ4_API int32_t k4lz4_frame_writer_group_write(k4lz4_frame_writer_group *g, co
 K4LZ4_API int32_t k4lz4_frame_writer_group_close(k4lz4_frame_writer_group *g, const int32_t *streams,
                                                  uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
                                                  int32_t *outLen, int32_t n, int32_t memKind, void *cudaStream);
+/* Write and close with the 32-bit engine (the blocks as k4lz4_frame_encode_batch_x32 encodes them).  The engine is
+ * chosen per call, not per group: each call's blocks use its own, and streams keep one state layout for both. */
+K4LZ4_API int32_t k4lz4_frame_writer_group_write_x32(k4lz4_frame_writer_group *g, const int32_t *streams,
+                                                     const uint8_t *srcBase, const int64_t *srcOff,
+                                                     const int32_t *srcLen, uint8_t *dstBase, const int64_t *dstOff,
+                                                     const int32_t *dstCap, int32_t *outLen, int32_t n,
+                                                     int32_t memKind, void *cudaStream);
+K4LZ4_API int32_t k4lz4_frame_writer_group_close_x32(k4lz4_frame_writer_group *g, const int32_t *streams,
+                                                     uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                                     int32_t *outLen, int32_t n, int32_t memKind, void *cudaStream);
 /* The most one write of `length` bytes appends: 7 + floor((B - 1 + length) / B) * (4 + B + 4 with block
  * checksums).  K4LZ4_E_ARG for a null group or a negative length. */
 K4LZ4_API int64_t k4lz4_frame_writer_bound(const k4lz4_frame_writer_group *g, int64_t length);
@@ -511,6 +545,12 @@ K4LZ4_API int32_t k4lz4_pickle_batch(const uint8_t *srcBase, const int64_t *srcO
                                      uint8_t *dstBase, const int64_t *dstOff,
                                      int32_t *outLen, int32_t nMessages, int32_t level,
                                      int32_t memKind, void *cudaStream, int32_t device);
+/* The same under LL.Enforce32: messages of >= 65 547 bytes are encoded by the 32-bit engine (LZ4Codec.Encode,
+ * k4lz4_encode_x32); shorter ones give the plain call's bytes.  Likewise k4lz4_pickle_writer_batch_x32 below. */
+K4LZ4_API int32_t k4lz4_pickle_batch_x32(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                         uint8_t *dstBase, const int64_t *dstOff,
+                                         int32_t *outLen, int32_t nMessages, int32_t level,
+                                         int32_t memKind, void *cudaStream, int32_t device);
 
 /* LZ4Pickler.Pickle<TBufferWriter>(ReadOnlySpan<byte>, writer, level) -- LZ4Pickler.pickle.cs:113-148.
  * Different bytes than the byte[] variant: the header width is chosen from the full length before
@@ -522,6 +562,10 @@ K4LZ4_API int32_t k4lz4_pickle_writer_batch(const uint8_t *srcBase, const int64_
                                             uint8_t *dstBase, const int64_t *dstOff,
                                             int32_t *outLen, int32_t nMessages, int32_t level,
                                             int32_t memKind, void *cudaStream, int32_t device);
+K4LZ4_API int32_t k4lz4_pickle_writer_batch_x32(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                uint8_t *dstBase, const int64_t *dstOff,
+                                                int32_t *outLen, int32_t nMessages, int32_t level,
+                                                int32_t memKind, void *cudaStream, int32_t device);
 
 /* LZ4Pickler.UnpickledSize(ReadOnlySpan<byte>) -- LZ4Pickler.unpickle.cs:83-92,131-148.
  * outSize[i] = unpickled size, or K4LZ4_R_CORRUPT where the reference throws. */

@@ -36,13 +36,16 @@ inline int check_codec(int r) {
 
 struct LZ4Codec {
     static constexpr int Version = 192;                                            // LZ4Codec.cs:13
+    // LZ4Codec.Enforce32 (LZ4Codec.cs:21-25): every encode below that starts while it is set uses the 32-bit engine
+    // (the k4lz4_*_x32 exports), as the reference reads its switch at each call.  Decoding is unaffected.
+    static inline bool Enforce32 = false;
     static int MaximumOutputSize(int length) { return k4lz4_max_output_size(length); }   // :30-31
 
     // LZ4Codec.Encode(byte*,int,byte*,int,LZ4Level) -- LZ4Codec.cs:40-52
     static int Encode(const uint8_t* source, int sourceLength, uint8_t* target, int targetLength,
                       LZ4Level level = LZ4Level::L00_FAST) {
         if (sourceLength <= 0) return 0;
-        const int r = check_codec(k4lz4_encode(source, sourceLength, target, targetLength, (int)level));
+        const int r = check_codec((Enforce32 ? k4lz4_encode_x32 : k4lz4_encode)(source, sourceLength, target, targetLength, (int)level));
         if (r == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("HC/OPT levels stay with the managed engine");
         return r;
     }
@@ -115,7 +118,7 @@ public:
         std::vector<int32_t> sl((size_t)nb), cap((size_t)nb, bound), res((size_t)nb, -1);
         for (int i = 0; i < nb; i++) { so[(size_t)i] = (int64_t)i * block_; dof[(size_t)i] = (int64_t)i * bound; sl[(size_t)i] = fill_[(size_t)i]; }
         std::vector<uint8_t> dst((size_t)nb * bound);
-        const int rc = k4lz4_encode_batch(buf_.data(), so.data(), sl.data(), dst.data(), dof.data(), cap.data(),
+        const int rc = (LZ4Codec::Enforce32 ? k4lz4_encode_batch_x32 : k4lz4_encode_batch)(buf_.data(), so.data(), sl.data(), dst.data(), dof.data(), cap.data(),
                                           res.data(), nb, (int)level_, K4LZ4_MEM_HOST, nullptr, K4LZ4_ALL_DEVICES);
         if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
         for (int i = 0; i < nb; i++) {
@@ -252,7 +255,7 @@ public:
     void Encode(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                 uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int n,
                 LZ4Level level = LZ4Level::L00_FAST, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
-        check(k4lz4_chain_group_encode(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
+        check((LZ4Codec::Enforce32 ? k4lz4_chain_group_encode_x32 : k4lz4_chain_group_encode)(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
                                        (int)level, memKind, cudaStream));
     }
     std::vector<uint8_t> State(int stream) const {
@@ -304,12 +307,12 @@ public:
     void Write(const int32_t* streams, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int n,
                int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
-        check(k4lz4_frame_writer_group_write(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
+        check((LZ4Codec::Enforce32 ? k4lz4_frame_writer_group_write_x32 : k4lz4_frame_writer_group_write)(g_, streams, srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n,
                                              memKind, cudaStream));
     }
     void Close(const int32_t* streams, uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
                int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
-        check(k4lz4_frame_writer_group_close(g_, streams, dstBase, dstOff, dstCap, outLen, n, memKind, cudaStream));
+        check((LZ4Codec::Enforce32 ? k4lz4_frame_writer_group_close_x32 : k4lz4_frame_writer_group_close)(g_, streams, dstBase, dstOff, dstCap, outLen, n, memKind, cudaStream));
     }
     void Reset(const int32_t* streams, int n, int memKind = K4LZ4_MEM_HOST, void* cudaStream = nullptr) {
         check(k4lz4_frame_writer_group_reset(g_, streams, n, memKind, cudaStream));
@@ -368,7 +371,7 @@ struct LZ4Pickler {
         if (length == 0) return {};
         std::vector<uint8_t> out((size_t)k4lz4_pickle_bound(length));
         int64_t so = 0, dof = 0; int32_t n = length, r = -1;
-        const int rc = k4lz4_pickle_batch(source, &so, &n, out.data(), &dof, &r, 1, (int)level, K4LZ4_MEM_HOST, nullptr, 0);
+        const int rc = (LZ4Codec::Enforce32 ? k4lz4_pickle_batch_x32 : k4lz4_pickle_batch)(source, &so, &n, out.data(), &dof, &r, 1, (int)level, K4LZ4_MEM_HOST, nullptr, 0);
         if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
         if (r == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("HC/OPT levels stay with the managed engine");
         out.resize((size_t)r);
@@ -428,7 +431,7 @@ struct LZ4Frame {
             dofs[i] = d; dc[i] = (int32_t)Bound(sl[i], s); d += dc[i];
         }
         src.resize(src.size() + 1); dst.resize((size_t)d + 1);
-        const int rc = k4lz4_frame_encode_batch(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
+        const int rc = (LZ4Codec::Enforce32 ? k4lz4_frame_encode_batch_x32 : k4lz4_frame_encode_batch)(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
                                                 out.data(), (int32_t)n, s.blockSize, flags(s), (int)s.level,
                                                 K4LZ4_MEM_HOST, nullptr, device);
         if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());

@@ -45,9 +45,12 @@ SIGNATURES = {
     "k4lz4_decode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
+    "k4lz4_encode_chain_batch_x32": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_unpickle_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_pickle_batch": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),
+    "k4lz4_pickle_batch_x32": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_pickle_writer_batch": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),
+    "k4lz4_pickle_writer_batch_x32": ([_vp] * 6 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_unpickled_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_xxh32": ([_vp, _i64, _u32], _u32),
     "k4lz4_xxh32_batch": ([_vp, _vp, _vp, _u32, _vp, _i32] + _CALL, _i32),
@@ -60,19 +63,23 @@ SIGNATURES = {
     "k4lz4_chain_group_destroy": ([_vp], _i32),
     "k4lz4_chain_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
     "k4lz4_chain_group_encode": ([_vp] * 9 + [_i32, _i32, _i32, _vp], _i32),
+    "k4lz4_chain_group_encode_x32": ([_vp] * 9 + [_i32, _i32, _i32, _vp], _i32),
     "k4lz4_chain_group_decode": ([_vp] * 9 + [_i32, _i32, _vp], _i32),
     "k4lz4_chain_group_inject": ([_vp] * 5 + [_i32, _i32, _vp], _i32),
     "k4lz4_chain_group_state": ([_vp, _i32, _vp], _i32),
     "k4lz4_chain_group_history": ([_vp, _i32, _vp, _i32], _i32),
     "k4lz4_frame_bound": ([_i64, _i32, _i32], _i64),
     "k4lz4_frame_encode_batch": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
+    "k4lz4_frame_encode_batch_x32": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
     "k4lz4_frame_content_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_frame_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_frame_writer_group_create": ([_i32, _i32, _i32, _i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_destroy": ([_vp], _i32),
     "k4lz4_frame_writer_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_write": ([_vp] * 9 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_group_write_x32": ([_vp] * 9 + [_i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_close": ([_vp] * 6 + [_i32, _i32, _vp], _i32),
+    "k4lz4_frame_writer_group_close_x32": ([_vp] * 6 + [_i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_bound": ([_vp, _i64], _i64),
     "k4lz4_frame_writer_close_bound": ([_vp], _i64),
     "k4lz4_frame_reader_group_create": ([_i32, _i32, _i32, _vp], _i32),

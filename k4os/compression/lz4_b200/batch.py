@@ -26,14 +26,19 @@ def _i32(a) -> np.ndarray:
     return np.ascontiguousarray(a, dtype=np.int32)
 
 
+def encoder_fn(name: str, x32: bool):
+    """The export `name` of an encoder call, or its _x32 twin (the 32-bit engine, LZ4Codec.Enforce32)."""
+    return getattr(N.lib(), name + "_x32" if x32 else name)
+
+
 # ---- flat host API: caller supplies base buffers + offset/length arrays ------------------------
 
 def encode_batch_flat_host(src: np.ndarray, src_off, src_len, dst: np.ndarray, dst_off, dst_cap,
-                           level: int = 0, device: int = 0) -> np.ndarray:
+                           level: int = 0, device: int = 0, x32: bool = False) -> np.ndarray:
     src_off, dst_off, src_len, dst_cap = _i64(src_off), _i64(dst_off), _i32(src_len), _i32(dst_cap)
     n = int(src_len.shape[0])
     out = np.full(n, -1, dtype=np.int32)
-    N.check(N.lib().k4lz4_encode_batch(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
+    N.check(encoder_fn("k4lz4_encode_batch", x32)(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
                                        dst.ctypes.data, dst_off.ctypes.data, dst_cap.ctypes.data,
                                        out.ctypes.data, n, int(level), N.MEM_HOST, None, int(device)))
     return out
@@ -97,27 +102,27 @@ def decode_batch_host(blocks: Sequence, caps: Sequence[int], device: int = 0):
     return _slices(dst, do, out), out
 
 
-def pickle_batch_host(messages: Sequence, level: int = 0, device: int = 0):
-    """LZ4Pickler.Pickle over a batch -> (list[bytes], outLen int32[n])."""
+def pickle_batch_host(messages: Sequence, level: int = 0, device: int = 0, x32: bool = False):
+    """LZ4Pickler.Pickle over a batch -> (list[bytes], outLen int32[n]); x32: the 32-bit engine."""
     src, so, sl = _pack(messages)
     n = len(sl)
     dst, do, _ = _slots(np.where(sl > 0, sl + 1, 0))
     out = np.full(n, -1, dtype=np.int32)
-    N.check(N.lib().k4lz4_pickle_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
+    N.check(encoder_fn("k4lz4_pickle_batch", x32)(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
                                        dst.ctypes.data, do.ctypes.data, out.ctypes.data,
                                        n, int(level), N.MEM_HOST, None, int(device)))
     return _slices(dst, do, out), out
 
 
-def pickle_writer_batch_host(messages: Sequence, level: int = 0, device: int = 0):
+def pickle_writer_batch_host(messages: Sequence, level: int = 0, device: int = 0, x32: bool = False):
     """LZ4Pickler.Pickle<TBufferWriter> over a batch -> (list[bytes], outLen int32[n]): what the
-    reference would have advanced each writer by (LZ4Pickler.pickle.cs:113-148)."""
+    reference would have advanced each writer by (LZ4Pickler.pickle.cs:113-148); x32: the 32-bit engine."""
     src, so, sl = _pack(messages)
     n = len(sl)
     L = N.lib()
     dst, do, _ = _slots([L.k4lz4_pickle_writer_bound(int(v)) for v in sl])
     out = np.full(n, -1, dtype=np.int32)
-    N.check(L.k4lz4_pickle_writer_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
+    N.check(encoder_fn("k4lz4_pickle_writer_batch", x32)(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
                                         dst.ctypes.data, do.ctypes.data, out.ctypes.data,
                                         n, int(level), N.MEM_HOST, None, int(device)))
     return _slices(dst, do, out), out
@@ -177,8 +182,8 @@ def decode_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_pt
 
 
 def pickle_batch_device(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, out_len_ptr, n,
-                        level: int = 0, stream: int = 0, device: int = -1) -> None:
-    N.check(N.lib().k4lz4_pickle_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr,
+                        level: int = 0, stream: int = 0, device: int = -1, x32: bool = False) -> None:
+    N.check(encoder_fn("k4lz4_pickle_batch", x32)(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr,
                                        out_len_ptr, int(n), int(level), N.MEM_DEVICE,
                                        stream or None, int(device)))
 
@@ -304,18 +309,18 @@ def partial_decode_batch_host(blocks: Sequence, targets: Sequence[int], device: 
 
 
 def encode_chain_batch_host(src: np.ndarray, src_off, src_len, prefix_len, dst: np.ndarray, dst_off, dst_cap,
-                            state: np.ndarray, state_off, level: int = 0, device: int = 0) -> np.ndarray:
+                            state: np.ndarray, state_off, level: int = 0, device: int = 0, x32: bool = False) -> np.ndarray:
     """LZ4FastChainEncoder's block encode over a batch of streams (k4lz4_encode_chain_batch, host memory).
     Block i encodes src[src_off[i] .. + src_len[i]) behind the prefix_len[i] bytes in front of it (its stream's
     history) into dst[dst_off[i] .. + dst_cap[i]), reading and advancing the 16 400-byte state record at
     state[state_off[i]] (16-aligned; all zero = a new stream).  One block per stream per call.  Returns int32
     results: bytes written, 0 for an empty block, -1 where Encode would throw (state advanced), R_DELEGATE for
-    level >= 3."""
+    level >= 3.  x32: the 32-bit engine (k4lz4_encode_chain_batch_x32), which keeps the same state record."""
     src_off, dst_off, state_off = _i64(src_off), _i64(dst_off), _i64(state_off)
     src_len, dst_cap, prefix_len = _i32(src_len), _i32(dst_cap), _i32(prefix_len)
     n = int(src_len.shape[0])
     out = np.full(n, -1, dtype=np.int32)
-    N.check(N.lib().k4lz4_encode_chain_batch(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
+    N.check(encoder_fn("k4lz4_encode_chain_batch", x32)(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
                                              prefix_len.ctypes.data, dst.ctypes.data, dst_off.ctypes.data,
                                              dst_cap.ctypes.data, state.ctypes.data, state_off.ctypes.data,
                                              out.ctypes.data, n, int(level), N.MEM_HOST, None, int(device)))
@@ -324,8 +329,9 @@ def encode_chain_batch_host(src: np.ndarray, src_off, src_len, prefix_len, dst: 
 
 def encode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, prefix_len_ptr: int, dst_ptr: int,
                               dst_off_ptr: int, dst_cap_ptr: int, state_ptr: int, state_off_ptr: int,
-                              out_len_ptr: int, n: int, level: int = 0, stream: int = 0, device: int = -1) -> None:
+                              out_len_ptr: int, n: int, level: int = 0, stream: int = 0, device: int = -1,
+                              x32: bool = False) -> None:
     """Device-pointer form of encode_chain_batch_host: only enqueues the kernel on `stream`."""
-    N.check(N.lib().k4lz4_encode_chain_batch(src_ptr, src_off_ptr, src_len_ptr, prefix_len_ptr, dst_ptr, dst_off_ptr,
+    N.check(encoder_fn("k4lz4_encode_chain_batch", x32)(src_ptr, src_off_ptr, src_len_ptr, prefix_len_ptr, dst_ptr, dst_off_ptr,
                                              dst_cap_ptr, state_ptr, state_off_ptr, out_len_ptr, int(n), int(level),
                                              N.MEM_DEVICE, stream or None, int(device)))

@@ -68,6 +68,13 @@ class LZ4Codec:
 
     Version = 192                      # LZ4Codec.cs:13
 
+    # LZ4Codec.Enforce32 (LZ4Codec.cs:21-25, Engine/LL.tools.cs:29-36): every L00_FAST encode call made while it is
+    # set uses the 32-bit engine LL32 (hash4 for the u32 table), so its bytes differ from LL64's for inputs of
+    # >= 65 547 bytes and for chained blocks of any size.  Read at each call, as the reference reads it
+    # (Engine/LLxx.cs:65-91): Encode, LZ4Pickler.Pickle / PickleTo, LZ4BlockEncoder, LZ4FastChainEncoder,
+    # LZ4Frame / write_frames, ChainEncoderGroup.encode and FrameWriterGroup.write / close.  Decoding is unaffected.
+    Enforce32 = False
+
     @staticmethod
     def MaximumOutputSize(length: int) -> int:
         """LZ4Codec.cs:30-31."""
@@ -98,7 +105,8 @@ class LZ4Codec:
         n = int(src.shape[0])
         if n <= 0:
             return 0                                                      # LZ4Codec.cs:45-46,64-65
-        r = int(N.lib().k4lz4_encode(src.ctypes.data, n, dst.ctypes.data, int(dst.shape[0]), int(level)))
+        enc = N.lib().k4lz4_encode_x32 if LZ4Codec.Enforce32 else N.lib().k4lz4_encode
+        r = int(enc(src.ctypes.data, n, dst.ctypes.data, int(dst.shape[0]), int(level)))
         if r == N.R_DELEGATE:
             raise DelegateToManagedEngine(f"level {int(level)} is not on the accelerated path")
         if r <= N.E_NODEVICE:

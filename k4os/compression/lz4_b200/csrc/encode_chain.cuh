@@ -6,13 +6,16 @@
 // sets up: LZ4EncoderBase.cs:90-97 with LZ4_saveDict).  That is LZ4_compress_generic with
 //   byU32 table (4 096 slots of absolute indices, hash5), limitedOutput, withPrefix64k, dictSmall or
 //   noDictIssue (LL64.fast.cs:582-667; upstream orig/lib/lz4.c:851-1240, 1545-1637).
+// With H4 = true it is the 32-bit engine's instead (LZ4Codec.Enforce32: LL32.fast.cs, whose only difference is
+// hash4 over 4 bytes for the byU32 table, LL32.tools.cs:143-150).  Both engines keep the same state record, so a
+// stream may alternate between them.
 // The table is the caller's state record (K4LZ4_CHAIN_STATE_BYTES) in global memory, accessed through L2
 // (.cg) like the global-table warps of encode_tile.cuh; it is never zeroed.
 //
 // The match search is encode_spec_warp's (encode_tile.cuh): 32 consecutive probes of a search run at once,
 // `__match_any_sync` on the hash substitutes the nearest earlier lane's store, the first hitting lane wins
 // and lanes up to it commit their stores.  What differs:
-//   * the hash (hash5 over 8 bytes, 12 bits) and the slots (absolute index = currentOffset-based, no tag);
+//   * the hash (hash5 over 8 bytes or, with H4, hash4 over 4 bytes, 12 bits) and the slots (absolute index = currentOffset-based, no tag);
 //   * an index below startIndex lies in the history at src - (startIndex - index);
 //   * the accept tests: index + 65535 >= current, and under dictSmall index >= startIndex - dictSize
 //     (lz4.c:1001-1006, 1187-1188);
@@ -42,7 +45,8 @@ static_assert(sizeof(ChainState) == 16400, "K4LZ4_CHAIN_STATE_BYTES");
 constexpr int ENC_CHAIN_WARPS = K4_ENC_CHAIN_WARPS;
 
 // Returns the engine's value: bytes written, or 0 when a limitedOutput check fails (the state has then
-// advanced as far as upstream's has).  `P` is the caller's prefixLen (>= 0).
+// advanced as far as upstream's has).  `P` is the caller's prefixLen (>= 0).  H4: hash4 (the 32-bit engine).
+template <bool H4>
 __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t n, const uint32_t P,
                                  uint8_t* __restrict__ dst, const int cap, ChainState* st) {
     const int lane = lane_id();
@@ -72,7 +76,7 @@ __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t
     };
 #define RD32(p) ldg_u32u(src + (int)(p))
 #define RD8(p) ((uint32_t)__ldg(src + (int)(p)))
-#define HASH(p) hash5(ldg_u64u(src + (p)), 12)
+#define HASH(p) (H4 ? hash4(ldg_u32u(src + (p)), 12) : hash5(ldg_u64u(src + (p)), 12))
     const int64_t olimit = cap;                                               // limitedOutput, always
     uint32_t ip = 0, anchor = 0, op = 0;
 
@@ -91,9 +95,15 @@ __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t
             const uint32_t q = q0 + (uint32_t)lane - (post ? 1u : 0u);
             const uint32_t pos = isPost ? ip : base + probe_advance(q);
             const bool valid = isPost || (base + probe_advance(q + 1) <= mfl1);   // :969
-            const uint64_t v64 = valid ? ldg_u64u(src + pos) : 0ull;
-            const uint32_t v = (uint32_t)v64;
-            const uint32_t h = valid ? hash5(v64, 12) : (0x10000u + (uint32_t)lane);
+            uint32_t v, h;
+            if constexpr (H4) {                                               // one word: all the compare needs
+                v = valid ? ldg_u32u(src + pos) : 0u;
+                h = valid ? hash4(v, 12) : (0x10000u + (uint32_t)lane);
+            } else {
+                const uint64_t v64 = valid ? ldg_u64u(src + pos) : 0ull;
+                v = (uint32_t)v64;
+                h = valid ? hash5(v64, 12) : (0x10000u + (uint32_t)lane);
+            }
             uint32_t cand = valid ? __ldcg(table + h) : 0u;
             if (h == h2) cand = startIndex + ip - 2;                          // sees the put(ip-2)
             const unsigned peers = __match_any_sync(FULL, h);
@@ -223,7 +233,8 @@ __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t
 // Persistent: one-warp CTAs pull blocks from a device counter.  Block b's result: 0 for n == 0 and -2
 // (K4LZ4_R_DELEGATE) for level >= 3, both without touching the state; -1 for a negative prefix length or a
 // state record not 16-aligned (state untouched) and where the engine returns 0 (state advanced); otherwise
-// the bytes written.
+// the bytes written.  H4: the 32-bit engine (k4lz4_*_x32).
+template <bool H4>
 __global__ void __launch_bounds__(32, ENC_CHAIN_WARPS)
 encode_chain_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
                     const int32_t* __restrict__ srcLen, const int32_t* __restrict__ prefixLen,
@@ -243,7 +254,7 @@ encode_chain_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restri
         const int P = prefixLen[b];
         uint8_t* const sp = stateBase + stateOff[b];
         if (P < 0 || (reinterpret_cast<uintptr_t>(sp) & 15)) { if (lane == 0) outLen[b] = -1; continue; }
-        const int r = encode_chain_warp(srcBase + srcOff[b], (uint32_t)n, (uint32_t)P, dstBase + dstOff[b],
+        const int r = encode_chain_warp<H4>(srcBase + srcOff[b], (uint32_t)n, (uint32_t)P, dstBase + dstOff[b],
                                         dstCap[b], reinterpret_cast<ChainState*>(sp));
         if (lane == 0) {
             outLen[b] = r <= 0 ? -1 : r;

@@ -87,7 +87,7 @@ struct Batch {
     int32_t* outLen;                  // OP_XXH32: the uint32 checksums
     int64_t n;
     int level = 0;                    // OP_ENCODE: 0..255; OP_PICKLE(W): passed through
-    bool x32 = false;                 // OP_ENCODE: reproduce the 32-bit engine (k4lz4_encode*_x32)
+    bool x32 = false;                 // OP_ENCODE, OP_ENCCHAIN, OP_PICKLE(W): the 32-bit engine (k4lz4_*_x32)
     const uint8_t* dictBase = nullptr; const int64_t* dictOff = nullptr; const int32_t* dictLen = nullptr;
     const int32_t* prefixLen = nullptr;   // OP_CHAIN: history in front of each destination; OP_ENCCHAIN: of each source
     uint8_t* stateBase = nullptr; const int64_t* stateOff = nullptr;   // OP_ENCCHAIN: K4LZ4_CHAIN_STATE_BYTES per block
@@ -221,8 +221,9 @@ Dev* dev_state(int dev) {
         // best effort, as their results never decide anything: the pickler's shared memory, and the split of
         // shared memory / L1 both encoder kernels ask for (they share SMs): just enough for the shared-memory
         // tables (+1 KiB the hardware reserves per CTA), the rest stays L1 for the input windows
-        cudaFuncSetAttribute(k4::pickle_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES);
+        for (auto* pk : {k4::pickle_kernel<false>, k4::pickle_kernel<true>})
+            cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES);
         const int carve = (k4::ENC_SM_WARPS * (k4::ENC_SLOT_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
         cudaFuncSetAttribute(k4::encode_spec_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
         cudaFuncSetAttribute(k4::encode_spec_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
@@ -337,8 +338,8 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
     case OP_PICKLE:
     case OP_PICKLEW: {
         const int ctas = (n + k4::ENC_WARPS_PER_CTA - 1) / k4::ENC_WARPS_PER_CTA;
-        k4::pickle_kernel<<<ctas, k4::ENC_WARPS_PER_CTA * 32,
-                            k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES, st>>>(
+        (a.x32 ? k4::pickle_kernel<true> : k4::pickle_kernel<false>)<<<ctas, k4::ENC_WARPS_PER_CTA * 32,
+                                                                        k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES, st>>>(
             a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.outLen, n, a.level, op == OP_PICKLEW ? 1 : 0);
         g_launches++;
         break;
@@ -367,9 +368,9 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
         if (e == cudaSuccess) e = cudaMemsetAsync(counter, 0, 4, st);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return e; }
         const int wave = D->sms * k4::ENC_CHAIN_WARPS;
-        k4::encode_chain_kernel<<<n < wave ? n : wave, 32, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.prefixLen,
-                                                                    a.dstBase, a.dstOff, a.dstCap, a.stateBase,
-                                                                    a.stateOff, a.outLen, n, a.level, counter);
+        (a.x32 ? k4::encode_chain_kernel<true> : k4::encode_chain_kernel<false>)<<<n < wave ? n : wave, 32, 0, st>>>(
+            a.srcBase, a.srcOff, a.srcLen, a.prefixLen, a.dstBase, a.dstOff, a.dstCap, a.stateBase, a.stateOff,
+            a.outLen, n, a.level, counter);
         g_launches++;
         cudaFreeAsync(counter, st);
         break;
@@ -1089,7 +1090,7 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
         if (!linked) {
             for (int64_t b0 = 0; b0 < nB; b0 += E) {
                 const int64_t m = std::min<int64_t>(E, nB - b0);
-                Batch kb{b.srcBase, t.srcOff + b0, t.len + b0, scratch, eDst, eCap, e.res, m, b.level};
+                Batch kb{b.srcBase, t.srcOff + b0, t.len + b0, scratch, eDst, eCap, e.res, m, b.level, b.x32};
                 FR_TRY(launch_op(OP_ENCODE, kb, st));
                 FR_TRY(place(-1, b0, b0 + m, 0, n, m));
             }
@@ -1110,7 +1111,7 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
                     k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fr, t, so, sl, pre, bs);
                     FR_LAUNCH();
                     g_launches++;
-                    Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level};
+                    Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level, b.x32};
                     kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
                     FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
                     FR_TRY(place(k, 0, 0, f0, f0 + m, m));
@@ -1481,7 +1482,7 @@ cudaError_t group_codec(k4lz4_chain_group* g, int cg, const Batch& b, const int3
     if (e == cudaSuccess && cg != k4::CG_DECODE)
         e = launch_op(OP_COPY, Batch{b.srcBase, t.copyOff, t.copyLen, g->rings, t.ringOff, nullptr, nullptr, n}, st);
     if (e == cudaSuccess && cg == k4::CG_ENCODE) {
-        Batch kb{g->rings, t.ringOff, t.len, b.dstBase, b.dstOff, b.dstCap, b.outLen, n, b.level};
+        Batch kb{g->rings, t.ringOff, t.len, b.dstBase, b.dstOff, b.dstCap, b.outLen, n, b.level, b.x32};
         kb.prefixLen = t.prefix; kb.stateBase = g->states; kb.stateOff = t.stateOff;
         e = launch_op(OP_ENCCHAIN, kb, st);
     }
@@ -1642,7 +1643,7 @@ cudaError_t fw_device(k4lz4_frame_writer_group* g, bool closing, const Batch& b,
                 g_launches++;
                 if (!closing)
                     FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.copyOff, t.copyLen, g->rings, copyDst, nullptr, nullptr, m}, st));
-                Batch kb{g->rings, t.ringOff, t.len, scratch, eDst, eCap, e.res, m, g->level};
+                Batch kb{g->rings, t.ringOff, t.len, scratch, eDst, eCap, e.res, m, g->level, b.x32};
                 if (linked) { kb.prefixLen = t.prefix; kb.stateBase = g->states; kb.stateOff = t.stateOff; }
                 FR_TRY(launch_op(linked ? OP_ENCCHAIN : OP_ENCODE, kb, st));
                 k4::frame_writer_place_kernel<<<grid_of(m), 128, 0, st>>>(e0, m, ent, g->fw, t, e, b.dstBase, bound,
@@ -1697,7 +1698,7 @@ int fw_host_part(k4lz4_frame_writer_group* g, bool closing, const Batch& b, cons
                      streams[idx[k]], (int32_t)piece[k], (int32_t)room, 0};
     }, up, st);
     if (rc != K4LZ4_OK) return rc;
-    const Batch kb{up.src, up.srcOff, up.len, up.dst, up.dstOff, up.cap, up.res, m, g->level};
+    const Batch kb{up.src, up.srcOff, up.len, up.dst, up.dstOff, up.cap, up.res, m, g->level, b.x32};
     const cudaError_t e = fw_device(g, closing, kb, up.stream, st);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame writer step: %s", cudaGetErrorString(e)); }
     res.resize((size_t)m);
@@ -2135,14 +2136,33 @@ int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, 
     return run(OP_CHAIN, b, memKind, cudaStream, device);
 }
 
+namespace {
+int encode_chain_batch(bool x32, const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                       const int32_t* prefixLen, uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                       uint8_t* stateBase, const int64_t* stateOff, int32_t* outLen, int32_t nBlocks, int32_t level,
+                       int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level, x32};
+    b.prefixLen = prefixLen; b.stateBase = stateBase; b.stateOff = stateOff;
+    return run(OP_ENCCHAIN, b, memKind, cudaStream, device);
+}
+}  // namespace
+
 int32_t k4lz4_encode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                  const int32_t* prefixLen, uint8_t* dstBase, const int64_t* dstOff,
                                  const int32_t* dstCap, uint8_t* stateBase, const int64_t* stateOff,
                                  int32_t* outLen, int32_t nBlocks, int32_t level, int32_t memKind, void* cudaStream,
                                  int32_t device) {
-    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level};
-    b.prefixLen = prefixLen; b.stateBase = stateBase; b.stateOff = stateOff;
-    return run(OP_ENCCHAIN, b, memKind, cudaStream, device);
+    return encode_chain_batch(false, srcBase, srcOff, srcLen, prefixLen, dstBase, dstOff, dstCap, stateBase, stateOff,
+                              outLen, nBlocks, level, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_encode_chain_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                     const int32_t* prefixLen, uint8_t* dstBase, const int64_t* dstOff,
+                                     const int32_t* dstCap, uint8_t* stateBase, const int64_t* stateOff,
+                                     int32_t* outLen, int32_t nBlocks, int32_t level, int32_t memKind,
+                                     void* cudaStream, int32_t device) {
+    return encode_chain_batch(true, srcBase, srcOff, srcLen, prefixLen, dstBase, dstOff, dstCap, stateBase, stateOff,
+                              outLen, nBlocks, level, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_chain_group_create(int32_t kind, int32_t nStreams, int32_t blockSize, int32_t device,
@@ -2173,6 +2193,14 @@ int32_t k4lz4_chain_group_encode(k4lz4_chain_group* g, const int32_t* streams, c
                                  const int32_t* dstCap, int32_t* outLen, int32_t n, int32_t level, int32_t memKind,
                                  void* cudaStream) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n, level};
+    return group_run(g, K4LZ4_CHAIN_ENCODER, k4::CG_ENCODE, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_chain_group_encode_x32(k4lz4_chain_group* g, const int32_t* streams, const uint8_t* srcBase,
+                                     const int64_t* srcOff, const int32_t* srcLen, uint8_t* dstBase,
+                                     const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int32_t n,
+                                     int32_t level, int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n, level, true};
     return group_run(g, K4LZ4_CHAIN_ENCODER, k4::CG_ENCODE, b, streams, memKind, cudaStream);
 }
 
@@ -2257,6 +2285,14 @@ int32_t k4lz4_pickle_batch(const uint8_t* srcBase, const int64_t* srcOff, const 
                memKind, cudaStream, device);
 }
 
+int32_t k4lz4_pickle_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                               uint8_t* dstBase, const int64_t* dstOff, int32_t* outLen,
+                               int32_t nMessages, int32_t level, int32_t memKind, void* cudaStream,
+                               int32_t device) {
+    return run(OP_PICKLE, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level, true},
+               memKind, cudaStream, device);
+}
+
 int32_t k4lz4_pickle_writer_bound(int32_t length) { return length <= 0 ? 0 : length + 1 + k4::pickle_diff_width(length); }
 
 int32_t k4lz4_pickle_writer_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2264,6 +2300,14 @@ int32_t k4lz4_pickle_writer_batch(const uint8_t* srcBase, const int64_t* srcOff,
                                   int32_t nMessages, int32_t level, int32_t memKind, void* cudaStream,
                                   int32_t device) {
     return run(OP_PICKLEW, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level},
+               memKind, cudaStream, device);
+}
+
+int32_t k4lz4_pickle_writer_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                      uint8_t* dstBase, const int64_t* dstOff, int32_t* outLen,
+                                      int32_t nMessages, int32_t level, int32_t memKind, void* cudaStream,
+                                      int32_t device) {
+    return run(OP_PICKLEW, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, nullptr, outLen, nMessages, level, true},
                memKind, cudaStream, device);
 }
 
@@ -2353,6 +2397,14 @@ int32_t k4lz4_frame_encode_batch(const uint8_t* srcBase, const int64_t* srcOff, 
     return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
 }
 
+int32_t k4lz4_frame_encode_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                     uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                                     int32_t nFrames, int32_t blockSize, int32_t flags, int32_t level,
+                                     int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level, true};
+    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
+}
+
 int32_t k4lz4_frame_content_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                        int32_t* outSize, int32_t nFrames, int32_t memKind, void* cudaStream,
                                        int32_t device) {
@@ -2405,10 +2457,27 @@ int32_t k4lz4_frame_writer_group_write(k4lz4_frame_writer_group* g, const int32_
     return fw_run(g, false, b, streams, memKind, cudaStream);
 }
 
+int32_t k4lz4_frame_writer_group_write_x32(k4lz4_frame_writer_group* g, const int32_t* streams,
+                                           const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                           uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                           int32_t* outLen, int32_t n, int32_t memKind, void* cudaStream) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, n};
+    b.x32 = true;
+    return fw_run(g, false, b, streams, memKind, cudaStream);
+}
+
 int32_t k4lz4_frame_writer_group_close(k4lz4_frame_writer_group* g, const int32_t* streams, uint8_t* dstBase,
                                        const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int32_t n,
                                        int32_t memKind, void* cudaStream) {
     Batch b{nullptr, nullptr, nullptr, dstBase, dstOff, dstCap, outLen, n};
+    return fw_run(g, true, b, streams, memKind, cudaStream);
+}
+
+int32_t k4lz4_frame_writer_group_close_x32(k4lz4_frame_writer_group* g, const int32_t* streams, uint8_t* dstBase,
+                                           const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen, int32_t n,
+                                           int32_t memKind, void* cudaStream) {
+    Batch b{nullptr, nullptr, nullptr, dstBase, dstOff, dstCap, outLen, n};
+    b.x32 = true;
     return fw_run(g, true, b, streams, memKind, cudaStream);
 }
 

@@ -38,6 +38,8 @@ __device__ __forceinline__ void warp_shift_up(uint8_t* p, int len, int d, int la
 
 // LZ4Pickler.Pickle<TBufferWriter> (pickle.cs:113-148): the header width is fixed from the full
 // length before encoding (:129,161-165) and the payload is encoded in place with capacity n (:130-133).
+// X32 (both variants): LZ4Codec.Enforce32, the 32-bit engine's hash4 for messages of LIMIT_64K bytes or more.
+template <bool X32>
 __device__ int pickle_writer_message_warp(const uint8_t* __restrict__ src, int n, uint8_t* __restrict__ dst,
                                           int level, void* table) {
     const int lane = lane_id();
@@ -47,7 +49,7 @@ __device__ int pickle_writer_message_warp(const uint8_t* __restrict__ src, int n
     const int hs = 1 + k;
     int enc = (n < LIMIT_64K)
         ? encode_spec_warp<false>(src, nullptr, (uint32_t)n, dst + hs, n, n - 1, reinterpret_cast<uint16_t*>(table))
-        : encode_block_warp(src, n, dst + hs, n, n - 1, table, false);
+        : encode_block_warp(src, n, dst + hs, n, n - 1, table, X32);
     __syncwarp();
     if (enc <= 0 || enc >= n) {                                  // :135-140
         if (lane == 0) dst[0] = 0;
@@ -62,6 +64,7 @@ __device__ int pickle_writer_message_warp(const uint8_t* __restrict__ src, int n
     return hs + enc;                                             // :146
 }
 
+template <bool X32>
 __device__ int pickle_message_warp(const uint8_t* __restrict__ src, int n, uint8_t* __restrict__ dst,
                                    int level, void* table) {
     const int lane = lane_id();
@@ -70,7 +73,7 @@ __device__ int pickle_message_warp(const uint8_t* __restrict__ src, int n, uint8
     const int cap = n <= 1024 ? 1024 : n;                        // :57-67
     int enc = (n < LIMIT_64K)                                                 // :83
         ? encode_spec_warp<false>(src, nullptr, (uint32_t)n, dst + 2, cap, n - 1, reinterpret_cast<uint16_t*>(table))
-        : encode_block_warp(src, n, dst + 2, cap, n - 1, table, false);
+        : encode_block_warp(src, n, dst + 2, cap, n - 1, table, X32);
     __syncwarp();
     if (enc <= 0 || enc >= n) {                                  // :85-94
         if (lane == 0) dst[0] = 0;
@@ -118,6 +121,7 @@ __device__ int unpickle_message_warp(const uint8_t* __restrict__ src, int n, uin
     return dec != expected ? R_CORRUPT : expected;               // :126-128
 }
 
+template <bool X32>
 __global__ void __launch_bounds__(ENC_WARPS_PER_CTA * 32)
 pickle_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
               const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
@@ -128,8 +132,8 @@ pickle_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ s
     const int b = blockIdx.x * ENC_WARPS_PER_CTA + wInCta;
     if (b >= nMessages) return;
     int r = writerVariant
-        ? pickle_writer_message_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES)
-        : pickle_message_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES);
+        ? pickle_writer_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES)
+        : pickle_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES);
     if (lane_id() == 0) outLen[b] = r;
 }
 

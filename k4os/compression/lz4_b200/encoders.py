@@ -116,7 +116,8 @@ class LZ4BlockEncoder:
         dst_off = np.zeros(nb, dtype=np.int64)
         dst_off[1:] = np.cumsum(caps[:-1].astype(np.int64))
         dst = np.zeros(int(caps.astype(np.int64).sum()) + 16, dtype=np.uint8)
-        out_len = encode_batch_flat_host(self._buf, src_off, lens, dst, dst_off, caps, int(self._level))
+        out_len = encode_batch_flat_host(self._buf, src_off, lens, dst, dst_off, caps, int(self._level),
+                                         x32=LZ4Codec.Enforce32)
         res = []
         for i in range(nb):
             enc = int(out_len[i])
@@ -478,7 +479,8 @@ class LZ4FastChainEncoder:
         doff[1:] = np.cumsum(caps[:-1].astype(np.int64))
         state = np.concatenate([encoders[i]._state for i in todo])
         soff = np.arange(len(todo), dtype=np.int64) * N.CHAIN_STATE_BYTES
-        out = encode_chain_batch_host(base, src_off, src_len, prefix, dst, doff, caps, state, soff, 0, device)
+        out = encode_chain_batch_host(base, src_off, src_len, prefix, dst, doff, caps, state, soff, 0, device,
+                                      LZ4Codec.Enforce32)
         failed = False
         for k, i in enumerate(todo):
             e, r, n = encoders[i], int(out[k]), int(src_len[k])

@@ -20,7 +20,8 @@ import struct
 import numpy as np
 
 from . import _native as N
-from .batch import _pack, _slices, _slots
+from .batch import _pack, _slices, _slots, encoder_fn
+from .codec import LZ4Codec
 
 MAGIC = 0x184D2204
 _BLOCK_SIZES = {4: 1 << 16, 5: 1 << 18, 6: 1 << 20, 7: 1 << 22}
@@ -68,7 +69,7 @@ def _native_block_size(block_size: int) -> int:
 
 class LZ4Frame:
     """LZ4Frame.Encode / Decode over whole buffers (k4lz4_frame_*): every frame of a call is encoded or decoded on
-    the GPU, header, block walk, layout and checksums included.  Host memory takes bytes / numpy arrays; the
+    the GPU, header, block walk, layout and checksums included.  Encoding follows LZ4Codec.Enforce32 at each call.  Host memory takes bytes / numpy arrays; the
     *_device forms take torch tensors on the GPU (uint8 data, int64 offsets, int32 lengths and results) and only
     enqueue work on `stream` (after one wait for the block and step counts)."""
 
@@ -90,7 +91,7 @@ class LZ4Frame:
         caps = [LZ4Frame.Bound(int(x), block_size, chaining, block_checksum, content_checksum) for x in sl]
         dst, do, dc = _slots(caps)
         out = np.full(len(sl), -1, dtype=np.int32)
-        N.check(N.lib().k4lz4_frame_encode_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+        N.check(encoder_fn("k4lz4_frame_encode_batch", LZ4Codec.Enforce32)(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
                                                  do.ctypes.data, dc.ctypes.data, out.ctypes.data, len(sl), bs, fl,
                                                  int(level), N.MEM_HOST, None, int(device)))
         return _slices(dst, do, out), out
@@ -136,7 +137,7 @@ class LZ4Frame:
     def encode_many_device(src, src_off, src_len, dst, dst_off, dst_cap, out_len, block_size: int = 65536,
                            chaining: bool = True, block_checksum: bool = False, content_checksum: bool = False,
                            level: int = 0, stream: int = 0, device: int = -1) -> None:
-        N.check(N.lib().k4lz4_frame_encode_batch(
+        N.check(encoder_fn("k4lz4_frame_encode_batch", LZ4Codec.Enforce32)(
             src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(), dst.data_ptr(), dst_off.data_ptr(),
             dst_cap.data_ptr(), out_len.data_ptr(), int(src_len.numel()), _native_block_size(block_size),
             _flags(chaining, block_checksum, content_checksum), int(level), N.MEM_DEVICE, stream or None, int(device)))

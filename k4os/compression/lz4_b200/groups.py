@@ -17,7 +17,8 @@ from typing import Sequence
 import numpy as np
 
 from . import _native as N
-from .batch import _i32, _pack, _slices, _slots
+from .batch import _i32, _pack, _slices, _slots, encoder_fn
+from .codec import LZ4Codec
 
 
 class _Group:
@@ -81,7 +82,8 @@ class _ChainGroup(_Group):
 
 
 class ChainEncoderGroup(_ChainGroup):
-    """S LZ4FastChainEncoder streams at L00_FAST whose input rings and LZ4_stream_t records live on the GPU."""
+    """S LZ4FastChainEncoder streams at L00_FAST whose input rings and LZ4_stream_t records live on the GPU.  Each
+    call encodes with the engine LZ4Codec.Enforce32 names at that call."""
     _kind = N.CHAIN_ENCODER
 
     def encode(self, blocks: Sequence, streams: Sequence[int] | None = None, caps: Sequence[int] | None = None,
@@ -94,7 +96,7 @@ class ChainEncoderGroup(_ChainGroup):
             caps = [N.lib().k4lz4_max_output_size(int(x)) for x in sl]
         dst, do, dc = _slots(caps)
         out = np.full(len(sl), -1, dtype=np.int32)
-        N.check(N.lib().k4lz4_chain_group_encode(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
+        N.check(encoder_fn("k4lz4_chain_group_encode", LZ4Codec.Enforce32)(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
                                                  sl.ctypes.data, dst.ctypes.data, do.ctypes.data, dc.ctypes.data,
                                                  out.ctypes.data, len(sl), int(level), N.MEM_HOST, None))
         return _slices(dst, do, out), out
@@ -103,7 +105,7 @@ class ChainEncoderGroup(_ChainGroup):
                       dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int, n: int, level: int = 0,
                       stream: int = 0) -> None:
         """Device-pointer form of encode: only enqueues work on `stream`."""
-        N.check(N.lib().k4lz4_chain_group_encode(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr, dst_ptr,
+        N.check(encoder_fn("k4lz4_chain_group_encode", LZ4Codec.Enforce32)(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr, dst_ptr,
                                                  dst_off_ptr, dst_cap_ptr, out_len_ptr, int(n), int(level),
                                                  N.MEM_DEVICE, stream or None))
 
@@ -156,7 +158,8 @@ class FrameWriterGroup(_Group):
     chain states and content checksums live on the GPU.  Each call writes one chunk of any size to (or closes) any
     subset of the streams and returns the frame bytes it produced; for every stream the concatenation of what its
     writes and its close returned is the LZ4 frame of everything written to it.  ``close(streams)`` ends frames;
-    ``free()`` (or ``with``) frees the group's device memory, abandoning frames not closed."""
+    ``free()`` (or ``with``) frees the group's device memory, abandoning frames not closed.  Each write and close
+    encodes with the engine LZ4Codec.Enforce32 names at that call."""
     _destroy, _reset = "k4lz4_frame_writer_group_destroy", "k4lz4_frame_writer_group_reset"
 
     def __init__(self, n_streams: int, block_size: int = 65536, chaining: bool = True, block_checksum: bool = False,
@@ -190,7 +193,7 @@ class FrameWriterGroup(_Group):
         s = self._streams(streams, len(sl))
         dst, do, dc = _slots([self.bound(int(x)) for x in sl] if caps is None else caps)
         out = np.full(len(sl), -1, dtype=np.int32)
-        N.check(N.lib().k4lz4_frame_writer_group_write(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
+        N.check(encoder_fn("k4lz4_frame_writer_group_write", LZ4Codec.Enforce32)(self.handle, s.ctypes.data, src.ctypes.data, so.ctypes.data,
                                                        sl.ctypes.data, dst.ctypes.data, do.ctypes.data,
                                                        dc.ctypes.data, out.ctypes.data, len(sl), N.MEM_HOST, None))
         return _slices(dst, do, out), out
@@ -201,21 +204,21 @@ class FrameWriterGroup(_Group):
         s = self._streams(streams, self.n_streams)
         dst, do, dc = _slots([self.close_bound()] * len(s) if caps is None else caps)
         out = np.full(len(s), -1, dtype=np.int32)
-        N.check(N.lib().k4lz4_frame_writer_group_close(self.handle, s.ctypes.data, dst.ctypes.data, do.ctypes.data,
+        N.check(encoder_fn("k4lz4_frame_writer_group_close", LZ4Codec.Enforce32)(self.handle, s.ctypes.data, dst.ctypes.data, do.ctypes.data,
                                                        dc.ctypes.data, out.ctypes.data, len(s), N.MEM_HOST, None))
         return _slices(dst, do, out), out
 
     def write_device(self, streams_ptr: int, src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int,
                      dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int, n: int, stream: int = 0) -> None:
         """Device-pointer form of write: enqueues work on `stream` (and waits once for the number of steps)."""
-        N.check(N.lib().k4lz4_frame_writer_group_write(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
+        N.check(encoder_fn("k4lz4_frame_writer_group_write", LZ4Codec.Enforce32)(self.handle, streams_ptr, src_ptr, src_off_ptr, src_len_ptr,
                                                        dst_ptr, dst_off_ptr, dst_cap_ptr, out_len_ptr, int(n),
                                                        N.MEM_DEVICE, stream or None))
 
     def close_device(self, streams_ptr: int, dst_ptr: int, dst_off_ptr: int, dst_cap_ptr: int, out_len_ptr: int,
                      n: int, stream: int = 0) -> None:
         """Device-pointer form of close: only enqueues work on `stream`."""
-        N.check(N.lib().k4lz4_frame_writer_group_close(self.handle, streams_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
+        N.check(encoder_fn("k4lz4_frame_writer_group_close", LZ4Codec.Enforce32)(self.handle, streams_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
                                                        out_len_ptr, int(n), N.MEM_DEVICE, stream or None))
 
 

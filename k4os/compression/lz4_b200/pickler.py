@@ -10,7 +10,7 @@ import numpy as np
 
 from . import _native as N
 from .batch import pickle_batch_host, pickle_writer_batch_host, unpickle_batch_host, unpickled_size_batch_host
-from .codec import LZ4Level, DelegateToManagedEngine, _ro, _rw
+from .codec import LZ4Codec, LZ4Level, DelegateToManagedEngine, _ro, _rw
 
 
 class InvalidDataException(ValueError):
@@ -24,7 +24,7 @@ class LZ4Pickler:
         src = _ro(source)
         if src.shape[0] == 0:
             return b""
-        out, lens = pickle_batch_host([src], level=int(level))
+        out, lens = pickle_batch_host([src], level=int(level), x32=LZ4Codec.Enforce32)
         if lens[0] == N.R_DELEGATE:
             raise DelegateToManagedEngine(f"level {int(level)} is not on the accelerated path")
         return out[0]
@@ -39,7 +39,7 @@ class LZ4Pickler:
         src = _ro(source)
         if src.shape[0] == 0:
             return
-        out, lens = pickle_writer_batch_host([src], level=int(level))
+        out, lens = pickle_writer_batch_host([src], level=int(level), x32=LZ4Codec.Enforce32)
         if lens[0] == N.R_DELEGATE:
             raise DelegateToManagedEngine(f"level {int(level)} is not on the accelerated path")
         if isinstance(writer, bytearray):

@@ -13,7 +13,9 @@ the same raw bytes compressed as independent blocks.
 S streams x B linked 64 KiB blocks of datagen: one k4lz4_encode_chain_batch call per step (device memory) encodes
 block k of every stream behind its history; GB/s of input over all B steps, next to one k4lz4_encode_batch call
 over the same raw bytes, with the encoder's path counters and a spot check against upstream's chained encoder.
-The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
+The 32-bit engine (k4lz4_encode_chain_batch_x32, LZ4Codec.Enforce32) runs the same steps in the same process,
+timed alternately with the plain one, with a spot check against upstream's chained encoder built as LL32; the card's
+name and power limit are printed with it.  The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
 chained call also moves each block's history and its 16 400-byte state each way).
 Both chain arms also time a chain group (k4lz4_chain_group_*: rings and states resident on the GPU) and print
 per-step times (one block of every stream) through host memory -- LZ4FastChainEncoder.EncodeMany /
@@ -247,12 +249,12 @@ if a.what == "chain-encode":
                   torch.arange(S, dtype=torch.int64, device=dev) * (Bk * bound) + k * bound,
                   torch.zeros(S, dtype=torch.int32, device=dev)) for k in range(Bk)]
         rl, cc = rlen[:S], ccap[:S]
-        def chain():
+        def chain(x32=False):
             state.zero_()
             for t_so, t_pre, t_do, t_out in steps:
                 B.encode_chain_batch_device(raw.data_ptr(), t_so.data_ptr(), rl.data_ptr(), t_pre.data_ptr(),
                                             dstc.data_ptr(), t_do.data_ptr(), cc.data_ptr(), state.data_ptr(),
-                                            soff.data_ptr(), t_out.data_ptr(), S, 0, st)
+                                            soff.data_ptr(), t_out.data_ptr(), S, 0, st, x32=x32)
         B.encode_stats(0, reset=True)
         chain(); torch.cuda.synchronize()
         stats = B.encode_stats(0, reset=True)
@@ -267,6 +269,27 @@ if a.what == "chain-encode":
                 o = (s_ * Bk + k) * bound
                 ok &= int(lens[k][s_]) == len(want[k]) and hd[o:o + len(want[k])].tobytes() == want[k]
         cbytes = sum(int(l.sum()) for l in lens)
+        # the 32-bit engine: the same steps, timed alternately with the plain engine, and its own spot check
+        from tests import enforce32_ref as E32
+        t64, t32 = [], []
+        for _ in range(3):
+            t64.append(timeit(chain, a.reps)[1]); t32.append(timeit(lambda: chain(True), a.reps)[1])
+        chain(True); torch.cuda.synchronize()
+        hd32, lens32, ok32 = dstc.cpu().numpy(), [steps[k][3].cpu().numpy() for k in range(Bk)], True
+        up32 = E32.EncUpstream32()
+        for s_ in (0, S - 1):
+            want = up32.encode_chain(hraw[s_ * Bk * bs:(s_ + 1) * Bk * bs].tobytes(), bs)
+            for k in range(Bk):
+                o = (s_ * Bk + k) * bound
+                ok32 &= int(lens32[k][s_]) == len(want[k]) and hd32[o:o + len(want[k])].tobytes() == want[k]
+        m64, m32 = float(np.median(t64)), float(np.median(t32))
+        import subprocess
+        card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                              capture_output=True, text=True).stdout.strip()
+        print(f"chain-encode-x32[{a.data}{a.mp}] S={S} B={Bk}: plain {m64:.3f} ms {n2*bs/m64/1e6:.1f} GB/s, x32 "
+              f"{m32:.3f} ms {n2*bs/m32/1e6:.1f} GB/s (medians of 3 alternating runs of {a.reps}) x32/plain "
+              f"{m32/m64:.3f} ratio32 {sum(int(l.sum()) for l in lens32)/(n2*bs):.3f} ok32={ok32} | {card}", flush=True)
+        chain(); torch.cuda.synchronize()
         def indep():
             B.encode_batch_device(raw.data_ptr(), roff.data_ptr(), rlen.data_ptr(), slots.data_ptr(), coff.data_ptr(),
                                   ccap.data_ptr(), clen.data_ptr(), n2, 0, st)
