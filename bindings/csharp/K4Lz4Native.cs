@@ -28,6 +28,10 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* outLen, int nBlocks, int memKind, void* cudaStream, int device);
+        // the decoded length of every raw block (no reference counterpart: sizes for blocks stored without them)
+        [DllImport(Lib)] public static extern int k4lz4_decoded_size_batch(
+            byte* srcBase, long* srcOff, int* srcLen, int* outSize, int nBlocks,
+            int memKind, void* cudaStream, int device);
         [DllImport(Lib)] public static extern int k4lz4_pickle_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff,
             int* outLen, int nMessages, int level, int memKind, void* cudaStream, int device);

@@ -34,6 +34,18 @@ namespace K4os.Compression.LZ4
                     K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
         }
 
+        // sizes[i]: what Decode needs as targetCapacities[i] -- 0 for an empty block, -1 where the token chain does
+        // not parse (Decode then fails at any capacity)
+        public static void DecodedSizes(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<int> sizes)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (int* os = sizes)
+                Check(K4Lz4Native.k4lz4_decoded_size_batch(s, so, sl, os, sizes.Length,
+                    K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
+        }
+
         private static void Check(int rc)
         {
             if (rc != 0) throw new InvalidOperationException("libk4lz4: " + K4Lz4Native.LastError());

@@ -125,6 +125,19 @@ K4LZ4_API int32_t k4lz4_decode_batch(const uint8_t *srcBase, const int64_t *srcO
                                      int32_t *outLen, int32_t nBlocks,
                                      int32_t memKind, void *cudaStream, int32_t device);
 
+/* The decoded length of every raw LZ4 block, to size the destinations of k4lz4_decode_batch (as
+ * k4lz4_unpickled_size_batch does for pickles and k4lz4_frame_content_size_batch for frames).  No reference call
+ * corresponds: it is the batch analogue of LZ4Pickler.UnpickledSize for blocks whose sizes were not stored.
+ * outSize[i] = 0 for srcLen[i] <= 0; else the sum of the literal runs plus matchlen + 4 of the token chain, or -1
+ * where the chain runs past the end of the block or the length exceeds 2^31 - 1.  Offsets and the decoder's
+ * end-of-block rules are not checked, so the call runs one way: wherever k4lz4_decode returns r > 0 for some
+ * dstCap, outSize[i] == r; where outSize[i] == -1, k4lz4_decode fails for every dstCap.  Argument checks and codes
+ * as k4lz4_xxh32_batch.  Device memory only enqueues work on `cudaStream`; host memory is synchronous and runs on
+ * one GPU (`device`, K4LZ4_ALL_DEVICES = GPU 0).  One warp walks each block (csrc/size_walk.cuh). */
+K4LZ4_API int32_t k4lz4_decoded_size_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                           int32_t *outSize, int32_t nBlocks,
+                                           int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- decode with an external dictionary, partial decode (SURVEY 8f rows 3 and 4) ------------ */
 
 /* LZ4Codec.Decode(byte*,int,byte*,int,byte*,int) -- LZ4Codec.cs:144-157; replaces the call to

@@ -65,6 +65,23 @@ struct LZ4Codec {
         if (sourceLength <= 0) return 0;
         return check_codec(k4lz4_partial_decode(source, sourceLength, target, targetLength));
     }
+    // The decoded length of every raw block (k4lz4_decoded_size_batch; no reference counterpart): 0 for an empty
+    // block, -1 where its token chain does not parse.  Sizes the targets of Decode for blocks stored without them.
+    static std::vector<int32_t> DecodedSizes(const std::vector<std::vector<uint8_t>>& blocks, int device = 0) {
+        const size_t n = blocks.size();
+        std::vector<int64_t> so(n);
+        std::vector<int32_t> sl(n), out(n, -1);
+        std::vector<uint8_t> src;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)blocks[i].size();
+            src.insert(src.end(), blocks[i].begin(), blocks[i].end());
+        }
+        src.resize(src.size() + 1);
+        const int rc = k4lz4_decoded_size_batch(src.data(), so.data(), sl.data(), out.data(), (int32_t)n,
+                                                K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        return out;
+    }
 };
 
 // Independent-block stream pair with a batched top-up (SURVEY 8f row 1):

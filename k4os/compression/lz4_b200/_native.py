@@ -41,6 +41,7 @@ SIGNATURES = {
     "k4lz4_encode_batch": (_BATCH + [_i32, _i32] + _CALL, _i32),
     "k4lz4_encode_batch_x32": (_BATCH + [_i32, _i32] + _CALL, _i32),
     "k4lz4_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
+    "k4lz4_decoded_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_partial_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_decode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),

@@ -102,6 +102,17 @@ def decode_batch_host(blocks: Sequence, caps: Sequence[int], device: int = 0):
     return _slices(dst, do, out), out
 
 
+def decoded_size_batch_host(blocks: Sequence, device: int = 0) -> np.ndarray:
+    """The decoded length of every raw LZ4 block (k4lz4_decoded_size_batch): 0 for an empty block, -1 where the
+    token chain does not parse or its length exceeds 2^31 - 1."""
+    src, so, sl = _pack(blocks)
+    n = len(sl)
+    out = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_decoded_size_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
+                                             out.ctypes.data, n, N.MEM_HOST, None, int(device)))
+    return out
+
+
 def pickle_batch_host(messages: Sequence, level: int = 0, device: int = 0, x32: bool = False):
     """LZ4Pickler.Pickle over a batch -> (list[bytes], outLen int32[n]); x32: the 32-bit engine."""
     src, so, sl = _pack(messages)
@@ -179,6 +190,12 @@ def decode_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_pt
     N.check(N.lib().k4lz4_decode_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr,
                                        dst_cap_ptr, out_len_ptr, int(n), N.MEM_DEVICE,
                                        stream or None, int(device)))
+
+
+def decoded_size_batch_device(src_ptr, src_off_ptr, src_len_ptr, out_size_ptr, n,
+                              stream: int = 0, device: int = -1) -> None:
+    N.check(N.lib().k4lz4_decoded_size_batch(src_ptr, src_off_ptr, src_len_ptr, out_size_ptr,
+                                             int(n), N.MEM_DEVICE, stream or None, int(device)))
 
 
 def pickle_batch_device(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, out_len_ptr, n,

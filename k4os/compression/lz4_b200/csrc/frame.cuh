@@ -5,7 +5,7 @@
 //
 // Format: orig/doc/lz4_Frame_format.md; the reference's writer and reader: Streams/Frames/LZ4FrameWriter.cs:57-189,
 // LZ4FrameReader.cs:55-59, LZ4FrameReader.blocking.cs:57-144.  The CPU restatement of the parse is frame.py's
-// _Frame; of the walk, tests/test_frame_model.py.
+// _Frame; of the walk (size_walk.cuh), tests/test_frame_model.py.
 //
 // Decode keeps one error KEY per frame: (block index << 4) | kind, the smallest one wins, because the reference
 // reads a frame in order and throws at the first problem.  Kinds: FK_TRUNC (the block's length code, body or
@@ -14,6 +14,7 @@
 #pragma once
 #include "common.cuh"
 #include "xxh32.cuh"
+#include "size_walk.cuh"
 
 namespace k4 {
 
@@ -227,42 +228,17 @@ __global__ void __launch_bounds__(1024) frame_scan_kernel(FrameRec* __restrict__
     if (threadIdx.x == 0) { tot->blocks = carry[0]; tot->slots = carry[1]; }
 }
 
-// The decoded length of an LZ4 block from its token chain alone: literal runs plus matchlen + 4; offsets are not
-// read.  For every block LZ4_decompress_safe accepts this equals its result.  -1 where the chain runs past the end.
-__device__ int64_t frame_walk(const uint8_t* s, int64_t n) {
-    int64_t p = 0, out = 0;
-    while (p < n) {
-        const uint32_t tok = s[p++];
-        int64_t lit = tok >> 4;
-        if (lit == 15) {
-            uint32_t x;
-            do { if (p >= n) return -1; x = s[p++]; lit += x; } while (x == 255);
-        }
-        out += lit;
-        p += lit;
-        if (p == n) return out;
-        if (p + 2 > n) return -1;
-        p += 2;
-        int64_t ml = tok & 15;
-        if (ml == 15) {
-            uint32_t x;
-            do { if (p >= n) return -1; x = s[p++]; ml += x; } while (x == 255);
-        }
-        out += ml + 4;
-    }
-    return -1;
-}
-
-// One thread per row: the decoded length of a compressed block (a raw block's is its length).  A chain that does
-// not parse is an error of its block (the decoder rejects it too); its size is then the lower bound, so that the
-// layout's scratch rule still holds.
+// One warp per row: the decoded length of a compressed block (a raw block's is its length), by the warp walk of
+// size_walk.cuh.  A chain that does not parse is an error of its block (the decoder rejects it too); its size is
+// then the lower bound, so that the layout's scratch rule still holds.  Launch with 32 * nB threads.
 __global__ void block_size_walk_kernel(const uint8_t* __restrict__ srcBase, FrameTable t, int64_t nB,
                                        FrameRec* __restrict__ fr) {
-    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t b = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (b >= nB) return;
     const int32_t L = t.len[b];
     const bool raw = t.kind[b] & RK_RAW;
-    int64_t s = raw ? L : frame_walk(srcBase + t.srcOff[b], L);
+    int64_t s = raw ? L : sw_walk_warp(srcBase + t.srcOff[b], L, threadIdx.x & 31);
+    if (threadIdx.x & 31) return;
     if (s < 0) {
         atomicMin(&fr[t.frame[b]].err, ((unsigned long long)t.idx[b] << 4) | FK_BLOCK);
         s = frame_lb(L, false);

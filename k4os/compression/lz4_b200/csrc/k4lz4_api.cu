@@ -76,7 +76,7 @@ int device_count_cached() {
 
 enum Op {
     OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY,
-    OP_ENCCHAIN
+    OP_ENCCHAIN, OP_DSIZE
 };
 
 // Block i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]) and outLen[i].
@@ -110,8 +110,9 @@ constexpr Needs NEEDS[] = {
     /* OP_XXH32    */ {false, false, true,  false, false, false},
     /* OP_COPY     */ {true,  false, false, false, false, false},
     /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true},
+    /* OP_DSIZE    */ {false, false, true,  false, false, false},
 };
-static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_ENCCHAIN + 1, "one row per op");
+static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_DSIZE + 1, "one row per op");
 
 // The machine part of check(): a device must exist, an empty batch is then done (the caller returns OK for
 // n == 0), and `device` (K4LZ4_ALL_DEVICES or the current device when negative) must name a visible GPU.
@@ -375,6 +376,11 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
         cudaFreeAsync(counter, st);
         break;
     }
+    case OP_DSIZE:     // one warp per block
+        k4::decoded_size_kernel<<<(unsigned)(((int64_t)n * 32 + 127) / 128), 128, 0, st>>>(a.srcBase, a.srcOff,
+                                                                                       a.srcLen, a.outLen, n);
+        g_launches++;
+        break;
     }
     return cudaGetLastError();
 }
@@ -833,7 +839,7 @@ int run(Op op, const Batch& b, int memKind, void* stream, int device) {
     const int rc = check(op, b, memKind, device);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     if (memKind == K4LZ4_MEM_HOST)
-        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN)
+        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN || op == OP_DSIZE)
                    ? run_staged(op, b, device < 0 ? 0 : device) : run_host(op, b, device);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
@@ -967,7 +973,7 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
     FR_LAUNCH();
     g_launches++;
     if (nB > 0) {
-        k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, fr);
+        k4::block_size_walk_kernel<<<grid_of(nB * 32), 128, 0, st>>>(b.srcBase, t, nB, fr);
         FR_LAUNCH();
         g_launches++;
     }
@@ -1860,7 +1866,7 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, int mode, const Batch& b, con
     FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, c.upOff, c.upLen, g->stash, c.upDst, nullptr, nullptr, n}, st));
     if (bytes) {
         if (nB > 0) {
-            k4::block_size_walk_kernel<<<grid_of(nB), 128, 0, st>>>(b.srcBase, t, nB, walkFr);
+            k4::block_size_walk_kernel<<<grid_of(nB * 32), 128, 0, st>>>(b.srcBase, t, nB, walkFr);
             FR_LAUNCH();
             g_launches++;
         }
@@ -2323,6 +2329,13 @@ int32_t k4lz4_unpickle_batch(const uint8_t* srcBase, const int64_t* srcOff, cons
                              int32_t* outLen, int32_t nMessages, int32_t memKind, void* cudaStream,
                              int32_t device) {
     return run(OP_UNPICKLE, Batch{srcBase, srcOff, srcLen, dstBase, dstOff, dstLen, outLen, nMessages},
+               memKind, cudaStream, device);
+}
+
+int32_t k4lz4_decoded_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                 int32_t* outSize, int32_t nBlocks, int32_t memKind, void* cudaStream,
+                                 int32_t device) {
+    return run(OP_DSIZE, Batch{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nBlocks},
                memKind, cudaStream, device);
 }
 

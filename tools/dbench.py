@@ -13,6 +13,10 @@ the same raw bytes compressed as independent blocks.
 S streams x B linked 64 KiB blocks of datagen: one k4lz4_encode_chain_batch call per step (device memory) encodes
 block k of every stream behind its history; GB/s of input over all B steps, next to one k4lz4_encode_batch call
 over the same raw bytes, with the encoder's path counters and a spot check against upstream's chained encoder.
+    python tools/dbench.py --what size [--blocks 65536] [--size-libs scratch/libk4lz4_A.so,...]
+k4lz4_decoded_size_batch over the compressed blocks in device memory: GB/s of compressed input, every size checked
+equal to the block length; other builds (segment length and warm-up, K4_SW_SEG / K4_SW_WARM) alternate with the
+shipped one in three rounds.  The card's name and power limit are printed with it.
 The 32-bit engine (k4lz4_encode_chain_batch_x32, LZ4Codec.Enforce32) runs the same steps in the same process,
 timed alternately with the plain one, with a spot check against upstream's chained encoder built as LL32; the card's
 name and power limit are printed with it.  The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
@@ -42,6 +46,8 @@ ap.add_argument("--check", type=int, default=0, help="encode: compare every CHEC
 ap.add_argument("--lib", default=None, help="alternative build of libk4lz4.so (e.g. a -DK4_DT_PROFILE build under scratch/)")
 ap.add_argument("--streams", default="264,1024,4096", help="chain: stream counts")
 ap.add_argument("--chain-blocks", type=int, default=16, help="chain: linked blocks per stream")
+ap.add_argument("--size-libs", default="", help="size: other builds of libk4lz4.so (tools/build_variant.py), "
+                                                "timed alternately with the shipped one in this process")
 a = ap.parse_args()
 
 
@@ -156,6 +162,35 @@ if a.what in ("decode", "both"):
     algo = (int(clen.sum()) + nb * bs)
     print(f"decode[{a.data}{a.mp}]: {ms:.3f} ms (median {med:.3f})  {nb*bs/ms/1e6:.1f} GB/s out  {algo/ms/1e6:.1f} GB/s algorithmic  "
           f"ok={ok} ratio {ratio:.3f} stats {stats}", flush=True)
+if a.what == "size":
+    import ctypes as C
+    import subprocess
+    poff = torch.cumsum(clen.to(torch.int64), 0) - clen.to(torch.int64)
+    packed = torch.empty(int(clen.sum()) + 64, dtype=torch.uint8, device=dev)
+    B.copy_blocks_device(slots.data_ptr(), coff.data_ptr(), packed.data_ptr(), poff.data_ptr(), clen.data_ptr(), nb, st)
+    osz = torch.zeros(nb, dtype=torch.int32, device=dev)
+    libs = [("shipped", N.lib())] + [(os.path.basename(p), C.CDLL(os.path.abspath(p))) for p in a.size_libs.split(",") if p]
+    def size_call(L):
+        fn = L.k4lz4_decoded_size_batch
+        fn.argtypes, fn.restype = N.SIGNATURES["k4lz4_decoded_size_batch"]
+        return lambda: N.check(fn(packed.data_ptr(), poff.data_ptr(), clen.data_ptr(), osz.data_ptr(), nb, N.MEM_DEVICE,
+                                  st or None, -1))
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True).stdout.strip()
+    cbytes = int(clen.sum())
+    res = {name: [] for name, _ in libs}
+    for _ in range(3):
+        for name, L in libs:
+            f = size_call(L)
+            osz.fill_(-7); f(); torch.cuda.synchronize()
+            ok = bool((osz == bs).all())
+            ms, med = timeit(f, a.reps)
+            res[name].append((ms, med, ok))
+    for name, rs in res.items():
+        best = min(r[0] for r in rs)
+        print(f"size[{a.data}{a.mp}] {name}: {best:.3f} ms (medians {', '.join(f'{r[1]:.3f}' for r in rs)})  "
+              f"{cbytes/best/1e6:.1f} GB/s compressed  {nb*bs/best/1e6:.1f} GB/s decoded  ok={all(r[2] for r in rs)} "
+              f"| {card}", flush=True)
 if a.what == "chain":
     from concurrent.futures import ThreadPoolExecutor
     from tests import chain_ref as CR
