@@ -178,6 +178,24 @@ struct Buf {           // grows, never shrinks: device memory, or pinned host me
     }
 };
 
+// One row of a synchronous host-memory step (stage_up): `send` source bytes at src, with the `pre` bytes in front of
+// them; a destination slot of `room` bytes, with the `dstPre` bytes in front of dst as its history; the table columns
+// stream len cap aux; an optional blob (a dictionary, or a state record that comes back whole to `back`).  dst is
+// where stage_down puts the row's output.
+struct UpRow {
+    const uint8_t* src; int64_t send, room; int32_t stream, len, cap, aux;
+    uint8_t* dst = nullptr;
+    int32_t pre = 0, dstPre = 0;
+    const uint8_t* blob = nullptr; int32_t blobLen = 0; uint8_t* back = nullptr;
+};
+
+// The buffers of the synchronous host-memory path (stage_up / stage_down) and the rows of the step in flight.
+struct Staging {
+    Buf dStage, dDown, hUp{true}, hDown{true};
+    std::vector<UpRow> rows;
+    void release() { for (Buf* b : {&dStage, &dDown, &hUp, &hDown}) b->release(); }
+};
+
 struct Slot {          // one in-flight chunk of the pipelined host path
     cudaStream_t stream = nullptr;
     Buf dSrc, dDst, dMeta, dPack, dPackOff;
@@ -202,8 +220,9 @@ constexpr int NSLOT = 4;                // chunks in flight per device (see run_
 
 // Everything the library keeps per GPU, set up once on first use with that GPU current: its SM count, a
 // PRIVATE stream-ordered memory pool for the decoder's work lists and the encoder's tables (the process-wide
-// default pool is never touched), the encoder's helper stream, the kernels' function attributes and the
-// slots of the pipelined host path (guarded by `mu`).
+// default pool is never touched), the encoder's helper stream, the kernels' function attributes, the
+// slots of the pipelined host path (guarded by `mu`) and the staging of the synchronous host calls (guarded
+// by `stageMu`, so that they never wait behind a pipelined call).
 struct Dev {
     std::once_flag once;
     cudaError_t err = cudaSuccess;
@@ -212,6 +231,8 @@ struct Dev {
     cudaStream_t helper = nullptr;    // side stream of the encoder (encode_launch)
     std::mutex mu;
     Slot slot[NSLOT];
+    std::mutex stageMu;
+    Staging stage;
 };
 
 Dev* dev_state(int dev) {
@@ -730,47 +751,129 @@ int run_host(Op op, const Batch& a, int device) {
     return K4LZ4_OK;
 }
 
-// ---- synchronous host path: dictionary / partial / chained decode and XXH32 ------------------------
+// ---- synchronous host path: one staging routine, used by every host-memory call outside run_host ----------
 
-struct DevMem {         // the call's device buffer: grows with the chunks, freed when the call returns
-    void* p = nullptr; size_t cap = 0;
-    ~DevMem() { if (p) cudaFree(p); }
-    cudaError_t ensure(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        cap = 0;
-        const cudaError_t e = cudaMalloc(&p, n);
-        if (e == cudaSuccess) cap = n; else p = nullptr;
-        return e;
-    }
+constexpr int64_t STAGE_BYTES = 256ll << 20;   // staged bytes per chunk; source bytes per group sub-write / sub-read
+
+// One synchronous host-memory step's upload, in one copy into dStage: the table srcOff dstOff blobOff (int64) |
+// stream len cap aux blobLen (int32) of the m rows row(k) describes, then their sources (the `pre` bytes in front
+// of each go up with it, and the source lands 16-aligned), then their blobs (16-aligned).  Behind it in dStage:
+// resInts * m int32 results, m compact offsets (stage_down), `extra` bytes for the caller, and the rows'
+// destination slots, `room` bytes each at dstOff (16-aligned) with `dstPre` bytes of history in front.  When a row
+// has history the copy extends over the slots, the history filled in from in front of the row's dst.
+struct StageUp {                      // device pointers into dStage
+    const uint8_t* src; const int64_t* srcOff; const int64_t* dstOff; const int64_t* blobOff;
+    const int32_t* stream; const int32_t* len; const int32_t* cap; const int32_t* aux; const int32_t* blobLen;
+    int32_t* res; int64_t* coff; uint8_t* extra; uint8_t* dst; uint8_t* blob;
+    int64_t blobAt, blobBytes;        // where the blobs are in dStage (and were in hUp)
+    bool back;                        // a row's blob comes back (stage_down)
 };
 
-constexpr int64_t STAGE_BYTES = 256ll << 20;   // staged payload per chunk
+template <class Row>
+int stage_up(Staging& S, int64_t m, int64_t resInts, int64_t extra, Row row, StageUp& up, cudaStream_t st) {
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    S.rows.resize((size_t)m);
+    int64_t sp = 0, bp = 0, dp = 0;
+    bool hist = false, back = false;
+    for (int64_t k = 0; k < m; k++) {
+        const UpRow& x = S.rows[(size_t)k] = row(k);
+        sp = a16(sp + x.pre) + x.send; bp = a16(bp) + x.blobLen; dp = a16(dp + x.dstPre) + x.room;
+        hist |= x.dstPre > 0; back |= x.back != nullptr;
+    }
+    const int64_t sendAt = a16(m * (8 * 3 + 4 * 5)), blobAt = sendAt + a16(sp), blobBytes = a16(bp);
+    const int64_t resAt = blobAt + blobBytes, coffAt = resAt + a16(m * 4 * resInts), extraAt = coffAt + a16(m * 8);
+    const int64_t dstAt = extraAt + a16(extra), upBytes = hist ? dstAt + dp : resAt;
+    CU_TRY(S.hUp.ensure((size_t)std::max(upBytes, m * 8) + 16));   // stage_down sends the compact offsets through it
+    CU_TRY(S.dStage.ensure((size_t)(dstAt + dp) + 16));
+    uint8_t* H = (uint8_t*)S.hUp.p;
+    int64_t* hso = (int64_t*)H; int64_t* hdo = hso + m; int64_t* hbo = hdo + m;
+    int32_t* hs = (int32_t*)(hbo + m); int32_t* hl = hs + m; int32_t* hc = hl + m; int32_t* ha = hc + m; int32_t* hb = ha + m;
+    sp = bp = dp = 0;
+    for (int64_t k = 0; k < m; k++) {
+        const UpRow& x = S.rows[(size_t)k];
+        hs[k] = x.stream; hl[k] = x.len; hc[k] = x.cap; ha[k] = x.aux; hb[k] = x.blobLen;
+        hso[k] = a16(sp + x.pre); hbo[k] = a16(bp); hdo[k] = a16(dp + x.dstPre);
+        sp = hso[k] + x.send; bp = hbo[k] + x.blobLen; dp = hdo[k] + x.room;
+    }
+    parallel_for_blocks(0, m, upBytes, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++) {
+            const UpRow& x = S.rows[(size_t)k];
+            if (x.pre + x.send > 0) memcpy(H + sendAt + hso[k] - x.pre, x.src - x.pre, (size_t)(x.pre + x.send));
+            if (x.blobLen > 0) memcpy(H + blobAt + hbo[k], x.blob, (size_t)x.blobLen);
+            if (x.dstPre > 0) memcpy(H + dstAt + hdo[k] - x.dstPre, x.dst - x.dstPre, (size_t)x.dstPre);
+        }
+    });
+    uint8_t* D = (uint8_t*)S.dStage.p;
+    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
+    const int64_t* dso = (const int64_t*)D;
+    const int32_t* ds = (const int32_t*)(dso + 3 * m);
+    up = StageUp{D + sendAt, dso, dso + m, dso + 2 * m, ds, ds + m, ds + 2 * m, ds + 3 * m, ds + 4 * m,
+                 (int32_t*)(D + resAt), (int64_t*)(D + coffAt), D + extraAt, D + dstAt, D + blobAt, blobAt, blobBytes, back};
+    return K4LZ4_OK;
+}
 
-// One GPU, no pipelining: per chunk of at most STAGE_BYTES, everything the kernel reads is packed into one
-// host buffer -- the block table, the sources, the dictionaries (when the batch has them) and, with a
-// prefix, the destination slots [history | capacity] (16-aligned, history filled in: all the decoder reads
-// of a stream is its last <= 65535 bytes) -- and goes up in one copy.  The chained encoder's history goes in
-// front of its source instead ([history | source], 16-aligned) and its state records (16-aligned) go up and
-// come back whole.  The results and the destination region come back, and exactly outLen[i] > 0 bytes of
-// each block are copied to the caller.  A batch without dstCap (XXH32) has no destination: its per-block
+// One synchronous host-memory step's download, behind the device work on `st`: the resInts * m results come back
+// into hRes (the first m are the rows' lengths), and each row's blob comes back whole to its `back` where it has
+// one.  With a gather source, row k's hRes[k] bytes at from + fromOff[k] on the device are gathered into dDown where
+// any is positive, come down in one copy and go to the row's dst, exactly hRes[k] > 0 bytes each; without one
+// (from == nullptr) only the results come down, as their positive values need not be byte counts.  `after` (may be
+// empty) is enqueued behind the gather, or alone when nothing was produced, and the call waits for it.
+int stage_down(Staging& S, const StageUp& up, int64_t m, int32_t* hRes, int64_t resInts, const uint8_t* from,
+               const int64_t* fromOff, const std::function<cudaError_t()>& after, cudaStream_t st) {
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    uint8_t* H = (uint8_t*)S.hUp.p;
+    CU_TRY(cudaMemcpyAsync(hRes, up.res, (size_t)(m * 4 * resInts), cudaMemcpyDeviceToHost, st));
+    if (up.back) CU_TRY(cudaMemcpyAsync(H + up.blobAt, up.blob, (size_t)up.blobBytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    const int64_t* hbo = (const int64_t*)H + 2 * m;     // stage_up's table, still in hUp
+    for (int64_t k = 0; up.back && k < m; k++) {
+        const UpRow& x = S.rows[(size_t)k];
+        if (x.back) memcpy(x.back, H + up.blobAt + hbo[k], (size_t)x.blobLen);
+    }
+    std::vector<int64_t> co((size_t)m);
+    int64_t total = 0;
+    for (int64_t k = 0; from && k < m; k++) { co[(size_t)k] = total; if (hRes[k] > 0) total = a16(total + hRes[k]); }
+    if (total == 0) {
+        if (after) { CU_TRY(after()); CU_TRY(cudaStreamSynchronize(st)); }
+        return K4LZ4_OK;
+    }
+    CU_TRY(S.dDown.ensure((size_t)total + 16));
+    CU_TRY(S.hDown.ensure((size_t)total + 16));
+    memcpy(H, co.data(), (size_t)m * 8);            // the upload buffer is free again
+    CU_TRY(cudaMemcpyAsync(up.coff, H, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+    CU_TRY(launch_op(OP_COPY, Batch{from, fromOff, up.res, (uint8_t*)S.dDown.p, up.coff, nullptr, nullptr, m}, st));
+    if (after) CU_TRY(after());
+    CU_TRY(cudaMemcpyAsync(S.hDown.p, S.dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    const uint8_t* stage = (const uint8_t*)S.hDown.p;
+    parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
+        for (int64_t k = lo; k < hi; k++)
+            if (hRes[k] > 0) memcpy(S.rows[(size_t)k].dst, stage + co[(size_t)k], (size_t)hRes[k]);
+    });
+    return K4LZ4_OK;
+}
+
+// Dictionary / partial / chained decode, chained encode, XXH32 and decoded sizes: one GPU, on the legacy default
+// stream, in chunks of whole blocks of at most STAGE_BYTES through the device's staging.  Chained decode's history
+// (the last <= 65535 bytes in front of each destination: all the decoder reads) goes in front of its slot, the
+// chained encoder's in front of its source; the dictionaries and the encoder's state records are the blobs, and the
+// state records come back whole.  A batch without dstCap (XXH32, decoded sizes) has no destination: its per-block
 // result is the whole output.
 int run_staged(Op op, const Batch& b, int dev) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
+    Dev* D = dev_state(dev);
+    if (!D) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
+    std::lock_guard<std::mutex> lk(D->stageMu);
     const bool dict = b.dictBase != nullptr, prefix = b.prefixLen != nullptr, dst = b.dstCap != nullptr;
     const bool enc = op == OP_ENCCHAIN;
     constexpr int64_t SB = K4LZ4_CHAIN_STATE_BYTES;
-    auto hist = [&](int64_t i) -> int64_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
+    auto hist = [&](int64_t i) -> int32_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
     auto cap = [&](int64_t i) -> int64_t {      // the encoder never writes more than compressBound(srcLen)
         const int64_t c = dst ? std::max<int32_t>(b.dstCap[i], 0) : 0;
         return enc ? std::min<int64_t>(c, b.srcLen[i] > 0 ? k4::max_output_size(b.srcLen[i]) : 0) : c;
     };
-    auto dlen = [&](int64_t i) -> int64_t { return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0; };
-    auto up = [](int64_t x) { return (x + 255) & ~int64_t(255); };
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
-    std::vector<uint8_t> h;          // reused by every chunk: the kernel reads only bytes the chunk has written
-    DevMem d;
+    auto dlen = [&](int64_t i) -> int32_t { return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0; };
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
         for (j = i; j < b.n; j++) {
@@ -779,58 +882,29 @@ int run_staged(Op op, const Batch& b, int dev) {
             bytes += add;
         }
         const int64_t nb = j - i;
-        // block table: srcOff dstOff dictOff stateOff (int64) | srcLen dstCap dictLen prefixLen outLen (int32)
-        int64_t sTot = 0, diTot = 0, dTot = 0;
-        for (int64_t k = 0; k < nb; k++) {
-            sTot = (enc ? a16(sTot + hist(i + k)) : sTot) + src_size(b, i + k);
-            diTot += dlen(i + k);
-            dTot = (prefix && !enc ? a16(dTot + hist(i + k)) : dTot) + cap(i + k);
-        }
-        const int64_t stTot = enc ? nb * SB : 0;
-        const int64_t srcAt = up(nb * (4 * 8 + 5 * 4)), dictAt = up(srcAt + sTot), stateAt = up(dictAt + diTot);
-        const int64_t dstAt = up(stateAt + stTot);
-        const int64_t total = dstAt + dTot;
-        if (h.size() < (size_t)total + 16) h.resize((size_t)total + 16);
-        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* dio = doff + nb; int64_t* sto = dio + nb;
-        int32_t* sl = (int32_t*)(sto + nb); int32_t* dc = sl + nb; int32_t* dl = dc + nb; int32_t* pl = dl + nb;
-        int32_t* res = pl + nb;
-        for (int64_t k = 0, sp = 0, dip = 0, dp = 0; k < nb; k++) {
-            const int64_t x = i + k, hl = hist(x);
-            sl[k] = b.srcLen[x]; dc[k] = dst ? b.dstCap[x] : 0; dl[k] = (int32_t)dlen(x);
-            pl[k] = enc ? b.prefixLen[x] : (int32_t)hl;   // the encoder's dictSize clamp needs the caller's value
-            so[k] = enc ? a16(sp + hl) : sp; dio[k] = dip; sto[k] = k * SB;
-            doff[k] = prefix && !enc ? a16(dp + hl) : dp;
-            if (enc && hl > 0) memcpy(h.data() + srcAt + so[k] - hl, b.srcBase + b.srcOff[x] - hl, (size_t)hl);
-            if (sl[k] > 0) memcpy(h.data() + srcAt + so[k], b.srcBase + b.srcOff[x], (size_t)sl[k]);
-            if (dl[k] > 0) memcpy(h.data() + dictAt + dip, b.dictBase + b.dictOff[x], (size_t)dl[k]);
-            if (enc) memcpy(h.data() + stateAt + sto[k], b.stateBase + b.stateOff[x], (size_t)SB);
-            else if (prefix && hl > 0) memcpy(h.data() + dstAt + doff[k] - hl, b.dstBase + b.dstOff[x] - hl, (size_t)hl);
-            sp = so[k] + src_size(b, x); dip += dl[k]; dp = doff[k] + cap(x);
-        }
-        CU_TRY(d.ensure((size_t)total + 16));
-        uint8_t* D = (uint8_t*)d.p;
-        CU_TRY(cudaMemcpy(D, h.data(), (size_t)(prefix && !enc ? total : dstAt), cudaMemcpyHostToDevice));
-        int32_t* dRes = (int32_t*)(D + ((uint8_t*)res - h.data()));
+        StageUp up;
+        int rc = stage_up(D->stage, nb, 1, 0, [&](int64_t k) {
+            const int64_t x = i + k;
+            const int32_t hl = hist(x);
+            // the encoder's dictSize clamp needs the caller's prefixLen
+            UpRow r{b.srcBase + b.srcOff[x], src_size(b, x), cap(x), 0, b.srcLen[x], dst ? b.dstCap[x] : 0,
+                    enc ? b.prefixLen[x] : hl, dst ? b.dstBase + b.dstOff[x] : nullptr};
+            if (enc) { r.pre = hl; r.blob = r.back = b.stateBase + b.stateOff[x]; r.blobLen = (int32_t)SB; }
+            else r.dstPre = hl;
+            if (dict) { r.blob = b.dictBase + b.dictOff[x]; r.blobLen = dlen(x); }
+            return r;
+        }, up, nullptr);
+        if (rc != K4LZ4_OK) return rc;
         Batch kb = b;                                // the same batch, on the device
-        kb.srcBase = D + srcAt; kb.srcOff = (int64_t*)D; kb.srcLen = (int32_t*)(D + ((uint8_t*)sl - h.data()));
-        kb.dstBase = D + dstAt; kb.dstOff = kb.srcOff + nb; kb.dstCap = dst ? kb.srcLen + nb : nullptr;
-        kb.dictBase = dict ? D + dictAt : nullptr; kb.dictOff = kb.srcOff + 2 * nb; kb.dictLen = kb.srcLen + 2 * nb;
-        kb.prefixLen = prefix ? kb.srcLen + 3 * nb : nullptr;
-        kb.stateBase = enc ? D + stateAt : nullptr; kb.stateOff = enc ? kb.srcOff + 3 * nb : nullptr;
-        kb.outLen = dRes; kb.n = nb;
+        kb.srcBase = up.src; kb.srcOff = up.srcOff; kb.srcLen = up.len;
+        kb.dstBase = up.dst; kb.dstOff = up.dstOff; kb.dstCap = dst ? up.cap : nullptr;
+        kb.dictBase = dict ? up.blob : nullptr; kb.dictOff = up.blobOff; kb.dictLen = up.blobLen;
+        kb.prefixLen = prefix ? up.aux : nullptr;
+        kb.stateBase = enc ? up.blob : nullptr; kb.stateOff = up.blobOff;
+        kb.outLen = up.res; kb.n = nb;
         CU_TRY(launch_op(op, kb, nullptr));
-        CU_TRY(cudaMemcpy(b.outLen + i, dRes, (size_t)nb * 4, cudaMemcpyDeviceToHost));
-        if (enc) {
-            CU_TRY(cudaMemcpy(h.data() + stateAt, D + stateAt, (size_t)stTot, cudaMemcpyDeviceToHost));
-            for (int64_t k = 0; k < nb; k++)
-                memcpy(b.stateBase + b.stateOff[i + k], h.data() + stateAt + sto[k], (size_t)SB);
-        }
-        if (!dst || dTot == 0) continue;
-        CU_TRY(cudaMemcpy(h.data() + dstAt, D + dstAt, (size_t)dTot, cudaMemcpyDeviceToHost));
-        for (int64_t k = 0; k < nb; k++) {
-            const int32_t r = b.outLen[i + k];
-            if (r > 0) memcpy(b.dstBase + b.dstOff[i + k], h.data() + dstAt + doff[k], (size_t)r);
-        }
+        rc = stage_down(D->stage, up, nb, b.outLen + i, 1, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
+        if (rc != K4LZ4_OK) return rc;
     }
     return K4LZ4_OK;
 }
@@ -1144,10 +1218,9 @@ cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_
 }
 
 // Host memory, one GPU, synchronous: chunks of whole frames (a frame is never split: its linked blocks and its
-// content checksum need all of it).  Per chunk, the offsets, lengths and packed frames go up in one copy; the
-// device path runs on them; the results come down, the produced bytes are gathered on the device and come down in
-// one copy, and exactly outLen[i] > 0 bytes of each frame go to the caller.  The device region of a frame is
-// min(dstCap, frame bound) when encoding (a frame never needs more) and dstCap when decoding.
+// content checksum need all of it) through the device's staging, the device path on each, on the legacy default
+// stream.  The device region of a frame is min(dstCap, frame bound) when encoding (a frame never needs more) and
+// dstCap when decoding; content sizes have none.
 int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
@@ -1155,15 +1228,16 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
         for (int64_t i = 0; i < b.n; i++) b.outLen[i] = K4LZ4_R_DELEGATE;
         return K4LZ4_OK;
     }
+    Dev* D = dev_state(dev);
+    if (!D) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
+    std::lock_guard<std::mutex> lk(D->stageMu);
+    const bool dst = fo != FO_SIZE;
     auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
     auto room = [&](int64_t i) -> int64_t {
-        if (fo == FO_SIZE) return 0;
+        if (!dst) return 0;
         const int64_t c = std::max<int32_t>(b.dstCap[i], 0);
         return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags)) : c;
     };
-    std::vector<uint8_t> h;
-    std::vector<int64_t> pack;
-    DevMem d;
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
         for (j = i; j < b.n; j++) {
@@ -1172,49 +1246,20 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
             bytes += add;
         }
         const int64_t nb = j - i;
-        // up: srcOff dstOff packOff (int64) | srcLen dstCap outLen (int32) | frames; then the regions and the pack
-        const int64_t srcAt = a16(nb * (3 * 8 + 3 * 4));
-        int64_t sTot = 0, dTot = 0;
-        for (int64_t k = 0; k < nb; k++) { sTot += a16(src_size(b, i + k)); dTot += a16(room(i + k)); }
-        const int64_t dstAt = a16(srcAt + sTot), packAt = a16(dstAt + dTot), total = packAt + dTot;
-        if (h.size() < (size_t)srcAt + (size_t)sTot + 16) h.resize((size_t)srcAt + (size_t)sTot + 16);
-        int64_t* so = (int64_t*)h.data(); int64_t* doff = so + nb; int64_t* po = doff + nb;
-        int32_t* sl = (int32_t*)(po + nb); int32_t* dc = sl + nb; int32_t* res = dc + nb;
-        for (int64_t k = 0, sp = 0, dp = 0; k < nb; k++) {
+        StageUp up;
+        int rc = stage_up(D->stage, nb, 1, 0, [&](int64_t k) {
             const int64_t x = i + k, s = src_size(b, x), r = room(x);
-            so[k] = sp; doff[k] = dp; sl[k] = (int32_t)s; dc[k] = (int32_t)r; po[k] = 0;
-            sp += a16(s); dp += a16(r);
-        }
-        parallel_for_blocks(0, nb, sTot, [&](int64_t lo, int64_t hi) {
-            for (int64_t k = lo; k < hi; k++)
-                if (sl[k] > 0) memcpy(h.data() + srcAt + so[k], b.srcBase + b.srcOff[i + k], (size_t)sl[k]);
-        });
-        CU_TRY(d.ensure((size_t)total + 16));
-        uint8_t* Dp = (uint8_t*)d.p;
-        CU_TRY(cudaMemcpy(Dp, h.data(), (size_t)(srcAt + sTot), cudaMemcpyHostToDevice));
+            return UpRow{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, 0, dst ? b.dstBase + b.dstOff[x] : nullptr};
+        }, up, nullptr);
+        if (rc != K4LZ4_OK) return rc;
         Batch kb = b;
-        kb.srcBase = Dp + srcAt; kb.srcOff = (int64_t*)Dp; kb.srcLen = (int32_t*)(Dp + ((uint8_t*)sl - h.data()));
-        kb.dstBase = Dp + dstAt; kb.dstOff = kb.srcOff + nb; kb.dstCap = fo == FO_SIZE ? nullptr : kb.srcLen + nb;
-        kb.outLen = (int32_t*)(Dp + ((uint8_t*)res - h.data())); kb.n = nb;
+        kb.srcBase = up.src; kb.srcOff = up.srcOff; kb.srcLen = up.len;
+        kb.dstBase = up.dst; kb.dstOff = up.dstOff; kb.dstCap = dst ? up.cap : nullptr;
+        kb.outLen = up.res; kb.n = nb;
         const cudaError_t e = frame_dev(fo, kb, bs, flags, header, nullptr);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
-        CU_TRY(cudaMemcpy(b.outLen + i, kb.outLen, (size_t)nb * 4, cudaMemcpyDeviceToHost));
-        if (fo == FO_SIZE) continue;
-        pack.resize((size_t)nb);
-        int64_t got = 0;
-        for (int64_t k = 0; k < nb; k++) { pack[(size_t)k] = got; if (b.outLen[i + k] > 0) got = a16(got + b.outLen[i + k]); }
-        if (got == 0) continue;
-        CU_TRY(cudaMemcpy(Dp + ((uint8_t*)po - h.data()), pack.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
-        CU_TRY(launch_op(OP_COPY, Batch{kb.dstBase, kb.dstOff, kb.outLen, Dp + packAt, (int64_t*)(Dp + ((uint8_t*)po - h.data())),
-                                        nullptr, nullptr, nb}, nullptr));
-        if (h.size() < (size_t)got + 16) { h.resize((size_t)got + 16); }
-        CU_TRY(cudaMemcpy(h.data(), Dp + packAt, (size_t)got, cudaMemcpyDeviceToHost));
-        parallel_for_blocks(0, nb, got, [&](int64_t lo, int64_t hi) {
-            for (int64_t k = lo; k < hi; k++) {
-                const int32_t r = b.outLen[i + k];
-                if (r > 0) memcpy(b.dstBase + b.dstOff[i + k], h.data() + pack[(size_t)k], (size_t)r);
-            }
-        });
+        rc = stage_down(D->stage, up, nb, b.outLen + i, 1, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
+        if (rc != K4LZ4_OK) return rc;
     }
     return K4LZ4_OK;
 }
@@ -1249,7 +1294,7 @@ struct GroupCore {
     int64_t ring = 0, slot = 0;       // bytes per ring; the room a block or an injection may need at the write position
     uint8_t* rings = nullptr;
     k4::ChainGroupHdr* hdr = nullptr;
-    Buf dStage, dDown, hUp{true}, hDown{true};
+    Staging stage;
     std::vector<void*> owned;
     cudaError_t allocErr = cudaSuccess;   // the first failure of alloc(), after which it allocates nothing
 
@@ -1264,7 +1309,7 @@ struct GroupCore {
     }
     ~GroupCore() {
         for (void* p : owned) cudaFree(p);
-        for (Buf* b : {&dStage, &dDown, &hUp, &hDown}) b->release();
+        stage.release();
     }
 };
 
@@ -1333,11 +1378,11 @@ int group_streams_run(GroupCore* g, const int32_t* streams, int32_t n, int memKi
     cudaStream_t st = (cudaStream_t)stream;
     const int32_t* ds = streams;
     if (memKind == K4LZ4_MEM_HOST) {
-        CU_TRY(g->hUp.ensure((size_t)n * 4));
-        CU_TRY(g->dStage.ensure((size_t)n * 8));
-        memcpy(g->hUp.p, streams, (size_t)n * 4);
-        CU_TRY(cudaMemcpyAsync(g->dStage.p, g->hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        ds = (const int32_t*)g->dStage.p;
+        CU_TRY(g->stage.hUp.ensure((size_t)n * 4));
+        CU_TRY(g->stage.dStage.ensure((size_t)n * 8));
+        memcpy(g->stage.hUp.p, streams, (size_t)n * 4);
+        CU_TRY(cudaMemcpyAsync(g->stage.dStage.p, g->stage.hUp.p, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        ds = (const int32_t*)g->stage.dStage.p;
     }
     CU_TRY(enqueue(ds, st));
     if (memKind == K4LZ4_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
@@ -1384,85 +1429,6 @@ int check_step(const GroupCore* g, const Batch& b, const int32_t* streams, bool 
 }
 
 const auto no_entry_check = [](int64_t) { return K4LZ4_OK; };
-
-// One host-memory step's upload, in one copy into dStage: the table srcOff dstOff (int64) | stream len cap aux
-// (int32) of the m entries row(k) describes, then their `send` source bytes packed 16-aligned.  Behind it in dStage:
-// resInts * m int32 results, m compact offsets (stage_down), `extra` bytes for the caller, and the entries'
-// destination slots, `room` bytes each at dstOff (16-aligned).
-struct UpRow { const uint8_t* src; int64_t send, room; int32_t stream, len, cap, aux; };
-struct StageUp {                      // device pointers into dStage
-    const uint8_t* src; const int64_t* srcOff; const int64_t* dstOff;
-    const int32_t* stream; const int32_t* len; const int32_t* cap; const int32_t* aux;
-    int32_t* res; int64_t* coff; uint8_t* extra; uint8_t* dst;
-};
-
-template <class Row>
-int stage_up(GroupCore* g, int64_t m, int64_t resInts, int64_t extra, Row row, StageUp& up, cudaStream_t st) {
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
-    std::vector<UpRow> r((size_t)m);
-    int64_t srcBytes = 0, dstBytes = 0;
-    for (int64_t k = 0; k < m; k++) {
-        r[(size_t)k] = row(k);
-        srcBytes += a16(r[(size_t)k].send); dstBytes += a16(r[(size_t)k].room);
-    }
-    const int64_t sendAt = a16(m * (8 * 2 + 4 * 4)), upBytes = sendAt + srcBytes;
-    const int64_t resAt = a16(upBytes), coffAt = resAt + a16(m * 4 * resInts), extraAt = coffAt + a16(m * 8);
-    const int64_t dstAt = extraAt + a16(extra);
-    CU_TRY(g->hUp.ensure((size_t)std::max(upBytes, m * 8) + 16));   // stage_down sends the compact offsets through it
-    CU_TRY(g->dStage.ensure((size_t)(dstAt + dstBytes) + 16));
-    uint8_t* H = (uint8_t*)g->hUp.p;
-    int64_t* hso = (int64_t*)H; int64_t* hdo = hso + m;
-    int32_t* hs = (int32_t*)(hdo + m); int32_t* hl = hs + m; int32_t* hc = hl + m; int32_t* ha = hc + m;
-    for (int64_t k = 0, sp = 0, dp = 0; k < m; k++) {
-        const UpRow& x = r[(size_t)k];
-        hs[k] = x.stream; hl[k] = x.len; hc[k] = x.cap; ha[k] = x.aux;
-        hso[k] = sp; hdo[k] = dp;
-        sp += a16(x.send); dp += a16(x.room);
-    }
-    parallel_for_blocks(0, m, srcBytes, [&](int64_t lo, int64_t hi) {
-        for (int64_t k = lo; k < hi; k++)
-            if (r[(size_t)k].send > 0) memcpy(H + sendAt + hso[k], r[(size_t)k].src, (size_t)r[(size_t)k].send);
-    });
-    uint8_t* D = (uint8_t*)g->dStage.p;
-    CU_TRY(cudaMemcpyAsync(D, H, (size_t)upBytes, cudaMemcpyHostToDevice, st));
-    const int32_t* ds = (const int32_t*)(D + m * 16);
-    up = StageUp{D + sendAt, (const int64_t*)D, (const int64_t*)D + m, ds, ds + m, ds + 2 * m, ds + 3 * m,
-                 (int32_t*)(D + resAt), (int64_t*)(D + coffAt), D + extraAt, D + dstAt};
-    return K4LZ4_OK;
-}
-
-// One host-memory step's download, behind the device work on `st`: the resInts * m results come back into hRes (the
-// first m are the entries' lengths) and, where any is positive, entry k's hRes[k] bytes at from + fromOff[k] on the
-// device are gathered into dDown and come down in one copy, then go to to(k), exactly hRes[k] > 0 bytes each.
-// `after` (may be empty) is enqueued behind the gather, or alone when nothing was produced, and the call waits for it.
-template <class To>
-int stage_down(GroupCore* g, const StageUp& up, int64_t m, int32_t* hRes, int64_t resInts, const uint8_t* from,
-               const int64_t* fromOff, const std::function<cudaError_t()>& after, To to, cudaStream_t st) {
-    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
-    CU_TRY(cudaMemcpyAsync(hRes, up.res, (size_t)(m * 4 * resInts), cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    std::vector<int64_t> co((size_t)m);
-    int64_t total = 0;
-    for (int64_t k = 0; k < m; k++) { co[(size_t)k] = total; if (hRes[k] > 0) total = a16(total + hRes[k]); }
-    if (total == 0) {
-        if (after) { CU_TRY(after()); CU_TRY(cudaStreamSynchronize(st)); }
-        return K4LZ4_OK;
-    }
-    CU_TRY(g->dDown.ensure((size_t)total + 16));
-    CU_TRY(g->hDown.ensure((size_t)total + 16));
-    memcpy(g->hUp.p, co.data(), (size_t)m * 8);     // the upload buffer is free again
-    CU_TRY(cudaMemcpyAsync(up.coff, g->hUp.p, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(launch_op(OP_COPY, Batch{from, fromOff, up.res, (uint8_t*)g->dDown.p, up.coff, nullptr, nullptr, m}, st));
-    if (after) CU_TRY(after());
-    CU_TRY(cudaMemcpyAsync(g->hDown.p, g->dDown.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    const uint8_t* stage = (const uint8_t*)g->hDown.p;
-    parallel_for_blocks(0, m, total, [&](int64_t lo, int64_t hi) {
-        for (int64_t k = lo; k < hi; k++)
-            if (hRes[k] > 0) memcpy(to(k), stage + co[(size_t)k], (size_t)hRes[k]);
-    });
-    return K4LZ4_OK;
-}
 
 // ---- chain groups -----------------------------------------------------------------------------------
 
@@ -1538,13 +1504,13 @@ int group_host(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* stre
     const int64_t n = b.n;
     const bool enc = cg == k4::CG_ENCODE, inj = cg == k4::CG_INJECT;
     StageUp up;
-    const int rc = stage_up(g, n, 1, n * TABLE_BYTES, [&](int64_t i) {
+    const int rc = stage_up(g->stage, n, 1, n * TABLE_BYTES, [&](int64_t i) {
         const int32_t L = b.srcLen[i];
         const bool fits = L > 0 && L <= g->blockSize;
         const int64_t send = L <= 0 ? 0 : inj ? std::min<int64_t>(L, k4::CG_WINDOW) : enc && !fits ? 0 : L;
         const int64_t room = enc && fits ? std::min<int64_t>(std::max<int32_t>(b.dstCap[i], 0), k4::max_output_size(L)) : 0;
         return UpRow{send > 0 ? b.srcBase + b.srcOff[i] + (L - send) : nullptr, send, room, streams[i],
-                     inj ? (int32_t)send : L, inj ? 0 : b.dstCap[i], 0};
+                     inj ? (int32_t)send : L, inj ? 0 : b.dstCap[i], 0, inj ? nullptr : b.dstBase + b.dstOff[i]};
     }, up, st);
     if (rc != K4LZ4_OK) return rc;
     Batch kb = b;
@@ -1557,8 +1523,7 @@ int group_host(k4lz4_chain_group* g, int cg, const Batch& b, const int32_t* stre
     if (e == cudaSuccess && inj) e = commit();
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "chain group step: %s", cudaGetErrorString(e)); }
     if (inj) { CU_TRY(cudaStreamSynchronize(st)); return K4LZ4_OK; }
-    return stage_down(g, up, n, b.outLen, 1, enc ? up.dst : g->rings, enc ? up.dstOff : t.ringOff, commit,
-                      [&](int64_t i) { return b.dstBase + b.dstOff[i]; }, st);
+    return stage_down(g->stage, up, n, b.outLen, 1, enc ? up.dst : g->rings, enc ? up.dstOff : t.ringOff, commit, st);
 }
 
 int group_run(k4lz4_chain_group* g, int kind, int cg, const Batch& b, const int32_t* streams, int memKind, void* stream) {
@@ -1592,8 +1557,6 @@ struct k4lz4_frame_writer_group : GroupCore {
 };
 
 namespace {
-
-constexpr int64_t FW_STAGE_BYTES = 256ll << 20;   // source bytes of one host-memory sub-write
 
 // One write (or close) of b.n entries in device memory on `st`: plan, the content checksum, one host
 // synchronisation for the number of steps (a close has at most one and does not wait), the steps over chunks of at
@@ -1697,26 +1660,25 @@ int fw_host_part(k4lz4_frame_writer_group* g, bool closing, const Batch& b, cons
     const int64_t m = (int64_t)idx.size();
     const int64_t cb = k4::fw_close_bound(g->B, g->bc(), g->cc());
     StageUp up;
-    const int rc = stage_up(g, m, 1, 0, [&](int64_t k) {
+    const int rc = stage_up(g->stage, m, 1, 0, [&](int64_t k) {
         const int64_t room = closing ? std::min<int64_t>(std::max<int32_t>(b.dstCap[idx[k]], 0), cb)
                                      : k4::fw_write_bound(piece[k], g->B, g->bc());
         return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[idx[k]] + srcAt[k] : nullptr, piece[k], room,
-                     streams[idx[k]], (int32_t)piece[k], (int32_t)room, 0};
+                     streams[idx[k]], (int32_t)piece[k], (int32_t)room, 0, b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k]};
     }, up, st);
     if (rc != K4LZ4_OK) return rc;
     const Batch kb{up.src, up.srcOff, up.len, up.dst, up.dstOff, up.cap, up.res, m, g->level, b.x32};
     const cudaError_t e = fw_device(g, closing, kb, up.stream, st);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame writer step: %s", cudaGetErrorString(e)); }
     res.resize((size_t)m);
-    const int rd = stage_down(g, up, m, res.data(), 1, up.dst, up.dstOff, nullptr,
-                              [&](int64_t k) { return b.dstBase + b.dstOff[idx[k]] + wrote[(size_t)k]; }, st);
+    const int rd = stage_down(g->stage, up, m, res.data(), 1, up.dst, up.dstOff, nullptr, st);
     if (rd != K4LZ4_OK) return rd;
     for (int64_t k = 0; k < m; k++) if (res[(size_t)k] > 0) wrote[(size_t)k] += res[(size_t)k];
     return K4LZ4_OK;
 }
 
 // Host memory: entries whose capacity is below their bound get -1 and are left out; the others are written in
-// sub-writes of at most FW_STAGE_BYTES source bytes, in entry order (cutting a write in two changes nothing of what
+// sub-writes of at most STAGE_BYTES source bytes, in entry order (cutting a write in two changes nothing of what
 // a stream emits).  The first sub-write lists every such entry, so that a 0-byte write still opens its frame.
 int fw_host(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int32_t* streams, cudaStream_t st) {
     std::vector<int32_t> res;
@@ -1736,7 +1698,7 @@ int fw_host(k4lz4_frame_writer_group* g, bool closing, const Batch& b, const int
     std::vector<int64_t> used(all.size(), 0), total(all.size(), 0);
     for (bool first = true;; first = false) {
         std::vector<int64_t> idx, at, piece, wrote, which;
-        int64_t budget = FW_STAGE_BYTES;
+        int64_t budget = STAGE_BYTES;
         for (size_t k = 0; k < all.size(); k++) {
             const int64_t take = std::min(src_size(b, all[k]) - used[k], budget);
             if (!first && take == 0) continue;
@@ -1948,7 +1910,7 @@ cudaError_t fr_device(k4lz4_frame_reader_group* g, int mode, const Batch& b, con
     return cudaSuccess;
 }
 
-// Host memory, synchronous: sub-reads of at most FW_STAGE_BYTES chunk bytes, in entry order.  Each sub-read is
+// Host memory, synchronous: sub-reads of at most STAGE_BYTES chunk bytes, in entry order.  Each sub-read is
 // one fr_device call on stage_up's table -- cap / aux: a plain read's dstCap and the blocks earlier sub-reads
 // decoded, or the room a byte read has left (dstCap minus the bytes earlier sub-reads appended) -- and its output
 // comes down behind it, exactly outLen bytes per entry.  The first sub-read lists every entry, so that a byte read
@@ -1972,7 +1934,7 @@ int fr_host(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t
     for (int64_t i = 0; i < n; i++) { b.outLen[i] = 0; srcUsed[i] = 0; frameEnded[i] = 0; }
     for (bool first = true;; first = false) {
         std::vector<int64_t> idx, at, piece;
-        int64_t budget = FW_STAGE_BYTES;
+        int64_t budget = STAGE_BYTES;
         for (int64_t i = 0; i < n; i++) {
             if (!active[(size_t)i]) continue;
             if (!first && budget == 0) break;
@@ -1984,11 +1946,12 @@ int fr_host(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t
         if (idx.empty()) break;
         const int64_t m = (int64_t)idx.size();
         StageUp up;
-        const int rc = stage_up(g, m, 4, m * 8, [&](int64_t k) {
+        const int rc = stage_up(g->stage, m, 4, m * 8, [&](int64_t k) {
             const int64_t i = idx[(size_t)k];
             const int64_t room = std::max<int64_t>(b.dstCap[i], 0) - outTot[(size_t)i];
             return UpRow{piece[k] > 0 ? b.srcBase + b.srcOff[i] + at[k] : nullptr, piece[k], 0, streams[i],
-                         (int32_t)piece[k], bytes ? (int32_t)room : b.dstCap[i], bytes ? 0 : spentTot[(size_t)i]};
+                         (int32_t)piece[k], bytes ? (int32_t)room : b.dstCap[i], bytes ? 0 : spentTot[(size_t)i],
+                         b.dstBase + b.dstOff[i] + outTot[(size_t)i]};
         }, up, st);
         if (rc != K4LZ4_OK) return rc;
         int64_t* dOff = (int64_t*)up.extra;
@@ -2000,9 +1963,7 @@ int fr_host(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t
             e = fr_device(g, mode, kb, up.stream, up.res + m, up.res + 2 * m, up.aux, up.res + 3 * m, dOff, &stage, P, st);
             if (e == cudaSuccess) {
                 std::vector<int32_t> down((size_t)m * 4);
-                const int rd = stage_down(g, up, m, down.data(), 4, stage, dOff, nullptr, [&](int64_t k) {
-                    return b.dstBase + b.dstOff[idx[(size_t)k]] + outTot[(size_t)idx[(size_t)k]];
-                }, st);
+                const int rd = stage_down(g->stage, up, m, down.data(), 4, stage, dOff, nullptr, st);
                 if (rd != K4LZ4_OK) return rd;
                 for (int64_t k = 0; k < m; k++) {
                     const int64_t i = idx[(size_t)k];
@@ -2046,7 +2007,7 @@ int fr_run(k4lz4_frame_reader_group* g, int mode, const Batch& b, const int32_t*
     if (!reading)             // with host memory the statuses come back from behind the stream list in dStage
         return group_streams_run(g, streams, n, memKind, stream, [&](const int32_t* ds, cudaStream_t st) {
             const bool host = memKind == K4LZ4_MEM_HOST;
-            int32_t* dStatus = host ? (int32_t*)g->dStage.p + n : b.outLen;
+            int32_t* dStatus = host ? (int32_t*)g->stage.dStage.p + n : b.outLen;
             k4::frame_reader_end_kernel<<<grid_of(n), 128, 0, st>>>(ds, n, g->nStreams, g->st, g->hdr, g->drain, dStatus);
             g_launches++;
             cudaError_t e = cudaGetLastError();
