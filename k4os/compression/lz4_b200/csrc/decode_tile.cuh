@@ -25,8 +25,9 @@
 //      for short runs, by the whole warp in 4-byte words for long ones.  The remaining "near"
 //      matches (source reaches into the step's own output) are compacted into a sorted interval
 //      list; a near match is copied as soon as no still-pending interval intersects its source
-//      (binary search once, then a flag scan per round); rounds are separated by CTA barriers,
-//      chains inside one warp resolve without a barrier.
+//      (binary search once, then a flag scan per round).  A pending entry polls the flags of the
+//      earlier entries it waits for, with no CTA barrier between rounds; the barrier that ends the
+//      step sits behind the next step's literal copies.
 //
 // The fast path accepts a block only when every sequence satisfies the reference decoder's
 // accept tests with room to spare (so the shortcut and the general path of the reference agree);
@@ -43,7 +44,6 @@
 #include "common.cuh"
 #include "decode_generic.cuh"
 #include "parse_table.cuh"
-#include "lane_copy.cuh"
 
 namespace k4 {
 
@@ -59,11 +59,8 @@ constexpr int DT_K = DT_THREADS;         // sequences per step
 #define K4_DT_WARM 256
 #endif
 constexpr int DT_WARM = K4_DT_WARM;      // speculative warm-up before the segment
-#ifndef K4_DT_NEARSPIN
-#define K4_DT_NEARSPIN 1
-#endif
-#ifndef K4_DT_LATEBAR
-#define K4_DT_LATEBAR 1                    // the barrier that ends a step sits behind the NEXT step's literal copies
+#ifndef K4_DT_SPINNS
+#define K4_DT_SPINNS 40                  // back-off between two polls of the near-match flags, ns
 #endif
 #ifndef K4_DT_LSHORT
 #define K4_DT_LSHORT 32
@@ -332,24 +329,8 @@ __device__ __forceinline__ void warp_copy_match_smem(uint32_t d, const int off, 
 // loads back to back and only then its stores, so a tier costs one shared-memory round trip instead of
 // one per group of bytes (measured: the byte-group loop was the longest serial chain of a step).
 // `ovl` lanes (LZ77 copy whose source runs into its destination) are done byte by byte afterwards.
-#ifndef K4_DT_WORDCOPY
-#define K4_DT_WORDCOPY 0                   // 1: lane_copy.cuh (4-byte words) instead of byte tiers
-#endif
-struct SmemOps {
-    __device__ __forceinline__ uint32_t ld8(uint32_t a) const { return lds8(a); }
-    __device__ __forceinline__ uint32_t ld32(uint32_t a) const { return lds32(a); }
-    __device__ __forceinline__ void st8(uint32_t a, uint32_t v) const { sts8(a, v); }
-    __device__ __forceinline__ void st32(uint32_t a, uint32_t v) const { sts32(a, v); }
-};
 __device__ __forceinline__ void lanes_copy(const uint32_t d, const uint32_t s, const int len, const bool ovl) {
     const int plain = ovl ? 0 : len;
-#if K4_DT_WORDCOPY
-    static_assert(DT_LSHORT <= LC_MAX, "lane copies are bounded by LC_MAX");
-    SmemOps m;
-    lc_copy(m, d, s, plain, __reduce_max_sync(FULL, lc_words(d, plain)));
-    if (ovl) for (int j = 0; j < len; j++) sts8(d + j, lds8(s + j));
-    return;
-#endif
     const int top = __reduce_max_sync(FULL, plain);
     for (int base = 0; base < top; base += 8) {
         const int left = plain - base;
@@ -587,14 +568,12 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
             }
         }
         DT_PROF(6);
-#if K4_DT_LATEBAR
         // The previous step's near matches must be final before a far match may read them -- but not before this
         // step's headers and literals (stage -> bytes beyond everything earlier steps write): warps that are
         // done with the near phase early do those instead of waiting (the step-end barrier was 17 % of all
         // warp stall samples).  The near arrays are first touched behind barrier #1 below.
         if (r > 0) __syncthreads();
         DT_PROF(11);
-#endif
         lanes_copy(sT + (uint32_t)d, sT + (uint32_t)a, farM && ml <= DT_LSHORT ? ml : 0, off < ml);
         for (unsigned m = __ballot_sync(FULL, farM && ml > DT_LSHORT); m; m &= m - 1) {
             const int l = __ffs(m) - 1;
@@ -665,29 +644,14 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
                     } while (progress && __any_sync(FULL, pend));
                 }
                 DT_PROF(10);
-#if K4_DT_NEARSPIN
                 // no CTA barrier between rounds: a pending entry only ever waits for entries with a LOWER
                 // index (same warp, lower lane, or an earlier warp), entry 0 waits for nothing, so polling
-                // the flags terminates; one barrier after the loop publishes the step
+                // the flags terminates; the next step's first barrier (or the one before the store) publishes the step
                 if (!warpHasWork || !__any_sync(FULL, pend)) break;
-#ifndef K4_DT_SPINNS
-#define K4_DT_SPINNS 40
-#endif
                 __nanosleep(K4_DT_SPINNS);
                 DT_PROF_COUNT(18, 1);
                 if (round > (1 << 20)) break;                     // (bounded for safety; never reached)
-#else
-                const bool more = __syncthreads_or(pend);
-                DT_PROF(11);
-                DT_PROF_COUNT(18, 1);
-                if (!more) break;
-                if (round > DT_K + 2) return -1;                 // cannot happen: each round retires the first pending match
-#endif
             }
-#if K4_DT_NEARSPIN && !K4_DT_LATEBAR
-            __syncthreads();
-            DT_PROF(11);
-#endif
         }
         dCur = dNext;
         Sr = SrNext;

@@ -19,17 +19,8 @@ namespace k4 {
 
 constexpr int ENC_TABLE_BYTES = 16384;   // LZ4_stream_t hash table, LL.types.cs:18-39
 constexpr int ENC_FLAG_X32 = 0x100;      // `level` bit: reproduce the 32-bit engine (LL32) for inputs >= 65 547 bytes
-#ifndef K4_ENC_TAGS
-#define K4_ENC_TAGS 0
-#endif
-constexpr int ENC_TAG_BYTES = K4_ENC_TAGS ? 8192 : 0;   // one filter byte per u16 slot (encode_tile.cuh)
-constexpr int ENC_SLOT_BYTES = ENC_TABLE_BYTES + ENC_TAG_BYTES;   // shared memory per warp
-// the global-table encoder warps (encode_tile.cuh) filter their candidate reads by a tag: see TAGMODE there
-#ifndef K4_ENC_GTAG
-#define K4_ENC_GTAG 2        // 32-bit slots: position | 16-bit tag
-#endif
-constexpr int ENC_GTAG = K4_ENC_GTAG;
-constexpr int ENC_GSLOT_BYTES = ENC_GTAG == 2 ? 2 * ENC_TABLE_BYTES : (ENC_GTAG ? ENC_TABLE_BYTES + ENC_TABLE_BYTES / 2 : ENC_TABLE_BYTES);
+// the global-table encoder warps (encode_tile.cuh, GTAB) keep 32-bit slots: position | 16-bit tag
+constexpr int ENC_GSLOT_BYTES = 2 * ENC_TABLE_BYTES;
 
 struct EncCtx {
     const uint8_t* src;
@@ -215,16 +206,7 @@ last_literals:
     return (int)op;
 }
 
-// LZ4Codec.Encode post-processing (LZ4Codec.cs:40-52).
-__device__ __forceinline__ int codec_encode_warp(const uint8_t* src, int n, uint8_t* dst, int cap,
-                                                 int level, void* table, bool enforce32) {
-    if (n <= 0) return 0;
-    if (level >= 3) return -2;   // K4LZ4_R_DELEGATE: HC/OPT stay with the managed engine
-    int r = encode_block_warp(src, n, dst, cap, 0x7fffffff, table, enforce32);
-    return r <= 0 ? -1 : r;
-}
-
-constexpr int ENC_WARPS_PER_CTA = K4_ENC_TAGS ? 9 : 7;   // pickle_kernel: 2 CTAs x 7 warps x 16 KiB of tables fill the SM
+constexpr int ENC_WARPS_PER_CTA = 7;   // pickle_kernel: 2 CTAs x 7 warps x 16 KiB of tables fill the SM
 // encode_spec_kernel / encode_spec_gtab_kernel (one warp per CTA, see encode_tile.cuh): resident warps per SM
 #ifndef K4_ENC_SM_WARPS
 #define K4_ENC_SM_WARPS 10      // shared-memory tables: 10 x (16 KiB + 1 KiB the hardware reserves per CTA); the rest of the 256 KiB stays L1

@@ -245,8 +245,8 @@ Dev* dev_state(int dev) {
         // tables (+1 KiB the hardware reserves per CTA), the rest stays L1 for the input windows
         for (auto* pk : {k4::pickle_kernel<false>, k4::pickle_kernel<true>})
             cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES);
-        const int carve = (k4::ENC_SM_WARPS * (k4::ENC_SLOT_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
+                                 k4::ENC_WARPS_PER_CTA * k4::ENC_TABLE_BYTES);
+        const int carve = (k4::ENC_SM_WARPS * (k4::ENC_TABLE_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
         cudaFuncSetAttribute(k4::encode_spec_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
         cudaFuncSetAttribute(k4::encode_spec_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
         cudaError_t e = cudaDeviceGetAttribute(&d->sms, cudaDevAttrMultiProcessorCount, dev);
@@ -315,8 +315,8 @@ cudaError_t encode_launch(const Batch& a, int level, const Dev& D, cudaStream_t 
         if (e == cudaSuccess) e = cudaEventRecord(join, hs);
     }
     if (e == cudaSuccess && gridS > 0) {
-        k4::encode_spec_kernel<<<gridS, 32, k4::ENC_SLOT_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
-                                                                      a.dstOff, a.dstCap, a.outLen, n, level, counter);
+        k4::encode_spec_kernel<<<gridS, 32, k4::ENC_TABLE_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
+                                                                       a.dstOff, a.dstCap, a.outLen, n, level, counter);
         e = cudaGetLastError();
         (*launches)++;
     }
@@ -361,7 +361,7 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
     case OP_PICKLEW: {
         const int ctas = (n + k4::ENC_WARPS_PER_CTA - 1) / k4::ENC_WARPS_PER_CTA;
         (a.x32 ? k4::pickle_kernel<true> : k4::pickle_kernel<false>)<<<ctas, k4::ENC_WARPS_PER_CTA * 32,
-                                                                        k4::ENC_WARPS_PER_CTA * k4::ENC_SLOT_BYTES, st>>>(
+                                                                        k4::ENC_WARPS_PER_CTA * k4::ENC_TABLE_BYTES, st>>>(
             a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.outLen, n, a.level, op == OP_PICKLEW ? 1 : 0);
         g_launches++;
         break;

@@ -48,7 +48,7 @@ __device__ int pickle_writer_message_warp(const uint8_t* __restrict__ src, int n
     const int k = pickle_diff_width(n);
     const int hs = 1 + k;
     int enc = (n < LIMIT_64K)
-        ? encode_spec_warp<false>(src, nullptr, (uint32_t)n, dst + hs, n, n - 1, reinterpret_cast<uint16_t*>(table))
+        ? encode_spec_warp<true>(src, (uint32_t)n, dst + hs, n, n - 1, reinterpret_cast<uint16_t*>(table))
         : encode_block_warp(src, n, dst + hs, n, n - 1, table, X32);
     __syncwarp();
     if (enc <= 0 || enc >= n) {                                  // :135-140
@@ -72,7 +72,7 @@ __device__ int pickle_message_warp(const uint8_t* __restrict__ src, int n, uint8
     if (level >= 3) return -2;                                   // delegate HC/OPT
     const int cap = n <= 1024 ? 1024 : n;                        // :57-67
     int enc = (n < LIMIT_64K)                                                 // :83
-        ? encode_spec_warp<false>(src, nullptr, (uint32_t)n, dst + 2, cap, n - 1, reinterpret_cast<uint16_t*>(table))
+        ? encode_spec_warp<true>(src, (uint32_t)n, dst + 2, cap, n - 1, reinterpret_cast<uint16_t*>(table))
         : encode_block_warp(src, n, dst + 2, cap, n - 1, table, X32);
     __syncwarp();
     if (enc <= 0 || enc >= n) {                                  // :85-94
@@ -132,8 +132,8 @@ pickle_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ s
     const int b = blockIdx.x * ENC_WARPS_PER_CTA + wInCta;
     if (b >= nMessages) return;
     int r = writerVariant
-        ? pickle_writer_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES)
-        : pickle_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_SLOT_BYTES);
+        ? pickle_writer_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_TABLE_BYTES)
+        : pickle_message_warp<X32>(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], level, smem + wInCta * ENC_TABLE_BYTES);
     if (lane_id() == 0) outLen[b] = r;
 }
 

@@ -82,16 +82,3 @@ def test_table_on_mutated_and_random_streams(chk):
         fails, st = chk(s, it % 16, 0xFF if it % 2 else 0x1000 + it)
         assert fails == 0, (it, int(st[4]) - 1)
     assert n_checked > 100_000
-
-
-def test_lane_copy_words_equal_byte_copies():
-    """csrc/lane_copy.cuh: word-granular per-lane copies == byte copies, nothing outside the destinations changes."""
-    src = os.path.join(HERE, "native", "lane_copy_check.cpp")
-    so = os.path.join(HERE, "native", "_lane_copy_check.so")
-    hdr = os.path.join(HERE, "..", "k4os", "compression", "lz4_b200", "csrc", "lane_copy.cuh")
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-x", "c++", "-shared", "-fPIC", "-o", so, src], check=True)
-    lib = C.CDLL(so)
-    lib.lc_check.restype = C.c_long
-    lib.lc_check.argtypes = [C.c_int, C.c_uint]
-    assert lib.lc_check(20000, 12345) == 0

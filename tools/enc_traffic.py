@@ -7,14 +7,16 @@ Replays the L00_FAST matcher for blocks below 64 KiB + 11 bytes (LL64.fast.cs, b
 each search run `win` lanes wide (K4_ENC_WIN) and every later one 32, the put(ip-2) of the post-match probe and
 the stores of earlier lanes forwarded to later lanes, the stores of lanes up to the first hit committed.  It
 emits the LZ4 block, so the counts can be pinned to the real parse (tests/test_enc_traffic_model.py compares
-the bytes with the oracle), and counts per batch what each warp kind loads:
+the bytes with the oracle), and counts per batch what each table layout loads.  Mode 0 is the shared-memory
+warps' (plain u16 slots), mode 2 the global-table warps' (32-bit slots, position | 16-bit tag); mode 3 (an 8-bit
+tag table in front of the u16 slots) was measured on the GPU and is not in the encoder (DESIGN §7.2):
 
   probe words      4-byte reads of the lanes' own positions (two LDGs where the position is not 4-aligned)
-  slot loads       TAGMODE 2, the global-table warps: one 32-bit slot (position | 16-bit tag) per lane
-  tag loads        TAGMODE 3: one 8-bit tag per lane ...
+  slot loads       mode 2: one 32-bit slot per lane
+  tag loads        mode 3: one 8-bit tag per lane ...
   pos loads        ... and the 16-bit position, only where the tag agrees and no earlier store is forwarded
-  cand words       4-byte candidate reads: TAGMODE 0 (shared-memory warps) on every lane, TAGMODE 2 / 3 where
-                   the tag agrees; counted in LDGs as above
+  cand words       4-byte candidate reads: mode 0 on every lane, modes 2 / 3 where the tag agrees; counted in
+                   LDGs as above
 
 The data is the bench's encode input (the reference generator, matchProba mp/1000, seed 1234 + chunk), from
 the first block on.  The model counts requests, not time: which variant is faster is measured on the GPU.

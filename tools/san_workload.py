@@ -11,7 +11,7 @@ import numpy as np
 
 import oracle
 import k4os.compression.lz4_b200 as k4
-if len(sys.argv) > 2 and sys.argv[1] == "--lib":       # another build of the library (e.g. -DK4_DT_NEARSPIN=0)
+if len(sys.argv) > 2 and sys.argv[1] == "--lib":       # another build of the library (e.g. -DK4_DT_SPINNS=0)
     from k4os.compression.lz4_b200 import _native as _N
     _N.SO_PATH = os.path.abspath(sys.argv[2])
 from tests import inputs
