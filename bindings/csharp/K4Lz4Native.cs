@@ -50,6 +50,13 @@ namespace K4os.Compression.LZ4.Engine.Native
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             byte* dictBase, long* dictOff, int* dictLen, int* outLen, int nBlocks,
             int memKind, void* cudaStream, int device);
+        // the blocks LZ4Codec.Decode(source, target, dictionary) reads: upstream's LZ4_loadDict + LZ4_compress_fast_continue
+        [DllImport(Lib)] public static extern int k4lz4_encode_dict(
+            byte* src, int srcLen, byte* dst, int dstCap, byte* dict, int dictLen);
+        [DllImport(Lib)] public static extern int k4lz4_encode_dict_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* dictBase, long* dictOff, int* dictLen, int* outLen, int nBlocks,
+            int memKind, void* cudaStream, int device);
         [DllImport(Lib)] public static extern int k4lz4_partial_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* targetLen,
             int* outLen, int nBlocks, int memKind, void* cudaStream, int device);

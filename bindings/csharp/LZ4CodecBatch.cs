@@ -34,6 +34,24 @@ namespace K4os.Compression.LZ4
                     K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
         }
 
+        // Block i against dictionaryBase[dictionaryOffsets[i] .. +dictionaryLengths[i]): what
+        // LZ4Codec.Decode(source, target, dictionary) reads back.  Blocks with equal (offset, length) share one
+        // loaded table and one staged copy of the dictionary.  lengths[i]: bytes written, 0 for an empty block,
+        // -1 where it does not fit targetCapacities[i].
+        public static void EncodeWithDictionary(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            ReadOnlySpan<byte> dictionaryBase, ReadOnlySpan<long> dictionaryOffsets,
+            ReadOnlySpan<int> dictionaryLengths, Span<int> lengths)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (byte* x = dictionaryBase) fixed (long* xo = dictionaryOffsets) fixed (int* xl = dictionaryLengths)
+            fixed (int* ol = lengths)
+                Check(K4Lz4Native.k4lz4_encode_dict_batch(s, so, sl, d, dof, dc, x, xo, xl, ol, lengths.Length,
+                    K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
+        }
+
         // sizes[i]: what Decode needs as targetCapacities[i] -- 0 for an empty block, -1 where the token chain does
         // not parse (Decode then fails at any capacity)
         public static void DecodedSizes(

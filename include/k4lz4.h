@@ -164,6 +164,29 @@ K4LZ4_API int32_t k4lz4_partial_decode_batch(const uint8_t *srcBase, const int64
                                              int32_t *outLen, int32_t nBlocks,
                                              int32_t memKind, void *cudaStream, int32_t device);
 
+/* Encode against an external dictionary: the blocks LZ4Codec.Decode(source, target, dictionary) (and
+ * k4lz4_decode_dict) read back.  No reference call corresponds (the reference has no LZ4_loadDict); the result is
+ * upstream lz4's 64-bit engine for
+ *     LZ4_loadDict(s, dict, dictLen); LZ4_compress_fast_continue(s, src, dst, srcLen, dstCap, 1);
+ * with the dictionary in a buffer of its own (the extDict mode).  Only the last 65 536 bytes of a longer dictionary
+ * count, and one of fewer than 8 bytes encodes like none.  Result: bytes written; 0 for srcLen <= 0; -1 when the
+ * block does not fit dstCap (upstream returns 0).  Nothing is written at or beyond dstCap.  Host pointers; dict may
+ * be NULL when dictLen <= 0. */
+K4LZ4_API int32_t k4lz4_encode_dict(const uint8_t *src, int32_t srcLen, uint8_t *dst, int32_t dstCap,
+                                    const uint8_t *dict, int32_t dictLen);
+/* Batched form; block i encodes against dictBase[dictOff[i] .. +dictLen[i]).  Arguments, checks and codes as
+ * k4lz4_decode_dict_batch, except that dictBase / dictOff / dictLen are required when nBlocks > 0.  Blocks whose
+ * (dictOff, dictLen) are equal share one loaded table; with host memory they also share one staged copy of the
+ * dictionary bytes per chunk.  With device memory a block that does not fit may write anything below its dstCap;
+ * with host memory exactly outLen[i] > 0 bytes come back.  memKind == K4LZ4_MEM_HOST is synchronous and runs on one
+ * GPU (`device`, K4LZ4_ALL_DEVICES = GPU 0); device memory only enqueues work on `cudaStream`.  Blocks are counted in
+ * k4lz4_encode_stats out4[3].  There is no _x32 twin: the reference has no dictionary encoder to reproduce. */
+K4LZ4_API int32_t k4lz4_encode_dict_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                          uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                          const uint8_t *dictBase, const int64_t *dictOff, const int32_t *dictLen,
+                                          int32_t *outLen, int32_t nBlocks,
+                                          int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- chained (linked) blocks: LZ4ChainDecoder, one block per stream per call ------------------ */
 
 /* LZ4ChainDecoder.Decode -> LLxx.LZ4_decompress_safe_continue in prefix mode
@@ -633,7 +656,7 @@ K4LZ4_API int32_t k4lz4_decode_stats(int32_t device, uint64_t *out4, int32_t res
  * hash table in shared memory, [1] by a warp with its table in global memory (only launched when a
  * call has more blocks than the shared-memory warps take in one round), [2] blocks of >= 65 547
  * bytes (the u32-table engine, either warp kind), [3] chained blocks (k4lz4_encode_chain_batch, any
- * size).  Empty blocks, delegated levels and rejected arguments are not counted.
+ * size) and blocks encoded against a dictionary (k4lz4_encode_dict_batch).  Empty blocks, delegated levels and rejected arguments are not counted.
  * Synchronises the device.  Diagnostics only. */
 K4LZ4_API int32_t k4lz4_encode_stats(int32_t device, uint64_t *out4, int32_t reset);
 

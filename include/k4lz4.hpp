@@ -60,6 +60,51 @@ struct LZ4Codec {
         if (sourceLength <= 0) return 0;
         return check_codec(k4lz4_decode_dict(source, sourceLength, target, targetLength, dictionary, dictionaryLength));
     }
+    // Encodes the block the dictionary Decode above reads back (k4lz4_encode_dict; the reference has no such call):
+    // upstream lz4's LZ4_loadDict + LZ4_compress_fast_continue.  -1 when it does not fit targetLength.
+    static int EncodeWithDictionary(const uint8_t* source, int sourceLength, uint8_t* target, int targetLength,
+                                    const uint8_t* dictionary, int dictionaryLength) {
+        if (sourceLength <= 0) return 0;
+        return check_codec(k4lz4_encode_dict(source, sourceLength, target, targetLength, dictionary, dictionaryLength));
+    }
+    // The same over a batch (k4lz4_encode_dict_batch, host memory): block i against dictionaries[which[i]], each
+    // distinct dictionary passed once.  -> one result per block (bytes written, 0 for an empty block, -1 where it does
+    // not fit MaximumOutputSize) and the encoded bytes.
+    static std::vector<int32_t> EncodeWithDictionary(const std::vector<std::vector<uint8_t>>& blocks,
+                                                     const std::vector<std::vector<uint8_t>>& dictionaries,
+                                                     const std::vector<int32_t>& which,
+                                                     std::vector<std::vector<uint8_t>>& encoded, int device = 0) {
+        const size_t n = blocks.size();
+        if (which.size() != n) throw std::invalid_argument("one dictionary index per block");
+        std::vector<int64_t> so(n), dof(n), uo(dictionaries.size()), xo(n);
+        std::vector<int32_t> sl(n), dc(n), xl(n), out(n, -1);
+        std::vector<uint8_t> src, dic;
+        int64_t at = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)blocks[i].size();
+            src.insert(src.end(), blocks[i].begin(), blocks[i].end());
+            dof[i] = at; dc[i] = k4lz4_max_output_size(sl[i]); at += dc[i];
+        }
+        for (size_t k = 0; k < dictionaries.size(); k++) {
+            uo[k] = (int64_t)dic.size();
+            dic.insert(dic.end(), dictionaries[k].begin(), dictionaries[k].end());
+        }
+        for (size_t i = 0; i < n; i++) {
+            const size_t k = (size_t)which.at(i);
+            if (k >= dictionaries.size()) throw std::out_of_range("dictionary index");
+            xo[i] = uo[k]; xl[i] = (int32_t)dictionaries[k].size();
+        }
+        src.resize(src.size() + 1); dic.resize(dic.size() + 1);
+        std::vector<uint8_t> dst((size_t)at + 1);
+        const int rc = k4lz4_encode_dict_batch(src.data(), so.data(), sl.data(), dst.data(), dof.data(), dc.data(),
+                                               dic.data(), xo.data(), xl.data(), out.data(), (int32_t)n,
+                                               K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        encoded.assign(n, {});
+        for (size_t i = 0; i < n; i++)
+            if (out[i] > 0) encoded[i].assign(dst.begin() + dof[i], dst.begin() + dof[i] + out[i]);
+        return out;
+    }
     // LZ4Codec.PartialDecode(byte*,int,byte*,int) -- LZ4Codec.cs:123-134
     static int PartialDecode(const uint8_t* source, int sourceLength, uint8_t* target, int targetLength) {
         if (sourceLength <= 0) return 0;

@@ -44,6 +44,8 @@ SIGNATURES = {
     "k4lz4_decoded_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_partial_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
     "k4lz4_decode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
+    "k4lz4_encode_dict": ([_vp, _i32, _vp, _i32, _vp, _i32], _i32),
+    "k4lz4_encode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch_x32": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),

@@ -352,3 +352,44 @@ def encode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, 
     N.check(encoder_fn("k4lz4_encode_chain_batch", x32)(src_ptr, src_off_ptr, src_len_ptr, prefix_len_ptr, dst_ptr, dst_off_ptr,
                                              dst_cap_ptr, state_ptr, state_off_ptr, out_len_ptr, int(n), int(level),
                                              N.MEM_DEVICE, stream or None, int(device)))
+
+
+def encode_dict_batch_host(blocks: Sequence, dicts: Sequence, caps: Sequence[int] | None = None, device: int = 0):
+    """Encode each block against its dictionary (k4lz4_encode_dict_batch, host memory): upstream lz4's LZ4_loadDict
+    followed by LZ4_compress_fast_continue, the blocks LZ4Codec.Decode(source, target, dictionary) reads back.
+    `dicts` holds one dictionary per block; equal objects are passed to the library once, so that blocks sharing a
+    dictionary share its staging and its loaded table.  caps default to MaximumOutputSize(len).
+    Returns (list of bytes, int32 results: bytes written, 0 for an empty block, -1 where it does not fit)."""
+    src, so, sl = _pack(blocks)
+    n = len(sl)
+    if len(dicts) != n:
+        raise ValueError(f"{n} blocks but {len(dicts)} dictionaries")
+    first: dict = {}
+    uniq: list = []
+    which = np.zeros(n, dtype=np.int64)
+    for i, d in enumerate(dicts):
+        key = id(d)
+        if key not in first:
+            first[key] = len(uniq)
+            uniq.append(d)
+        which[i] = first[key]
+    dic, uo, ul = _pack(uniq)
+    do, dl = _i64(uo[which]), _i32(ul[which])
+    if caps is None:
+        caps = [N.lib().k4lz4_max_output_size(int(x)) for x in sl]
+    dst, doff, dc = _slots(caps)
+    out = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_encode_dict_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+                                            doff.ctypes.data, dc.ctypes.data, dic.ctypes.data, do.ctypes.data,
+                                            dl.ctypes.data, out.ctypes.data, n, N.MEM_HOST, None, int(device)))
+    return _slices(dst, doff, out), out
+
+
+def encode_dict_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int, dst_off_ptr: int,
+                             dst_cap_ptr: int, dict_ptr: int, dict_off_ptr: int, dict_len_ptr: int,
+                             out_len_ptr: int, n: int, stream: int = 0, device: int = -1) -> None:
+    """Device-pointer form of encode_dict_batch_host: only enqueues the kernels on `stream`.  Blocks whose
+    (dict_off, dict_len) are equal share one loaded table."""
+    N.check(N.lib().k4lz4_encode_dict_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
+                                            dict_ptr, dict_off_ptr, dict_len_ptr, out_len_ptr, int(n), N.MEM_DEVICE,
+                                            stream or None, int(device)))

@@ -20,6 +20,7 @@
 #include <cstdio>
 #include <cstring>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -31,6 +32,7 @@
 #include "encode_generic.cuh"
 #include "encode_tile.cuh"
 #include "encode_chain.cuh"
+#include "encode_dict.cuh"
 #include "chain_group.cuh"
 #include "pickle.cuh"
 #include "synth.cuh"
@@ -76,7 +78,7 @@ int device_count_cached() {
 
 enum Op {
     OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY,
-    OP_ENCCHAIN, OP_DSIZE
+    OP_ENCCHAIN, OP_DSIZE, OP_ENCDICT
 };
 
 // Block i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]) and outLen[i].
@@ -96,23 +98,24 @@ struct Batch {
 };
 
 // The pointers each op needs when n > 0, besides srcBase / srcOff / srcLen.  A dictionary is optional
-// wherever it is read: with dictBase set, dictOff and dictLen are required too.
-struct Needs { bool dst, cap, out, prefix, level, state; };
+// wherever it is read unless `dict` says otherwise: with dictBase set, dictOff and dictLen are required too.
+struct Needs { bool dst, cap, out, prefix, level, state, dict; };
 constexpr Needs NEEDS[] = {
-    /* OP_ENCODE   */ {true,  true,  true,  false, true,  false},
-    /* OP_DECODE   */ {true,  true,  true,  false, false, false},
-    /* OP_CHAIN    */ {true,  true,  true,  true,  false, false},
-    /* OP_GENERAL  */ {true,  true,  true,  false, false, false},
-    /* OP_PICKLE   */ {true,  false, true,  false, false, false},
-    /* OP_PICKLEW  */ {true,  false, true,  false, false, false},
-    /* OP_UNPICKLE */ {true,  true,  true,  false, false, false},
-    /* OP_USIZE    */ {false, false, true,  false, false, false},
-    /* OP_XXH32    */ {false, false, true,  false, false, false},
-    /* OP_COPY     */ {true,  false, false, false, false, false},
-    /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true},
-    /* OP_DSIZE    */ {false, false, true,  false, false, false},
+    /* OP_ENCODE   */ {true,  true,  true,  false, true,  false, false},
+    /* OP_DECODE   */ {true,  true,  true,  false, false, false, false},
+    /* OP_CHAIN    */ {true,  true,  true,  true,  false, false, false},
+    /* OP_GENERAL  */ {true,  true,  true,  false, false, false, false},
+    /* OP_PICKLE   */ {true,  false, true,  false, false, false, false},
+    /* OP_PICKLEW  */ {true,  false, true,  false, false, false, false},
+    /* OP_UNPICKLE */ {true,  true,  true,  false, false, false, false},
+    /* OP_USIZE    */ {false, false, true,  false, false, false, false},
+    /* OP_XXH32    */ {false, false, true,  false, false, false, false},
+    /* OP_COPY     */ {true,  false, false, false, false, false, false},
+    /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true,  false},
+    /* OP_DSIZE    */ {false, false, true,  false, false, false, false},
+    /* OP_ENCDICT  */ {true,  true,  true,  false, false, false, true},
 };
-static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_DSIZE + 1, "one row per op");
+static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_ENCDICT + 1, "one row per op");
 
 // The machine part of check(): a device must exist, an empty batch is then done (the caller returns OK for
 // n == 0), and `device` (K4LZ4_ALL_DEVICES or the current device when negative) must name a visible GPU.
@@ -132,7 +135,7 @@ int check(Op op, const Batch& b, int memKind, int device) {
     if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
     if (b.n > 0 && (!b.srcBase || !b.srcOff || !b.srcLen || (w.out && !b.outLen) || (w.dst && (!b.dstBase || !b.dstOff)) ||
                     (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen)) ||
-                    (w.state && (!b.stateBase || !b.stateOff))))
+                    (w.state && (!b.stateBase || !b.stateOff)) || (w.dict && !b.dictBase)))
         return fail(K4LZ4_E_ARG, "null pointer argument");
     if (w.prefix && memKind == K4LZ4_MEM_HOST)       // device arrays cannot be checked here: there a negative prefix gives -1
         for (int64_t i = 0; i < b.n; i++)
@@ -180,13 +183,15 @@ struct Buf {           // grows, never shrinks: device memory, or pinned host me
 
 // One row of a synchronous host-memory step (stage_up): `send` source bytes at src, with the `pre` bytes in front of
 // them; a destination slot of `room` bytes, with the `dstPre` bytes in front of dst as its history; the table columns
-// stream len cap aux; an optional blob (a dictionary, or a state record that comes back whole to `back`).  dst is
-// where stage_down puts the row's output.
+// stream len cap aux; an optional blob (a dictionary, or a state record that comes back whole to `back`), or the
+// blob of the earlier row `blobFrom` of the same step, staged once for both.  dst is where stage_down puts the
+// row's output.
 struct UpRow {
     const uint8_t* src; int64_t send, room; int32_t stream, len, cap, aux;
     uint8_t* dst = nullptr;
     int32_t pre = 0, dstPre = 0;
     const uint8_t* blob = nullptr; int32_t blobLen = 0; uint8_t* back = nullptr;
+    int64_t blobFrom = -1;
 };
 
 // The buffers of the synchronous host-memory path (stage_up / stage_down) and the rows of the step in flight.
@@ -402,6 +407,39 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
                                                                                        a.srcLen, a.outLen, n);
         g_launches++;
         break;
+    case OP_ENCDICT: {   // key map -> loaded records -> persistent encoder warps; one workspace from the private pool
+        const int wave = D->sms * k4::ENC_CHAIN_WARPS;
+        const int grid = n < wave ? n : wave;
+        const int nrec = n < k4::DICT_RECORDS ? n : k4::DICT_RECORDS;
+        uint32_t slots = 1;
+        while (slots < 2u * (uint32_t)n) slots <<= 1;
+        auto a256 = [](size_t x) { return (x + 255) & ~size_t(255); };
+        constexpr size_t SB = sizeof(k4::ChainState);
+        const size_t mapAt = 256, repAt = mapAt + a256((size_t)slots * 4), idAt = repAt + a256((size_t)n * 4);
+        const size_t blkAt = idAt + a256((size_t)n * 4), recAt = blkAt + a256((size_t)nrec * 4);
+        const size_t workAt = recAt + (size_t)nrec * SB, total = workAt + (size_t)grid * SB;
+        uint8_t* ws = nullptr;
+        cudaError_t e = cudaMallocFromPoolAsync((void**)&ws, total, D->pool, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(ws, 0, 8, st);                      // block counter, record count
+        if (e == cudaSuccess) e = cudaMemsetAsync(ws + mapAt, 0, (size_t)slots * 4, st);
+        if (e != cudaSuccess) { (void)cudaGetLastError(); return e; }
+        uint32_t* const counter = reinterpret_cast<uint32_t*>(ws);
+        int32_t* const rep = reinterpret_cast<int32_t*>(ws + repAt);
+        int32_t* const recId = reinterpret_cast<int32_t*>(ws + idAt);
+        int32_t* const recBlock = reinterpret_cast<int32_t*>(ws + blkAt);
+        k4::ChainState* const recs = reinterpret_cast<k4::ChainState*>(ws + recAt);
+        k4::dict_key_kernel<<<(n + 127) / 128, 128, 0, st>>>(a.dictOff, a.dictLen, a.srcLen, n,
+                                                             reinterpret_cast<int32_t*>(ws + mapAt), slots - 1, rep,
+                                                             recId, recBlock, counter + 1);
+        k4::dict_load_kernel<<<nrec, 32, 0, st>>>(a.dictBase, a.dictOff, a.dictLen, recBlock, counter + 1, recs);
+        k4::encode_dict_kernel<<<grid, 32, 0, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.dstCap,
+                                                    a.dictBase, a.dictOff, a.dictLen, rep, recId, recs,
+                                                    reinterpret_cast<k4::ChainState*>(ws + workAt), a.outLen, n,
+                                                    counter);
+        g_launches += 3;
+        cudaFreeAsync(ws, st);
+        break;
+    }
     }
     return cudaGetLastError();
 }
@@ -777,7 +815,8 @@ int stage_up(Staging& S, int64_t m, int64_t resInts, int64_t extra, Row row, Sta
     bool hist = false, back = false;
     for (int64_t k = 0; k < m; k++) {
         const UpRow& x = S.rows[(size_t)k] = row(k);
-        sp = a16(sp + x.pre) + x.send; bp = a16(bp) + x.blobLen; dp = a16(dp + x.dstPre) + x.room;
+        sp = a16(sp + x.pre) + x.send; dp = a16(dp + x.dstPre) + x.room;
+        if (x.blobFrom < 0) bp = a16(bp) + x.blobLen;
         hist |= x.dstPre > 0; back |= x.back != nullptr;
     }
     const int64_t sendAt = a16(m * (8 * 3 + 4 * 5)), blobAt = sendAt + a16(sp), blobBytes = a16(bp);
@@ -791,15 +830,17 @@ int stage_up(Staging& S, int64_t m, int64_t resInts, int64_t extra, Row row, Sta
     sp = bp = dp = 0;
     for (int64_t k = 0; k < m; k++) {
         const UpRow& x = S.rows[(size_t)k];
-        hs[k] = x.stream; hl[k] = x.len; hc[k] = x.cap; ha[k] = x.aux; hb[k] = x.blobLen;
-        hso[k] = a16(sp + x.pre); hbo[k] = a16(bp); hdo[k] = a16(dp + x.dstPre);
-        sp = hso[k] + x.send; bp = hbo[k] + x.blobLen; dp = hdo[k] + x.room;
+        hs[k] = x.stream; hl[k] = x.len; hc[k] = x.cap; ha[k] = x.aux;
+        hso[k] = a16(sp + x.pre); hdo[k] = a16(dp + x.dstPre);
+        sp = hso[k] + x.send; dp = hdo[k] + x.room;
+        if (x.blobFrom >= 0) { hbo[k] = hbo[x.blobFrom]; hb[k] = hb[x.blobFrom]; }
+        else { hbo[k] = a16(bp); hb[k] = x.blobLen; bp = hbo[k] + x.blobLen; }
     }
     parallel_for_blocks(0, m, upBytes, [&](int64_t lo, int64_t hi) {
         for (int64_t k = lo; k < hi; k++) {
             const UpRow& x = S.rows[(size_t)k];
             if (x.pre + x.send > 0) memcpy(H + sendAt + hso[k] - x.pre, x.src - x.pre, (size_t)(x.pre + x.send));
-            if (x.blobLen > 0) memcpy(H + blobAt + hbo[k], x.blob, (size_t)x.blobLen);
+            if (x.blobLen > 0 && x.blobFrom < 0) memcpy(H + blobAt + hbo[k], x.blob, (size_t)x.blobLen);
             if (x.dstPre > 0) memcpy(H + dstAt + hdo[k] - x.dstPre, x.dst - x.dstPre, (size_t)x.dstPre);
         }
     });
@@ -853,12 +894,13 @@ int stage_down(Staging& S, const StageUp& up, int64_t m, int32_t* hRes, int64_t 
     return K4LZ4_OK;
 }
 
-// Dictionary / partial / chained decode, chained encode, XXH32 and decoded sizes: one GPU, on the legacy default
-// stream, in chunks of whole blocks of at most STAGE_BYTES through the device's staging.  Chained decode's history
-// (the last <= 65535 bytes in front of each destination: all the decoder reads) goes in front of its slot, the
-// chained encoder's in front of its source; the dictionaries and the encoder's state records are the blobs, and the
-// state records come back whole.  A batch without dstCap (XXH32, decoded sizes) has no destination: its per-block
-// result is the whole output.
+// Dictionary / partial / chained decode, chained and dictionary encode, XXH32 and decoded sizes: one GPU, on the
+// legacy default stream, in chunks of whole blocks of at most STAGE_BYTES through the device's staging.  Chained
+// decode's history (the last <= 65535 bytes in front of each destination: all the decoder reads) goes in front of
+// its slot, the chained encoder's in front of its source; the dictionaries and the encoder's state records are the
+// blobs, and the state records come back whole.  The dictionary encoder stages only the bytes LZ4_loadDict keeps,
+// and each distinct dictionary once per chunk, so that many messages against one dictionary move it once.  A batch
+// without dstCap (XXH32, decoded sizes) has no destination: its per-block result is the whole output.
 int run_staged(Op op, const Batch& b, int dev) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
@@ -866,20 +908,38 @@ int run_staged(Op op, const Batch& b, int dev) {
     if (!D) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
     std::lock_guard<std::mutex> lk(D->stageMu);
     const bool dict = b.dictBase != nullptr, prefix = b.prefixLen != nullptr, dst = b.dstCap != nullptr;
-    const bool enc = op == OP_ENCCHAIN;
+    const bool enc = op == OP_ENCCHAIN, edict = op == OP_ENCDICT;
     constexpr int64_t SB = K4LZ4_CHAIN_STATE_BYTES;
     auto hist = [&](int64_t i) -> int32_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
-    auto cap = [&](int64_t i) -> int64_t {      // the encoder never writes more than compressBound(srcLen)
+    auto cap = [&](int64_t i) -> int64_t {      // the encoders never write more than compressBound(srcLen)
         const int64_t c = dst ? std::max<int32_t>(b.dstCap[i], 0) : 0;
-        return enc ? std::min<int64_t>(c, b.srcLen[i] > 0 ? k4::max_output_size(b.srcLen[i]) : 0) : c;
+        return enc || edict ? std::min<int64_t>(c, b.srcLen[i] > 0 ? k4::max_output_size(b.srcLen[i]) : 0) : c;
     };
-    auto dlen = [&](int64_t i) -> int32_t { return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0; };
+    auto dlen = [&](int64_t i) -> int32_t {
+        if (edict) return b.srcLen[i] > 0 ? k4::dict_kept(b.dictLen[i]) : 0;
+        return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0;
+    };
+    // the dictionary encoder's first row of each distinct dictionary in the chunk, and each row's sharer
+    std::map<std::pair<const uint8_t*, int32_t>, int64_t> first;
+    std::vector<int64_t> from;
+    auto dkey = [&](int64_t i) { return std::make_pair(b.dictBase + b.dictOff[i] + (b.dictLen[i] - dlen(i)), dlen(i)); };
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
+        first.clear(); from.clear();
         for (j = i; j < b.n; j++) {
-            const int64_t add = src_size(b, j) + dlen(j) + cap(j) + (prefix ? hist(j) + 16 : 0) + (enc ? SB : 0);
+            int64_t shared = -1;
+            if (edict && dlen(j) > 0) {
+                auto it = first.find(dkey(j));
+                if (it != first.end()) shared = it->second;
+            }
+            const int64_t add = src_size(b, j) + (shared >= 0 ? 0 : dlen(j)) + cap(j) +
+                                (prefix ? hist(j) + 16 : 0) + (enc ? SB : 0);
             if (j > i && bytes + add > STAGE_BYTES) break;
             bytes += add;
+            if (edict) {
+                if (shared < 0 && dlen(j) > 0) first.emplace(dkey(j), j - i);
+                from.push_back(shared);
+            }
         }
         const int64_t nb = j - i;
         StageUp up;
@@ -891,7 +951,8 @@ int run_staged(Op op, const Batch& b, int dev) {
                     enc ? b.prefixLen[x] : hl, dst ? b.dstBase + b.dstOff[x] : nullptr};
             if (enc) { r.pre = hl; r.blob = r.back = b.stateBase + b.stateOff[x]; r.blobLen = (int32_t)SB; }
             else r.dstPre = hl;
-            if (dict) { r.blob = b.dictBase + b.dictOff[x]; r.blobLen = dlen(x); }
+            if (edict) { r.blob = dkey(x).first; r.blobLen = dlen(x); r.blobFrom = from[(size_t)k]; }
+            else if (dict) { r.blob = b.dictBase + b.dictOff[x]; r.blobLen = dlen(x); }
             return r;
         }, up, nullptr);
         if (rc != K4LZ4_OK) return rc;
@@ -913,7 +974,8 @@ int run(Op op, const Batch& b, int memKind, void* stream, int device) {
     const int rc = check(op, b, memKind, device);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     if (memKind == K4LZ4_MEM_HOST)
-        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN || op == OP_DSIZE)
+        return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN || op == OP_DSIZE ||
+                op == OP_ENCDICT)
                    ? run_staged(op, b, device < 0 ? 0 : device) : run_host(op, b, device);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
@@ -928,13 +990,14 @@ int32_t run_one(Op op, const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t
     if (op == OP_ENCODE && level >= 3) return K4LZ4_R_DELEGATE;
     if (!src || (!dst && dstCap > 0) || (!dict && dictLen > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
     if (dstCap <= 0) return -1;                      // nothing fits in an empty target (LL64.dec.cs:162-168; LZ4Codec.cs:135)
-    int64_t zero = 0; int32_t out = -1;
+    int64_t zero = 0; int32_t zero32 = 0, out = -1;
     Batch b{src, &zero, &srcLen, dst, &zero, &dstCap, &out, 1};
     // the encoder reads bits 0-7 of its level word as the level and bit 8 as the 32-bit switch: a level
     // below 0 reaches it as that word
     const int word = level | (x32 ? k4::ENC_FLAG_X32 : 0);
     b.level = word & 0xFF; b.x32 = (word & k4::ENC_FLAG_X32) != 0;
     if (dictLen > 0) { b.dictBase = dict; b.dictOff = &zero; b.dictLen = &dictLen; }
+    else if (op == OP_ENCDICT) { b.dictBase = src; b.dictOff = &zero; b.dictLen = &zero32; }   // no dictionary
     b.partial = partial;
     const int rc = run(op, b, K4LZ4_MEM_HOST, nullptr, 0);
     return rc != K4LZ4_OK ? rc : out;
@@ -2092,6 +2155,21 @@ int32_t k4lz4_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, c
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
     return run(OP_GENERAL, b, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_encode_dict(const uint8_t* src, int32_t srcLen, uint8_t* dst, int32_t dstCap,
+                          const uint8_t* dict, int32_t dictLen) {
+    return run_one(OP_ENCDICT, src, srcLen, dst, dstCap, 0, false, dict, dictLen);
+}
+
+int32_t k4lz4_encode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen,
+                                int32_t* outLen, int32_t nBlocks, int32_t memKind, void* cudaStream,
+                                int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
+    b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
+    return run(OP_ENCDICT, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,

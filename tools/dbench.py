@@ -17,6 +17,13 @@ over the same raw bytes, with the encoder's path counters and a spot check again
 k4lz4_decoded_size_batch over the compressed blocks in device memory: GB/s of compressed input, every size checked
 equal to the block length; other builds (segment length and warm-up, K4_SW_SEG / K4_SW_WARM) alternate with the
 shipped one in three rounds.  The card's name and power limit are printed with it.
+    python tools/dbench.py --what dict-encode [--messages 1000000] [--reps 5]
+k4lz4_encode_dict_batch in device memory: M messages of the pickler benchmark's length mix (256 B .. 4 KiB) of
+JSON-like records against one 64 KiB dictionary of other records, beside k4lz4_encode_batch over the same messages
+without one; then 65 536 x 64 KiB blocks of the same content against the dictionary, beside
+k4lz4_encode_chain_batch over the same blocks (new streams); then the host-memory rate of the message workload, and
+a torch.profiler run of one device call for the kernels' times (the dictionary load among them).  GB/s of source
+bytes, compressed ratios, spot checks against upstream (oracle/_ref/), and the card's name and power limit.
 The 32-bit engine (k4lz4_encode_chain_batch_x32, LZ4Codec.Enforce32) runs the same steps in the same process,
 timed alternately with the plain one, with a spot check against upstream's chained encoder built as LL32; the card's
 name and power limit are printed with it.  The host-memory form of one step is timed too, beside a host-memory k4lz4_encode_batch of the same blocks (the
@@ -46,6 +53,7 @@ ap.add_argument("--check", type=int, default=0, help="encode: compare every CHEC
 ap.add_argument("--lib", default=None, help="alternative build of libk4lz4.so (e.g. a -DK4_DT_PROFILE build under scratch/)")
 ap.add_argument("--streams", default="264,1024,4096", help="chain: stream counts")
 ap.add_argument("--chain-blocks", type=int, default=16, help="chain: linked blocks per stream")
+ap.add_argument("--messages", type=int, default=1000000, help="dict-encode: message count")
 ap.add_argument("--size-libs", default="", help="size: other builds of libk4lz4.so (tools/build_variant.py), "
                                                 "timed alternately with the shipped one in this process")
 a = ap.parse_args()
@@ -60,10 +68,150 @@ def host_ms(fn, reps):
     return float(np.median(t))
 
 
+def timeit(fn, reps):
+    fn(); torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(); fn(); e1.record(); torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
+    return min(ts), float(np.median(ts))
+
+
 def report(kind, S, Bk, host, dev):
     print(f"{kind}-group S={S} x {Bk} steps, ms per step | host memory: chained {host[0]:.2f}, group {host[1]:.2f}, "
           f"independent {host[2]:.2f} | device memory: chained {dev[0]:.3f}, group {dev[1]:.3f}, "
           f"independent {dev[2]:.3f}", flush=True)
+
+
+def dict_encode():
+    import subprocess
+    from tests import dict_enc_ref as DR
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True).stdout.strip()
+    print(f"card: {card}", flush=True)
+    up = DR.DictUpstream()
+    dev, st = torch.device("cuda", 0), torch.cuda.current_stream().cuda_stream
+    L = N.lib()
+    rng = np.random.default_rng(7)
+    pool = np.frombuffer(DR.records(8 << 20, 8), dtype=np.uint8)
+    d = np.frombuffer(DR.records(65536, 9), dtype=np.uint8)
+    M = a.messages
+    lens = rng.integers(256, 4097, M).astype(np.int32)
+    starts = rng.integers(0, len(pool) - 4096, M)
+    offs = np.zeros(M, dtype=np.int64)
+    offs[1:] = np.cumsum(lens[:-1], dtype=np.int64)
+    total = int(lens.sum())
+    hsrc = np.empty(total, dtype=np.uint8)
+    for i in range(M):
+        hsrc[offs[i]:offs[i] + lens[i]] = pool[starts[i]:starts[i] + lens[i]]
+    caps = (lens + lens // 255 + 16).astype(np.int32)
+    doffs = np.zeros(M, dtype=np.int64)
+    doffs[1:] = np.cumsum(caps[:-1], dtype=np.int64)
+    t = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)
+    src, so, sl, dc, do_ = t(hsrc), t(offs), t(lens), t(caps), t(doffs)
+    dst = torch.empty(int(caps.sum()), dtype=torch.uint8, device=dev)
+    out = torch.zeros(M, dtype=torch.int32, device=dev)
+    dd, zo, dlen = t(d), torch.zeros(M, dtype=torch.int64, device=dev), torch.full((M,), len(d), dtype=torch.int32, device=dev)
+
+    def denc(n=M):
+        B.encode_dict_batch_device(src.data_ptr(), so.data_ptr(), sl.data_ptr(), dst.data_ptr(), do_.data_ptr(),
+                                   dc.data_ptr(), dd.data_ptr(), zo.data_ptr(), dlen.data_ptr(), out.data_ptr(), n, st)
+
+    def penc():
+        B.encode_batch_device(src.data_ptr(), so.data_ptr(), sl.data_ptr(), dst.data_ptr(), do_.data_ptr(),
+                              dc.data_ptr(), out.data_ptr(), M, 0, st)
+    tm = {}
+    for _ in range(3):                                   # alternate the two calls
+        for name, fn in (("dict", denc), ("plain", penc)):
+            tm.setdefault(name, []).append(timeit(fn, a.reps)[1])
+    denc(); torch.cuda.synchronize()
+    ho, hd = out.cpu().numpy(), dst.cpu().numpy()
+    rd = float(ho.sum()) / total
+    bad = 0
+    for i in range(0, M, max(M // 500, 1)):
+        r, want = up.encode(hsrc[offs[i]:offs[i] + lens[i]].tobytes(), d.tobytes())
+        bad += int(ho[i]) != r or hd[doffs[i]:doffs[i] + r].tobytes() != want
+    penc(); torch.cuda.synchronize()
+    rp = float(out.sum()) / total
+    md, mp = float(np.median(tm["dict"])), float(np.median(tm["plain"]))
+    print(f"dict-encode messages M={M} ({total / 1e9:.2f} GB, 256 B..4 KiB) vs one 64 KiB dictionary: {md:.3f} ms "
+          f"{total / md / 1e6:.1f} GB/s ratio {rd:.3f} (spot check vs upstream: {bad} differ) | k4lz4_encode_batch, "
+          f"no dictionary: {mp:.3f} ms {total / mp / 1e6:.1f} GB/s ratio {rp:.3f} (medians of 3 alternating runs "
+          f"of {a.reps})", flush=True)
+
+    # host memory, the same messages (dictionary staged once per chunk)
+    hdst = np.empty(int(caps.sum()), dtype=np.uint8)
+    hout = np.zeros(M, dtype=np.int32)
+    hzo, hdl = np.zeros(M, dtype=np.int64), np.full(M, len(d), dtype=np.int32)
+
+    def henc():
+        N.check(L.k4lz4_encode_dict_batch(hsrc.ctypes.data, offs.ctypes.data, lens.ctypes.data, hdst.ctypes.data,
+                                          doffs.ctypes.data, caps.ctypes.data, d.ctypes.data, hzo.ctypes.data,
+                                          hdl.ctypes.data, hout.ctypes.data, M, N.MEM_HOST, None, 0))
+    hm = host_ms(henc, 3)
+    print(f"dict-encode host memory M={M}: {hm:.1f} ms {total / hm / 1e6:.2f} GB/s, results equal to device: "
+          f"{bool(np.array_equal(hout, ho))}", flush=True)
+    del src, dst, out, so, sl, dc, do_, zo, dlen, hdst
+
+    # 65 536 x 64 KiB blocks of the same content, against the dictionary and as new chained streams
+    nb, bs = 65536, 65536
+    big = t(pool).repeat((nb * bs + len(pool) - 1) // len(pool))[:nb * bs]
+    bound = bs + bs // 255 + 16
+    bo = torch.arange(nb, dtype=torch.int64, device=dev)
+    so2, do2 = bo * bs, bo * bound
+    sl2, dc2 = torch.full((nb,), bs, dtype=torch.int32, device=dev), torch.full((nb,), bound, dtype=torch.int32, device=dev)
+    dst2 = torch.empty(nb * bound, dtype=torch.uint8, device=dev)
+    out2 = torch.zeros(nb, dtype=torch.int32, device=dev)
+    zo2, dl2 = torch.zeros(nb, dtype=torch.int64, device=dev), torch.full((nb,), len(d), dtype=torch.int32, device=dev)
+    SB = N.CHAIN_STATE_BYTES
+    states = torch.zeros(nb * SB, dtype=torch.uint8, device=dev)
+    stoff, pre = bo * SB, torch.zeros(nb, dtype=torch.int32, device=dev)
+
+    def denc2():
+        B.encode_dict_batch_device(big.data_ptr(), so2.data_ptr(), sl2.data_ptr(), dst2.data_ptr(), do2.data_ptr(),
+                                   dc2.data_ptr(), dd.data_ptr(), zo2.data_ptr(), dl2.data_ptr(), out2.data_ptr(), nb, st)
+
+    def cenc2():
+        states.zero_()
+        B.encode_chain_batch_device(big.data_ptr(), so2.data_ptr(), sl2.data_ptr(), pre.data_ptr(), dst2.data_ptr(),
+                                    do2.data_ptr(), dc2.data_ptr(), states.data_ptr(), stoff.data_ptr(),
+                                    out2.data_ptr(), nb, 0, st)
+    tm = {}
+    for _ in range(3):
+        for name, fn in (("dict", denc2), ("chain", cenc2)):
+            tm.setdefault(name, []).append(timeit(fn, a.reps)[1])
+    denc2(); torch.cuda.synchronize()
+    rd2 = float(out2.sum()) / (nb * bs)
+    o0 = out2[:4].cpu().numpy()
+    h0 = dst2[:4 * bound].cpu().numpy()
+    hb = big[:4 * bs].cpu().numpy()
+    bad2 = sum(up.encode(hb[k * bs:(k + 1) * bs].tobytes(), d.tobytes())[1] != h0[k * bound:k * bound + o0[k]].tobytes()
+               for k in range(4))
+    cenc2(); torch.cuda.synchronize()
+    rc2 = float(out2.sum()) / (nb * bs)
+    md, mc = float(np.median(tm["dict"])), float(np.median(tm["chain"]))
+    print(f"dict-encode blocks {nb} x 64 KiB vs 64 KiB dictionary: {md:.3f} ms {nb * bs / md / 1e6:.1f} GB/s ratio "
+          f"{rd2:.3f} ({bad2} of 4 differ from upstream) | k4lz4_encode_chain_batch, new streams: {mc:.3f} ms "
+          f"{nb * bs / mc / 1e6:.1f} GB/s ratio {rc2:.3f}", flush=True)
+    del big, dst2, states
+
+    # kernel times of one message call, in a profiler run of its own
+    src, so, sl, dc, do_ = t(hsrc), t(offs), t(lens), t(caps), t(doffs)
+    dst = torch.empty(int(caps.sum()), dtype=torch.uint8, device=dev)
+    out = torch.zeros(M, dtype=torch.int32, device=dev)
+    zo, dlen = torch.zeros(M, dtype=torch.int64, device=dev), torch.full((M,), len(d), dtype=torch.int32, device=dev)
+    denc(); torch.cuda.synchronize()
+    from torch.profiler import profile, ProfilerActivity
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        denc(); torch.cuda.synchronize()
+    for ev in prof.key_averages():
+        if "dict" in ev.key:
+            print(f"   kernel {ev.key.split('(')[0]}: {ev.device_time_total / max(ev.count, 1) / 1e3:.3f} ms", flush=True)
+
+
+if a.what == "dict-encode":
+    dict_encode()
+    sys.exit(0)
 if a.what in ("chain", "chain-encode"):
     a.blocks = max(int(x) for x in a.streams.split(",")) * a.chain_blocks
 if a.lib:
@@ -97,13 +245,6 @@ clen = torch.zeros(nb, dtype=torch.int32, device=dev)
 def enc():
     B.encode_batch_device(raw.data_ptr(), roff.data_ptr(), rlen.data_ptr(), slots.data_ptr(), coff.data_ptr(),
                           ccap.data_ptr(), clen.data_ptr(), nb, 0, st)
-def timeit(fn, reps):
-    fn(); torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); fn(); e1.record(); torch.cuda.synchronize(); ts.append(e0.elapsed_time(e1))
-    return min(ts), float(np.median(ts))
 if a.what != "chain-encode":
     enc(); torch.cuda.synchronize()
 ratio = float(clen.sum()) / (nb * bs)
