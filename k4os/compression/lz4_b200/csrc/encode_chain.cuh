@@ -23,6 +23,9 @@
 //   * the state update (dictSize += n, currentOffset += n before the search, lz4.c:909-919) and the
 //     renormalisation near 2 GiB (LZ4_renormDictT, lz4.c:1545-1562).
 // The history a block may read is min(state.dictSize, prefixLen) bytes, and never more than 65 535 of them.
+//
+// The search itself (chain_search_warp) reads positions below 0 through a window: PrefixWindow here, whose
+// history lies directly in front of `src`, and ExtWindow (encode_dict.cuh), whose dictionary is a buffer of its own.
 #pragma once
 #include "common.cuh"
 #include "encode_generic.cuh"
@@ -44,38 +47,39 @@ static_assert(sizeof(ChainState) == 16400, "K4LZ4_CHAIN_STATE_BYTES");
 #endif
 constexpr int ENC_CHAIN_WARPS = K4_ENC_CHAIN_WARPS;
 
-// Returns the engine's value: bytes written, or 0 when a limitedOutput check fails (the state has then
-// advanced as far as upstream's has).  `P` is the caller's prefixLen (>= 0).  H4: hash4 (the 32-bit engine).
-template <bool H4>
-__device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t n, const uint32_t P,
-                                 uint8_t* __restrict__ dst, const int cap, ChainState* st) {
+// Reads in the prefix layout: position p < 0 is src[p], the `d` bytes of history directly in front of the source.
+// The catch-up's byte compare (same8) and its floor (floor/above) are window members rather than expressions over
+// rd8 and an int: a compare of the two bytes widened to uint32_t, or a floor hoisted into an int, changes the
+// chained kernels' SASS.  So same8 compares the bytes as uint8_t, and floor is an empty tag that keeps -d in the test.
+struct PrefixWindow {
+    uint32_t d;
+    struct Floor {};
+    __device__ __forceinline__ uint32_t rd8(const uint8_t* __restrict__ src, int p) const {
+        return (uint32_t)__ldg(src + p);
+    }
+    __device__ __forceinline__ uint32_t rd32(const uint8_t* __restrict__ src, int p) const { return ldg_u32u(src + p); }
+    __device__ __forceinline__ bool same8(const uint8_t* __restrict__ src, int a, int b) const {
+        return __ldg(src + a) == __ldg(src + b);
+    }
+    __device__ __forceinline__ Floor floor(int) const { return {}; }
+    __device__ __forceinline__ bool above(int x, Floor) const { return x > -(int)d; }         // lowLimit, :907
+};
+
+// The search of one block, from position 0 through the last literals: the table's slots hold absolute indices,
+// position 0 is `startIndex`, and the window `w` reads the `d` bytes of history below it.  Under dictSmall no index
+// below startIndex - d is accepted.  Returns the engine's value: bytes written, or 0 when a limitedOutput check fails.
+template <bool H4, class W>
+__device__ __forceinline__ int chain_search_warp(const W w, const uint8_t* __restrict__ src, const uint32_t n,
+                                                 const uint32_t startIndex, const uint32_t d, const bool dictSmall,
+                                                 uint32_t* table, uint8_t* __restrict__ dst, const int cap) {
     const int lane = lane_id();
-    uint32_t* const table = st->table;
-    uint32_t startIndex = __ldcg(&st->currentOffset), dsz = __ldcg(&st->dictSize);
-    if (startIndex + n > 0x80000000u) {                                       // LZ4_renormDictT
-        const uint32_t delta = startIndex - 65536u;
-        for (int i = lane; i < 4096; i += 32) {
-            const uint32_t t = __ldcg(table + i);
-            __stcg(table + i, t < delta ? 0u : t - delta);
-        }
-        startIndex = 65536u;
-        if (dsz > 65536u) dsz = 65536u;
-    }
-    if (n > (uint32_t)MAX_INPUT_SIZE) {                                       // lz4.c: before any state update
-        if (lane == 0) { __stcg(&st->currentOffset, startIndex); __stcg(&st->dictSize, dsz); }
-        __syncwarp();
-        return 0;
-    }
-    const uint32_t d = dsz < P ? dsz : P;                                     // LZ4_saveDict's clamp
-    const bool dictSmall = d < 65536u && d < startIndex;                      // lz4.c:1601
     const uint32_t prefixIdxLimit = startIndex - d;
-    if (lane == 0) { __stcg(&st->currentOffset, startIndex + n); __stcg(&st->dictSize, d + n); }
     // a candidate index passes the reference's tests (and lies below the probe, as every valid state's do)
     auto accept = [&](uint32_t idx, uint32_t cur) {
         return idx < cur && !(dictSmall && idx < prefixIdxLimit) && !(idx + (uint32_t)MAX_DISTANCE < cur);
     };
-#define RD32(p) ldg_u32u(src + (int)(p))
-#define RD8(p) ((uint32_t)__ldg(src + (int)(p)))
+#define RD32(p) w.rd32(src, (int)(p))
+#define RD8(p) w.rd8(src, (int)(p))
 #define HASH(p) (H4 ? hash4(ldg_u32u(src + (p)), 12) : hash5(ldg_u64u(src + (p)), 12))
     const int64_t olimit = cap;                                               // limitedOutput, always
     uint32_t ip = 0, anchor = 0, op = 0;
@@ -150,10 +154,11 @@ __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t
             }
             uint32_t caught = 0;
             if (!zeroLit) {                                                   // catch-up down to lowLimit, :1019
+                const auto low = w.floor(m);
                 for (int width = 8;; width = 32) {
                     const bool part = lane < width;
-                    const bool ok = !part || ((ip > anchor + lane) && (m - lane > -(int)d) &&
-                                              (RD8(ip - 1 - lane) == RD8(m - 1 - lane)));
+                    const bool ok = !part || ((ip > anchor + lane) && w.above(m - lane, low) &&
+                                              w.same8(src, ip - 1 - lane, m - 1 - lane));
                     const unsigned bad = __ballot_sync(FULL, !ok);
                     const int c = bad ? __ffs(bad) - 1 : width;
                     ip -= c; m -= c; caught += (uint32_t)c;
@@ -228,6 +233,34 @@ __device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t
 #undef RD32
 #undef RD8
 #undef HASH
+}
+
+// Returns the engine's value: bytes written, or 0 when a limitedOutput check fails (the state has then
+// advanced as far as upstream's has).  `P` is the caller's prefixLen (>= 0).  H4: hash4 (the 32-bit engine).
+template <bool H4>
+__device__ int encode_chain_warp(const uint8_t* __restrict__ src, const uint32_t n, const uint32_t P,
+                                 uint8_t* __restrict__ dst, const int cap, ChainState* st) {
+    const int lane = lane_id();
+    uint32_t* const table = st->table;
+    uint32_t startIndex = __ldcg(&st->currentOffset), dsz = __ldcg(&st->dictSize);
+    if (startIndex + n > 0x80000000u) {                                       // LZ4_renormDictT
+        const uint32_t delta = startIndex - 65536u;
+        for (int i = lane; i < 4096; i += 32) {
+            const uint32_t t = __ldcg(table + i);
+            __stcg(table + i, t < delta ? 0u : t - delta);
+        }
+        startIndex = 65536u;
+        if (dsz > 65536u) dsz = 65536u;
+    }
+    if (n > (uint32_t)MAX_INPUT_SIZE) {                                       // lz4.c: before any state update
+        if (lane == 0) { __stcg(&st->currentOffset, startIndex); __stcg(&st->dictSize, dsz); }
+        __syncwarp();
+        return 0;
+    }
+    const uint32_t d = dsz < P ? dsz : P;                                     // LZ4_saveDict's clamp
+    const bool dictSmall = d < 65536u && d < startIndex;                      // lz4.c:1601
+    if (lane == 0) { __stcg(&st->currentOffset, startIndex + n); __stcg(&st->dictSize, d + n); }
+    return chain_search_warp<H4>(PrefixWindow{d}, src, n, startIndex, d, dictSmall, table, dst, cap);
 }
 
 // Persistent: one-warp CTAs pull blocks from a device counter.  Block b's result: 0 for n == 0 and -2

@@ -8,8 +8,8 @@
 // with value 65 536 - (dictEnd - p), the last writer per slot winning; a dictionary of fewer than 8 bytes loads
 // nothing and leaves dictSize = 0 (lz4.c:1499-1501), so it encodes exactly like an empty one.
 //
-// The search (encode_dict_warp) is the chained encoder's with startIndex = 65 536, dictSmall for dictSize < 65 536,
-// and the extDict addressing and catch-up floor.
+// The search (encode_dict_warp) is the chained encoder's, chain_search_warp, through ExtWindow: startIndex = 65 536,
+// dictSmall for dictSize < 65 536, and the extDict addressing and catch-up floor.
 //
 // Blocks whose dictionaries are the same bytes range share one loaded table: dict_key_kernel gives every block
 // the first block that claimed its (start, size) key, and each distinct key one record, up to DICT_RECORDS;
@@ -62,185 +62,42 @@ __device__ void load_dict_warp(const uint8_t* __restrict__ dict, int len, ChainS
     }
 }
 
-// Reads in the extDict layout: position p < 0 is dictEnd[p], the dictionary that logically precedes the source in
-// a buffer of its own.  A word may straddle the two buffers.
-__device__ __forceinline__ uint32_t ext_rd8(const uint8_t* src, const uint8_t* dictEnd, int p) {
-    return p < 0 ? (uint32_t)__ldg(dictEnd + p) : (uint32_t)__ldg(src + p);
-}
-__device__ __forceinline__ uint32_t ext_rd32(const uint8_t* src, const uint8_t* dictEnd, int p) {
-    if (p >= 0) return ldg_u32u(src + p);
-    if (p <= -4) return ldg_u32u(dictEnd + p);
-    uint32_t v = 0;
-    for (int i = 0; i < 4; i++) v |= ext_rd8(src, dictEnd, p + i) << (8 * i);
-    return v;
-}
+// Reads in the extDict layout: position p < 0 is dictEnd[p], the `d` kept dictionary bytes that logically precede
+// the source in a buffer of its own.  A word may straddle the two buffers.  same8 and floor/above keep the forms
+// PrefixWindow (encode_chain.cuh) explains: a byte compare of the widened reads, and the floor hoisted into an int.
+struct ExtWindow {
+    const uint8_t* dictEnd;
+    uint32_t d;
+    __device__ __forceinline__ uint32_t rd8(const uint8_t* __restrict__ src, int p) const {
+        return p < 0 ? (uint32_t)__ldg(dictEnd + p) : (uint32_t)__ldg(src + p);
+    }
+    __device__ __forceinline__ uint32_t rd32(const uint8_t* __restrict__ src, int p) const {
+        if (p >= 0) return ldg_u32u(src + p);
+        if (p <= -4) return ldg_u32u(dictEnd + p);
+        uint32_t v = 0;
+        for (int i = 0; i < 4; i++) v |= rd8(src, p + i) << (8 * i);
+        return v;
+    }
+    __device__ __forceinline__ bool same8(const uint8_t* __restrict__ src, int a, int b) const {
+        return rd8(src, a) == rd8(src, b);
+    }
+    __device__ __forceinline__ int floor(int m) const { return m < 0 ? -(int)d : 0; }
+    __device__ __forceinline__ bool above(int x, int low) const { return x > low; }
+};
 
 // One block against its loaded table `table` (a private copy: the block's stores go into it) and the `d` kept
 // dictionary bytes that end at dictEnd.  Returns the engine's value: bytes written, or 0 when a limitedOutput check
-// fails.  This is encode_chain_warp<false> (encode_chain.cuh, whose comments give the upstream lines) with
-// startIndex = 65 536 and these differences of the usingExtDict mode:
+// fails.  This is chain_search_warp<false> (encode_chain.cuh, whose comments give the upstream lines) with
+// startIndex = 65 536, dictSmall for d < 65 536 (lz4.c:1626-1629), and the usingExtDict mode's reads and catch-up:
 //   * an index below startIndex lies in the dictionary at dictEnd - (startIndex - index), and reads that run past
 //     the dictionary's end continue at src[0], as upstream's match count does (lz4.c:1078-1089);
 //   * a match found in the source catches up no further than the source's start (lz4.c:992, 1180); one found in
 //     the dictionary down to the dictionary's start (lz4.c:989, 1177).
-// It is a function of its own because a template switch in encode_chain_warp changed the chained kernels' code.
 __device__ int encode_dict_warp(const uint8_t* __restrict__ src, const uint32_t n, const uint8_t* __restrict__ dictEnd,
                                 const uint32_t d, uint8_t* __restrict__ dst, const int cap, uint32_t* table) {
-    const int lane = lane_id();
     if (n > (uint32_t)MAX_INPUT_SIZE) return 0;
-    const uint32_t startIndex = (uint32_t)DICT_WINDOW;
-    const bool dictSmall = d < (uint32_t)DICT_WINDOW;                        // lz4.c:1626-1629
-    const uint32_t prefixIdxLimit = startIndex - d;
-    auto accept = [&](uint32_t idx, uint32_t cur) {
-        return idx < cur && !(dictSmall && idx < prefixIdxLimit) && !(idx + (uint32_t)MAX_DISTANCE < cur);
-    };
-#define RD32(p) ext_rd32(src, dictEnd, (int)(p))
-#define RD8(p) ext_rd8(src, dictEnd, (int)(p))
-#define HASH(p) hash5(ldg_u64u(src + (p)), 12)
-    const int64_t olimit = cap;
-    uint32_t ip = 0, anchor = 0, op = 0;
-
-    if (n >= (uint32_t)MINLENGTH) {
-        const uint32_t mfl1 = n - MFLIMIT + 1, mlim = n - LASTLITERALS;
-        if (lane == 0) __stcg(table + HASH(0), startIndex);
-        __syncwarp();
-        ip = 1;
-        bool post = false;
-        uint32_t q0 = 0;
-        uint32_t base = 1;
-        for (;;) {
-            uint32_t h2 = 0xFFFFFFFFu;
-            if (post) h2 = HASH(ip - 2);
-            const bool isPost = post && lane == 0;
-            const uint32_t q = q0 + (uint32_t)lane - (post ? 1u : 0u);
-            const uint32_t pos = isPost ? ip : base + probe_advance(q);
-            const bool valid = isPost || (base + probe_advance(q + 1) <= mfl1);
-            const uint64_t v64 = valid ? ldg_u64u(src + pos) : 0ull;
-            const uint32_t v = (uint32_t)v64;
-            const uint32_t h = valid ? hash5(v64, 12) : (0x10000u + (uint32_t)lane);
-            uint32_t cand = valid ? __ldcg(table + h) : 0u;
-            if (h == h2) cand = startIndex + ip - 2;
-            const unsigned peers = __match_any_sync(FULL, h);
-            const unsigned earlier = peers & ((1u << lane) - 1u);
-            const int fromLane = earlier ? 31 - __clz(earlier) : lane;
-            const uint32_t fwdPos = __shfl_sync(FULL, pos, fromLane);
-            if (earlier) cand = startIndex + fwdPos;
-            const uint32_t cur = startIndex + pos;
-            bool hit = false;
-            if (valid && accept(cand, cur)) hit = RD32(cand - startIndex) == v;
-            const unsigned hits = __ballot_sync(FULL, hit);
-            const unsigned ends = __ballot_sync(FULL, !valid);
-            const int f = hits ? __ffs(hits) - 1 : 32;
-            const int e = ends ? __ffs(ends) - 1 : 32;
-            {
-                const int last = e < f ? e - 1 : f;
-                const unsigned upto = (last >= 31) ? 0xffffffffu : ((1u << (last + 1)) - 1u);
-                const unsigned later = peers & ~((2u << lane) - 1u) & upto;
-                const bool doStore = valid && ((1u << lane) & upto) && !(lane < 31 ? later : 0u);
-                if (post) {
-                    const unsigned same2 = __ballot_sync(FULL, valid && h == h2) & upto;
-                    if (lane == 0 && !same2) __stcg(table + h2, startIndex + ip - 2);
-                }
-                if (doStore) __stcg(table + h, cur);
-                __syncwarp();
-            }
-            if (e < f) break;
-            if (f == 32) {
-                if (post) { post = false; base = ip + 1; q0 = 31; }
-                else q0 += 32;
-                continue;
-            }
-            const bool zeroLit = post && f == 0;
-            int m = (int)(__shfl_sync(FULL, cand, f) - startIndex);           // < 0: in the dictionary
-            ip = __shfl_sync(FULL, pos, f);
-            const uint32_t a0h = ip + MINMATCH;
-            const int b0h = m + MINMATCH;
-            uint32_t x1 = 0u;
-            {
-                const uint32_t a = a0h + 4u * lane;
-                if (lane < 8 && (int)mlim - (int)a > 0) x1 = RD32(a) ^ RD32(b0h + 4 * lane);
-            }
-            uint32_t caught = 0;
-            if (!zeroLit) {                                                   // catch-up down to lowLimit
-                const int low = m < 0 ? -(int)d : 0;
-                for (int width = 8;; width = 32) {
-                    const bool part = lane < width;
-                    const bool ok = !part || ((ip > anchor + lane) && (m - lane > low) &&
-                                              (RD8(ip - 1 - lane) == RD8(m - 1 - lane)));
-                    const unsigned bad = __ballot_sync(FULL, !ok);
-                    const int c = bad ? __ffs(bad) - 1 : width;
-                    ip -= c; m -= c; caught += (uint32_t)c;
-                    if (bad) break;
-                }
-            }
-            const uint32_t lit = ip - anchor;
-            if (!zeroLit && (int64_t)op + 1 + lit + 8 + lit / 255 > olimit) return 0;
-            uint32_t mc = caught;
-            {
-                uint32_t a0 = a0h;
-                int b0 = b0h;
-                for (int width = 8;; width = 32) {
-                    const uint32_t a = a0 + 4u * lane;
-                    const int bb = b0 + 4 * lane;
-                    const bool part = lane < width;
-                    const int room = (int)mlim - (int)a;
-                    const uint32_t x = width == 8 ? x1 : ((part && room > 0) ? (RD32(a) ^ RD32(bb)) : 0u);
-                    int eq = x ? ((__ffs(x) - 1) >> 3) : 4;
-                    if (eq > room) eq = room < 0 ? 0 : room;
-                    if (!part) eq = 4;
-                    const unsigned stop = __ballot_sync(FULL, eq < 4);
-                    if (stop) {
-                        const int s = __ffs(stop) - 1;
-                        mc += 4u * s + (uint32_t)__shfl_sync(FULL, eq, s);
-                        break;
-                    }
-                    mc += 4u * width; a0 += 4u * width; b0 += 4 * width;
-                }
-            }
-            const uint32_t hdr = run_header_size(lit);
-            const uint32_t afterOff = op + hdr + lit + 2;
-            if ((int64_t)afterOff + 6 + (mc + 240) / 255 > olimit) return 0;
-            {
-                const uint32_t mlTok = mc >= 15 ? 15u : mc;
-                const uint32_t off = (uint32_t)((int)ip - m);
-                if (lane == 0) {
-                    if (lit >= 15) {
-                        uint32_t o = op, rest = lit - 15;
-                        dst[o++] = (uint8_t)(0xF0 | mlTok);
-                        for (; rest >= 255; rest -= 255) dst[o++] = 255;
-                        dst[o] = (uint8_t)rest;
-                    } else dst[op] = (uint8_t)((lit << 4) | mlTok);
-                    dst[afterOff - 2] = (uint8_t)off;
-                    dst[afterOff - 1] = (uint8_t)(off >> 8);
-                }
-                for (uint32_t i = lane; i < lit; i += 32) dst[op + hdr + i] = (uint8_t)RD8(anchor + i);
-                op = afterOff;
-                if (mc >= 15) {
-                    const uint32_t rest = mc - 15, nff = rest / 255;
-                    for (uint32_t i = lane; i < nff; i += 32) dst[op + i] = 0xFF;
-                    if (lane == 0) dst[op + nff] = (uint8_t)(rest % 255);
-                    op += nff + 1;
-                }
-            }
-            ip += mc + MINMATCH;
-            anchor = ip;
-            if (ip >= mfl1) break;
-            post = true; q0 = 0; base = ip + 1;
-        }
-    }
-    {   // last literals
-        const uint32_t run = n - anchor;
-        if ((int64_t)op + run + 1 + (run + 255 - 15) / 255 > olimit) return 0;
-        const uint32_t hdr = run_header_size(run);
-        if (lane == 0) write_run_header(dst, op, run);
-        op += hdr;
-        for (uint32_t i = lane; i < run; i += 32) dst[op + i] = (uint8_t)RD8(anchor + i);
-        op += run;
-        return (int)op;
-    }
-#undef RD32
-#undef RD8
-#undef HASH
+    return chain_search_warp<false>(ExtWindow{dictEnd, d}, src, n, (uint32_t)DICT_WINDOW, d,
+                                    d < (uint32_t)DICT_WINDOW, table, dst, cap);
 }
 
 // The key of a block's dictionary: the (start, size) of the bytes the load keeps.  An empty one is (0, 0).
