@@ -64,6 +64,11 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_decode_chain_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* prefixLen, int* outLen, int nBlocks, int memKind, void* cudaStream, int device);
+        // whole chained streams in one call: every block of every stream in flight at once
+        [DllImport(Lib)] public static extern int k4lz4_decode_chain_streams(
+            byte* srcBase, long* srcOff, int* srcLen, byte* raw, int* dstCap, int* outLen, int nEntries,
+            int* entryStart, byte* dstBase, long* dstOff, int* prefixLen, int nStreams, int memKind, void* cudaStream,
+            int device);
         // LZ4FastChainEncoder.Encode (LZ4_compress_fast_continue, prefix mode) for one block of each of many streams;
         // state = K4LZ4_CHAIN_STATE_BYTES (16 400) per stream, all zero for a new one
         [DllImport(Lib)] public static extern int k4lz4_encode_chain_batch(

@@ -207,6 +207,33 @@ K4LZ4_API int32_t k4lz4_decode_chain_batch(const uint8_t *srcBase, const int64_t
                                            const int32_t *prefixLen, int32_t *outLen, int32_t nBlocks,
                                            int32_t memKind, void *cudaStream, int32_t device);
 
+/* Whole chained streams in one call: nStreams streams, all their blocks in flight at once (DESIGN 4.11).  Exact, but
+ * not yet faster: measured on an H100 it is about 4x slower than k4lz4_decode_chain_batch stepped one block per
+ * stream per call, at 1 to 64 streams.
+ * Stream s owns entries [entryStart[s], entryStart[s+1]), in stream order (entryStart holds nStreams + 1 values,
+ * from 0 to nEntries).  Entry e reads srcBase[srcOff[e] .. +srcLen[e]) with capacity dstCap[e] (the blockSize
+ * LZ4ChainDecoder.Decode receives).  raw (may be NULL) marks with raw[e] != 0 an entry stored uncompressed: it is
+ * copied as-is (LZ4ChainDecoder.Inject, LZ4ChainDecoder.cs:64-93), and is -1 if srcLen[e] < 0 or > dstCap[e].
+ * Stream s decodes its entries back to back at dstBase + dstOff[s]; the prefixLen[s] bytes directly in front of it
+ * are its history, as in k4lz4_decode_chain_batch (>= 65535 = withPrefix64k; read, never written).  The caller
+ * provides sum(max(dstCap[e], 0)) bytes at dstOff[s] for every stream, and no stream's history or region may
+ * overlap another stream's region.
+ * outLen[e] is what k4lz4_decode_chain_batch returns for the entry when the stream is decoded one block per call,
+ * in order, each behind prefixLen[s] + the bytes decoded so far; a stored entry's is its length.  From a stream's
+ * first failing entry on (where LZ4ChainDecoder.Decode would throw) every outLen of that stream is -1.  Bytes of
+ * a stream's region at or after its failing entry are unspecified; nothing is written outside the stream regions.
+ * Arguments, checks and codes as k4lz4_decode_chain_batch: with host memory a malformed entryStart or a negative
+ * prefixLen is K4LZ4_E_ARG; with device memory neither can be checked (an entry no stream holds, and every entry
+ * of a stream with a negative prefixLen, get -1).  Host memory is synchronous, runs on one GPU (`device`,
+ * K4LZ4_ALL_DEVICES = GPU 0) and splits a stream larger than a staging chunk into consecutive pieces; device
+ * memory only enqueues work on `cudaStream`.  The call takes 24 KiB of device workspace per entry from the library's
+ * private pool (with host memory, per entry of a chunk). */
+K4LZ4_API int32_t k4lz4_decode_chain_streams(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                             const uint8_t *raw, const int32_t *dstCap, int32_t *outLen,
+                                             int32_t nEntries, const int32_t *entryStart, uint8_t *dstBase,
+                                             const int64_t *dstOff, const int32_t *prefixLen, int32_t nStreams,
+                                             int32_t memKind, void *cudaStream, int32_t device);
+
 /* LZ4FastChainEncoder.Encode -> LLxx.LZ4_compress_fast_continue(state, src, dst, n, dstCap, 1)
  * (Encoders/LZ4FastChainEncoder.cs:35-41, Engine/x64/LL64.fast.cs:582-667) with the stream's history
  * contiguous in front of the source (the prefix mode the reference's ring buffer sets up).

@@ -282,6 +282,45 @@ private:
     std::vector<uint8_t> out_;
 };
 
+// One chained stream (LZ4ChainDecoder.Decode over consecutive blocks) in one call, every block in flight at once
+// (k4lz4_decode_chain_streams).  `history` is the stream's output so far (the last 64 KiB are read); a block with
+// raw = true was stored as is (LZ4ChainDecoder.Inject).  Returns the decoded bytes; throws InvalidOperationException
+// where LZ4ChainDecoder would, NativeError on a library-level failure.  Not a speed-up today: on an H100 one stream
+// decodes about 4x slower this way than one block per call (DESIGN 4.11).
+struct ChainStream {
+    struct Item { const uint8_t* data; int length; int blockSize; bool raw; };
+    static std::vector<uint8_t> Decode(const std::vector<Item>& items, const uint8_t* history = nullptr,
+                                       int historyLength = 0) {
+        const int n = (int)items.size();
+        const int32_t hl = historyLength < 65536 ? historyLength : 65536;
+        std::vector<int64_t> so((size_t)n);
+        std::vector<int32_t> sl((size_t)n), cap((size_t)n), got((size_t)n, -1);
+        std::vector<uint8_t> raw((size_t)n);
+        int64_t tot = 0, room = 0;
+        for (int i = 0; i < n; i++) {
+            const Item& it = items[(size_t)i];
+            so[(size_t)i] = tot; sl[(size_t)i] = it.length; tot += it.length > 0 ? it.length : 0;
+            cap[(size_t)i] = it.raw ? it.length : it.blockSize; room += cap[(size_t)i] > 0 ? cap[(size_t)i] : 0;
+            raw[(size_t)i] = it.raw ? 1 : 0;
+        }
+        std::vector<uint8_t> src((size_t)tot + 16), dst((size_t)(hl + room) + 16);
+        for (int i = 0; i < n; i++)
+            if (sl[(size_t)i] > 0) std::copy(items[(size_t)i].data, items[(size_t)i].data + sl[(size_t)i], src.begin() + so[(size_t)i]);
+        if (hl > 0) std::copy(history + historyLength - hl, history + historyLength, dst.begin());
+        const int32_t es[2] = {0, n};
+        const int64_t dof = hl;
+        const int rc = k4lz4_decode_chain_streams(src.data(), so.data(), sl.data(), raw.data(), cap.data(), got.data(), n,
+                                                  es, dst.data(), &dof, &hl, 1, K4LZ4_MEM_HOST, nullptr, K4LZ4_ALL_DEVICES);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        int64_t at = hl;
+        for (int i = 0; i < n; i++) {
+            if (got[(size_t)i] < 0) throw std::runtime_error("InvalidOperationException");
+            at += got[(size_t)i];
+        }
+        return std::vector<uint8_t>(dst.begin() + hl, dst.begin() + at);
+    }
+};
+
 // Chain groups (k4lz4_chain_group_*): S chained streams whose rings and encoder states stay on one GPU.  RAII owner
 // of the group; the calls take the C ABI's batch arrays (host or device memory) and throw NativeError on a
 // library-level failure.  Like the reference's encoder and decoder objects, not thread-safe.

@@ -47,6 +47,7 @@ SIGNATURES = {
     "k4lz4_encode_dict": ([_vp, _i32, _vp, _i32, _vp, _i32], _i32),
     "k4lz4_encode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),
+    "k4lz4_decode_chain_streams": ([_vp] * 6 + [_i32] + [_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch_x32": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),
     "k4lz4_unpickle_batch": (_BATCH + [_i32] + _CALL, _i32),

@@ -313,6 +313,35 @@ def decode_chain_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, 
                                              int(device)))
 
 
+def decode_chain_streams_host(src: np.ndarray, src_off, src_len, dst_cap, entry_start, dst: np.ndarray, dst_off,
+                              prefix_len, raw=None, device: int = 0) -> np.ndarray:
+    """Whole chained streams in one call (k4lz4_decode_chain_streams, host memory).  Stream s owns entries
+    entry_start[s] .. entry_start[s+1] and decodes them back to back into dst[dst_off[s] ..), behind the
+    prefix_len[s] bytes in front of it (its history); dst needs sum(max(dst_cap, 0)) bytes of each stream's entries
+    there.  raw[e] (optional) marks an entry stored uncompressed.  Returns int32 results per entry: what stepping
+    decode_chain_batch_host block by block gives, and -1 from a stream's first failing entry on."""
+    src_off, dst_off = _i64(src_off), _i64(dst_off)
+    src_len, dst_cap, entry_start, prefix_len = _i32(src_len), _i32(dst_cap), _i32(entry_start), _i32(prefix_len)
+    raw = None if raw is None else np.ascontiguousarray(raw, dtype=np.uint8)
+    n, m = int(src_len.shape[0]), int(entry_start.shape[0]) - 1
+    out = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_decode_chain_streams(src.ctypes.data, src_off.ctypes.data, src_len.ctypes.data,
+                                               None if raw is None else raw.ctypes.data, dst_cap.ctypes.data,
+                                               out.ctypes.data, n, entry_start.ctypes.data, dst.ctypes.data,
+                                               dst_off.ctypes.data, prefix_len.ctypes.data, max(m, 0), N.MEM_HOST,
+                                               None, int(device)))
+    return out
+
+
+def decode_chain_streams_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, raw_ptr: int, dst_cap_ptr: int,
+                                out_len_ptr: int, n: int, entry_start_ptr: int, dst_ptr: int, dst_off_ptr: int,
+                                prefix_len_ptr: int, m: int, stream: int = 0, device: int = -1) -> None:
+    """Device-pointer form of decode_chain_streams_host (raw_ptr may be 0): only enqueues the kernels on `stream`."""
+    N.check(N.lib().k4lz4_decode_chain_streams(src_ptr, src_off_ptr, src_len_ptr, raw_ptr or None, dst_cap_ptr,
+                                               out_len_ptr, int(n), entry_start_ptr, dst_ptr, dst_off_ptr,
+                                               prefix_len_ptr, int(m), N.MEM_DEVICE, stream or None, int(device)))
+
+
 def partial_decode_batch_host(blocks: Sequence, targets: Sequence[int], device: int = 0):
     """LZ4Codec.PartialDecode over a batch (k4lz4_partial_decode_batch, host memory)."""
     src, so, sl = _pack(blocks)

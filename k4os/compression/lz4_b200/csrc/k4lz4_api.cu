@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "decode_generic.cuh"
 #include "decode_tile.cuh"
+#include "decode_stream.cuh"
 #include "encode_generic.cuh"
 #include "encode_tile.cuh"
 #include "encode_chain.cuh"
@@ -967,6 +968,170 @@ int run_staged(Op op, const Batch& b, int dev) {
         rc = stage_down(D->stage, up, nb, b.outLen + i, 1, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
         if (rc != K4LZ4_OK) return rc;
     }
+    return K4LZ4_OK;
+}
+
+// ---- whole chained streams (k4lz4_decode_chain_streams) ------------------------------------------------------
+
+// Entry e reads srcBase[srcOff[e] .. +srcLen[e]) (stored as-is where raw[e]) into at most dstCap[e] bytes; stream s
+// owns entries [entryStart[s], entryStart[s+1]) and decodes them back to back at dstBase + dstOff[s], behind its
+// prefixLen[s] bytes of history.
+struct Streams {
+    const uint8_t* srcBase; const int64_t* srcOff; const int32_t* srcLen; const uint8_t* raw;
+    const int32_t* dstCap; int32_t* outLen; int64_t n;
+    const int32_t* entryStart; uint8_t* dstBase; const int64_t* dstOff; const int32_t* prefixLen; int64_t m;
+};
+
+// The checks of check(OP_CHAIN, ...) plus the stream table's; as there, device arrays cannot be checked here.
+int check_streams(const Streams& a, int memKind, int device) {
+    if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
+    if (a.n < 0 || a.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad entry count %lld", (long long)a.n);
+    if (a.m < 0 || a.m > INT32_MAX) return fail(K4LZ4_E_ARG, "bad stream count %lld", (long long)a.m);
+    if (a.n > 0 && a.m == 0) return fail(K4LZ4_E_ARG, "%lld entries but no stream", (long long)a.n);
+    if (a.n > 0 && (!a.srcBase || !a.srcOff || !a.srcLen || !a.dstCap || !a.outLen || !a.entryStart || !a.dstBase ||
+                    !a.dstOff || !a.prefixLen))
+        return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (a.n > 0 && memKind == K4LZ4_MEM_HOST) {
+        if (a.entryStart[0] != 0 || a.entryStart[a.m] != a.n)
+            return fail(K4LZ4_E_ARG, "entryStart must run from 0 to the entry count %lld", (long long)a.n);
+        for (int64_t s = 0; s < a.m; s++) {
+            if (a.entryStart[s + 1] < a.entryStart[s]) return fail(K4LZ4_E_ARG, "entryStart decreases at stream %lld", (long long)s);
+            if (a.prefixLen[s] < 0) return fail(K4LZ4_E_ARG, "negative prefix length at stream %lld", (long long)s);
+        }
+    }
+    return check_device(device, a.n);
+}
+
+// Host memory: one GPU, in chunks of at most STAGE_BYTES through the device's staging (stage_up / stage_down), one
+// row per entry; an entry counts its bytes and the 24 KiB of device workspace its deferred list takes.  A stream whose entries do not fit one chunk continues in the next as a new piece, behind the last
+// <= 65535 bytes its earlier pieces produced (already in the caller's buffer), with prefix length prefixLen[s] plus
+// the bytes produced so far, clamped to 65535 (every larger value reads the same bytes).  The pieces' stream table
+// goes up beside the staged rows; each piece's output comes back in one copy.
+int run_streams_staged(const Streams& a, int dev) {
+    DeviceGuard guard(dev);
+    if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
+    Dev* D = dev_state(dev);
+    if (!D) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
+    if (D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d: %s", dev, cudaGetErrorString(D->err));
+    std::lock_guard<std::mutex> lk(D->stageMu);
+    Staging& S = D->stage;
+    auto a16 = [](int64_t x) { return (x + 15) & ~int64_t(15); };
+    auto cap = [&](int64_t e) -> int64_t { return std::max<int32_t>(a.dstCap[e], 0); };
+    auto send = [&](int64_t e) -> int64_t { return std::max<int32_t>(a.srcLen[e], 0); };
+    struct Piece { int64_t s, e0, e1, row0, room; int32_t hist; };
+    std::vector<int64_t> pos((size_t)a.m, 0);        // bytes stream s produced in earlier pieces
+    std::vector<char> dead((size_t)a.m, 0);
+    std::vector<Piece> pieces;
+    std::vector<int64_t> rows;
+    std::vector<int32_t> res;
+    std::vector<uint8_t> table;
+    int64_t s = 0, e = 0;
+    for (;;) {
+        pieces.clear(); rows.clear();
+        int64_t bytes = 0;
+        while (s < a.m) {
+            if (e >= a.entryStart[s + 1]) { s++; continue; }
+            if (dead[(size_t)s]) { a.outLen[e++] = -1; continue; }
+            const bool fresh = pieces.empty() || pieces.back().s != s;
+            const int32_t hist = (int32_t)std::min<int64_t>((int64_t)a.prefixLen[s] + pos[(size_t)s], 65535);
+            // the entry's bytes and its share of the device workspace (its deferred list)
+            const int64_t add = send(e) + cap(e) + 32 + (fresh ? hist + 16 : 0) +
+                                (int64_t)k4::DS_BUDGET * (int64_t)sizeof(k4::DeferCopy);
+            if (!rows.empty() && bytes + add > STAGE_BYTES) break;
+            bytes += add;
+            if (fresh) pieces.push_back(Piece{s, e, e, (int64_t)rows.size(), 0, hist});
+            pieces.back().e1 = e + 1;
+            pieces.back().room += cap(e);
+            rows.push_back(e++);
+        }
+        if (rows.empty()) return K4LZ4_OK;
+        const int64_t nb = (int64_t)rows.size(), np = (int64_t)pieces.size();
+        std::vector<int64_t> head((size_t)nb, -1);    // the piece whose first row this is
+        for (int64_t p = 0; p < np; p++) head[(size_t)pieces[(size_t)p].row0] = p;
+        // the device's stream table: entryStart (np + 1) | prefixLen (np) | dstOff (np) | raw (nb)
+        const int64_t esAt = 0, preAt = a16((np + 1) * 4), offAt = preAt + a16(np * 4), rawAt = offAt + np * 8;
+        const int64_t tabBytes = rawAt + a16(nb);
+        StageUp up;
+        int rc = stage_up(S, nb, 1, tabBytes, [&](int64_t k) {
+            const int64_t x = rows[(size_t)k];
+            UpRow r{a.srcBase + a.srcOff[x], send(x), 0, 0, a.srcLen[x],
+                    a.dstCap[x], 0};
+            const int64_t p = head[(size_t)k];
+            if (p >= 0) {
+                const Piece& q = pieces[(size_t)p];
+                r.room = q.room; r.dstPre = q.hist; r.dst = a.dstBase + a.dstOff[q.s] + pos[(size_t)q.s];
+            }
+            return r;
+        }, up, nullptr);
+        if (rc != K4LZ4_OK) return rc;
+        // each piece's device slot (stage_up's slot offset of its first row), before stage_down reuses hUp
+        std::vector<int64_t> slot((size_t)np);
+        for (int64_t p = 0; p < np; p++) slot[(size_t)p] = ((const int64_t*)S.hUp.p + nb)[pieces[(size_t)p].row0];
+        table.assign((size_t)tabBytes, 0);
+        int32_t* es = (int32_t*)(table.data() + esAt); int32_t* pre = (int32_t*)(table.data() + preAt);
+        int64_t* doff = (int64_t*)(table.data() + offAt);
+        for (int64_t p = 0; p < np; p++) {
+            const Piece& q = pieces[(size_t)p];
+            es[p] = (int32_t)q.row0; pre[p] = q.hist; doff[p] = slot[(size_t)p];
+        }
+        es[np] = (int32_t)nb;
+        for (int64_t k = 0; a.raw && k < nb; k++) table[(size_t)(rawAt + k)] = a.raw[rows[(size_t)k]] ? 1 : 0;
+        CU_TRY(cudaMemcpyAsync(up.extra, table.data(), (size_t)tabBytes, cudaMemcpyHostToDevice, nullptr));
+        const cudaError_t le = k4::stream_decode_launch(
+            up.src, up.srcOff, up.len, a.raw ? up.extra + rawAt : nullptr, up.cap, up.res, (int)nb,
+            (const int32_t*)(up.extra + esAt), up.dst, (const int64_t*)(up.extra + offAt),
+            (const int32_t*)(up.extra + preAt), (int)np, nullptr, D->pool, D->sms);
+        if (le != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "stream decode launch: %s", cudaGetErrorString(le)); }
+        g_launches += k4::DS_LAUNCHES;
+        res.assign((size_t)nb, -1);
+        rc = stage_down(S, up, nb, res.data(), 1, nullptr, nullptr, nullptr, nullptr);
+        if (rc != K4LZ4_OK) return rc;
+        // each piece's produced bytes: one copy down, then to the caller's buffer behind its earlier pieces
+        std::vector<int64_t> got((size_t)np, 0), co((size_t)np, 0);
+        int64_t total = 0;
+        for (int64_t p = 0; p < np; p++) {
+            const Piece& q = pieces[(size_t)p];
+            for (int64_t k = q.row0; k < q.row0 + (q.e1 - q.e0); k++) {
+                a.outLen[rows[(size_t)k]] = res[(size_t)k];
+                if (res[(size_t)k] < 0) dead[(size_t)q.s] = 1; else got[(size_t)p] += res[(size_t)k];
+            }
+            co[(size_t)p] = total;
+            total = a16(total + got[(size_t)p]);
+        }
+        if (total == 0) continue;
+        CU_TRY(S.hDown.ensure((size_t)total + 16));
+        for (int64_t p = 0; p < np; p++)
+            if (got[(size_t)p] > 0)
+                CU_TRY(cudaMemcpyAsync((uint8_t*)S.hDown.p + co[(size_t)p], up.dst + slot[(size_t)p],
+                                       (size_t)got[(size_t)p], cudaMemcpyDeviceToHost, nullptr));
+        CU_TRY(cudaStreamSynchronize(nullptr));
+        parallel_for_blocks(0, np, total, [&](int64_t lo, int64_t hi) {
+            for (int64_t p = lo; p < hi; p++) {
+                const Piece& q = pieces[(size_t)p];
+                if (got[(size_t)p] > 0)
+                    memcpy(a.dstBase + a.dstOff[q.s] + pos[(size_t)q.s], (const uint8_t*)S.hDown.p + co[(size_t)p],
+                           (size_t)got[(size_t)p]);
+            }
+        });
+        for (int64_t p = 0; p < np; p++) pos[(size_t)pieces[(size_t)p].s] += got[(size_t)p];
+    }
+}
+
+int run_streams(const Streams& a, int memKind, void* stream, int device) {
+    const int rc = check_streams(a, memKind, device);
+    if (rc != K4LZ4_OK || a.n == 0) return rc;
+    if (memKind == K4LZ4_MEM_HOST) return run_streams_staged(a, device < 0 ? 0 : device);
+    DeviceGuard g(device);
+    if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
+    int dev = 0;
+    CU_TRY(cudaGetDevice(&dev));
+    const Dev* D = dev_state(dev);
+    if (!D || D->err != cudaSuccess) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
+    const cudaError_t e = k4::stream_decode_launch(a.srcBase, a.srcOff, a.srcLen, a.raw, a.dstCap, a.outLen, (int)a.n,
+                                                   a.entryStart, a.dstBase, a.dstOff, a.prefixLen, (int)a.m,
+                                                   (cudaStream_t)stream, D->pool, D->sms);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "stream decode launch: %s", cudaGetErrorString(e)); }
+    g_launches += k4::DS_LAUNCHES;
     return K4LZ4_OK;
 }
 
@@ -2179,6 +2344,15 @@ int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, 
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
     b.prefixLen = prefixLen;
     return run(OP_CHAIN, b, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_decode_chain_streams(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                   const uint8_t* raw, const int32_t* dstCap, int32_t* outLen, int32_t nEntries,
+                                   const int32_t* entryStart, uint8_t* dstBase, const int64_t* dstOff,
+                                   const int32_t* prefixLen, int32_t nStreams,
+                                   int32_t memKind, void* cudaStream, int32_t device) {
+    return run_streams(Streams{srcBase, srcOff, srcLen, raw, dstCap, outLen, nEntries, entryStart, dstBase, dstOff,
+                               prefixLen, nStreams}, memKind, cudaStream, device);
 }
 
 namespace {
