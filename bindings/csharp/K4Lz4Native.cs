@@ -138,6 +138,18 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_frame_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* outLen, int nFrames, int memKind, void* cudaStream, int device);
+        // LZ4 frames against a dictionary (k4lz4.h "LZ4 Frame against a dictionary"; no reference call)
+        [DllImport(Lib)] public static extern int k4lz4_frame_encode_dict_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* dictBase, long* dictOff, int* dictLen, uint* dictId, int* outLen, int nFrames, int blockSize,
+            int flags, int level, int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_decode_dict_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* dictBase, long* dictOff, int* dictLen, int* outLen, int nFrames, int memKind, void* cudaStream,
+            int device);
+        [DllImport(Lib)] public static extern int k4lz4_frame_info_batch(
+            byte* srcBase, long* srcOff, int* srcLen, int* outSize, long* outDictId, int nFrames, int memKind,
+            void* cudaStream, int device);
         // LZ4EncoderStream / LZ4FrameWriter written incrementally, batched across streams (k4lz4.h "frame writer group")
         [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_create(
             int nStreams, int blockSize, int flags, int level, int device, void** group);

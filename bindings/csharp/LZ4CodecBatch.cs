@@ -52,6 +52,54 @@ namespace K4os.Compression.LZ4
                     K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
         }
 
+        // LZ4 frames against a dictionary, as upstream's LZ4F_compressBegin_usingCDict writes them
+        // (k4lz4_frame_encode_dict_batch): frame i holds source i, encoded against dictionary i, with the dictID
+        // dictionaryIds[i] unless it is 0 (an empty span: no IDs).  blockSize: 64 KiB, 256 KiB, 1 MiB or 4 MiB; flags:
+        // K4Lz4Native.FRAME_*.  lengths[i]: the frame's length, -1 where it does not fit targetCapacities[i].
+        public static void EncodeFramesWithDictionary(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            ReadOnlySpan<byte> dictionaryBase, ReadOnlySpan<long> dictionaryOffsets,
+            ReadOnlySpan<int> dictionaryLengths, ReadOnlySpan<uint> dictionaryIds, Span<int> lengths,
+            int blockSize = 65536, int flags = 0)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (byte* x = dictionaryBase) fixed (long* xo = dictionaryOffsets) fixed (int* xl = dictionaryLengths)
+            fixed (uint* xi = dictionaryIds) fixed (int* ol = lengths)
+                Check(K4Lz4Native.k4lz4_frame_encode_dict_batch(s, so, sl, d, dof, dc, x, xo, xl,
+                    dictionaryIds.Length > 0 ? xi : null, ol, lengths.Length, blockSize, flags, 0,
+                    K4Lz4Native.MEM_HOST, null, 0));
+        }
+
+        // Frames against a dictionary, with or without a dictID field (k4lz4_frame_decode_dict_batch); lengths[i]
+        // as k4lz4_frame_decode_batch gives them.  Pick the dictionaries with FrameInfo.
+        public static void DecodeFramesWithDictionary(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            ReadOnlySpan<byte> dictionaryBase, ReadOnlySpan<long> dictionaryOffsets,
+            ReadOnlySpan<int> dictionaryLengths, Span<int> lengths)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (byte* x = dictionaryBase) fixed (long* xo = dictionaryOffsets) fixed (int* xl = dictionaryLengths)
+            fixed (int* ol = lengths)
+                Check(K4Lz4Native.k4lz4_frame_decode_dict_batch(s, so, sl, d, dof, dc, x, xo, xl, ol, lengths.Length,
+                    K4Lz4Native.MEM_HOST, null, 0));
+        }
+
+        // sizes[i]: the content size (the dictionary flag accepted); dictionaryIds[i]: the header's dictID, -1 without
+        // a dictID field (k4lz4_frame_info_batch).
+        public static void FrameInfo(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<int> sizes, Span<long> dictionaryIds)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (int* os = sizes) fixed (long* oi = dictionaryIds)
+                Check(K4Lz4Native.k4lz4_frame_info_batch(s, so, sl, os, oi, sizes.Length,
+                    K4Lz4Native.MEM_HOST, null, 0));
+        }
+
         // sizes[i]: what Decode needs as targetCapacities[i] -- 0 for an empty block, -1 where the token chain does
         // not parse (Decode then fails at any capacity)
         public static void DecodedSizes(

@@ -423,6 +423,43 @@ K4LZ4_API int32_t k4lz4_frame_decode_batch(const uint8_t *srcBase, const int64_t
                                            int32_t *outLen, int32_t nFrames,
                                            int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- LZ4 Frame against a dictionary (upstream's LZ4F_compressBegin_usingCDict / LZ4F_decompress_usingDict,
+ * lz4 -D).  No reference call: the reference's frame code throws NotImplementedException for dictionaries. ---- */
+
+/* Frames against a dictionary: byte for byte what upstream writes with
+ * LZ4F_compressBegin_usingCDict(LZ4F_createCDict(dict_i)) + LZ4F_compressUpdate(all) + LZ4F_compressEnd,
+ * prefs = {blockSizeID of blockSize, linked unless K4LZ4_FRAME_INDEPENDENT, the checksums `flags` asks for,
+ * dictID = dictId[i], level 0, autoFlush 0, no content size}.  Frame i's dictionary is
+ * dictBase[dictOff[i] .. + dictLen[i]); only its last 64 KiB count, and one of fewer than 8 bytes loads nothing.
+ * dictId may be NULL; an ID of 0 writes no dictID field (as lz4 -D).  Every block is encoded with capacity n - 1 and
+ * stored raw when it does not fit (lz4frame.c:747-749; not k4lz4_frame_encode_batch's rule).  blockSize must be
+ * 65 536, 262 144, 1 048 576 or 4 194 304, flags as k4lz4_frame_bound.  The largest frame is
+ * k4lz4_frame_bound(length, blockSize, flags), + 4 when the ID is not 0.  outLen[i] = the frame's length; -1 when it
+ * does not fit dstCap[i]; K4LZ4_R_DELEGATE for level >= 3, nothing written.  Nothing is ever written at or beyond
+ * dstCap[i].  Argument errors as k4lz4_frame_encode_batch, then the dictionary arrays (required when nFrames > 0). */
+K4LZ4_API int32_t k4lz4_frame_encode_dict_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                                const uint8_t *dictBase, const int64_t *dictOff, const int32_t *dictLen,
+                                                const uint32_t *dictId, int32_t *outLen, int32_t nFrames,
+                                                int32_t blockSize, int32_t flags, int32_t level,
+                                                int32_t memKind, void *cudaStream, int32_t device);
+/* k4lz4_frame_decode_batch's results, codes, their order and capacities, except that the dictionary flag is
+ * accepted (its 4 ID bytes are covered by the header checksum and otherwise skipped) and every frame, with or without
+ * an ID, decodes against its dictionary.  The ID is not checked against the dictionary (as upstream); pick the
+ * dictionaries with k4lz4_frame_info_batch.  Linked block k decodes as k4lz4_decode_chain_batch would behind the last
+ * 64 KiB of (dictionary | blocks 0 .. k-1); independent blocks each as k4lz4_decode_dict against the dictionary.
+ * dictBase may be NULL: no dictionaries (every result then equals k4lz4_frame_decode_batch's, except for the flag). */
+K4LZ4_API int32_t k4lz4_frame_decode_dict_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                                uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                                const uint8_t *dictBase, const int64_t *dictOff, const int32_t *dictLen,
+                                                int32_t *outLen, int32_t nFrames,
+                                                int32_t memKind, void *cudaStream, int32_t device);
+/* outSize[i] as k4lz4_frame_content_size_batch, except that the dictionary flag is not a verdict;
+ * outDictId[i] = the header's dictID, or -1 when the frame has no dictID field (or no valid header). */
+K4LZ4_API int32_t k4lz4_frame_info_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                         int32_t *outSize, int64_t *outDictId, int32_t nFrames,
+                                         int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- LZ4 Frame, written incrementally: LZ4EncoderStream / LZ4FrameWriter, batched across streams ------ */
 
 /*

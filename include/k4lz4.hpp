@@ -11,6 +11,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "k4lz4.h"
@@ -592,6 +593,60 @@ struct LZ4Frame {
     }
     static std::vector<uint8_t> Decode(const std::vector<uint8_t>& frame, int device = 0) {
         return DecodeMany({frame}, device)[0];
+    }
+    // Against a dictionary (k4lz4_frame_encode_dict_batch): upstream's CDict frame, the ID written unless 0;
+    // s.blockSize is 64 KiB, 256 KiB, 1 MiB or 4 MiB.
+    static std::vector<uint8_t> EncodeWithDictionary(const std::vector<uint8_t>& source,
+                                                     const std::vector<uint8_t>& dictionary, uint32_t dictId = 0,
+                                                     const Settings& s = {}, int device = 0) {
+        const int64_t so = 0, dofs = 0, dictOff = 0;
+        const int32_t sl = (int32_t)source.size(), dl = (int32_t)dictionary.size();
+        const int32_t dc = (int32_t)(Bound(sl, s) + (dictId ? 4 : 0));
+        int32_t out = -1;
+        std::vector<uint8_t> src(source), dict(dictionary), dst((size_t)dc + 1);
+        src.resize(src.size() + 1); dict.resize(dict.size() + 1);
+        const int rc = k4lz4_frame_encode_dict_batch(src.data(), &so, &sl, dst.data(), &dofs, &dc, dict.data(), &dictOff,
+                                                     &dl, &dictId, &out, 1, s.blockSize, flags(s), (int)s.level,
+                                                     K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        if (out == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("dictionary frames at the HC levels");
+        if (out < 0) throw std::runtime_error("Failed to encode the frame.");
+        dst.resize((size_t)out);
+        return dst;
+    }
+    // The content sizes (as ContentSizes, the dictionary flag accepted) and the headers' dictIDs (-1: none).
+    static std::pair<std::vector<int32_t>, std::vector<int64_t>> Info(const std::vector<std::vector<uint8_t>>& frames,
+                                                                      int device = 0) {
+        const size_t n = frames.size();
+        std::vector<int64_t> so(n), ids(n, -1);
+        std::vector<int32_t> sl(n), out(n, -1);
+        std::vector<uint8_t> src;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)frames[i].size();
+            src.insert(src.end(), frames[i].begin(), frames[i].end());
+        }
+        src.resize(src.size() + 1);
+        const int rc = k4lz4_frame_info_batch(src.data(), so.data(), sl.data(), out.data(), ids.data(), (int32_t)n,
+                                              K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        return {out, ids};
+    }
+    // Against a dictionary, with or without a dictID field (k4lz4_frame_decode_dict_batch).
+    static std::vector<uint8_t> DecodeWithDictionary(const std::vector<uint8_t>& frame,
+                                                     const std::vector<uint8_t>& dictionary, int device = 0) {
+        const int32_t size = Info({frame}, device).first[0];
+        raise_for(size);
+        const int64_t so = 0, dofs = 0, dictOff = 0;
+        const int32_t sl = (int32_t)frame.size(), dl = (int32_t)dictionary.size(), dc = size;
+        int32_t out = -1;
+        std::vector<uint8_t> src(frame), dict(dictionary), dst((size_t)size + 1);
+        src.resize(src.size() + 1); dict.resize(dict.size() + 1);
+        const int rc = k4lz4_frame_decode_dict_batch(src.data(), &so, &sl, dst.data(), &dofs, &dc, dict.data(), &dictOff,
+                                                     &dl, &out, 1, K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        raise_for(out);
+        dst.resize((size_t)out);
+        return dst;
     }
 private:
     static void raise_for(int32_t r) {

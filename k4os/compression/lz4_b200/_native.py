@@ -77,6 +77,9 @@ SIGNATURES = {
     "k4lz4_frame_encode_batch_x32": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
     "k4lz4_frame_content_size_batch": ([_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_frame_decode_batch": (_BATCH + [_i32] + _CALL, _i32),
+    "k4lz4_frame_encode_dict_batch": ([_vp] * 11 + [_i32] * 4 + _CALL, _i32),
+    "k4lz4_frame_decode_dict_batch": ([_vp] * 10 + [_i32] + _CALL, _i32),
+    "k4lz4_frame_info_batch": ([_vp] * 5 + [_i32] + _CALL, _i32),
     "k4lz4_frame_writer_group_create": ([_i32, _i32, _i32, _i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_destroy": ([_vp], _i32),
     "k4lz4_frame_writer_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),

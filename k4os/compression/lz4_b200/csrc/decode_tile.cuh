@@ -370,9 +370,14 @@ __device__ __forceinline__ void warp_copy_hist(const uint32_t d, const uint8_t* 
 // whose source starts before the block is split the way the reference splits an external-dictionary match
 // (LL64.dec.cs:359-374): the history part is copied from global memory in the far phase, the remainder is
 // a match at d' = off with source 0 and is scheduled like any other.  With P = 0 nothing changes.
-template <int STAGE>
+//
+// EXT: the history is not in front of gdst but ends at `hist` (a dictionary in a buffer of its own, the usingExtDict
+// mode of LZ4_decompress_safe_usingDict): the history parts are read from hist + (d - off), P is the dictionary's
+// length for the offset test.  The instantiation without EXT never reads `hist`.
+template <int STAGE, bool EXT = false>
 __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__ src, const int n,
-                                 uint8_t* __restrict__ gdst, const int cap, const int P, uint32_t& barParity) {
+                                 uint8_t* __restrict__ gdst, const int cap, const int P, uint32_t& barParity,
+                                 const uint8_t* __restrict__ hist = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int shift = (int)(reinterpret_cast<uintptr_t>(src) & 15);
     uint8_t* const stg = S.stage + shift;                       // stg[p] == src[p]
@@ -538,7 +543,7 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
         }
         DT_PROF(5);
 
-        // history part of a match whose source starts before the block: hl bytes from gdst + d - off
+        // history part of a match whose source starts before the block: hl bytes from hEnd + d - off
         int d = op + lit;                                        // match destination
         const int hl = P > 0 && off > d ? (off - d < ml ? off - d : ml) : 0;
         const int hd = d;
@@ -560,11 +565,12 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
         if (P > 0) {
             // history parts: nothing else of this step reads or writes [hd, hd + hl) before barrier #1, and a
             // near remainder that reads it (off < its length) runs behind that barrier
-            lanes_copy_hist(sT + (uint32_t)hd, gdst + (hd - off), hl <= DT_LSHORT ? hl : 0);
+            const uint8_t* const hEnd = EXT ? hist : gdst;
+            lanes_copy_hist(sT + (uint32_t)hd, hEnd + (hd - off), hl <= DT_LSHORT ? hl : 0);
             for (unsigned m = __ballot_sync(FULL, hl > DT_LSHORT); m; m &= m - 1) {
                 const int l = __ffs(m) - 1;
                 const int ld = __shfl_sync(FULL, hd, l);
-                warp_copy_hist(sT + (uint32_t)ld, gdst + (ld - __shfl_sync(FULL, off, l)), __shfl_sync(FULL, hl, l), lane);
+                warp_copy_hist(sT + (uint32_t)ld, hEnd + (ld - __shfl_sync(FULL, off, l)), __shfl_sync(FULL, hl, l), lane);
             }
         }
         DT_PROF(6);
@@ -710,20 +716,34 @@ __device__ __forceinline__ int chain_prefix(const int32_t* prefixLen, int b) {
     return p < 65535 ? p : 65535;
 }
 
-// launch 1: one CTA per block, small stage, two CTAs per SM
-__global__ void __launch_bounds__(DT_THREADS, 2)
-decode_tile_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
-                   const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
-                   const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                   const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+// A dictionary block's history (EXT): the last <= 65 535 bytes of dictBase[dictOff[b] .. + dictLen[b]), which end
+// at *end; every offset an LZ4 block can hold reaches no further back than that.
+__device__ __forceinline__ int dict_hist(const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen, int b,
+                                         const uint8_t** end) {
+    const int len = dictLen[b] > 0 ? dictLen[b] : 0;
+    *end = dictBase + dictOff[b] + len;
+    return len < 65535 ? len : 65535;
+}
+
+// The kernels' bodies: without EXT a block's history is the prefixLen[b] bytes in front of its destination (none
+// when prefixLen is null); with EXT it is its dictionary (dict_hist), and the results are LZ4Codec.Decode's with
+// that dictionary.  decode_tile_kernel & co. are the bodies without EXT; decode_tile_dict_kernel & co. with it.
+template <bool EXT>
+__device__ __forceinline__ void decode_tile_body(
+        const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
+        uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+        const int32_t* __restrict__ prefixLen, const uint8_t* __restrict__ dictBase,
+        const int64_t* __restrict__ dictOff, const int32_t* __restrict__ dictLen, int32_t* __restrict__ outLen,
+        DecodeLists wl) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TileSmem<STAGE_SMALL>& S = *reinterpret_cast<TileSmem<STAGE_SMALL>*>(smem_raw);
     const int b = blockIdx.x;
     const int n = srcLen[b], cap = dstCap[b];
-    const int P = chain_prefix(prefixLen, b);
+    const uint8_t* hist = nullptr;
+    const int P = EXT ? dict_hist(dictBase, dictOff, dictLen, b, &hist) : chain_prefix(prefixLen, b);
     if (n <= 0 || cap <= 0 || P < 0) {
         if (threadIdx.x == 0) {
-            if (!prefixLen) decode_trivial(n, cap, &outLen[b]);
+            if (EXT || !prefixLen) decode_trivial(n, cap, &outLen[b]);
             else outLen[b] = P < 0 ? -1 : chain_trivial(n, cap, srcBase + srcOff[b]);
         }
         return;
@@ -735,19 +755,20 @@ decode_tile_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
     if (threadIdx.x == 0) mbar_init(&S.bar, 1);
     __syncthreads();
     uint32_t parity = 0;
-    const int r = tile_decode_block<STAGE_SMALL>(S, src, n, dstBase + dstOff[b], cap, P, parity);
+    const int r = tile_decode_block<STAGE_SMALL, EXT>(S, src, n, dstBase + dstOff[b], cap, P, parity, hist);
     if (threadIdx.x == 0) {
         if (r > 0) { outLen[b] = r; atomicAdd(&g_decode_stats[0], 1ull); }
         else wl_push(wl.gen, &wl.counts[1], (uint32_t)b);
     }
 }
 
-// launch 2: persistent, one CTA per SM, big stage: blocks whose compressed size needs it
-__global__ void __launch_bounds__(DT_THREADS, 1)
-decode_tile_big_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
-                       const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
-                       const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                       const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+template <bool EXT>
+__device__ __forceinline__ void decode_tile_big_body(
+        const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
+        uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+        const int32_t* __restrict__ prefixLen, const uint8_t* __restrict__ dictBase,
+        const int64_t* __restrict__ dictOff, const int32_t* __restrict__ dictLen, int32_t* __restrict__ outLen,
+        DecodeLists wl) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TileSmem<STAGE_BIG>& S = *reinterpret_cast<TileSmem<STAGE_BIG>*>(smem_raw);
     const uint32_t count = wl.counts[0];
@@ -758,8 +779,15 @@ decode_tile_big_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __res
     for (uint32_t e = blockIdx.x; e < count; e += gridDim.x) {
         const int b = (int)wl.big[e];
         const uint8_t* src = srcBase + srcOff[b];
-        const int r = tile_decode_block<STAGE_BIG>(S, src, srcLen[b], dstBase + dstOff[b], dstCap[b],
-                                                   chain_prefix(prefixLen, b), parity);
+        int r;
+        if constexpr (EXT) {
+            const uint8_t* hist;
+            const int P = dict_hist(dictBase, dictOff, dictLen, b, &hist);
+            r = tile_decode_block<STAGE_BIG, true>(S, src, srcLen[b], dstBase + dstOff[b], dstCap[b], P, parity, hist);
+        } else {
+            r = tile_decode_block<STAGE_BIG>(S, src, srcLen[b], dstBase + dstOff[b], dstCap[b],
+                                             chain_prefix(prefixLen, b), parity);
+        }
         if (threadIdx.x == 0) {
             if (r > 0) { outLen[b] = r; atomicAdd(&g_decode_stats[1], 1ull); }
             else wl_push(wl.gen, &wl.counts[1], (uint32_t)b);
@@ -768,18 +796,28 @@ decode_tile_big_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __res
     }
 }
 
-// launch 3: persistent, warp per block: the exact decoder for everything the tile path declined
-__global__ void __launch_bounds__(128)
-decode_rest_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
-                   const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
-                   const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                   const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+template <bool EXT>
+__device__ __forceinline__ void decode_rest_body(
+        const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
+        uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+        const int32_t* __restrict__ prefixLen, const uint8_t* __restrict__ dictBase,
+        const int64_t* __restrict__ dictOff, const int32_t* __restrict__ dictLen, int32_t* __restrict__ outLen,
+        DecodeLists wl) {
     const uint32_t count = wl.counts[1];
     const uint32_t nwarps = gridDim.x * (blockDim.x >> 5);
     for (uint32_t e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < count; e += nwarps) {
         const int b = (int)wl.gen[e];
         int r;
-        if (!prefixLen) r = codec_decode_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b]);
+        if constexpr (EXT) {                     // the general engine's dictionary form (decode_general_kernel)
+            const int n = srcLen[b];
+            if (n <= 0) r = 0;
+            else {
+                const int dl = dictLen[b];
+                r = decode_block_warp_general(srcBase + srcOff[b], n, dstBase + dstOff[b], dstCap[b] < 0 ? 0 : dstCap[b],
+                                              false, dl > 0 ? dictBase + dictOff[b] : nullptr, dl > 0 ? dl : 0);
+                r = r <= 0 ? -1 : r;
+            }
+        } else if (!prefixLen) r = codec_decode_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b]);
         else {                                   // LZ4_decompress_safe_continue in prefix mode, raw engine result
             r = decode_block_warp_general(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b], false,
                                           nullptr, 0, chain_prefix(prefixLen, b));
@@ -789,20 +827,67 @@ decode_rest_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restric
     }
 }
 
+#define K4_DT_ARGS const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff, \
+    const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff, \
+    const int32_t* __restrict__ dstCap
+#define K4_DT_DICT const uint8_t* __restrict__ dictBase, const int64_t* __restrict__ dictOff, \
+    const int32_t* __restrict__ dictLen
+
+// launch 1: one CTA per block, small stage, two CTAs per SM
+__global__ void __launch_bounds__(DT_THREADS, 2)
+decode_tile_kernel(K4_DT_ARGS, const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_tile_body<false>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, nullptr, nullptr, nullptr,
+                            outLen, wl);
+}
+__global__ void __launch_bounds__(DT_THREADS, 2)
+decode_tile_dict_kernel(K4_DT_ARGS, K4_DT_DICT, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_tile_body<true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, nullptr, dictBase, dictOff, dictLen,
+                           outLen, wl);
+}
+
+// launch 2: persistent, one CTA per SM, big stage: blocks whose compressed size needs it
+__global__ void __launch_bounds__(DT_THREADS, 1)
+decode_tile_big_kernel(K4_DT_ARGS, const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_tile_big_body<false>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, nullptr, nullptr, nullptr,
+                                outLen, wl);
+}
+__global__ void __launch_bounds__(DT_THREADS, 1)
+decode_tile_big_dict_kernel(K4_DT_ARGS, K4_DT_DICT, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_tile_big_body<true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, nullptr, dictBase, dictOff, dictLen,
+                               outLen, wl);
+}
+
+// launch 3: persistent, warp per block: the exact decoder for everything the tile path declined
+__global__ void __launch_bounds__(128)
+decode_rest_kernel(K4_DT_ARGS, const int32_t* __restrict__ prefixLen, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_rest_body<false>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, nullptr, nullptr, nullptr,
+                            outLen, wl);
+}
+__global__ void __launch_bounds__(128)
+decode_rest_dict_kernel(K4_DT_ARGS, K4_DT_DICT, int32_t* __restrict__ outLen, DecodeLists wl) {
+    decode_rest_body<true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, nullptr, dictBase, dictOff, dictLen,
+                           outLen, wl);
+}
+#undef K4_DT_ARGS
+#undef K4_DT_DICT
+
 // ------------------------------------------------------------------------------------------------
 // launcher (host)
 // ------------------------------------------------------------------------------------------------
 // Enqueues the decode of n blocks on `st` (current device).  prefixLen (device array, may be null:
 // independent blocks) gives each block's history length, the bytes in front of its destination; with it the
-// results are those of LZ4_decompress_safe_continue in prefix mode (bytes decoded or -1).  On success
-// DECODE_LAUNCHES kernels were launched.  The work lists come from `pool`, a private stream-ordered
-// pool of the current device (the process-wide default pool is never touched); `sms` is its SM count.  The
-// tile kernels must have been granted their dynamic shared memory (sizeof(TileSmem<...>)).
+// results are those of LZ4_decompress_safe_continue in prefix mode (bytes decoded or -1).  With dictBase (then
+// prefixLen is null) block b's history is the dictionary dictBase[dictOff[b] .. + dictLen[b]) in a buffer of its own,
+// and the results are LZ4Codec.Decode's with it (LZ4_decompress_safe_usingDict).  On success DECODE_LAUNCHES kernels
+// were launched.  The work lists come from `pool`, a private stream-ordered pool of the current device (the
+// process-wide default pool is never touched); `sms` is its SM count.  The tile kernels must have been granted their
+// dynamic shared memory (sizeof(TileSmem<...>)).
 constexpr int DECODE_LAUNCHES = 3;
 inline cudaError_t decode_launch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                  uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
                                  const int32_t* prefixLen, int32_t* outLen, int n, cudaStream_t st,
-                                 cudaMemPool_t pool, int sms) {
+                                 cudaMemPool_t pool, int sms, const uint8_t* dictBase = nullptr,
+                                 const int64_t* dictOff = nullptr, const int32_t* dictLen = nullptr) {
     uint32_t* scratch = nullptr;
     cudaError_t e = cudaMallocFromPoolAsync((void**)&scratch, ((size_t)2 * n + 4) * sizeof(uint32_t), pool, st);
     if (e != cudaSuccess) return e;
@@ -812,15 +897,24 @@ inline cudaError_t decode_launch(const uint8_t* srcBase, const int64_t* srcOff, 
     wl.gen = scratch + 4 + n;
     e = cudaMemsetAsync(wl.counts, 0, 4 * sizeof(uint32_t), st);
     if (e == cudaSuccess) {
-        decode_tile_kernel<<<n, DT_THREADS, sizeof(TileSmem<STAGE_SMALL>), st>>>(
-            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
         const int gridBig = n < sms ? n : sms;
-        decode_tile_big_kernel<<<gridBig, DT_THREADS, sizeof(TileSmem<STAGE_BIG>), st>>>(
-            srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
         const int want = (n + 3) / 4;
         const int gridRest = want < sms * 8 ? want : sms * 8;
-        decode_rest_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen,
-                                                      outLen, wl);
+        if (dictBase) {
+            decode_tile_dict_kernel<<<n, DT_THREADS, sizeof(TileSmem<STAGE_SMALL>), st>>>(
+                srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, dictBase, dictOff, dictLen, outLen, wl);
+            decode_tile_big_dict_kernel<<<gridBig, DT_THREADS, sizeof(TileSmem<STAGE_BIG>), st>>>(
+                srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, dictBase, dictOff, dictLen, outLen, wl);
+            decode_rest_dict_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap,
+                                                               dictBase, dictOff, dictLen, outLen, wl);
+        } else {
+            decode_tile_kernel<<<n, DT_THREADS, sizeof(TileSmem<STAGE_SMALL>), st>>>(
+                srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
+            decode_tile_big_kernel<<<gridBig, DT_THREADS, sizeof(TileSmem<STAGE_BIG>), st>>>(
+                srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen, outLen, wl);
+            decode_rest_kernel<<<gridRest, 128, 0, st>>>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, prefixLen,
+                                                          outLen, wl);
+        }
         e = cudaGetLastError();
     }
     cudaFreeAsync(scratch, st);

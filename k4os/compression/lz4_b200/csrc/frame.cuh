@@ -15,11 +15,13 @@
 #include "common.cuh"
 #include "xxh32.cuh"
 #include "size_walk.cuh"
+#include "encode_dict.cuh"
 
 namespace k4 {
 
 constexpr uint32_t FRAME_MAGIC = 0x184D2204u;
 constexpr int FR_INDEPENDENT = 1, FR_BLOCK_SUM = 2, FR_CONTENT_SUM = 4;   // K4LZ4_FRAME_* (and the parsed FLG bits)
+constexpr int FR_DICT_ID = 8;                // parsed (dictionary calls): the header has a dictID field
 constexpr int FR_CORRUPT = -1000, FR_DELEGATE = -2, FR_DST_SMALL = -1001;   // K4LZ4_R_*
 constexpr unsigned long long FK_NONE = ~0ull;
 constexpr int FK_TRUNC = 0, FK_SUM = 1, FK_RAW = 2, FK_BLOCK = 3;
@@ -40,7 +42,7 @@ struct FrameRec {            // per frame, on the device
     int32_t maxBlock;        // BD maximum
     int32_t k0;              // decode: first block that may need a scratch slot
     uint32_t expect;         // decode: stored content checksum
-    int32_t reserved;
+    uint32_t dictId;         // decode (dictionary calls): the header's dictID
 };
 
 struct FrameTotals { int64_t blocks, slots; int32_t maxSteps, maxCap; };
@@ -85,16 +87,18 @@ __device__ __forceinline__ int64_t frame_lb(int64_t L, bool raw) {
 
 // The header checks on the first L bytes of a frame, in frame.py's _Frame order: magic, version with the
 // reference's 0x11 mask, dictionary flag, HC.  -> 0 or the verdict (R_CORRUPT / R_DELEGATE); *p = the offset of the
-// HC byte (6 or 14); *flg, *bd = the FLG and BD bytes (0 when L < 7).
+// HC byte (6 or 14, 4 more with a dictID); *flg, *bd = the FLG and BD bytes (0 when L < 7).  DICT (the dictionary
+// calls): the dictionary flag is no verdict, its 4 ID bytes lie in front of HC and are covered by it.
+template <bool DICT = false>
 __device__ __forceinline__ int frame_header_check(const uint8_t* f, int64_t L, int64_t* p, int* flg, int* bd) {
     int status = 0;
     if (L < 7 || fr_rd32(f) != FRAME_MAGIC) status = FR_CORRUPT;
     *flg = L >= 7 ? f[4] : 0;
     *bd = L >= 7 ? f[5] : 0;
     if (!status && ((*flg >> 6) & 0x11) != 1) status = FR_CORRUPT;
-    if (!status && (*flg & 1)) status = FR_DELEGATE;
+    if (!DICT && !status && (*flg & 1)) status = FR_DELEGATE;
     const bool hasSize = (*flg >> 3) & 1;
-    *p = 6 + (hasSize ? 8 : 0);
+    *p = 6 + (hasSize ? 8 : 0) + (DICT && (*flg & 1) ? 4 : 0);
     if (!status) {
         if (L < *p + 1) status = FR_CORRUPT;
         else {
@@ -112,9 +116,12 @@ __device__ __forceinline__ int frame_flags_of(int flg) {
 // One thread per frame.  Pass 0: header (frame.py's _Frame order: magic, version with the reference's 0x11 mask,
 // dictionary flag, HC), the block length codes, the first block that may need a scratch slot, and the frame's
 // counts.  Pass 1: the table rows.
-__global__ void frame_parse_kernel(int pass, const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
-                                   const int32_t* __restrict__ srcLen, int n, FrameRec* __restrict__ fr,
-                                   FrameTable t, FrameTotals* __restrict__ tot) {
+// DICT: frame_header_check<true>, and the dictID goes to r.dictId (FR_DICT_ID in r.flags).
+template <bool DICT>
+__device__ __forceinline__ void frame_parse_body(int pass, const uint8_t* __restrict__ srcBase,
+                                                 const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
+                                                 int n, FrameRec* __restrict__ fr, FrameTable t,
+                                                 FrameTotals* __restrict__ tot) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     FrameRec r = fr[i];
@@ -125,10 +132,12 @@ __global__ void frame_parse_kernel(int pass, const uint8_t* __restrict__ srcBase
     if (pass == 0) {
         r.status = 0; r.err = FK_NONE; r.nb = 0; r.nslot = 0; r.flags = 0; r.maxBlock = 1 << 16; r.k0 = 0; r.expect = 0;
         r.pos = 0;
+        if (DICT) r.dictId = 0;
         int flg, bd;
-        r.status = frame_header_check(f, L, &p, &flg, &bd);
+        r.status = frame_header_check<DICT>(f, L, &p, &flg, &bd);
         if (r.status) { r.nb = 0; fr[i] = r; return; }
         r.flags = frame_flags_of(flg);
+        if (DICT && (flg & 1)) { r.flags |= FR_DICT_ID; r.dictId = fr_rd32(f + p - 4); }
         r.maxBlock = frame_max_block((bd >> 4) & 7);
         p += 1;
         r.pos = p;               // where the first length code is, for pass 1
@@ -190,6 +199,16 @@ __global__ void frame_parse_kernel(int pass, const uint8_t* __restrict__ srcBase
         t.sum[b] = bc ? fr_rd32(f + p) : 0;
         p += bc ? 4 : 0;
     }
+}
+__global__ void frame_parse_kernel(int pass, const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
+                                   const int32_t* __restrict__ srcLen, int n, FrameRec* __restrict__ fr,
+                                   FrameTable t, FrameTotals* __restrict__ tot) {
+    frame_parse_body<false>(pass, srcBase, srcOff, srcLen, n, fr, t, tot);
+}
+__global__ void frame_parse_dict_kernel(int pass, const uint8_t* __restrict__ srcBase,
+                                        const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen, int n,
+                                        FrameRec* __restrict__ fr, FrameTable t, FrameTotals* __restrict__ tot) {
+    frame_parse_body<true>(pass, srcBase, srcOff, srcLen, n, fr, t, tot);
 }
 
 // Single CTA: exclusive scan of the frames' block and slot counts -> first row and first slot; totals.
@@ -290,6 +309,33 @@ __global__ void frame_layout_kernel(FrameRec* __restrict__ fr, int n, FrameTable
     fr[i].err = r.err;
 }
 
+// Dictionary decode, one thread per frame, after frame_layout_kernel: every row gets its frame's dictionary
+// (rowDictOff / rowDictLen: independent blocks decode against it), and a linked block k >= 1 whose 64 KiB window
+// reaches back past the content's start into a non-empty dictionary (fewer than 65 535 bytes decoded before it)
+// decodes in the frame's scratch slot, where frame_step_prepare_kernel<true> puts [dictionary tail | output so far]
+// in front of it.  A linked frame with blocks always has its one slot (frame_parse_kernel: k0 < nb).
+__global__ void frame_dict_layout_kernel(const FrameRec* __restrict__ fr, int n, FrameTable t,
+                                         const int64_t* __restrict__ dictOff, const int32_t* __restrict__ dictLen,
+                                         int64_t* __restrict__ rowDictOff, int32_t* __restrict__ rowDictLen,
+                                         int64_t scratchRel, int64_t slotBytes) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec& r = fr[i];
+    const int32_t dl = dictLen[i] > 0 ? dictLen[i] : 0;
+    const bool linked = !(r.flags & FR_INDEPENDENT);
+    int64_t pos = 0;
+    for (int k = 0; k < r.nb; k++) {
+        const int64_t b = r.first + k;
+        rowDictOff[b] = dictOff[i]; rowDictLen[b] = dl;
+        const int kind = t.kind[b];
+        if (linked && dl > 0 && k > 0 && pos < 65535 && !(kind & (RK_RAW | RK_SKIP | RK_SCRATCH))) {
+            t.kind[b] = kind | RK_SCRATCH;
+            t.dst[b] = scratchRel + r.slot * slotBytes + FR_HIST;
+        }
+        pos += t.size[b];
+    }
+}
+
 // Linked frames, step k: block k of every frame that has one (a compressed, not skipped block) decodes behind the
 // frame's output so far.  One entry per frame; the others get an empty source (no work).  A block in a scratch
 // slot gets the last <= 64 KiB of the output copied in front of it.
@@ -297,8 +343,16 @@ struct FrameStep {
     int64_t* srcOff; int32_t* srcLen; int64_t* dstOff; int32_t* cap; int32_t* prefix; int32_t* res;
     int64_t* hSrc; int64_t* hDst; int32_t* hLen;     // history copy, then copy-back
 };
-__global__ void frame_step_prepare_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t, FrameStep s,
-                                          const int64_t* __restrict__ dstOff) {
+struct FrameStepDict { int64_t* src; int64_t* dst; int32_t* len; };   // dictionary tail copy (source in dictBase)
+// DICT (dictionary decode): step 0 decodes against the dictionary itself (no copy: the caller launches the tile
+// decoder's dictionary form); a later block with fewer than 65 535 bytes decoded before it sits in the scratch slot
+// (frame_dict_layout_kernel) and gets the dictionary's last bytes in front of the output copied there, its prefix
+// then spanning both.
+template <bool DICT>
+__device__ __forceinline__ void frame_step_prepare_body(int k, const FrameRec* __restrict__ fr, int n, FrameTable t,
+                                                        FrameStep s, const int64_t* __restrict__ dstOff,
+                                                        const int64_t* __restrict__ dictOff,
+                                                        const int32_t* __restrict__ dictLen, FrameStepDict sd) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const FrameRec& r = fr[i];
@@ -317,8 +371,29 @@ __global__ void frame_step_prepare_kernel(int k, const FrameRec* __restrict__ fr
             }
         }
     }
+    if constexpr (DICT) {
+        int32_t dc = 0;
+        int64_t ds = 0, dd = 0;
+        const int32_t dl = dictLen[i] > 0 ? dictLen[i] : 0;
+        if (len > 0 && k > 0 && pre < 65535 && dl > 0) {     // pre = every byte decoded so far, all in the slot
+            dc = 65535 - pre < dl ? 65535 - pre : dl;
+            ds = dictOff[i] + dl - dc; dd = dof - pre - dc;
+            pre += dc;
+        }
+        sd.src[i] = ds; sd.dst[i] = dd; sd.len[i] = dc;
+    }
     s.srcOff[i] = so; s.srcLen[i] = len; s.dstOff[i] = dof; s.cap[i] = cap; s.prefix[i] = pre;
     s.hSrc[i] = hs; s.hDst[i] = hd; s.hLen[i] = hl;
+}
+__global__ void frame_step_prepare_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t, FrameStep s,
+                                          const int64_t* __restrict__ dstOff) {
+    frame_step_prepare_body<false>(k, fr, n, t, s, dstOff, nullptr, nullptr, FrameStepDict{});
+}
+__global__ void frame_step_prepare_dict_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t,
+                                               FrameStep s, const int64_t* __restrict__ dstOff,
+                                               const int64_t* __restrict__ dictOff,
+                                               const int32_t* __restrict__ dictLen, FrameStepDict sd) {
+    frame_step_prepare_body<true>(k, fr, n, t, s, dstOff, dictOff, dictLen, sd);
 }
 
 // After the step's decode: the result goes to the row, an accepted block in a scratch slot is copied back.
@@ -379,6 +454,14 @@ __global__ void frame_decode_finish_kernel(const FrameRec* __restrict__ fr, int 
         else out = r.pos > 0x7FFFFFFF ? FR_CORRUPT : (int32_t)r.pos;
     }
     outLen[i] = out;
+}
+
+// One thread per frame (k4lz4_frame_info_batch): the header's dictID, or -1 without a dictID field or a valid header.
+__global__ void frame_info_kernel(const FrameRec* __restrict__ fr, int n, int64_t* __restrict__ outId) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec& r = fr[i];
+    outId[i] = (!r.status && (r.flags & FR_DICT_ID)) ? (int64_t)r.dictId : -1;
 }
 
 // ---- encode ---------------------------------------------------------------------------------------------------
@@ -483,21 +566,104 @@ __global__ void frame_put_sum_kernel(uint8_t* __restrict__ dstBase, FrameEnc e, 
     fr_wr32(dstBase + e.ckOff[x] + e.ckLen[x], e.ckSum[x]);
 }
 
-// One thread per frame: header, end mark, content checksum, result.
-__global__ void frame_enc_finish_kernel(const FrameRec* __restrict__ fr, int n, uint8_t* __restrict__ dstBase,
-                                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                                        uint64_t header, int cc, const uint32_t* __restrict__ csum,
-                                        int32_t* __restrict__ outLen) {
+// One thread per frame: header, end mark, content checksum, result.  DICT: a frame whose dictId is not 0 gets the
+// dictionary flag and the 4-byte ID in front of HC, which covers it (dictId may be null: no IDs).
+template <bool DICT>
+__device__ __forceinline__ void frame_enc_finish_body(const FrameRec* __restrict__ fr, int n,
+                                                      uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff,
+                                                      const int32_t* __restrict__ dstCap, uint64_t header, int cc,
+                                                      const uint32_t* __restrict__ csum, int32_t* __restrict__ outLen,
+                                                      const uint32_t* __restrict__ dictId) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const FrameRec& r = fr[i];
     const int64_t total = r.pos + 4 + (cc ? 4 : 0);
     if (r.status || total > (dstCap[i] > 0 ? dstCap[i] : 0) || total > 0x7FFFFFFF) { outLen[i] = -1; return; }
     uint8_t* d = dstBase + dstOff[i];
-    for (int j = 0; j < 7; j++) d[j] = (uint8_t)(header >> (8 * j));
+    const uint32_t id = DICT && dictId ? dictId[i] : 0u;
+    if (DICT && id) {
+        uint8_t h[6] = {(uint8_t)((header >> 32) | 1), (uint8_t)(header >> 40), (uint8_t)id, (uint8_t)(id >> 8),
+                        (uint8_t)(id >> 16), (uint8_t)(id >> 24)};
+        fr_wr32(d, FRAME_MAGIC);
+        for (int j = 0; j < 6; j++) d[4 + j] = h[j];
+        d[10] = (uint8_t)(xx_finish(XXP5 + 6u, h, 6) >> 8);
+    } else {
+        for (int j = 0; j < 7; j++) d[j] = (uint8_t)(header >> (8 * j));
+    }
     fr_wr32(d + r.pos, 0);
     if (cc) fr_wr32(d + r.pos + 4, csum[i]);
     outLen[i] = (int32_t)total;
+}
+__global__ void frame_enc_finish_kernel(const FrameRec* __restrict__ fr, int n, uint8_t* __restrict__ dstBase,
+                                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+                                        uint64_t header, int cc, const uint32_t* __restrict__ csum,
+                                        int32_t* __restrict__ outLen) {
+    frame_enc_finish_body<false>(fr, n, dstBase, dstOff, dstCap, header, cc, csum, outLen, nullptr);
+}
+__global__ void frame_enc_finish_dict_kernel(const FrameRec* __restrict__ fr, int n, uint8_t* __restrict__ dstBase,
+                                             const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+                                             uint64_t header, int cc, const uint32_t* __restrict__ csum,
+                                             int32_t* __restrict__ outLen, const uint32_t* __restrict__ dictId) {
+    frame_enc_finish_body<true>(fr, n, dstBase, dstOff, dstCap, header, cc, csum, outLen, dictId);
+}
+
+// ---- dictionary encode (k4lz4_frame_encode_dict_batch): upstream's CDict frames ------------------------------
+// Every block is LZ4_compress_fast_continue with capacity n - 1 and is stored raw when that fails
+// (lz4frame.c:747-749); independent blocks each start from LZ4_loadDict of the frame's dictionary (OP_ENCDICT),
+// linked frames load it once, in front of block 0 (frame_dict_first_kernel).
+
+// One thread per frame, after the plan: the header grows by the dictID field where the ID is not 0, and every row
+// gets its frame's dictionary.
+__global__ void frame_enc_dict_plan_kernel(FrameRec* __restrict__ fr, int n, const int64_t* __restrict__ dictOff,
+                                           const int32_t* __restrict__ dictLen, const uint32_t* __restrict__ dictId,
+                                           int64_t* __restrict__ rowDictOff, int32_t* __restrict__ rowDictLen) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec r = fr[i];
+    if (dictId && dictId[i]) fr[i].pos = r.pos + 4;
+    for (int k = 0; k < r.nb; k++) { rowDictOff[r.first + k] = dictOff[i]; rowDictLen[r.first + k] = dictLen[i]; }
+}
+
+// Before an encode launch: capacity n - 1 for every entry.  After it: an entry that did not fit is stored raw
+// (frame_enc_place_kernel stores the source when the result is >= n).
+__global__ void frame_dict_cap_kernel(const int32_t* __restrict__ len, int32_t* __restrict__ cap, int m) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x < m) cap[x] = len[x] > 0 ? len[x] - 1 : 0;
+}
+__global__ void frame_dict_raw_kernel(const int32_t* __restrict__ len, int32_t* __restrict__ res, int m) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x < m && len[x] > 0 && res[x] <= 0) res[x] = len[x];
+}
+
+// Linked step 0, one warp per entry x (frame f0 + x): LZ4_loadDict of the frame's dictionary into its state record,
+// then block 0 in the usingExtDict mode against it (encode_dict_warp, capacity n0 - 1), then what
+// LZ4_compress_fast_continue leaves for the blocks behind it: currentOffset = 65 536 + n0 (lz4.c:918) and
+// dictSize = n0 (lz4.c:1633-1634), also when the block did not fit (its table stops where upstream's does).  The
+// result is as frame_dict_raw_kernel leaves it; steps 1.. are the chained encoder's (OP_ENCCHAIN).
+__global__ void __launch_bounds__(32)
+frame_dict_first_kernel(int f0, const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ so,
+                        const int32_t* __restrict__ sl, uint8_t* __restrict__ dstBase, int64_t bound,
+                        const uint8_t* __restrict__ dictBase, const int64_t* __restrict__ dictOff,
+                        const int32_t* __restrict__ dictLen, ChainState* __restrict__ state,
+                        int32_t* __restrict__ res) {
+    const int x = blockIdx.x, i = f0 + x, lane = lane_id();
+    ChainState* const st = state + x;
+    const int len = dictLen[i] > 0 ? dictLen[i] : 0;
+    const uint8_t* const dict = dictBase + dictOff[i];
+    load_dict_warp(dict, len, st);
+    const int n0 = sl[x];
+    int r = 0;
+    if (n0 > 0) {
+        r = encode_dict_warp(srcBase + so[x], (uint32_t)n0, dict + len, (uint32_t)dict_kept(len),
+                             dstBase + x * bound, n0 - 1, st->table);
+        if (lane == 0) {
+            __stcg(&st->currentOffset, (uint32_t)DICT_WINDOW + (uint32_t)n0);
+            __stcg(&st->dictSize, (uint32_t)n0);
+            atomicAdd(&g_encode_stats[3], 1ull);
+        }
+        r = r <= 0 ? n0 : r;
+    }
+    if (lane == 0) res[x] = r;
 }
 
 // off[x] = x * stride and, when cap is given, cap[x] = capValue: the fixed slots of a launch.

@@ -129,14 +129,14 @@ int check_device(int device, int64_t n) {
 }
 
 // Every batched export: the arguments first, then the machine, so that a caller's mistake gets the same
-// code with or without a GPU.
-int check(Op op, const Batch& b, int memKind, int device) {
+// code with or without a GPU.  `missing`: a pointer the export itself requires when n > 0 is null.
+int check(Op op, const Batch& b, int memKind, int device, bool missing = false) {
     const Needs& w = NEEDS[op];
     if (memKind != K4LZ4_MEM_HOST && memKind != K4LZ4_MEM_DEVICE) return fail(K4LZ4_E_ARG, "unknown memKind %d", memKind);
     if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
     if (b.n > 0 && (!b.srcBase || !b.srcOff || !b.srcLen || (w.out && !b.outLen) || (w.dst && (!b.dstBase || !b.dstOff)) ||
                     (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen)) ||
-                    (w.state && (!b.stateBase || !b.stateOff)) || (w.dict && !b.dictBase)))
+                    (w.state && (!b.stateBase || !b.stateOff)) || (w.dict && !b.dictBase) || missing))
         return fail(K4LZ4_E_ARG, "null pointer argument");
     if (w.prefix && memKind == K4LZ4_MEM_HOST)       // device arrays cannot be checked here: there a negative prefix gives -1
         for (int64_t i = 0; i < b.n; i++)
@@ -262,6 +262,12 @@ Dev* dev_state(int dev) {
         if (e == cudaSuccess)
             e = cudaFuncSetAttribute(k4::decode_tile_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)sizeof(k4::TileSmem<k4::STAGE_BIG>));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(k4::decode_tile_dict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(k4::TileSmem<k4::STAGE_SMALL>));
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(k4::decode_tile_big_dict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(k4::TileSmem<k4::STAGE_BIG>));
         if (e == cudaSuccess) {
             cudaMemPoolProps props = {};
             props.allocType = cudaMemAllocationTypePinned;
@@ -351,8 +357,11 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
     }
     case OP_DECODE:
     case OP_CHAIN: {
+        // OP_DECODE with dictBase: each block against its dictionary in a buffer of its own (the tile decoder's form)
+        const bool dict = op == OP_DECODE && a.dictBase;
         const cudaError_t de = k4::decode_launch(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff, a.dstCap,
-                                                 op == OP_CHAIN ? a.prefixLen : nullptr, a.outLen, n, st, D->pool, D->sms);
+                                                 op == OP_CHAIN ? a.prefixLen : nullptr, a.outLen, n, st, D->pool,
+                                                 D->sms, dict ? a.dictBase : nullptr, a.dictOff, a.dictLen);
         if (de != cudaSuccess) { (void)cudaGetLastError(); return de; }
         g_launches += k4::DECODE_LAUNCHES;
         break;
@@ -1214,6 +1223,12 @@ uint64_t frame_header(int32_t blockSize, int flags) {
     return (uint64_t)k4::FRAME_MAGIC | ((uint64_t)fb[0] << 32) | ((uint64_t)fb[1] << 40) | ((uint64_t)hc << 48);
 }
 
+// The dictionary calls (k4lz4_frame_*_dict_batch, k4lz4_frame_info_batch): frame i's dictionary is the Batch's
+// dictBase[dictOff[i] .. + dictLen[i]) (decode: dictBase may be null, no dictionaries); `id` the IDs an encode writes
+// (may be null: none), `outId` where the info call puts the headers' IDs.  A null FrameDict is the frame calls as
+// they were without dictionaries.
+struct FrameDict { const uint32_t* id = nullptr; int64_t* outId = nullptr; };
+
 // Stream-ordered allocations of one frame call, from the device's private pool; freed (in stream order) at the end.
 struct FramePool {
     cudaMemPool_t pool; cudaStream_t st;
@@ -1238,7 +1253,9 @@ inline unsigned grid_of(int64_t n, int t = 128) { return (unsigned)std::max<int6
 // Decode (or, with sizeOnly, only the content sizes of) b.n frames in device memory on `st`: parse, scan, one
 // host synchronisation for the block and step counts, then everything else enqueued.  b.dstCap may be null
 // (sizeOnly).
-cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
+// With fd: the dictionary flag is accepted, every frame decodes against its dictionary (none without b.dictBase),
+// and fd->outId, where given, gets the headers' IDs.
+cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, const FrameDict* fd = nullptr) {
     int dev = 0;
     cudaGetDevice(&dev);
     const Dev* D = dev_state(dev);
@@ -1249,7 +1266,8 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
     k4::FrameTotals* tot = P.get<k4::FrameTotals>(1);
     FR_TRY(P.err);
     FR_TRY(cudaMemsetAsync(tot, 0, sizeof(k4::FrameTotals), st));
-    k4::frame_parse_kernel<<<grid_of(n), 128, 0, st>>>(0, b.srcBase, b.srcOff, b.srcLen, n, fr, k4::FrameTable{}, tot);
+    auto parse = fd ? k4::frame_parse_dict_kernel : k4::frame_parse_kernel;
+    parse<<<grid_of(n), 128, 0, st>>>(0, b.srcBase, b.srcOff, b.srcLen, n, fr, k4::FrameTable{}, tot);
     FR_LAUNCH();
     k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, sizeOnly ? 0 : 1);
     FR_LAUNCH();
@@ -1271,7 +1289,7 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
         t.cap = (int32_t*)take(nB * 4); t.ilen = (int32_t*)take(nB * 4); t.res = (int32_t*)take(nB * 4);
         t.ckLen = (int32_t*)take(nB * 4); t.got = (uint32_t*)take(nB * 4); t.cpyLen = (int32_t*)take(nB * 4);
     }
-    k4::frame_parse_kernel<<<grid_of(n), 128, 0, st>>>(1, b.srcBase, b.srcOff, b.srcLen, n, fr, t, nullptr);
+    parse<<<grid_of(n), 128, 0, st>>>(1, b.srcBase, b.srcOff, b.srcLen, n, fr, t, nullptr);
     FR_LAUNCH();
     g_launches++;
     if (nB > 0) {
@@ -1289,26 +1307,57 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
                                                        sizeOnly ? nullptr : b.dstCap, scratchRel, slotBytes, ccLen);
     FR_LAUNCH();
     g_launches++;
+    // the dictionaries: per frame (no dictionaries: empty ones) and per row
+    const uint8_t* dBase = b.dictBase;
+    const int64_t* dOff = b.dictOff;
+    const int32_t* dLen = b.dictLen;
+    int64_t* rowDictOff = nullptr;
+    int32_t* rowDictLen = nullptr;
+    if (fd && !sizeOnly) {
+        if (!dBase) {
+            int64_t* z = P.get<int64_t>(n);
+            FR_TRY(P.err);
+            FR_TRY(cudaMemsetAsync(z, 0, (size_t)n * 8, st));
+            dBase = b.srcBase; dOff = z; dLen = reinterpret_cast<const int32_t*>(z);
+        }
+        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
+        FR_TRY(P.err);
+        k4::frame_dict_layout_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, t, dOff, dLen, rowDictOff, rowDictLen,
+                                                                scratchRel, slotBytes);
+        FR_LAUNCH();
+        g_launches++;
+    }
     if (!sizeOnly && nB > 0) {
         const int nb = (int)nB;
         // stored blocks first: they are history for the linked blocks after them
         FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
         FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
-        FR_TRY(launch_op(OP_DECODE, Batch{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb}, st));
+        Batch ib{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb};
+        if (fd) { ib.dictBase = dBase; ib.dictOff = rowDictOff; ib.dictLen = rowDictLen; }
+        FR_TRY(launch_op(OP_DECODE, ib, st));
         if (h.maxSteps > 0) {
             k4::FrameStep s;
             s.srcOff = P.get<int64_t>(n); s.dstOff = P.get<int64_t>(n); s.hSrc = P.get<int64_t>(n); s.hDst = P.get<int64_t>(n);
             s.srcLen = P.get<int32_t>(n); s.cap = P.get<int32_t>(n); s.prefix = P.get<int32_t>(n); s.res = P.get<int32_t>(n);
             s.hLen = P.get<int32_t>(n);
+            k4::FrameStepDict sd{};
+            if (fd) { sd.src = P.get<int64_t>(n); sd.dst = P.get<int64_t>(n); sd.len = P.get<int32_t>(n); }
             FR_TRY(P.err);
             for (int k = 0; k < h.maxSteps; k++) {
-                k4::frame_step_prepare_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff);
+                if (fd) k4::frame_step_prepare_dict_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff, dOff, dLen, sd);
+                else k4::frame_step_prepare_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff);
                 FR_LAUNCH();
                 g_launches++;
                 FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, n}, st));
                 Batch cb{b.srcBase, s.srcOff, s.srcLen, b.dstBase, s.dstOff, s.cap, s.res, n};
-                cb.prefixLen = s.prefix;
-                FR_TRY(launch_op(OP_CHAIN, cb, st));
+                if (fd && k == 0) {          // block 0 against the dictionary itself
+                    cb.dictBase = dBase; cb.dictOff = dOff; cb.dictLen = dLen;
+                    FR_TRY(launch_op(OP_DECODE, cb, st));
+                } else {
+                    if (fd) FR_TRY(launch_op(OP_COPY, Batch{dBase, sd.src, sd.len, b.dstBase, sd.dst, nullptr, nullptr, n}, st));
+                    cb.prefixLen = s.prefix;
+                    FR_TRY(launch_op(OP_CHAIN, cb, st));
+                }
                 k4::frame_step_commit_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s);
                 FR_LAUNCH();
                 g_launches++;
@@ -1326,13 +1375,20 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st) {
                                                               sizeOnly ? nullptr : ccGot, ccLen, b.outLen);
     FR_LAUNCH();
     g_launches++;
+    if (fd && fd->outId) {
+        k4::frame_info_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, fd->outId);
+        FR_LAUNCH();
+        g_launches++;
+    }
     return cudaSuccess;
 }
 
 // Encode b.n frames in device memory on `st` (level < 3): plan, scan, one host synchronisation for the block and
 // step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of at most
-// FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.
-cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st) {
+// FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.  With fd: against
+// the Batch's dictionaries, upstream's CDict frames (frame.cuh, "dictionary encode").
+cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
+                             const FrameDict* fd = nullptr) {
     int dev = 0;
     cudaGetDevice(&dev);
     const Dev* D = dev_state(dev);
@@ -1361,6 +1417,29 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
     k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(1, b.srcOff, b.srcLen, n, bs, fr, t, tot);
     FR_LAUNCH();
     g_launches++;
+    int64_t* rowDictOff = nullptr;
+    int32_t* rowDictLen = nullptr;
+    if (fd) {
+        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
+        FR_TRY(P.err);
+        k4::frame_enc_dict_plan_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dictOff, b.dictLen, fd->id, rowDictOff,
+                                                                  rowDictLen);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    // capacity n - 1 in front of a dictionary encode, raw where it did not fit behind it
+    auto dict_cap = [&](const int32_t* len, int32_t* cap, int64_t m) -> cudaError_t {
+        k4::frame_dict_cap_kernel<<<grid_of(m), 128, 0, st>>>(len, cap, (int)m);
+        FR_LAUNCH();
+        g_launches++;
+        return cudaSuccess;
+    };
+    auto dict_raw = [&](const int32_t* len, int32_t* res, int64_t m) -> cudaError_t {
+        k4::frame_dict_raw_kernel<<<grid_of(m), 128, 0, st>>>(len, res, (int)m);
+        FR_LAUNCH();
+        g_launches++;
+        return cudaSuccess;
+    };
     if (cc) FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, b.srcOff, b.srcLen, nullptr, nullptr, nullptr, (int32_t*)csum, n}, st));
     const int32_t bound = k4::max_output_size(bs);
     const bool linked = !(flags & K4LZ4_FRAME_INDEPENDENT);
@@ -1399,7 +1478,14 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
             for (int64_t b0 = 0; b0 < nB; b0 += E) {
                 const int64_t m = std::min<int64_t>(E, nB - b0);
                 Batch kb{b.srcBase, t.srcOff + b0, t.len + b0, scratch, eDst, eCap, e.res, m, b.level, b.x32};
-                FR_TRY(launch_op(OP_ENCODE, kb, st));
+                if (fd) {
+                    FR_TRY(dict_cap(t.len + b0, eCap, m));
+                    kb.dictBase = b.dictBase; kb.dictOff = rowDictOff + b0; kb.dictLen = rowDictLen + b0;
+                    FR_TRY(launch_op(OP_ENCDICT, kb, st));
+                    FR_TRY(dict_raw(t.len + b0, e.res, m));
+                } else {
+                    FR_TRY(launch_op(OP_ENCODE, kb, st));
+                }
                 FR_TRY(place(-1, b0, b0 + m, 0, n, m));
             }
         } else {
@@ -1414,21 +1500,36 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
             g_launches++;
             for (int f0 = 0; f0 < n; f0 += (int)E) {
                 const int m = (int)std::min<int64_t>(E, n - f0);
-                FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
+                // with dictionaries, step 0 loads each frame's state record from its dictionary
+                if (!fd) FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
                 for (int k = 0; k < h.maxSteps; k++) {
                     k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fr, t, so, sl, pre, bs);
                     FR_LAUNCH();
                     g_launches++;
-                    Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level, b.x32};
-                    kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
-                    FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
+                    if (fd && k == 0) {
+                        k4::frame_dict_first_kernel<<<m, 32, 0, st>>>(f0, b.srcBase, so, sl, scratch, bound, b.dictBase,
+                                                                      b.dictOff, b.dictLen,
+                                                                      reinterpret_cast<k4::ChainState*>(state), e.res);
+                        FR_LAUNCH();
+                        g_launches++;
+                    } else {
+                        Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level, b.x32};
+                        kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
+                        if (fd) FR_TRY(dict_cap(sl, eCap, m));
+                        FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
+                        if (fd) FR_TRY(dict_raw(sl, e.res, m));
+                    }
                     FR_TRY(place(k, 0, 0, f0, f0 + m, m));
                 }
             }
         }
     }
-    k4::frame_enc_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header, cc ? 1 : 0,
-                                                           csum, b.outLen);
+    if (fd)
+        k4::frame_enc_finish_dict_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header,
+                                                                    cc ? 1 : 0, csum, b.outLen, fd->id);
+    else
+        k4::frame_enc_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header,
+                                                               cc ? 1 : 0, csum, b.outLen);
     FR_LAUNCH();
     g_launches++;
     return cudaSuccess;
@@ -1436,20 +1537,23 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
 
 enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE };
 
-cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st) {
+cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
+                      const FrameDict* fd) {
     if (fo == FO_ENCODE && b.level >= 3) {
         k4::frame_fill_kernel<<<grid_of(b.n), 128, 0, st>>>(b.outLen, (int)b.n, K4LZ4_R_DELEGATE);
         g_launches++;
         return cudaGetLastError();
     }
-    return fo == FO_ENCODE ? frame_encode_dev(b, bs, flags, header, st) : frame_decode_dev(b, fo == FO_SIZE, st);
+    return fo == FO_ENCODE ? frame_encode_dev(b, bs, flags, header, st, fd) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
 }
 
 // Host memory, one GPU, synchronous: chunks of whole frames (a frame is never split: its linked blocks and its
 // content checksum need all of it) through the device's staging, the device path on each, on the legacy default
 // stream.  The device region of a frame is min(dstCap, frame bound) when encoding (a frame never needs more) and
-// dstCap when decoding; content sizes have none.
-int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev) {
+// dstCap when decoding; content sizes have none.  With fd: each distinct dictionary of a chunk is staged once, only
+// its last 64 KiB (all that encode and decode read), and the IDs travel in the rows' aux column; the info call's
+// IDs come back behind the sizes.
+int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev, const FrameDict* fd) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
     if (fo == FO_ENCODE && b.level >= 3) {
@@ -1464,49 +1568,89 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
     auto room = [&](int64_t i) -> int64_t {
         if (!dst) return 0;
         const int64_t c = std::max<int32_t>(b.dstCap[i], 0);
-        return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags)) : c;
+        const int64_t idRoom = fd && fd->id && fd->id[i] ? 4 : 0;
+        return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags) + idRoom) : c;
     };
+    const bool dict = fd && b.dictBase;
+    auto dlen = [&](int64_t i) -> int32_t { return dict ? std::min<int32_t>(std::max<int32_t>(b.dictLen[i], 0), 65536) : 0; };
+    auto dkey = [&](int64_t i) { return std::make_pair(b.dictBase + b.dictOff[i] + (b.dictLen[i] - dlen(i)), dlen(i)); };
+    std::map<std::pair<const uint8_t*, int32_t>, int64_t> first;   // a chunk's first row of each distinct dictionary
+    std::vector<int64_t> from;
+    const bool ids = fd && fd->outId;
+    std::vector<int32_t> res;
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
+        first.clear(); from.clear();
         for (j = i; j < b.n; j++) {
-            const int64_t add = a16(src_size(b, j)) + 2 * a16(room(j)) + 64;
+            int64_t shared = -1;
+            if (dlen(j) > 0) {
+                auto it = first.find(dkey(j));
+                if (it != first.end()) shared = it->second;
+            }
+            const int64_t add = a16(src_size(b, j)) + 2 * a16(room(j)) + 64 + (shared >= 0 ? 0 : a16(dlen(j)));
             if (j > i && bytes + add > STAGE_BYTES) break;
             bytes += add;
+            if (dict) {
+                if (shared < 0 && dlen(j) > 0) first.emplace(dkey(j), j - i);
+                from.push_back(shared);
+            }
         }
         const int64_t nb = j - i;
         StageUp up;
-        int rc = stage_up(D->stage, nb, 1, 0, [&](int64_t k) {
+        const int64_t resInts = ids ? 4 : 1;          // the info call: the int64 IDs at res + 2 nb
+        int rc = stage_up(D->stage, nb, resInts, 0, [&](int64_t k) {
             const int64_t x = i + k, s = src_size(b, x), r = room(x);
-            return UpRow{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, 0, dst ? b.dstBase + b.dstOff[x] : nullptr};
+            UpRow u{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, fd && fd->id ? (int32_t)fd->id[x] : 0,
+                    dst ? b.dstBase + b.dstOff[x] : nullptr};
+            if (dict) { u.blob = dkey(x).first; u.blobLen = dlen(x); u.blobFrom = from[(size_t)k]; }
+            return u;
         }, up, nullptr);
         if (rc != K4LZ4_OK) return rc;
         Batch kb = b;
         kb.srcBase = up.src; kb.srcOff = up.srcOff; kb.srcLen = up.len;
         kb.dstBase = up.dst; kb.dstOff = up.dstOff; kb.dstCap = dst ? up.cap : nullptr;
         kb.outLen = up.res; kb.n = nb;
-        const cudaError_t e = frame_dev(fo, kb, bs, flags, header, nullptr);
+        if (dict) { kb.dictBase = up.blob; kb.dictOff = up.blobOff; kb.dictLen = up.blobLen; }
+        FrameDict kd;
+        if (fd) {
+            kd.id = fd->id ? reinterpret_cast<const uint32_t*>(up.aux) : nullptr;
+            kd.outId = ids ? reinterpret_cast<int64_t*>(up.res + 2 * nb) : nullptr;
+        }
+        const cudaError_t e = frame_dev(fo, kb, bs, flags, header, nullptr, fd ? &kd : nullptr);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
-        rc = stage_down(D->stage, up, nb, b.outLen + i, 1, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
+        res.resize((size_t)(nb * resInts));
+        rc = stage_down(D->stage, up, nb, ids ? res.data() : b.outLen + i, resInts, dst ? up.dst : nullptr, up.dstOff,
+                        nullptr, nullptr);
         if (rc != K4LZ4_OK) return rc;
+        if (ids) {
+            memcpy(b.outLen + i, res.data(), (size_t)nb * 4);
+            memcpy(fd->outId + i, res.data() + 2 * nb, (size_t)nb * 8);
+        }
     }
     return K4LZ4_OK;
 }
 
-// Every frame export: its own arguments, then the batch's (check()), then host or device.
-int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memKind, void* stream, int device) {
+// Every frame export: its own arguments, then the batch's (check()), then host or device.  fd: the dictionary calls
+// (their encode takes upstream's four block sizes only, and requires the dictionaries; the info call its ID array).
+int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memKind, void* stream, int device,
+              const FrameDict* fd = nullptr) {
     int32_t bs = 0;
     if (fo == FO_ENCODE) {
         bs = frame_block_size(blockSize);
-        if (!bs) return fail(K4LZ4_E_ARG, "bad frame block size %d (1 .. 4 MiB)", blockSize);
+        if (fd && blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22))
+            bs = 0;
+        if (!bs) return fail(K4LZ4_E_ARG, "bad frame block size %d (%s)", blockSize,
+                             fd ? "64 KiB, 256 KiB, 1 MiB or 4 MiB" : "1 .. 4 MiB");
         if (flags & ~FRAME_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
     }
-    const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device);
+    const bool missing = fd && (fo == FO_ENCODE ? !b.dictBase : fo == FO_SIZE ? !fd->outId : false);
+    const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     const uint64_t header = fo == FO_ENCODE ? frame_header(blockSize, flags) : 0;
-    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, bs, flags, header, device < 0 ? 0 : device);
+    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, bs, flags, header, device < 0 ? 0 : device, fd);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    const cudaError_t e = frame_dev(fo, b, bs, flags, header, (cudaStream_t)stream);
+    const cudaError_t e = frame_dev(fo, b, bs, flags, header, (cudaStream_t)stream, fd);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
 }
@@ -2643,6 +2787,37 @@ int32_t k4lz4_frame_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, 
                                  int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
     return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_frame_encode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                      uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                      const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen,
+                                      const uint32_t* dictId, int32_t* outLen, int32_t nFrames, int32_t blockSize,
+                                      int32_t flags, int32_t level, int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level};
+    b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
+    FrameDict fd;
+    fd.id = dictId;
+    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device, &fd);
+}
+
+int32_t k4lz4_frame_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                      uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                      const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen,
+                                      int32_t* outLen, int32_t nFrames, int32_t memKind, void* cudaStream,
+                                      int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
+    b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
+    FrameDict fd;
+    return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device, &fd);
+}
+
+int32_t k4lz4_frame_info_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen, int32_t* outSize,
+                               int64_t* outDictId, int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
+    FrameDict fd;
+    fd.outId = outDictId;
+    return frame_run(FO_SIZE, b, 0, 0, memKind, cudaStream, device, &fd);
 }
 
 int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int32_t flags, int32_t level,

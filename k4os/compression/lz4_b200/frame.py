@@ -11,7 +11,9 @@ decoded by the library's frame calls (k4lz4_frame_encode_batch / _decode_batch /
 per call: header, block walk, raw/compressed choice, layout and checksums run on the GPU.  This module is a thin
 mirror over them.  Frames are interoperable with upstream lz4 (tests decode them with orig/lib/lz4frame.c and
 decode upstream's frames here); content size and dictionary ids are not written (the reference itself throws
-NotImplemented for them, LZ4FrameWriter.cs:89-95).  _Frame restates the device parse on the CPU.
+NotImplemented for them, LZ4FrameWriter.cs:89-95).  The *WithDictionary calls and Info go beyond the reference:
+upstream's frames against a dictionary (LZ4F_compressBegin_usingCDict, lz4 -D), encoded and decoded on the GPU.
+_Frame restates the device parse on the CPU (dictionary=True: the dictionary calls' parse).
 """
 from __future__ import annotations
 
@@ -156,6 +158,111 @@ class LZ4Frame:
                                                  out_len.data_ptr(), int(src_len.numel()), N.MEM_DEVICE,
                                                  stream or None, int(device)))
 
+    # ---- against a dictionary (k4lz4_frame_encode_dict_batch / _decode_dict_batch / k4lz4_frame_info_batch):
+    # upstream's LZ4F_compressBegin_usingCDict frames and lz4 -D; the reference has no dictionary frames.
+
+    @staticmethod
+    def EncodeManyWithDictionary(datas, dictionaries, dict_ids=None, block_size: int = 65536, chaining: bool = True,
+                                 block_checksum: bool = False, content_checksum: bool = False, level: int = 0,
+                                 device: int = 0):
+        """-> (list of frames, int32 results): frame i of datas[i] against dictionaries[i], byte for byte upstream's
+        CDict frame (dictID = dict_ids[i]; 0 or None writes no ID); K4LZ4_R_DELEGATE for level >= 3.  block_size is
+        64 KiB, 256 KiB, 1 MiB or 4 MiB."""
+        src, so, sl = _pack([_u8(d) for d in datas])
+        dic, do_, dl = _pack([_u8(d) for d in dictionaries])
+        ids = np.zeros(len(sl), dtype=np.uint32) if dict_ids is None else np.ascontiguousarray(dict_ids, dtype=np.uint32)
+        if len(dl) != len(sl) or len(ids) != len(sl):
+            raise ValueError("one dictionary and one ID per frame")
+        fl = _flags(chaining, block_checksum, content_checksum)
+        caps = [LZ4Frame.Bound(int(x), block_size, chaining, block_checksum, content_checksum) + (4 if ids[i] else 0)
+                for i, x in enumerate(sl)]
+        dst, do, dc = _slots(caps)
+        out = np.full(len(sl), -1, dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_encode_dict_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+                                                      do.ctypes.data, dc.ctypes.data, dic.ctypes.data,
+                                                      do_.ctypes.data, dl.ctypes.data, ids.ctypes.data,
+                                                      out.ctypes.data, len(sl), int(block_size), fl, int(level),
+                                                      N.MEM_HOST, None, int(device)))
+        return _slices(dst, do, out), out
+
+    @staticmethod
+    def Info(frames, device: int = 0):
+        """-> (int32 content sizes or verdicts, as ContentSizes but with the dictionary flag accepted;
+        int64 dictIDs, -1 for a frame without a dictID field)."""
+        src, so, sl = _pack([_u8(f) for f in frames])
+        out = np.full(len(sl), -1, dtype=np.int32)
+        ids = np.full(len(sl), -1, dtype=np.int64)
+        N.check(N.lib().k4lz4_frame_info_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, out.ctypes.data,
+                                               ids.ctypes.data, len(sl), N.MEM_HOST, None, int(device)))
+        return out, ids
+
+    @staticmethod
+    def DecodeManyWithDictionary(frames, dictionaries, caps=None, device: int = 0):
+        """-> (list of contents, int32 results), frame i against dictionaries[i] (with or without a dictID field:
+        the ID is not checked).  caps default to each frame's content size."""
+        frames = [_u8(f) for f in frames]
+        if caps is None:
+            caps = np.maximum(LZ4Frame.Info(frames, device)[0], 0)
+        src, so, sl = _pack(frames)
+        dic, do_, dl = _pack([_u8(d) for d in dictionaries])
+        if len(dl) != len(sl):
+            raise ValueError("one dictionary per frame")
+        dst, do, dc = _slots(caps)
+        out = np.full(len(sl), -1, dtype=np.int32)
+        N.check(N.lib().k4lz4_frame_decode_dict_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+                                                      do.ctypes.data, dc.ctypes.data, dic.ctypes.data,
+                                                      do_.ctypes.data, dl.ctypes.data, out.ctypes.data, len(sl),
+                                                      N.MEM_HOST, None, int(device)))
+        return _slices(dst, do, out), out
+
+    @staticmethod
+    def EncodeWithDictionary(data, dictionary, dict_id: int = 0, block_size: int = 65536, chaining: bool = True,
+                             block_checksum: bool = False, content_checksum: bool = False, level: int = 0,
+                             device: int = 0) -> bytes:
+        if level >= 3:
+            raise NotImplementedError("dictionary frames at the HC levels are not implemented")
+        frames, out = LZ4Frame.EncodeManyWithDictionary([data], [dictionary], [dict_id], block_size, chaining,
+                                                        block_checksum, content_checksum, level, device)
+        if out[0] < 0:
+            raise RuntimeError("Failed to encode the frame")
+        return frames[0]
+
+    @staticmethod
+    def DecodeWithDictionary(frame, dictionary, device: int = 0) -> bytes:
+        contents, out = LZ4Frame.DecodeManyWithDictionary([frame], [dictionary], None, device)
+        _raise_for(int(out[0]))
+        return contents[0]
+
+    @staticmethod
+    def encode_many_with_dictionary_device(src, src_off, src_len, dst, dst_off, dst_cap, dict_base, dict_off,
+                                           dict_len, dict_id, out_len, block_size: int = 65536, chaining: bool = True,
+                                           block_checksum: bool = False, content_checksum: bool = False,
+                                           level: int = 0, stream: int = 0, device: int = -1) -> None:
+        """dict_id: a uint32-sized tensor (torch.int32 holding the IDs' bits) or None."""
+        N.check(N.lib().k4lz4_frame_encode_dict_batch(
+            src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(), dst.data_ptr(), dst_off.data_ptr(),
+            dst_cap.data_ptr(), dict_base.data_ptr(), dict_off.data_ptr(), dict_len.data_ptr(),
+            dict_id.data_ptr() if dict_id is not None else None, out_len.data_ptr(), int(src_len.numel()),
+            int(block_size), _flags(chaining, block_checksum, content_checksum), int(level), N.MEM_DEVICE,
+            stream or None, int(device)))
+
+    @staticmethod
+    def decode_many_with_dictionary_device(src, src_off, src_len, dst, dst_off, dst_cap, dict_base, dict_off,
+                                           dict_len, out_len, stream: int = 0, device: int = -1) -> None:
+        """dict_base None: no dictionaries (dict_off / dict_len are then ignored)."""
+        N.check(N.lib().k4lz4_frame_decode_dict_batch(
+            src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(), dst.data_ptr(), dst_off.data_ptr(),
+            dst_cap.data_ptr(), dict_base.data_ptr() if dict_base is not None else None,
+            dict_off.data_ptr() if dict_base is not None else None,
+            dict_len.data_ptr() if dict_base is not None else None, out_len.data_ptr(), int(src_len.numel()),
+            N.MEM_DEVICE, stream or None, int(device)))
+
+    @staticmethod
+    def info_device(src, src_off, src_len, out_size, out_dict_id, stream: int = 0, device: int = -1) -> None:
+        N.check(N.lib().k4lz4_frame_info_batch(src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(),
+                                               out_size.data_ptr(), out_dict_id.data_ptr(), int(src_len.numel()),
+                                               N.MEM_DEVICE, stream or None, int(device)))
+
 
 def write_frames(datas, block_size: int = 65536, block_checksum: bool = False, content_checksum: bool = False,
                  level: int = 0, device: int = 0, chaining: bool = True) -> list:
@@ -180,7 +287,7 @@ def write_frame(data, block_size: int = 65536, block_checksum: bool = False,
 class _Frame:
     """A parsed frame: header flags and the position, length and raw flag of every block."""
 
-    def __init__(self, f: bytes):
+    def __init__(self, f: bytes, dictionary: bool = False):
         if len(f) < 7 or struct.unpack_from("<I", f, 0)[0] != MAGIC:
             raise InvalidDataException("LZ4 frame magic number expected")
         flg, bd = f[4], f[5]
@@ -190,11 +297,12 @@ class _Frame:
         self.block_checksum = bool((flg >> 4) & 1)
         has_size = bool((flg >> 3) & 1)
         content_checksum = bool((flg >> 2) & 1)
-        if flg & 1:
+        if flg & 1 and not dictionary:
             raise NotImplementedError("Predefined dictionaries feature is not implemented")   # :108-110
-        p = 6 + (8 if has_size else 0)
+        p = 6 + (8 if has_size else 0) + (4 if flg & 1 else 0)
         if len(f) < p + 1 or ((xxh32(f[4:p]) >> 8) & 0xFF) != f[p]:
             raise InvalidDataException("Invalid LZ4 frame header checksum")
+        self.dict_id = struct.unpack_from("<I", f, p - 4)[0] if flg & 1 else None
         p += 1
         self.max_block = _BLOCK_SIZES.get((bd >> 4) & 7, 1 << 16)    # LZ4FrameReader.cs:55-59
         pos, lens, raws, sums = [], [], [], []
