@@ -11,18 +11,18 @@
 //               so that a failing block cannot move a later one out of its stream's region; the stream of each
 //               entry.  Then one CTA scans the sizes over all entries; an entry's offset in its stream is its scan
 //               value minus that of the stream's first entry.
-//   2. decode   persistent warps, one entry each, the prefix-mode tests of decode_block_warp_general in the
-//               reference's order, so the verdict is final here.  Literals and the matches whose source is final
-//               (the caller's history, or bytes of this block that are not deferred) are written.  A match that
-//               reads bytes of an earlier block of this call, or a deferred interval of its own block, is recorded
-//               as (op, len, offset) on the block's deferred list; the list's destinations are the block's deferred
-//               intervals (increasing and disjoint, so membership is a binary search over the list).  A block with more than DS_BUDGET
-//               deferred matches is marked "whole".
+//   2. decode   persistent warps, one entry each: the exact engine (decode_block_warp) in prefix mode, so the
+//               verdict is final here, with its writes going through DeferOut.  Literals and the matches whose
+//               source is final (the caller's history, or bytes of this block that are not deferred) are written.
+//               A match that reads bytes of an earlier block of this call, or a deferred interval of its own block,
+//               is recorded as (op, len, offset) on the block's deferred list; the list's destinations are the
+//               block's deferred intervals (increasing and disjoint, so membership is a binary search over the
+//               list).  A block with more than DS_BUDGET deferred matches is marked "whole".
 //   3. verdicts and
 //   4. replay   one warp per stream, streams handed out by a counter: the stream's entries in order, -1 from its
 //               first failing entry on; each block's deferred records replayed with the exact engine's copy
 //               semantics (the records that read only earlier blocks 32 at a time, then the rest in order, in runs
-//               of independent records), or a "whole" block decoded again with decode_block_warp_general, whose
+//               of independent records), or a "whole" block decoded again by the engine with DirectOut, whose
 //               history is final by then.  Every stream's chain runs on its own warp, so all resident streams
 //               advance side by side, and no warp ever waits on another.
 //
@@ -117,23 +117,24 @@ __global__ void __launch_bounds__(DS_SCAN_THREADS) stream_scan_kernel(StreamWork
     }
 }
 
-// The prefix-mode engine of decode_block_warp_general (outputSize = cap, no dictionary, not partial), with the
-// match copies split into written-now and deferred.  `off` = the block's offset in its stream: bytes in
-// [-off, 0) are this call's earlier blocks.  Returns the engine's result (bytes or < 0); *nd = deferred copies
-// or -1 (whole).
-__device__ int stream_decode_block(const uint8_t* __restrict__ src, int n, uint8_t* dst, int cap, int prefix,
-                                   int64_t off, DeferCopy* copies, int* nd) {
-    const int lane = lane_id();
-    int64_t ip = 0, op = 0;
-    const int64_t iend = n, oend = cap;
-    const int64_t shortiend = iend - 16, shortoend = oend - 32;
-    const int64_t lowPrefix = -(int64_t)prefix;
+// The engine's output in pass 2 (prefix mode, outputSize = cap, no dictionary, not partial).  `off` = the block's
+// offset in its stream: bytes in [-off, 0) are this call's earlier blocks.  Literals and the match copies whose
+// source is final are written; a match that touches [-off, 0) or a deferred interval of this block is recorded on
+// `copies` instead.  The block's deferred intervals increase and are disjoint, so membership is a binary search over
+// the earlier records.  Past DS_BUDGET records the block is "whole": nothing more is written.  After the engine
+// returns, nd = the deferred copies or -1 (whole).
+struct DeferOut {
+    int64_t off;
+    DeferCopy* copies;
     int ndef = 0;
     bool whole = false;
     int64_t lastLo = 0, lastHi = -1;                 // the last deferred interval (in registers)
+    int nd = 0;
 
-    // A match's source is final unless it touches [-off, 0) or a deferred interval of this block.
-    auto copy_match = [&](int64_t match, int len, int offset) {
+    __device__ __forceinline__ void literals(uint8_t* d, const uint8_t* __restrict__ s, int len, int lane) {
+        if (!whole) warp_copy_in(d, s, len, lane);
+    }
+    __device__ __forceinline__ void match(uint8_t* dst, int64_t op, int64_t match, int len, int offset, int lane) {
         if (whole) return;
         if (offset == 0) { warp_copy_match(dst, op, match, len, offset, lane); return; }
         const int64_t lo = match, hi = match + (offset < len ? offset : len);
@@ -154,60 +155,11 @@ __device__ int stream_decode_block(const uint8_t* __restrict__ src, int n, uint8
         if (lane == 0) copies[ndef] = DeferCopy{(int32_t)op, len, offset};
         ndef++;
         lastLo = op; lastHi = op + len;
-    };
-    auto finish = [&](int r) { *nd = whole ? -1 : ndef; return r; };
-
-    for (;;) {
-        const uint32_t token = __ldg(src + ip); ip++;
-        int64_t len = token >> 4;
-        const bool shortcut = (len != 15) && (ip < shortiend) && (op <= shortoend);
-        if (!shortcut) {
-            if (len == 15) {
-                if (ip >= iend - 15) return finish(-1);
-                for (;;) {
-                    uint32_t s = __ldg(src + ip); ip++;
-                    len += s;
-                    if (ip >= iend - 15) break;
-                    if (s != 255) break;
-                }
-            }
-            const int64_t cpy = op + len;
-            if (cpy > oend - MFLIMIT || ip + len > iend - (2 + 1 + LASTLITERALS)) {
-                if (ip + len != iend || cpy > oend) return finish(-1);
-                if (!whole) warp_copy_in(dst + op, src + ip, (int)len, lane);
-                return finish((int)(op + len));
-            }
-        }
-        if (!whole) warp_copy_in(dst + op, src + ip, (int)len, lane);
-        ip += len; op += len;
-
-        const int offset = (int)__ldg(src + ip) | ((int)__ldg(src + ip + 1) << 8);
-        ip += 2;
-        const int64_t match = op - offset;
-        len = token & 15;
-
-        if (shortcut && len != 15 && offset >= 8 && match >= lowPrefix) {
-            len += MINMATCH;
-            copy_match(match, (int)len, offset);
-            op += len;
-            continue;
-        }
-        if (len == 15) {
-            for (;;) {
-                uint32_t s = __ldg(src + ip); ip++;
-                len += s;
-                if (ip >= iend - LASTLITERALS + 1) return finish(-1);
-                if (s != 255) break;
-            }
-        }
-        len += MINMATCH;
-        if (match < lowPrefix) return finish(-1);
-        const int64_t cpy = op + len;
-        if (cpy > oend - LASTLITERALS) return finish(-1);
-        copy_match(match, (int)len, offset);
-        op = cpy;
     }
-}
+    // never reached: a chained stream has no dictionary
+    __device__ __forceinline__ void window(uint8_t*, int64_t, int64_t, int, int, const uint8_t*, int, int) {}
+    __device__ __forceinline__ int done(int r) { nd = whole ? -1 : ndef; return r; }
+};
 
 // pass 2: persistent warps, one entry at a time
 __global__ void stream_decode_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
@@ -229,8 +181,10 @@ __global__ void stream_decode_kernel(const uint8_t* __restrict__ srcBase, const 
             } else if (L <= 0 || cap <= 0) {
                 r = chain_trivial(L, cap, src);
             } else {
-                r = stream_decode_block(src, L, dst, cap, p.P, p.off, w.copies + (int64_t)e * DS_BUDGET, &nd);
+                DeferOut out{p.off, w.copies + (int64_t)e * DS_BUDGET};
+                r = decode_block_warp(out, src, L, dst, cap, false, nullptr, 0, p.P);
                 r = r < 0 ? -1 : r;
+                nd = out.nd;
             }
         }
         if (lane == 0) { outLen[e] = r; w.ndef[e] = nd; }
@@ -324,7 +278,7 @@ __device__ void replay_block(uint8_t* dst, const DeferCopy* c, int nd, int lane)
 
 // passes 3 and 4: one warp per stream at a time (streams handed out by a counter), its chain in order: from the
 // stream's first failing entry on every entry is -1; a deferred list is replayed, a "whole" block decoded again
-// with decode_block_warp_general (its history is final by then).  A warp reads only bytes it wrote itself or that
+// by the engine with DirectOut (its history is final by then).  A warp reads only bytes it wrote itself or that
 // an earlier kernel wrote, so no warp ever waits on another and the chains of all resident streams run side by side.
 __global__ void __launch_bounds__(128)
 stream_replay_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
@@ -351,7 +305,8 @@ stream_replay_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restr
             const Place p = ds_place(w, entryStart, prefixLen, e);
             uint8_t* dst = dstBase + dstOff[s] + p.off;
             __syncwarp();
-            if (nd < 0) decode_block_warp_general(srcBase + srcOff[e], srcLen[e], dst, dstCap[e], false, nullptr, 0, p.P);
+            if (nd < 0) decode_block_warp(DirectOut{}, srcBase + srcOff[e], srcLen[e], dst, dstCap[e], false, nullptr, 0,
+                                          p.P);
             else replay_block(dst, w.copies + (int64_t)e * DS_BUDGET, nd, lane);
         }
     }

@@ -684,9 +684,6 @@ __device__ int tile_decode_block(TileSmem<STAGE>& S, const uint8_t* __restrict__
 // ------------------------------------------------------------------------------------------------
 // kernels
 // ------------------------------------------------------------------------------------------------
-// Work-list entry of the second and third launch: block index, bit 31 = "exact decoder only".
-constexpr uint32_t WL_GENERIC = 0x80000000u;
-
 struct DecodeLists {
     uint32_t* big;      // blocks for the big-stage tile kernel
     uint32_t* gen;      // blocks for the exact generic decoder
@@ -808,19 +805,13 @@ __device__ __forceinline__ void decode_rest_body(
     for (uint32_t e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < count; e += nwarps) {
         const int b = (int)wl.gen[e];
         int r;
-        if constexpr (EXT) {                     // the general engine's dictionary form (decode_general_kernel)
-            const int n = srcLen[b];
-            if (n <= 0) r = 0;
-            else {
-                const int dl = dictLen[b];
-                r = decode_block_warp_general(srcBase + srcOff[b], n, dstBase + dstOff[b], dstCap[b] < 0 ? 0 : dstCap[b],
-                                              false, dl > 0 ? dictBase + dictOff[b] : nullptr, dl > 0 ? dl : 0);
-                r = r <= 0 ? -1 : r;
-            }
+        if constexpr (EXT) {                     // the engine's dictionary form (decode_general_kernel)
+            r = codec_decode_general_warp(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, false, dictBase, dictOff,
+                                          dictLen, b);
         } else if (!prefixLen) r = codec_decode_warp(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b]);
         else {                                   // LZ4_decompress_safe_continue in prefix mode, raw engine result
-            r = decode_block_warp_general(srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b], false,
-                                          nullptr, 0, chain_prefix(prefixLen, b));
+            r = decode_block_warp(DirectOut{}, srcBase + srcOff[b], srcLen[b], dstBase + dstOff[b], dstCap[b], false,
+                                  nullptr, 0, chain_prefix(prefixLen, b));
             r = r < 0 ? -1 : r;
         }
         if (lane_id() == 0) { outLen[b] = r; atomicAdd(&g_decode_stats[2], 1ull); }

@@ -80,7 +80,7 @@ def _final(known: bytearray, a: int, b: int) -> bool:
 
 def _deferred_decode(src: bytes, cap: int, P: int, off: int, out: bytearray, known: bytearray, base: int,
                      budget: int):
-    """stream_decode_block: -> (r, copies or None for whole).  Block byte x is out[base + x]; [base - off, base)
+    """decode_block_warp with DeferOut: -> (r, copies or None for whole).  Block byte x is out[base + x]; [base - off, base)
     are this call's earlier blocks."""
     n = len(src)
     low = -min(P, 65535)
