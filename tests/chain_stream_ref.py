@@ -3,14 +3,17 @@
 ``decode_streams`` runs the four passes of k4lz4_decode_chain_streams over lists of blocks: place (the size walk
 and the per-stream scan), the deferred decode of every block on its own (literals and final-source matches
 written, the rest recorded on the block's deferred list, a block past the budget marked whole), the verdicts and
-the replay in stream order (a block's records that read only earlier blocks first, then the rest in order).  Every
-copy it makes asserts that the bytes it reads are already final, so the deferral rule and the replay's order are
-checked, not only the end result.  ``step_reference`` is the authority: upstream's
+the replay in stream order.  It makes the kernel's decisions in the kernel's form: the own-block test through the
+last deferred interval and a binary search over the unmerged records (checked against merged spans at every match),
+phase A in groups of 32 and phase B in the kernel's runs of lanes.  Every run of copies the kernel makes at the same
+time asserts that all the bytes it reads are final before any of it is written, so the deferral rule and the
+replay's partition are checked, not only the end result; ``Stats`` counts which rule decided what.  ``step_reference`` is the authority: upstream's
 LZ4_decompress_safe_continue stepped block by block (what k4lz4_decode_chain_batch does per call).
 """
 from __future__ import annotations
 
 import bisect
+from collections import Counter
 from dataclasses import dataclass, field
 
 from tests import chain_ref as CR
@@ -59,9 +62,37 @@ class Stats:
     deferred_bytes: int = 0
     deferred_copies: int = 0
     blocks: int = 0
-    whole_blocks: int = 0
+    whole_blocks: int = 0                  # accepted blocks decoded whole
     max_copies: int = 0
     per_block: list = field(default_factory=list)
+    # pass 2: which test of DeferOut::match decided each match with a nonzero offset
+    dec_earlier: int = 0                   # deferred: the source touches an earlier block of the call
+    dec_last: int = 0                      # deferred: the source touches the last deferred interval
+    dec_search: int = 0                    # deferred: the binary search over the older records found one
+    dec_gap: int = 0                       # written: the search ran and the source lies between intervals
+    whole_failed: int = 0                  # blocks over the budget that then fail (the stream's first failure)
+    whole_prewritten: int = 0              # blocks over the budget after pass 2 wrote some of their bytes
+    # pass 4
+    phase_a: int = 0                       # phase-A records
+    phase_a_long: int = 0                  # ... longer than the lane copy (one by one with the whole warp)
+    runs: int = 0                          # phase-B windows
+    stops_dep: int = 0                     # windows stopped by a lane that reads an earlier lane's destination
+    stops_len: int = 0                     # ... by a long lane
+    stop_lanes: Counter = field(default_factory=Counter)
+    dep_pairs: Counter = field(default_factory=Counter)      # (earlier lane, stop lane) of every dependency stop
+    cross_window: int = 0                  # phase-B records reading a record of the window before theirs
+
+
+@dataclass(frozen=True)
+class Rules:
+    """The replay's partition rules (decode_stream.cuh replay_block).  The defaults are the kernel's; the others
+    exist so that a test can check that the model's finality assertions catch a wrong rule."""
+    lane_copy: int = 64                    # DS_LANE_COPY
+    dep_gap: int = 0                       # lane i is an earlier lane of lane l when i + dep_gap < l
+    phase_a_hi: int = 0                    # phase A: the source ends at or before block byte phase_a_hi
+
+
+KERNEL = Rules()
 
 
 def _periodic(buf: bytearray, at: int, match: int, length: int, offset: int) -> None:
@@ -79,45 +110,75 @@ def _final(known: bytearray, a: int, b: int) -> bool:
 
 
 def _deferred_decode(src: bytes, cap: int, P: int, off: int, out: bytearray, known: bytearray, base: int,
-                     budget: int):
-    """decode_block_warp with DeferOut: -> (r, copies or None for whole).  Block byte x is out[base + x]; [base - off, base)
-    are this call's earlier blocks."""
+                     budget: int, st: Stats):
+    """decode_block_warp with DeferOut: -> (r, copies or None for whole), also for a failing block.  Block byte x is
+    out[base + x]; [base - off, base) are this call's earlier blocks.  The own-block test is made twice: in the
+    kernel's form (the last interval in registers, then a binary search over the unmerged records before it) and over
+    merged spans; the two must agree at every match."""
     n = len(src)
     low = -min(P, 65535)
     copies, spans = [], []                     # spans: [lo, hi) deferred intervals, increasing
+    last_lo, last_hi = 0, -1                   # DeferOut::lastLo / lastHi
     whole = False
+    written = 0                                # bytes pass 2 wrote
     ip = op = 0
     iend, oend = n, cap
     shortiend, shortoend = iend - 16, oend - 32
 
     def copy_match(match: int, length: int, offset: int) -> None:
-        nonlocal whole
+        nonlocal whole, last_lo, last_hi, written
         if whole:
             return
         lo, hi = match, match + min(length, offset)
         dep = offset != 0 and max(lo, -off) < min(hi, 0)
+        if offset != 0:
+            st.dec_earlier += dep
         if offset != 0 and not dep and hi > 0:
             qlo = max(lo, 0)
             k = bisect.bisect_left(spans, (hi, -1)) - 1
-            dep = k >= 0 and spans[k][1] > qlo
+            by_spans = k >= 0 and spans[k][1] > qlo
+            # DeferOut::match
+            dep = last_lo < hi and last_hi > qlo
+            st.dec_last += dep
+            if not dep and len(copies) > 1 and qlo < last_lo:
+                a, b = 0, len(copies) - 2
+                while a < b:
+                    m = (a + b + 1) >> 1
+                    if copies[m][0] < hi:
+                        a = m
+                    else:
+                        b = m - 1
+                c_op, c_len, _ = copies[a]
+                dep = c_op < hi and c_op + c_len > qlo
+                st.dec_search += dep
+                st.dec_gap += not dep and c_op < hi
+            assert dep == by_spans, ("the kernel's own-block test and the spans disagree", match, length, offset)
         if not dep:
             assert offset == 0 or _final(known, base + lo, base + hi), "a final-source copy reads a deferred byte"
             _periodic(out, base + op, base + match, length, offset)
             known[base + op:base + op + length] = b"\x01" * length
+            written += length
             return
         if len(copies) == budget:
             whole = True
+            st.whole_prewritten += written > 0
             return
         copies.append((op, length, offset))
+        last_lo, last_hi = op, op + length
         if spans and spans[-1][1] == op:
             spans[-1] = (spans[-1][0], op + length)
         else:
             spans.append((op, op + length))
 
     def lits(a: int, length: int) -> None:
+        nonlocal written
         if not whole:
             out[base + op:base + op + length] = src[a:a + length]
             known[base + op:base + op + length] = b"\x01" * length
+            written += length
+
+    def fail():
+        return -1, (None if whole else copies)
 
     while True:
         token = src[ip]; ip += 1
@@ -126,7 +187,7 @@ def _deferred_decode(src: bytes, cap: int, P: int, off: int, out: bytearray, kno
         if not shortcut:
             if length == 15:
                 if ip >= iend - 15:
-                    return -1, None
+                    return fail()
                 while True:
                     s = src[ip]; ip += 1; length += s
                     if ip >= iend - 15 or s != 255:
@@ -134,7 +195,7 @@ def _deferred_decode(src: bytes, cap: int, P: int, off: int, out: bytearray, kno
             cpy = op + length
             if cpy > oend - MFLIMIT or ip + length > iend - (2 + 1 + LASTLITERALS):
                 if ip + length != iend or cpy > oend:
-                    return -1, None
+                    return fail()
                 lits(ip, length)
                 return op + length, (None if whole else copies)
         lits(ip, length)
@@ -150,21 +211,78 @@ def _deferred_decode(src: bytes, cap: int, P: int, off: int, out: bytearray, kno
             while True:
                 s = src[ip]; ip += 1; length += s
                 if ip >= iend - LASTLITERALS + 1:
-                    return -1, None
+                    return fail()
                 if s != 255:
                     break
         length += MINMATCH
         if match < low:
-            return -1, None
+            return fail()
         if op + length > oend - LASTLITERALS:
-            return -1, None
+            return fail()
         copy_match(match, length, offset)
         op += length
 
 
-def decode_streams(streams, budget: int = BUDGET, stats: Stats | None = None):
+def _run(out: bytearray, known: bytearray, base: int, recs) -> None:
+    """Records copied at the same time (the lanes of one run, or one record by the whole warp): every byte any of
+    them reads must be final before the first of them writes."""
+    for op, length, offset in recs:
+        lo = base + op - offset
+        assert _final(known, lo, lo + min(length, offset)), "a replay run reads a byte that is not final yet"
+    for op, length, offset in recs:
+        _periodic(out, base + op, base + op - offset, length, offset)
+        known[base + op:base + op + length] = b"\x01" * length
+
+
+def _replay(out: bytearray, known: bytearray, base: int, cp, rules: Rules, st: Stats) -> None:
+    """replay_block: phase A in groups of 32 (the short records together, then the long ones one by one), then
+    phase B in windows of 32 that stop at the first lane that reads an earlier phase-B lane's destination or is long:
+    the lanes before it together, then it alone, and the next window starts behind it."""
+    nd = len(cp)
+    src_hi = [op - offset + min(length, offset) for op, length, offset in cp]
+    for k0 in range(0, nd, 32):
+        grp = [cp[k] for k in range(k0, min(k0 + 32, nd)) if src_hi[k] <= rules.phase_a_hi]
+        _run(out, known, base, [c for c in grp if c[1] <= rules.lane_copy])
+        for c in grp:
+            if c[1] > rules.lane_copy:
+                _run(out, known, base, [c])
+                st.phase_a_long += 1
+        st.phase_a += len(grp)
+    k, prev = 0, []
+    while k < nd:
+        lanes = [j for j in range(k, min(k + 32, nd))]
+        b = [src_hi[j] > 0 for j in lanes]
+        m, why, pairs = 32, None, []
+        for lane, j in enumerate(lanes):
+            if not b[lane]:
+                continue
+            op, length, offset = cp[j]
+            lo, hi = op - offset, src_hi[j]
+            deps = [i for i in range(31) if i + rules.dep_gap < lane and b[i] and cp[lanes[i]][0] < hi
+                    and cp[lanes[i]][0] + cp[lanes[i]][1] > lo]
+            st.cross_window += any(p_op < hi and p_op + p_len > lo for p_op, p_len, _ in prev)
+            if deps or length > rules.lane_copy:
+                m, why, pairs = lane, ("dep" if deps else "len"), deps
+                break
+        _run(out, known, base, [cp[lanes[i]] for i in range(min(m, len(lanes))) if b[i]])
+        st.runs += 1
+        if m < 32:
+            _run(out, known, base, [cp[lanes[m]]])
+            st.stop_lanes[m] += 1
+            st.stops_dep += why == "dep"
+            st.stops_len += why == "len"
+            st.dep_pairs.update((i, m) for i in pairs)
+            prev = [cp[lanes[i]] for i in range(m + 1) if b[i]]
+            k += m + 1
+        else:
+            prev = [cp[lanes[i]] for i in range(len(lanes)) if b[i]]
+            k += 32
+
+
+def decode_streams(streams, budget: int = BUDGET, stats: Stats | None = None, rules: Rules = KERNEL):
     """streams: list of (history bytes, prefixLen, [(src, cap, raw)]).  -> list of (outLen list, decoded bytes of
     the stream's region up to its first failing entry)."""
+    st = stats if stats is not None else Stats()
     res = []
     for hist, prefix, entries in streams:
         # pass 1: place
@@ -197,12 +315,13 @@ def decode_streams(streams, budget: int = BUDGET, stats: Stats | None = None):
             elif len(src) <= 0 or cap <= 0:
                 r2.append(0 if cap == 0 and len(src) == 1 and src[0] == 0 else -1); lists.append([])
             else:
-                r, cp = _deferred_decode(src, cap, prefix + offs[k], offs[k], out, known, base, budget)
+                r, cp = _deferred_decode(src, cap, prefix + offs[k], offs[k], out, known, base, budget, st)
                 r2.append(r if r >= 0 else -1); lists.append(cp)
         # passes 3 and 4: verdicts and replay, in stream order
         outlen, failed = [], False
         for k, (src, cap, raw) in enumerate(entries):
             if failed or r2[k] < 0:
+                st.whole_failed += not failed and lists[k] is None
                 failed = True
                 outlen.append(-1)
                 continue
@@ -216,28 +335,20 @@ def decode_streams(streams, budget: int = BUDGET, stats: Stats | None = None):
                 out[base:base + r] = data
                 known[base:base + r] = b"\x01" * r
             else:
-                # phase A: the records that read only earlier blocks; phase B: the rest, in order
-                in_front = [op - offset + min(length, offset) <= 0 for op, length, offset in cp]
-                for phase in (True, False):
-                    for (op, length, offset), a in zip(cp, in_front):
-                        if a != phase:
-                            continue
-                        assert _final(known, base + op - offset, base + op - offset + min(length, offset))
-                        _periodic(out, base + op, base + op - offset, length, offset)
-                        known[base + op:base + op + length] = b"\x01" * length
+                _replay(out, known, base, cp, rules, st)
             assert _final(known, base, base + r2[k]), "a byte of an accepted block was never written"
             outlen.append(r2[k])
-            if stats is not None and not raw:
-                stats.blocks += 1
-                stats.out_bytes += r2[k]
+            if not raw:
+                st.blocks += 1
+                st.out_bytes += r2[k]
                 if cp is None:
-                    stats.whole_blocks += 1
-                    stats.per_block.append(-1)
+                    st.whole_blocks += 1
+                    st.per_block.append(-1)
                 else:
-                    stats.deferred_copies += len(cp)
-                    stats.deferred_bytes += sum(c[1] for c in cp)
-                    stats.max_copies = max(stats.max_copies, len(cp))
-                    stats.per_block.append(len(cp))
+                    st.deferred_copies += len(cp)
+                    st.deferred_bytes += sum(c[1] for c in cp)
+                    st.max_copies = max(st.max_copies, len(cp))
+                    st.per_block.append(len(cp))
         good = sum(r for r in outlen if r > 0)
         res.append((outlen, bytes(out[H:H + good])))
     return res
