@@ -57,6 +57,12 @@ namespace K4os.Compression.LZ4.Engine.Native
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             byte* dictBase, long* dictOff, int* dictLen, int* outLen, int nBlocks,
             int memKind, void* cudaStream, int device);
+        // upstream's LZ4_compress_destSize: the longest prefix whose block fits the target; *srcSize becomes its length
+        [DllImport(Lib)] public static extern int k4lz4_encode_dest_size(
+            byte* src, byte* dst, int* srcSize, int targetDstSize);
+        [DllImport(Lib)] public static extern int k4lz4_encode_dest_size_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* outLen, int* srcUsed, int nBlocks, int memKind, void* cudaStream, int device);
         [DllImport(Lib)] public static extern int k4lz4_partial_decode_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* targetLen,
             int* outLen, int nBlocks, int memKind, void* cudaStream, int device);

@@ -52,6 +52,21 @@ namespace K4os.Compression.LZ4
                     K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
         }
 
+        // Fixed-size destinations (k4lz4_encode_dest_size_batch; the reference has no such call): block i encodes the
+        // longest prefix of its source whose block fits targetCapacities[i], as upstream's LZ4_compress_destSize.
+        // lengths[i]: bytes written; consumed[i]: the source bytes the block holds (both 0 where nothing is written).
+        public static void EncodeDestSize(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            Span<int> lengths, Span<int> consumed)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (int* ol = lengths) fixed (int* su = consumed)
+                Check(K4Lz4Native.k4lz4_encode_dest_size_batch(s, so, sl, d, dof, dc, ol, su, lengths.Length,
+                    K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
+        }
+
         // LZ4 frames against a dictionary, as upstream's LZ4F_compressBegin_usingCDict writes them
         // (k4lz4_frame_encode_dict_batch): frame i holds source i, encoded against dictionary i, with the dictID
         // dictionaryIds[i] unless it is 0 (an empty span: no IDs).  blockSize: 64 KiB, 256 KiB, 1 MiB or 4 MiB; flags:

@@ -187,6 +187,30 @@ K4LZ4_API int32_t k4lz4_encode_dict_batch(const uint8_t *srcBase, const int64_t 
                                           int32_t *outLen, int32_t nBlocks,
                                           int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- encode into fixed-size destinations (upstream's LZ4_compress_destSize) ------------------ */
+
+/* Encode the longest prefix of src whose block fits targetDstSize bytes.  No reference call corresponds (the
+ * reference's engine has the fillOutput branch, Engine/x64/LL64.fast.cs, but no public call reaches it); the result
+ * is upstream lz4's 64-bit engine for
+ *     n = *srcSize; r = LZ4_compress_destSize(src, dst, &n, targetDstSize);
+ * at acceleration 1: the return value is r and *srcSize becomes n, the source bytes the block holds.  A target of
+ * at least LZ4_compressBound(*srcSize) gives k4lz4_encode's bytes and consumes everything; an empty source with a
+ * target of at least 1 gives the one-byte block 0x00.  Nothing is written at or beyond the returned length.
+ * Where nothing is written (targetDstSize < 1, *srcSize < 0 or *srcSize > 0x7E000000) the result is 0 and *srcSize
+ * becomes 0.  Upstream leaves *srcSize as it was in that case; a loop that packs a source into fixed-size pages and
+ * reads it as "consumed" would then drop data.  Host pointers; src may be NULL when *srcSize is 0. */
+K4LZ4_API int32_t k4lz4_encode_dest_size(const uint8_t *src, uint8_t *dst, int32_t *srcSize, int32_t targetDstSize);
+/* Batched form: block i encodes srcBase[srcOff[i] .. +srcLen[i]) into at most dstCap[i] bytes at dstBase + dstOff[i];
+ * outLen[i] is the single call's result and srcUsed[i] what it leaves in *srcSize.  Argument checks and codes as
+ * k4lz4_encode_dict_batch, with srcUsed required instead of the dictionary arrays.  memKind == K4LZ4_MEM_HOST is
+ * synchronous and runs on one GPU (`device`, K4LZ4_ALL_DEVICES = GPU 0); device memory only enqueues work on
+ * `cudaStream`.  Blocks are counted in k4lz4_encode_stats out4[0..2] by the warp kind that encoded them, as
+ * k4lz4_encode_batch's are.  There is no _x32 twin and no level: the reference has no destSize call to reproduce. */
+K4LZ4_API int32_t k4lz4_encode_dest_size_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                               uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                               int32_t *outLen, int32_t *srcUsed, int32_t nBlocks,
+                                               int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- chained (linked) blocks: LZ4ChainDecoder, one block per stream per call ------------------ */
 
 /* LZ4ChainDecoder.Decode -> LLxx.LZ4_decompress_safe_continue in prefix mode
@@ -719,7 +743,7 @@ K4LZ4_API int32_t k4lz4_decode_stats(int32_t device, uint64_t *out4, int32_t res
 /* Encoder path counters of `device` since the last reset: out4[0] blocks encoded by a warp with its
  * hash table in shared memory, [1] by a warp with its table in global memory (only launched when a
  * call has more blocks than the shared-memory warps take in one round), [2] blocks of >= 65 547
- * bytes (the u32-table engine, either warp kind), [3] chained blocks (k4lz4_encode_chain_batch, any
+ * bytes (the u32-table engine, either warp kind); [0..2] count k4lz4_encode_dest_size_batch's blocks too; [3] chained blocks (k4lz4_encode_chain_batch, any
  * size) and blocks encoded against a dictionary (k4lz4_encode_dict_batch).  Empty blocks, delegated levels and rejected arguments are not counted.
  * Synchronises the device.  Diagnostics only. */
 K4LZ4_API int32_t k4lz4_encode_stats(int32_t device, uint64_t *out4, int32_t reset);

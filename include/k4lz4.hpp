@@ -106,6 +106,44 @@ struct LZ4Codec {
             if (out[i] > 0) encoded[i].assign(dst.begin() + dof[i], dst.begin() + dof[i] + out[i]);
         return out;
     }
+    // Encodes the longest prefix of source whose block fits targetLength bytes (k4lz4_encode_dest_size; the reference
+    // has no such call): upstream lz4's LZ4_compress_destSize.  -> bytes written; sourceLength becomes the source bytes
+    // the block holds (0 where nothing is written).
+    static int EncodeDestSize(const uint8_t* source, int& sourceLength, uint8_t* target, int targetLength) {
+        int32_t n = sourceLength;
+        const int r = check_codec(k4lz4_encode_dest_size(source, target, &n, targetLength));
+        sourceLength = n;
+        return r;
+    }
+    // The same over a batch (k4lz4_encode_dest_size_batch, host memory): block i into at most targets[i] bytes.
+    // -> one result per block (bytes written) and, in consumed, the source bytes each encoded block holds.
+    static std::vector<int32_t> EncodeDestSize(const std::vector<std::vector<uint8_t>>& blocks,
+                                               const std::vector<int32_t>& targets,
+                                               std::vector<std::vector<uint8_t>>& encoded,
+                                               std::vector<int32_t>& consumed, int device = 0) {
+        const size_t n = blocks.size();
+        if (targets.size() != n) throw std::invalid_argument("one target per block");
+        std::vector<int64_t> so(n), dof(n);
+        std::vector<int32_t> sl(n), out(n, 0);
+        std::vector<uint8_t> src;
+        int64_t at = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)blocks[i].size();
+            src.insert(src.end(), blocks[i].begin(), blocks[i].end());
+            dof[i] = at; at += targets[i] > 0 ? targets[i] : 0;
+        }
+        src.resize(src.size() + 1);
+        std::vector<uint8_t> dst((size_t)at + 1);
+        consumed.assign(n, 0);
+        const int rc = k4lz4_encode_dest_size_batch(src.data(), so.data(), sl.data(), dst.data(), dof.data(),
+                                                    targets.data(), out.data(), consumed.data(), (int32_t)n,
+                                                    K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        encoded.assign(n, {});
+        for (size_t i = 0; i < n; i++)
+            if (out[i] > 0) encoded[i].assign(dst.begin() + dof[i], dst.begin() + dof[i] + out[i]);
+        return out;
+    }
     // LZ4Codec.PartialDecode(byte*,int,byte*,int) -- LZ4Codec.cs:123-134
     static int PartialDecode(const uint8_t* source, int sourceLength, uint8_t* target, int targetLength) {
         if (sourceLength <= 0) return 0;

@@ -46,6 +46,8 @@ SIGNATURES = {
     "k4lz4_decode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
     "k4lz4_encode_dict": ([_vp, _i32, _vp, _i32, _vp, _i32], _i32),
     "k4lz4_encode_dict_batch": (_BATCH[:6] + [_vp] * 3 + [_vp, _i32] + _CALL, _i32),
+    "k4lz4_encode_dest_size": ([_vp, _vp, _vp, _i32], _i32),
+    "k4lz4_encode_dest_size_batch": (_BATCH + [_vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_batch": (_BATCH[:6] + [_vp, _vp, _i32] + _CALL, _i32),
     "k4lz4_decode_chain_streams": ([_vp] * 6 + [_i32] + [_vp] * 4 + [_i32] + _CALL, _i32),
     "k4lz4_encode_chain_batch": ([_vp] * 10 + [_i32, _i32] + _CALL, _i32),

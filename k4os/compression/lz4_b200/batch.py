@@ -422,3 +422,31 @@ def encode_dict_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, d
     N.check(N.lib().k4lz4_encode_dict_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
                                             dict_ptr, dict_off_ptr, dict_len_ptr, out_len_ptr, int(n), N.MEM_DEVICE,
                                             stream or None, int(device)))
+
+
+def encode_dest_size_batch_host(blocks: Sequence, targets: Sequence[int], device: int = 0):
+    """Encode the longest prefix of each block whose LZ4 block fits its target (k4lz4_encode_dest_size_batch, host
+    memory): upstream lz4's LZ4_compress_destSize, for destinations of a fixed size (pages, packet payloads, slabs).
+    Returns (list of bytes, int32 results: bytes written, int32 source bytes each output holds).  Where nothing is
+    written (a target below 1) both are 0; an empty block with a target of at least 1 gives the byte 0x00."""
+    src, so, sl = _pack(blocks)
+    n = len(sl)
+    if len(targets) != n:
+        raise ValueError(f"{n} blocks but {len(targets)} targets")
+    dst, doff, dc = _slots(targets)
+    out = np.full(n, -1, dtype=np.int32)
+    used = np.full(n, -1, dtype=np.int32)
+    N.check(N.lib().k4lz4_encode_dest_size_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+                                                 doff.ctypes.data, dc.ctypes.data, out.ctypes.data, used.ctypes.data,
+                                                 n, N.MEM_HOST, None, int(device)))
+    return _slices(dst, doff, out), out, used
+
+
+def encode_dest_size_batch_device(src_ptr: int, src_off_ptr: int, src_len_ptr: int, dst_ptr: int, dst_off_ptr: int,
+                                  dst_cap_ptr: int, out_len_ptr: int, src_used_ptr: int, n: int, stream: int = 0,
+                                  device: int = -1) -> None:
+    """Device-pointer form of encode_dest_size_batch_host: only enqueues the kernels on `stream`; dst_cap holds the
+    targets."""
+    N.check(N.lib().k4lz4_encode_dest_size_batch(src_ptr, src_off_ptr, src_len_ptr, dst_ptr, dst_off_ptr, dst_cap_ptr,
+                                                 out_len_ptr, src_used_ptr, int(n), N.MEM_DEVICE, stream or None,
+                                                 int(device)))

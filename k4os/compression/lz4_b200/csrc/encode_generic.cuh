@@ -60,9 +60,12 @@ __device__ __forceinline__ void write_run_header(uint8_t* dst, uint32_t op, uint
  * notLimited/limitedOutput choice and every olimit test).  `hardCap` is a physical write
  * bound used only by the pickler (see pickle.cuh): as soon as the stream would grow past it
  * the function returns 0; pass 0x7fffffff otherwise.
+ * FILL: upstream's fillOutput directive, as in encode_spec_warp (encode_tile.cuh): with cap below the bound the
+ * longest prefix whose block fits cap is encoded, and lane 0 stores the input bytes it took at *used.
  */
+template <bool FILL = false>
 __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_t* __restrict__ dst,
-                                 int cap, int hardCap, void* tableSmem, bool enforce32) {
+                                 int cap, int hardCap, void* tableSmem, bool enforce32, int32_t* used = nullptr) {
     const int lane = lane_id();
     if ((uint32_t)n_ > (uint32_t)MAX_INPUT_SIZE) return 0;                     // LL64.fast.cs:90
     EncCtx c;
@@ -71,7 +74,8 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
     c.use5 = !c.by16 && !enforce32;                                       // LL64.tools.cs:135-143
     c.t16 = reinterpret_cast<uint16_t*>(tableSmem);
     c.t32 = reinterpret_cast<uint32_t*>(tableSmem);
-    const bool limited = !(cap >= max_output_size(n_));                   // :524
+    const bool limited = !FILL && !(cap >= max_output_size(n_));          // :524
+    const bool fill = FILL && !(cap >= max_output_size(n_));              // lz4.c:1387
     const int64_t olimit = cap;
     const int64_t hard = hardCap;
     const uint32_t n = c.n;
@@ -125,6 +129,8 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
                 const uint32_t lit = ip - anchor;
                 if (limited && (int64_t)op + 1 + lit + 8 + lit / 255 > olimit) return 0;   // :246-251
                 const uint32_t hdr = run_header_size(lit);
+                // fill rule 1 (lz4.c:1028-1032): the sequence would pass the target; drop it unwritten
+                if (fill && (int64_t)op + hdr + lit + 2 + 1 + (MFLIMIT - MINMATCH) > olimit) goto last_literals;
                 if ((int64_t)op + hdr + lit > hard) return 0;
                 tokpos = op;
                 if (lane == 0) write_run_header(dst, op, lit);
@@ -151,6 +157,15 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
                 }
                 ip += mc + MINMATCH;
                 if (limited && (int64_t)op + 6 + (mc + 240) / 255 > olimit) return 0;   // :332-362
+                // fill rule 3 (lz4.c:1097-1104): shorten the match to what fits; no later sequence can pass rules
+                // 1 and 2 from here, so the block goes to last literals (encode_spec_warp says why)
+                bool cut = false;
+                if (fill && (int64_t)op + 6 + (mc + 240) / 255 > olimit) {
+                    const uint32_t mc2 = 14u + (uint32_t)(olimit - op - 6) * 255u;
+                    ip -= mc - mc2;
+                    mc = mc2;
+                    cut = true;
+                }
                 if (mc >= 15) {                                           // :365-379
                     const uint32_t rest = mc - 15;
                     const uint32_t nff = rest / 255;
@@ -166,7 +181,7 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
                 }
                 __syncwarp();
                 anchor = ip;                                              // :388
-                if (ip >= mfl1) goto last_literals;                       // :391
+                if (ip >= mfl1 || cut) goto last_literals;                // :391
 
                 // ---- step 8: post-match insert + immediate probe, lane 0 ---------------
                 uint32_t hit = 0;
@@ -183,6 +198,8 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
                 hit = __shfl_sync(FULL, hit, 0);
                 if (!hit) { ip++; break; }
                 m = __shfl_sync(FULL, m, 0);
+                // fill rule 2 (lz4.c:1057-1062): the zero-literal sequence would pass the target; drop it unwritten
+                if (fill && (int64_t)op + 1 + 2 + 1 + (MFLIMIT - MINMATCH) > olimit) goto last_literals;
                 if ((int64_t)op + 1 > hard) return 0;
                 tokpos = op;
                 if (lane == 0) dst[op] = 0;                               // :459-460
@@ -194,14 +211,19 @@ __device__ int encode_block_warp(const uint8_t* __restrict__ src, int n_, uint8_
 
 last_literals:
     {   // ---- step 9, :469-503 ----------------------------------------------------------
-        const uint32_t run = n - anchor;
+        uint32_t run = n - anchor;
         if (limited && (int64_t)op + run + 1 + (run + 255 - 15) / 255 > olimit) return 0;
+        if (fill && (int64_t)op + run + 1 + (run + 255 - 15) / 255 > olimit) {     // fill rule 4, lz4.c:1209-1213
+            run = (uint32_t)(olimit - op) - 1;
+            run -= (run + 256 - 15) / 256;
+        }
         const uint32_t hdr = run_header_size(run);
         if ((int64_t)op + hdr + run > hard) return 0;
         if (lane == 0) write_run_header(dst, op, run);
         op += hdr;
         for (uint32_t i = lane; i < run; i += 32) dst[op + i] = __ldg(src + anchor + i);
         op += run;
+        if (FILL && lane == 0) *used = (int32_t)(anchor + run);
     }
     return (int)op;
 }

@@ -50,9 +50,13 @@ __device__ __forceinline__ uint32_t probe_advance(uint32_t q) {
 // accessed through L2 (.cg) so that the little L1 left beside 224 KiB of shared memory keeps the input
 // windows of all warps of the SM.  Otherwise it holds plain u16 slots (shared memory) and every candidate is fetched.
 // WIN: lanes of the first batch of every search run (32 = all; K4_ENC_WIN).
-template <bool HARD = true, bool GTAB = false, int WIN = 32>
+// FILL: upstream's fillOutput directive (LZ4_compress_destSize, lz4.c:1382-1396): with cap below the bound, encode
+// the longest prefix whose block fits `cap` instead of failing; lane 0 stores the input bytes it took at *used.
+// The search never reads the output limit, so the sequences are the plain encoder's up to the cut (DESIGN 4.12).
+template <bool HARD = true, bool GTAB = false, int WIN = 32, bool FILL = false>
 __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint32_t n,
-                                uint8_t* __restrict__ dst, const int cap, const int hardCap, uint16_t* table) {
+                                uint8_t* __restrict__ dst, const int cap, const int hardCap, uint16_t* table,
+                                int32_t* used = nullptr) {
     const int lane = lane_id();
     const int64_t hard = hardCap;       // physical write bound (pickler, see pickle.cuh); 0x7fffffff otherwise
 #define RD32(p) ldg_u32u(src + (p))
@@ -77,7 +81,8 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint32_t 
         }
         __syncwarp();
     }
-    const bool limited = !(cap >= max_output_size((int)n));                           // LL64.fast.cs:524
+    const bool limited = !FILL && !(cap >= max_output_size((int)n));                  // LL64.fast.cs:524
+    const bool fill = FILL && !(cap >= max_output_size((int)n));                      // lz4.c:1387
     const int64_t olimit = cap;
     uint32_t ip = 0, anchor = 0, op = 0;
 
@@ -208,6 +213,10 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint32_t 
             // ---- step 5/6: literal run, offset, match length -----------------------------------------
             const uint32_t lit = ip - anchor;
             if (!zeroLit && limited && (int64_t)op + 1 + lit + 8 + lit / 255 > olimit) return 0;   // :246-251
+            // fill rules 1 and 2 (lz4.c:1028-1032, 1057-1062): token, literal run, offset and MFLIMIT - MINMATCH would
+            // pass the target.  (lit + 240) / 255 is the run header's extra bytes, so both tests read the same; the
+            // sequence is dropped before any byte of it is written and the rest goes to last literals.
+            if (fill && (int64_t)op + run_header_size(lit) + lit + 2 + 1 + (MFLIMIT - MINMATCH) > olimit) break;
             uint32_t mc = caught;
             {   // LZ4_count(ip+4, m+4, matchlimit), 4 bytes per lane, :328; the first round looks at 32 bytes
                 // (eight lanes: half of all matches end there and the other lanes' lines are not fetched)
@@ -232,6 +241,15 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint32_t 
             const uint32_t hdr = run_header_size(lit);
             const uint32_t afterOff = op + hdr + lit + 2;
             if (limited && (int64_t)afterOff + 6 + (mc + 240) / 255 > olimit) return 0;   // :332-362
+            // fill rule 3 (lz4.c:1097-1104): the match-length bytes would pass the target, so the match is shortened
+            // to what fits; op then ends at olimit - 6, where rules 1 and 2 stop every later sequence, so the block
+            // goes straight to last literals.  Upstream's hash clearing after the cut (:1105-1116) only matters to a
+            // table that is used again, and this one is not.
+            bool cut = false;
+            if (fill && (int64_t)afterOff + 6 + (mc + 240) / 255 > olimit) {
+                mc = 14u + (uint32_t)(olimit - afterOff - 6) * 255u;
+                cut = true;
+            }
             if (HARD && (int64_t)afterOff + (mc >= 15 ? (mc - 15) / 255 + 1 : 0) > hard) return 0;
             // emit: token, literal length bytes, literals, offset, match length bytes
             {
@@ -257,19 +275,24 @@ __device__ int encode_spec_warp(const uint8_t* __restrict__ src, const uint32_t 
             }
             ip += mc + MINMATCH;
             anchor = ip;                                                          // :388
-            if (ip >= mfl1) break;                                                // :391
+            if (ip >= mfl1 || cut) break;                                         // :391
             post = true; q0 = 0; base = ip + 1; width = WIN0;                     // step 8 rides with the next batch
         }
     }
     {   // ---- step 9: last literals, :469-503 -----------------------------------------------------------
-        const uint32_t run = n - anchor;
+        uint32_t run = n - anchor;
         if (limited && (int64_t)op + run + 1 + (run + 255 - 15) / 255 > olimit) return 0;
+        if (fill && (int64_t)op + run + 1 + (run + 255 - 15) / 255 > olimit) {     // fill rule 4, lz4.c:1209-1213
+            run = (uint32_t)(olimit - op) - 1;
+            run -= (run + 256 - 15) / 256;
+        }
         const uint32_t hdr = run_header_size(run);
         if (HARD && (int64_t)op + hdr + run > hard) return 0;
         if (lane == 0) write_run_header(dst, op, run);
         op += hdr;
         for (uint32_t i = lane; i < run; i += 32) dst[op + i] = RD8(anchor + i);
         op += run;
+        if (FILL && lane == 0) *used = (int32_t)(anchor + run);
         return (int)op;
     }
 #undef RD32
@@ -286,13 +309,16 @@ __device__ unsigned long long g_encode_stats[4];
 // the same counter and run concurrently: `encode_spec_kernel` keeps its 16 KiB hash table in shared
 // memory (ENC_SM_WARPS of them fill an SM), `encode_spec_gtab_kernel` keeps it in an L2-resident
 // workspace -- slower per block, but those warps use issue slots and registers the others leave idle.
-template <bool GTAB>
+// FILL: the destSize kernels (k4lz4_encode_dest_size_batch): dstCap is the target, outLen gets upstream's
+// LZ4_compress_destSize result and srcUsed the input bytes it consumed; no level, no 32-bit engine.
+template <bool GTAB, bool FILL = false>
 __device__ __forceinline__ void encode_persistent_warp(
         const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
         const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
         const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
         int32_t* __restrict__ outLen, const int nBlocks, int level,
-        uint32_t* __restrict__ nextBlock, uint16_t* const table, const int reserve) {
+        uint32_t* __restrict__ nextBlock, uint16_t* const table, const int reserve,
+        int32_t* __restrict__ srcUsed = nullptr) {
     const int lane = lane_id();
     const bool enforce32 = (level & ENC_FLAG_X32) != 0;   // LL.Enforce32 (LL.tools.cs:29): hash4 for the byU32 table
     level &= 0xFF;
@@ -309,13 +335,28 @@ __device__ __forceinline__ void encode_persistent_warp(
         const uint8_t* __restrict__ src = srcBase + srcOff[b];
         uint8_t* __restrict__ dst = dstBase + dstOff[b];
         const int cap = dstCap[b];
-        if (n_ <= 0) { if (lane == 0) outLen[b] = 0; continue; }
-        if (level >= 3) { if (lane == 0) outLen[b] = -2; continue; }
+        if (FILL) {
+            // nothing to encode: upstream's one-byte empty block where the target holds it (lz4.c:1263-1273), else
+            // nothing written and nothing consumed
+            if (n_ <= 0 || n_ > MAX_INPUT_SIZE || cap < 1) {
+                if (lane == 0) {
+                    const bool empty = n_ == 0 && cap >= 1;
+                    if (empty) dst[0] = 0;
+                    outLen[b] = empty ? 1 : 0;
+                    srcUsed[b] = 0;
+                }
+                continue;
+            }
+        } else {
+            if (n_ <= 0) { if (lane == 0) outLen[b] = 0; continue; }
+            if (level >= 3) { if (lane == 0) outLen[b] = -2; continue; }
+        }
         int r;
-        if (n_ >= LIMIT_64K) r = encode_block_warp(src, n_, dst, cap, 0x7fffffff, table, enforce32);
-        else r = encode_spec_warp<false, GTAB, K4_ENC_WIN>(src, (uint32_t)n_, dst, cap, 0x7fffffff, table);
+        if (n_ >= LIMIT_64K) r = encode_block_warp<FILL>(src, n_, dst, cap, 0x7fffffff, table, enforce32, srcUsed + b);
+        else r = encode_spec_warp<false, GTAB, K4_ENC_WIN, FILL>(src, (uint32_t)n_, dst, cap, 0x7fffffff, table,
+                                                                 srcUsed + b);
         if (lane == 0) {
-            outLen[b] = r <= 0 ? -1 : r;
+            outLen[b] = FILL ? r : (r <= 0 ? -1 : r);
             atomicAdd(&g_encode_stats[n_ >= LIMIT_64K ? 2 : (GTAB ? 1 : 0)], 1ull);
         }
         __syncwarp();
@@ -340,6 +381,30 @@ encode_spec_gtab_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __re
                         uint8_t* __restrict__ gtab, int reserve) {
     encode_persistent_warp<true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, level, nextBlock,
                                  reinterpret_cast<uint16_t*>(gtab + (size_t)blockIdx.x * ENC_GSLOT_BYTES), reserve);
+}
+
+// The destSize pair (k4lz4_encode_dest_size_batch): the two kernels above with the fill policy on, launched the same
+// way and pulling from one counter.  A block whose target reaches compressBound(n) runs the plain path.
+__global__ void __launch_bounds__(32)
+encode_fill_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
+                   const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
+                   const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+                   int32_t* __restrict__ outLen, int32_t* __restrict__ srcUsed, int nBlocks,
+                   uint32_t* __restrict__ nextBlock) {
+    extern __shared__ __align__(128) uint8_t smem_encf[];
+    encode_persistent_warp<false, true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, 0,
+                                        nextBlock, reinterpret_cast<uint16_t*>(smem_encf), 0, srcUsed);
+}
+
+__global__ void __launch_bounds__(32)
+encode_fill_gtab_kernel(const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ srcOff,
+                        const int32_t* __restrict__ srcLen, uint8_t* __restrict__ dstBase,
+                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
+                        int32_t* __restrict__ outLen, int32_t* __restrict__ srcUsed, int nBlocks,
+                        uint32_t* __restrict__ nextBlock, uint8_t* __restrict__ gtab, int reserve) {
+    encode_persistent_warp<true, true>(srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks, 0, nextBlock,
+                                       reinterpret_cast<uint16_t*>(gtab + (size_t)blockIdx.x * ENC_GSLOT_BYTES),
+                                       reserve, srcUsed);
 }
 
 }  // namespace k4

@@ -79,7 +79,7 @@ int device_count_cached() {
 
 enum Op {
     OP_ENCODE, OP_DECODE, OP_CHAIN, OP_GENERAL, OP_PICKLE, OP_PICKLEW, OP_UNPICKLE, OP_USIZE, OP_XXH32, OP_COPY,
-    OP_ENCCHAIN, OP_DSIZE, OP_ENCDICT
+    OP_ENCCHAIN, OP_DSIZE, OP_ENCDICT, OP_ENCFILL
 };
 
 // Block i reads srcBase[srcOff[i] .. +srcLen[i]) and writes dstBase[dstOff[i] .. +dstCap[i]) and outLen[i].
@@ -96,27 +96,29 @@ struct Batch {
     uint8_t* stateBase = nullptr; const int64_t* stateOff = nullptr;   // OP_ENCCHAIN: K4LZ4_CHAIN_STATE_BYTES per block
     bool partial = false;             // OP_GENERAL: PartialDecode semantics (dstCap = target length)
     uint32_t seed = 0;                // OP_XXH32
+    int32_t* srcUsed = nullptr;       // OP_ENCFILL: the source bytes each block's output holds
 };
 
 // The pointers each op needs when n > 0, besides srcBase / srcOff / srcLen.  A dictionary is optional
 // wherever it is read unless `dict` says otherwise: with dictBase set, dictOff and dictLen are required too.
-struct Needs { bool dst, cap, out, prefix, level, state, dict; };
+struct Needs { bool dst, cap, out, prefix, level, state, dict, used; };
 constexpr Needs NEEDS[] = {
-    /* OP_ENCODE   */ {true,  true,  true,  false, true,  false, false},
-    /* OP_DECODE   */ {true,  true,  true,  false, false, false, false},
-    /* OP_CHAIN    */ {true,  true,  true,  true,  false, false, false},
-    /* OP_GENERAL  */ {true,  true,  true,  false, false, false, false},
-    /* OP_PICKLE   */ {true,  false, true,  false, false, false, false},
-    /* OP_PICKLEW  */ {true,  false, true,  false, false, false, false},
-    /* OP_UNPICKLE */ {true,  true,  true,  false, false, false, false},
-    /* OP_USIZE    */ {false, false, true,  false, false, false, false},
-    /* OP_XXH32    */ {false, false, true,  false, false, false, false},
-    /* OP_COPY     */ {true,  false, false, false, false, false, false},
-    /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true,  false},
-    /* OP_DSIZE    */ {false, false, true,  false, false, false, false},
-    /* OP_ENCDICT  */ {true,  true,  true,  false, false, false, true},
+    /* OP_ENCODE   */ {true,  true,  true,  false, true,  false, false, false},
+    /* OP_DECODE   */ {true,  true,  true,  false, false, false, false, false},
+    /* OP_CHAIN    */ {true,  true,  true,  true,  false, false, false, false},
+    /* OP_GENERAL  */ {true,  true,  true,  false, false, false, false, false},
+    /* OP_PICKLE   */ {true,  false, true,  false, false, false, false, false},
+    /* OP_PICKLEW  */ {true,  false, true,  false, false, false, false, false},
+    /* OP_UNPICKLE */ {true,  true,  true,  false, false, false, false, false},
+    /* OP_USIZE    */ {false, false, true,  false, false, false, false, false},
+    /* OP_XXH32    */ {false, false, true,  false, false, false, false, false},
+    /* OP_COPY     */ {true,  false, false, false, false, false, false, false},
+    /* OP_ENCCHAIN */ {true,  true,  true,  true,  true,  true,  false, false},
+    /* OP_DSIZE    */ {false, false, true,  false, false, false, false, false},
+    /* OP_ENCDICT  */ {true,  true,  true,  false, false, false, true,  false},
+    /* OP_ENCFILL  */ {true,  true,  true,  false, false, false, false, true},
 };
-static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_ENCDICT + 1, "one row per op");
+static_assert(sizeof(NEEDS) / sizeof(NEEDS[0]) == OP_ENCFILL + 1, "one row per op");
 
 // The machine part of check(): a device must exist, an empty batch is then done (the caller returns OK for
 // n == 0), and `device` (K4LZ4_ALL_DEVICES or the current device when negative) must name a visible GPU.
@@ -136,7 +138,8 @@ int check(Op op, const Batch& b, int memKind, int device, bool missing = false) 
     if (b.n < 0 || b.n > INT32_MAX) return fail(K4LZ4_E_ARG, "bad block count %lld", (long long)b.n);
     if (b.n > 0 && (!b.srcBase || !b.srcOff || !b.srcLen || (w.out && !b.outLen) || (w.dst && (!b.dstBase || !b.dstOff)) ||
                     (w.cap && !b.dstCap) || (w.prefix && !b.prefixLen) || (b.dictBase && (!b.dictOff || !b.dictLen)) ||
-                    (w.state && (!b.stateBase || !b.stateOff)) || (w.dict && !b.dictBase) || missing))
+                    (w.state && (!b.stateBase || !b.stateOff)) || (w.dict && !b.dictBase) || (w.used && !b.srcUsed) ||
+                    missing))
         return fail(K4LZ4_E_ARG, "null pointer argument");
     if (w.prefix && memKind == K4LZ4_MEM_HOST)       // device arrays cannot be checked here: there a negative prefix gives -1
         for (int64_t i = 0; i < b.n; i++)
@@ -255,6 +258,8 @@ Dev* dev_state(int dev) {
         const int carve = (k4::ENC_SM_WARPS * (k4::ENC_TABLE_BYTES + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024);
         cudaFuncSetAttribute(k4::encode_spec_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
         cudaFuncSetAttribute(k4::encode_spec_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
+        cudaFuncSetAttribute(k4::encode_fill_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
+        cudaFuncSetAttribute(k4::encode_fill_gtab_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carve > 100 ? 100 : carve);
         cudaError_t e = cudaDeviceGetAttribute(&d->sms, cudaDevAttrMultiProcessorCount, dev);
         if (e == cudaSuccess)
             e = cudaFuncSetAttribute(k4::decode_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -293,7 +298,8 @@ Dev* dev_state(int dev) {
 // Enqueues the block encoder: a shared-memory-table kernel on `st` and, when the batch is big enough for
 // it to pay, a global-memory-table kernel on a helper stream that runs beside it (fork / join by events).
 // Both are persistent and pull blocks from one device counter.  The workspace (counter + the global
-// tables) comes from the private stream-ordered pool.
+// tables) comes from the private stream-ordered pool.  With a.srcUsed set it launches the destSize pair
+// (encode_fill_kernel / encode_fill_gtab_kernel) the same way.
 cudaError_t encode_launch(const Batch& a, int level, const Dev& D, cudaStream_t st, int* launches) {
     const int n = (int)a.n;
     const int wave = D.sms * k4::ENC_SM_WARPS;
@@ -319,16 +325,26 @@ cudaError_t encode_launch(const Batch& a, int level, const Dev& D, cudaStream_t 
         if (e == cudaSuccess) e = cudaEventRecord(fork, st);
         if (e == cudaSuccess) e = cudaStreamWaitEvent(hs, fork, 0);
         if (e == cudaSuccess) {
-            k4::encode_spec_gtab_kernel<<<gridG, 32, 0, hs>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
-                                                             a.dstCap, a.outLen, n, level, counter, ws + 256, wave);
+            if (a.srcUsed)
+                k4::encode_fill_gtab_kernel<<<gridG, 32, 0, hs>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
+                                                                 a.dstCap, a.outLen, a.srcUsed, n, counter, ws + 256,
+                                                                 wave);
+            else
+                k4::encode_spec_gtab_kernel<<<gridG, 32, 0, hs>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase, a.dstOff,
+                                                                 a.dstCap, a.outLen, n, level, counter, ws + 256, wave);
             e = cudaGetLastError();
             (*launches)++;
         }
         if (e == cudaSuccess) e = cudaEventRecord(join, hs);
     }
     if (e == cudaSuccess && gridS > 0) {
-        k4::encode_spec_kernel<<<gridS, 32, k4::ENC_TABLE_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
-                                                                       a.dstOff, a.dstCap, a.outLen, n, level, counter);
+        if (a.srcUsed)
+            k4::encode_fill_kernel<<<gridS, 32, k4::ENC_TABLE_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
+                                                                           a.dstOff, a.dstCap, a.outLen, a.srcUsed, n,
+                                                                           counter);
+        else
+            k4::encode_spec_kernel<<<gridS, 32, k4::ENC_TABLE_BYTES, st>>>(a.srcBase, a.srcOff, a.srcLen, a.dstBase,
+                                                                           a.dstOff, a.dstCap, a.outLen, n, level, counter);
         e = cudaGetLastError();
         (*launches)++;
     }
@@ -348,7 +364,8 @@ cudaError_t launch_op(Op op, const Batch& a, cudaStream_t st) {
     if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
     const int n = (int)a.n;
     switch (op) {
-    case OP_ENCODE: {
+    case OP_ENCODE:
+    case OP_ENCFILL: {     // OP_ENCFILL: a.srcUsed is set, so encode_launch picks the destSize kernels
         int nl = 0;
         const cudaError_t ee = encode_launch(a, a.level | (a.x32 ? k4::ENC_FLAG_X32 : 0), *D, st, &nl);
         g_launches += nl;
@@ -918,13 +935,17 @@ int run_staged(Op op, const Batch& b, int dev) {
     if (!D) return fail(K4LZ4_E_CUDA, "device %d: no state", dev);
     std::lock_guard<std::mutex> lk(D->stageMu);
     const bool dict = b.dictBase != nullptr, prefix = b.prefixLen != nullptr, dst = b.dstCap != nullptr;
-    const bool enc = op == OP_ENCCHAIN, edict = op == OP_ENCDICT;
+    const bool enc = op == OP_ENCCHAIN, edict = op == OP_ENCDICT, fill = op == OP_ENCFILL;
     constexpr int64_t SB = K4LZ4_CHAIN_STATE_BYTES;
     auto hist = [&](int64_t i) -> int32_t { return prefix ? std::min<int32_t>(b.prefixLen[i], 65535) : 0; };
     auto cap = [&](int64_t i) -> int64_t {      // the encoders never write more than compressBound(srcLen)
         const int64_t c = dst ? std::max<int32_t>(b.dstCap[i], 0) : 0;
+        if (fill) return std::min<int64_t>(c, b.srcLen[i] >= 0 ? k4::max_output_size(b.srcLen[i]) : 0);
         return enc || edict ? std::min<int64_t>(c, b.srcLen[i] > 0 ? k4::max_output_size(b.srcLen[i]) : 0) : c;
     };
+    // results per row: the length, and for the destSize encoder the source bytes consumed behind the lengths
+    const int64_t resInts = fill ? 2 : 1;
+    std::vector<int32_t> res;
     auto dlen = [&](int64_t i) -> int32_t {
         if (edict) return b.srcLen[i] > 0 ? k4::dict_kept(b.dictLen[i]) : 0;
         return dict ? std::max<int32_t>(b.dictLen[i], 0) : 0;
@@ -953,7 +974,7 @@ int run_staged(Op op, const Batch& b, int dev) {
         }
         const int64_t nb = j - i;
         StageUp up;
-        int rc = stage_up(D->stage, nb, 1, 0, [&](int64_t k) {
+        int rc = stage_up(D->stage, nb, resInts, 0, [&](int64_t k) {
             const int64_t x = i + k;
             const int32_t hl = hist(x);
             // the encoder's dictSize clamp needs the caller's prefixLen
@@ -973,9 +994,16 @@ int run_staged(Op op, const Batch& b, int dev) {
         kb.prefixLen = prefix ? up.aux : nullptr;
         kb.stateBase = enc ? up.blob : nullptr; kb.stateOff = up.blobOff;
         kb.outLen = up.res; kb.n = nb;
+        kb.srcUsed = fill ? up.res + nb : nullptr;
         CU_TRY(launch_op(op, kb, nullptr));
-        rc = stage_down(D->stage, up, nb, b.outLen + i, 1, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
+        res.resize((size_t)(nb * resInts));
+        int32_t* const hRes = fill ? res.data() : b.outLen + i;
+        rc = stage_down(D->stage, up, nb, hRes, resInts, dst ? up.dst : nullptr, up.dstOff, nullptr, nullptr);
         if (rc != K4LZ4_OK) return rc;
+        if (fill) {
+            std::copy(hRes, hRes + nb, b.outLen + i);
+            std::copy(hRes + nb, hRes + 2 * nb, b.srcUsed + i);
+        }
     }
     return K4LZ4_OK;
 }
@@ -1149,7 +1177,7 @@ int run(Op op, const Batch& b, int memKind, void* stream, int device) {
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     if (memKind == K4LZ4_MEM_HOST)
         return (op == OP_GENERAL || op == OP_CHAIN || op == OP_XXH32 || op == OP_ENCCHAIN || op == OP_DSIZE ||
-                op == OP_ENCDICT)
+                op == OP_ENCDICT || op == OP_ENCFILL)
                    ? run_staged(op, b, device < 0 ? 0 : device) : run_host(op, b, device);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
@@ -2479,6 +2507,31 @@ int32_t k4lz4_encode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, c
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
     return run(OP_ENCDICT, b, memKind, cudaStream, device);
+}
+
+int32_t k4lz4_encode_dest_size(const uint8_t* src, uint8_t* dst, int32_t* srcSize, int32_t targetDstSize) {
+    if (!srcSize) return fail(K4LZ4_E_ARG, "null pointer argument");
+    const int32_t n = *srcSize;
+    if (targetDstSize < 1 || n < 0 || n > k4::MAX_INPUT_SIZE) { *srcSize = 0; return 0; }   // nothing written
+    if (!dst || (!src && n > 0)) return fail(K4LZ4_E_ARG, "null pointer argument");
+    if (n == 0) { dst[0] = 0; return 1; }            // upstream's empty block (lz4.c:1263-1273); *srcSize stays 0
+    int64_t zero = 0;
+    int32_t out = 0, used = 0;
+    Batch b{src, &zero, &n, dst, &zero, &targetDstSize, &out, 1};
+    b.srcUsed = &used;
+    const int rc = run(OP_ENCFILL, b, K4LZ4_MEM_HOST, nullptr, 0);
+    if (rc != K4LZ4_OK) return rc;
+    *srcSize = used;
+    return out;
+}
+
+int32_t k4lz4_encode_dest_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                     uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                     int32_t* outLen, int32_t* srcUsed, int32_t nBlocks,
+                                     int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nBlocks};
+    b.srcUsed = srcUsed;
+    return run(OP_ENCFILL, b, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_decode_chain_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
