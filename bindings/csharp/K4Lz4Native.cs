@@ -156,6 +156,12 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_frame_info_batch(
             byte* srcBase, long* srcOff, int* srcLen, int* outSize, long* outDictId, int nFrames, int memKind,
             void* cudaStream, int device);
+        // LZ4 frames as upstream's LZ4F_compressFrame writes them (k4lz4.h "LZ4 Frame as upstream lz4 writes it")
+        public const int FRAME_CONTENT_SIZE = 8;
+        [DllImport(Lib)] public static extern long k4lz4_lz4f_compress_bound(long length, int blockSize, int flags);
+        [DllImport(Lib)] public static extern int k4lz4_lz4f_compress_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            int* outLen, int nFrames, int blockSize, int flags, int level, int memKind, void* cudaStream, int device);
         // LZ4EncoderStream / LZ4FrameWriter written incrementally, batched across streams (k4lz4.h "frame writer group")
         [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_create(
             int nStreams, int blockSize, int flags, int level, int device, void** group);

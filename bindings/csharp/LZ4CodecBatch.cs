@@ -67,6 +67,23 @@ namespace K4os.Compression.LZ4
                     K4Lz4Native.MEM_HOST, null, K4Lz4Native.ALL_DEVICES));
         }
 
+        // LZ4 frames as upstream's LZ4F_compressFrame writes them (k4lz4_lz4f_compress_batch; the reference has no
+        // such call): frame i holds source i; each frame's block size shrinks to fit it, a one-block frame is
+        // independent, and FRAME_CONTENT_SIZE writes the content size.  blockSize: 64 KiB, 256 KiB, 1 MiB or 4 MiB;
+        // flags: K4Lz4Native.FRAME_*; size targets with k4lz4_lz4f_compress_bound.  lengths[i]: the frame's length,
+        // -1 where it does not fit targetCapacities[i], K4Lz4Native.R_DELEGATE for HC levels.
+        public static void CompressFramesUpstream(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            Span<int> lengths, int blockSize = 65536, int flags = 0, LZ4Level level = LZ4Level.L00_FAST)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (int* ol = lengths)
+                Check(K4Lz4Native.k4lz4_lz4f_compress_batch(s, so, sl, d, dof, dc, ol, lengths.Length, blockSize,
+                    flags, (int)level, K4Lz4Native.MEM_HOST, null, 0));
+        }
+
         // LZ4 frames against a dictionary, as upstream's LZ4F_compressBegin_usingCDict writes them
         // (k4lz4_frame_encode_dict_batch): frame i holds source i, encoded against dictionary i, with the dictID
         // dictionaryIds[i] unless it is 0 (an empty span: no IDs).  blockSize: 64 KiB, 256 KiB, 1 MiB or 4 MiB; flags:

@@ -484,6 +484,39 @@ K4LZ4_API int32_t k4lz4_frame_info_batch(const uint8_t *srcBase, const int64_t *
                                          int32_t *outSize, int64_t *outDictId, int32_t nFrames,
                                          int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- LZ4 Frame as upstream lz4 writes it: LZ4F_compressFrame, batched across frames.  No reference call: the
+ * reference's writer has no content size and keeps the caller's block size (upstream liblz4, lz4 CLI, python-lz4). */
+
+/* Write the content-size field (FLG bit 3 + 8 bytes): LZ4F_preferences_t.frameInfo.contentSize != 0 */
+#define K4LZ4_FRAME_CONTENT_SIZE     8
+
+/* LZ4F_compressFrameBound(length, prefs) for prefs = {blockSizeID of blockSize, the checksums `flags` asks for}:
+ * 19 header bytes, per block 4 bytes of length code + at most the raw length (+ 4 with block checksums), the end
+ * mark (+ 4 with the content checksum).  blockSize must be 65 536, 262 144, 1 048 576 or 4 194 304; flags are
+ * K4LZ4_FRAME_INDEPENDENT, _BLOCK_CHECKSUM, _CONTENT_CHECKSUM and _CONTENT_SIZE.  A bad blockSize, a negative
+ * length or an unknown flag gives K4LZ4_E_ARG. */
+K4LZ4_API int64_t k4lz4_lz4f_compress_bound(int64_t length, int32_t blockSize, int32_t flags);
+
+/* LZ4F_compressFrame(dst, cap, src_i, n, prefs) per frame, byte for byte, with prefs = {blockSizeID of blockSize,
+ * linked unless K4LZ4_FRAME_INDEPENDENT, the checksums `flags` asks for, contentSize != 0 with
+ * K4LZ4_FRAME_CONTENT_SIZE, compressionLevel = level}.  As upstream decides each frame on its own size n
+ * (lz4frame.c:385-395), one call may mix modes and block sizes:
+ *   - the block size shrinks to the smallest of 64 KiB, 256 KiB and 1 MiB that holds n, up to blockSize;
+ *   - a frame of one block (n <= block size) is written independent;
+ *   - the content-size field is written only when asked for and n > 0.
+ * Every block is encoded with capacity n - 1 and stored raw (bit 31 of its length code) when that fails
+ * (lz4frame.c:747-749): independent blocks as LZ4_compress_fast, linked blocks as LZ4_compress_fast_continue on one
+ * fresh stream per frame.  There is no _x32 twin: this is upstream's call, not LZ4Codec's.
+ * Levels 0, 1 and 2 are acceleration 1, as upstream maps them; K4LZ4_R_DELEGATE for level >= 3 (HC) and for a
+ * negative level (acceleration > 1), nothing written.  outLen[i] = the frame's length; -1 when it does not fit
+ * dstCap[i] (upstream refuses any dstCap below LZ4F_compressFrameBound instead; here a frame is written whenever it
+ * fits).  Nothing is ever written at or beyond dstCap[i].  Argument errors, in order: blockSize and flags as
+ * k4lz4_lz4f_compress_bound, then as k4lz4_encode_batch (memKind, nFrames, null pointers, device). */
+K4LZ4_API int32_t k4lz4_lz4f_compress_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                            uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                            int32_t *outLen, int32_t nFrames, int32_t blockSize, int32_t flags,
+                                            int32_t level, int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- LZ4 Frame, written incrementally: LZ4EncoderStream / LZ4FrameWriter, batched across streams ------ */
 
 /*

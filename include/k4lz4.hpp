@@ -693,4 +693,49 @@ private:
     }
 };
 
+// Frames as upstream's LZ4F_compressFrame writes them (k4lz4_lz4f_compress_batch): each frame's block size shrinks
+// to fit it, a one-block frame is independent, contentSize writes the content-size field.  s.blockSize is 64 KiB,
+// 256 KiB, 1 MiB or 4 MiB; levels 0..2 (DelegateToManagedEngine for the others).
+struct LZ4F {
+    static int flags(const LZ4FrameSettings& s, bool contentSize) {
+        return LZ4Frame::flags(s) | (contentSize ? K4LZ4_FRAME_CONTENT_SIZE : 0);
+    }
+    static int64_t CompressFrameBound(int64_t length, const LZ4FrameSettings& s = {}, bool contentSize = false) {
+        const int64_t r = k4lz4_lz4f_compress_bound(length, s.blockSize, flags(s, contentSize));
+        if (r < 0) throw NativeError((int)r, k4lz4_last_error());
+        return r;
+    }
+    // frame i of the result holds sources[i]
+    static std::vector<std::vector<uint8_t>> CompressMany(const std::vector<std::vector<uint8_t>>& sources,
+                                                          const LZ4FrameSettings& s = {}, bool contentSize = false,
+                                                          int device = 0) {
+        const size_t n = sources.size();
+        std::vector<int64_t> so(n), dofs(n);
+        std::vector<int32_t> sl(n), dc(n), out(n, -1);
+        std::vector<uint8_t> src, dst;
+        int64_t d = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)sources[i].size();
+            src.insert(src.end(), sources[i].begin(), sources[i].end());
+            dofs[i] = d; dc[i] = (int32_t)CompressFrameBound(sl[i], s, contentSize); d += dc[i];
+        }
+        src.resize(src.size() + 1); dst.resize((size_t)d + 1);
+        const int rc = k4lz4_lz4f_compress_batch(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
+                                                 out.data(), (int32_t)n, s.blockSize, flags(s, contentSize),
+                                                 (int)s.level, K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        std::vector<std::vector<uint8_t>> frames(n);
+        for (size_t i = 0; i < n; i++) {
+            if (out[i] == K4LZ4_R_DELEGATE) throw DelegateToManagedEngine("LZ4F_compressFrame at this level stays managed");
+            if (out[i] < 0) throw std::runtime_error("ERROR_dstMaxSize_tooSmall");
+            frames[i].assign(dst.begin() + dofs[i], dst.begin() + dofs[i] + out[i]);
+        }
+        return frames;
+    }
+    static std::vector<uint8_t> CompressFrame(const std::vector<uint8_t>& source, const LZ4FrameSettings& s = {},
+                                              bool contentSize = false, int device = 0) {
+        return CompressMany({source}, s, contentSize, device)[0];
+    }
+};
+
 }  // namespace k4lz4

@@ -13,6 +13,7 @@ R_DELEGATE = -2
 R_CORRUPT = -1000
 R_DST_SMALL = -1001                       # K4LZ4_R_DST_SMALL (frame decode)
 FRAME_INDEPENDENT, FRAME_BLOCK_CHECKSUM, FRAME_CONTENT_CHECKSUM = 1, 2, 4
+FRAME_CONTENT_SIZE = 8                    # K4LZ4_FRAME_CONTENT_SIZE (k4lz4_lz4f_compress_batch)
 MEM_HOST, MEM_DEVICE = 0, 1
 ALL_DEVICES = -1
 CHAIN_STATE_BYTES = 16400                 # K4LZ4_CHAIN_STATE_BYTES
@@ -82,6 +83,8 @@ SIGNATURES = {
     "k4lz4_frame_encode_dict_batch": ([_vp] * 11 + [_i32] * 4 + _CALL, _i32),
     "k4lz4_frame_decode_dict_batch": ([_vp] * 10 + [_i32] + _CALL, _i32),
     "k4lz4_frame_info_batch": ([_vp] * 5 + [_i32] + _CALL, _i32),
+    "k4lz4_lz4f_compress_bound": ([_i64, _i32, _i32], _i64),
+    "k4lz4_lz4f_compress_batch": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
     "k4lz4_frame_writer_group_create": ([_i32, _i32, _i32, _i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_destroy": ([_vp], _i32),
     "k4lz4_frame_writer_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),

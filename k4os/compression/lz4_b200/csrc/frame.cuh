@@ -22,6 +22,7 @@ namespace k4 {
 constexpr uint32_t FRAME_MAGIC = 0x184D2204u;
 constexpr int FR_INDEPENDENT = 1, FR_BLOCK_SUM = 2, FR_CONTENT_SUM = 4;   // K4LZ4_FRAME_* (and the parsed FLG bits)
 constexpr int FR_DICT_ID = 8;                // parsed (dictionary calls): the header has a dictID field
+constexpr int FR_CONTENT_SIZE = 16;          // encode (k4lz4_lz4f_compress_batch): write the content size field
 constexpr int FR_CORRUPT = -1000, FR_DELEGATE = -2, FR_DST_SMALL = -1001;   // K4LZ4_R_*
 constexpr unsigned long long FK_NONE = ~0ull;
 constexpr int FK_TRUNC = 0, FK_SUM = 1, FK_RAW = 2, FK_BLOCK = 3;
@@ -664,6 +665,102 @@ frame_dict_first_kernel(int f0, const uint8_t* __restrict__ srcBase, const int64
         r = r <= 0 ? n0 : r;
     }
     if (lane == 0) res[x] = r;
+}
+
+// ---- upstream's LZ4F_compressFrame (k4lz4_lz4f_compress_batch) ----------------------------------------------
+// Per frame of n bytes (lz4frame.c:385-395): the block size shrinks to the smallest of 64 KiB, 256 KiB, 1 MiB that
+// holds n, up to the caller's (LZ4F_optimalBSID); a frame of one block (n <= block size) is independent; the content
+// size field is written when asked for and n > 0.  Every block is encoded with capacity n - 1 and stored raw when
+// that fails (frame_dict_cap_kernel / frame_dict_raw_kernel): independent blocks as LZ4_compress_fast, linked
+// blocks as LZ4_compress_fast_continue on one fresh stream.  A frame of more than one block keeps the caller's block
+// size, so every frame's blocks are bs bytes but its last.
+
+// Each frame is in one of two passes, and the existing encode kernels see it through the record of its pass:
+// fi, the independent view over all frames (frame_enc_place_kernel with k < 0; nb = 0 for a linked frame, first = its
+// first row of the compact table of independent blocks), and fl, the linked frames alone, compacted with their
+// destinations (lOff / lCap), so that the linked steps run over linked frames only.  A frame's layout and status live
+// in the record of its pass.
+// One thread per frame.  Pass 0: fr gets the frame's mode, block size and header length, nb its linked blocks and
+// nslot its independent blocks; fx.nb is 1 for a linked frame; the number of steps is the largest linked block count.
+// Pass 1, after frame_scan_kernel over fr (slots = 1: fr.first = first linked row, fr.slot = first independent row)
+// and over fx (fx.first = the linked frame's index in fl): the linked frames' rows in t, the independent frames' in
+// ti, fi, and fl / lOff / lCap.  `flags`: FR_* of the call plus FR_CONTENT_SIZE.
+__global__ void frame_lz4f_plan_kernel(int pass, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
+                                       const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap, int n,
+                                       int32_t bs, int flags, FrameRec* __restrict__ fr, FrameRec* __restrict__ fx,
+                                       FrameRec* __restrict__ fi, FrameRec* __restrict__ fl,
+                                       int64_t* __restrict__ lOff, int32_t* __restrict__ lCap, FrameTable t,
+                                       FrameTable ti, FrameTotals* __restrict__ tot) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t L = srcLen[i] > 0 ? srcLen[i] : 0;
+    const int nb = (int)((L + bs - 1) / bs);
+    if (pass == 0) {
+        FrameRec r = {};
+        int32_t size = 1 << 16;                          // LZ4F_optimalBSID
+        while (size < bs && L > size) size <<= 2;
+        const bool indep = (flags & FR_INDEPENDENT) || L <= size;
+        const bool cs = (flags & FR_CONTENT_SIZE) && L > 0;
+        r.flags = (indep ? FR_INDEPENDENT : 0) | (flags & (FR_BLOCK_SUM | FR_CONTENT_SUM)) | (cs ? FR_CONTENT_SIZE : 0);
+        r.maxBlock = size;
+        r.nb = indep ? 0 : nb; r.nslot = indep ? nb : 0; r.pos = cs ? 15 : 7; r.err = FK_NONE;
+        fr[i] = r;
+        fx[i].nb = indep ? 0 : 1;
+        if (!indep) atomicMax(&tot->maxSteps, nb);
+        return;
+    }
+    const FrameRec r = fr[i];
+    const bool indep = r.flags & FR_INDEPENDENT;
+    const int64_t first = indep ? r.slot : r.first;
+    int64_t* const rowOff = (indep ? ti.srcOff : t.srcOff) + first;
+    int32_t* const rowLen = (indep ? ti.len : t.len) + first;
+    for (int k = 0; k < nb; k++) {
+        rowOff[k] = srcOff[i] + (int64_t)k * bs;
+        rowLen[k] = (int32_t)((L - (int64_t)k * bs) < bs ? (L - (int64_t)k * bs) : bs);
+    }
+    FrameRec v = r;
+    v.first = r.slot; v.nb = r.nslot;
+    fi[i] = v;
+    if (!indep) {
+        const int64_t j = fx[i].first;
+        fl[j] = r; lOff[j] = dstOff[i]; lCap[j] = dstCap[i];
+    }
+}
+
+// One thread per frame: header (magic, FLG, BD of the frame's block size, the content size where the frame has
+// one, HC over FLG .. content size), end mark, content checksum, result.
+__global__ void frame_lz4f_finish_kernel(const FrameRec* __restrict__ fx, const FrameRec* __restrict__ fi,
+                                         const FrameRec* __restrict__ fl, int n, const int32_t* __restrict__ srcLen,
+                                         uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff,
+                                         const int32_t* __restrict__ dstCap, const uint32_t* __restrict__ csum,
+                                         int32_t* __restrict__ outLen) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FrameRec& r = (fi[i].flags & FR_INDEPENDENT) ? fi[i] : fl[fx[i].first];
+    const bool cc = r.flags & FR_CONTENT_SUM, cs = r.flags & FR_CONTENT_SIZE;
+    const int64_t total = r.pos + 4 + (cc ? 4 : 0);
+    if (r.status || total > (dstCap[i] > 0 ? dstCap[i] : 0) || total > 0x7FFFFFFF) { outLen[i] = -1; return; }
+    const int code = r.maxBlock == (1 << 16) ? 4 : r.maxBlock == (1 << 18) ? 5 : r.maxBlock == (1 << 20) ? 6 : 7;
+    uint8_t h[10];
+    h[0] = (uint8_t)((1 << 6) | ((r.flags & FR_INDEPENDENT) ? 1 << 5 : 0) | ((r.flags & FR_BLOCK_SUM) ? 1 << 4 : 0) |
+                     (cs ? 1 << 3 : 0) | (cc ? 1 << 2 : 0));
+    h[1] = (uint8_t)(code << 4);
+    const uint64_t size = (uint64_t)(srcLen[i] > 0 ? srcLen[i] : 0);
+#pragma unroll
+    for (int j = 0; j < 8; j++) h[2 + j] = (uint8_t)(size >> (8 * j));
+    uint8_t* d = dstBase + dstOff[i];
+    fr_wr32(d, FRAME_MAGIC);
+    if (cs) {                                        // constant lengths: h stays in registers
+#pragma unroll
+        for (int j = 0; j < 10; j++) d[4 + j] = h[j];
+        d[14] = (uint8_t)(xx_finish(XXP5 + 10u, h, 10) >> 8);
+    } else {
+        d[4] = h[0]; d[5] = h[1];
+        d[6] = (uint8_t)(xx_finish(XXP5 + 2u, h, 2) >> 8);
+    }
+    fr_wr32(d + r.pos, 0);
+    if (cc) fr_wr32(d + r.pos + 4, csum[i]);
+    outLen[i] = (int32_t)total;
 }
 
 // off[x] = x * stride and, when cap is given, cap[x] = capValue: the fixed slots of a launch.

@@ -1414,9 +1414,11 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
 // Encode b.n frames in device memory on `st` (level < 3): plan, scan, one host synchronisation for the block and
 // step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of at most
 // FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.  With fd: against
-// the Batch's dictionaries, upstream's CDict frames (frame.cuh, "dictionary encode").
+// the Batch's dictionaries, upstream's CDict frames (frame.cuh, "dictionary encode").  With up: upstream's
+// LZ4F_compressFrame (frame.cuh, "upstream's LZ4F_compressFrame"), each frame independent or linked by its own size,
+// so one call may run both passes; `flags` may then carry FR_CONTENT_SIZE.
 cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
-                             const FrameDict* fd = nullptr) {
+                             const FrameDict* fd = nullptr, bool up = false) {
     int dev = 0;
     cudaGetDevice(&dev);
     const Dev* D = dev_state(dev);
@@ -1425,24 +1427,53 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
     const bool bc = flags & K4LZ4_FRAME_BLOCK_CHECKSUM, cc = flags & K4LZ4_FRAME_CONTENT_CHECKSUM;
     FramePool P(D->pool, st);
     k4::FrameRec* fr = P.get<k4::FrameRec>(n);
-    k4::FrameTotals* tot = P.get<k4::FrameTotals>(1);
+    // up (frame_lz4f_plan_kernel): fx numbers the linked frames, fi is the independent view, fl the linked frames
+    // alone with their destinations lOff / lCap; otherwise all three are fr and the caller's destinations
+    k4::FrameRec* fx = up ? P.get<k4::FrameRec>(n) : fr;
+    k4::FrameRec* fi = up ? P.get<k4::FrameRec>(n) : fr;
+    k4::FrameTotals* tot = P.get<k4::FrameTotals>(2);
     FR_TRY(P.err);
-    FR_TRY(cudaMemsetAsync(tot, 0, sizeof(k4::FrameTotals), st));
-    k4::FrameTable t{};
-    k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(0, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+    FR_TRY(cudaMemsetAsync(tot, 0, 2 * sizeof(k4::FrameTotals), st));
+    k4::FrameTable t{}, ti{};
+    k4::FrameRec* fl = fr;
+    int64_t* flOff = nullptr;
+    int32_t* flCap = nullptr;
+    auto plan = [&](int pass) {
+        if (up)
+            k4::frame_lz4f_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, b.srcOff, b.srcLen, b.dstOff, b.dstCap, n, bs,
+                                                                  flags, fr, fx, fi, fl, flOff, flCap, t, ti, tot);
+        else k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+    };
+    plan(0);
     FR_LAUNCH();
-    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, 0);
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, up ? 1 : 0);
     FR_LAUNCH();
     g_launches += 2;
-    k4::FrameTotals h{};
-    FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    if (up) {
+        k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fx, n, tot + 1, 0);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    k4::FrameTotals h[2] = {};
+    FR_TRY(cudaMemcpyAsync(h, tot, (up ? 2 : 1) * sizeof(k4::FrameTotals), cudaMemcpyDeviceToHost, st));
     FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size and the number of steps
-    const int64_t nB = h.blocks;
+    const int64_t nB = h[0].blocks;
+    const bool linked = up ? h[0].maxSteps > 0 : !(flags & K4LZ4_FRAME_INDEPENDENT);
+    const int64_t nI = up ? h[0].slots : linked ? 0 : nB;    // blocks of the independent pass (up: in ti, nB in t)
+    const int64_t nL = up ? h[1].blocks : n;                  // frames of the linked pass
     t.srcOff = P.get<int64_t>(nB);
     t.len = P.get<int32_t>(nB);
+    if (up) {
+        ti.srcOff = P.get<int64_t>(nI); ti.len = P.get<int32_t>(nI);
+        fl = P.get<k4::FrameRec>(nL); flOff = P.get<int64_t>(nL); flCap = P.get<int32_t>(nL);
+    } else {
+        ti = t;
+    }
+    const int64_t* lOff = up ? flOff : b.dstOff;
+    const int32_t* lCap = up ? flCap : b.dstCap;
     uint32_t* csum = P.get<uint32_t>(n);
     FR_TRY(P.err);
-    k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(1, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+    plan(1);
     FR_LAUNCH();
     g_launches++;
     int64_t* rowDictOff = nullptr;
@@ -1469,11 +1500,11 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
         return cudaSuccess;
     };
     if (cc) FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, b.srcOff, b.srcLen, nullptr, nullptr, nullptr, (int32_t*)csum, n}, st));
+    const bool capm1 = fd || up;                       // capacity n - 1, raw where that fails (lz4frame.c:747-749)
     const int32_t bound = k4::max_output_size(bs);
-    const bool linked = !(flags & K4LZ4_FRAME_INDEPENDENT);
     const int64_t per = std::max<int64_t>(FRAME_SCRATCH / bound, 1);
-    const int64_t E = std::max<int64_t>(std::min<int64_t>(per, linked ? n : nB), 1);
-    if (nB > 0) {
+    const int64_t E = std::max<int64_t>(std::min<int64_t>(per, std::max<int64_t>(linked ? nL : 0, nI)), 1);
+    if (nB > 0 || nI > 0) {
         uint8_t* scratch = P.get<uint8_t>(E * bound);
         int64_t* eDst = P.get<int64_t>(E);
         int32_t* eCap = P.get<int32_t>(E);
@@ -1487,8 +1518,9 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
         g_launches++;
         // the bodies into place, then the block checksums over them
         auto place = [&](int k, int64_t b0, int64_t b1, int f0, int f1, int64_t m) -> cudaError_t {
-            k4::frame_enc_place_kernel<<<grid_of(f1 - f0), 128, 0, st>>>(k, b0, b1, f0, f1, fr, t, e, b.dstBase, b.dstOff,
-                                                                         b.dstCap, bound, bc ? 1 : 0);
+            k4::frame_enc_place_kernel<<<grid_of(f1 - f0), 128, 0, st>>>(k, b0, b1, f0, f1, k < 0 ? fi : fl, k < 0 ? ti : t,
+                                                                         e, b.dstBase, k < 0 ? b.dstOff : lOff,
+                                                                         k < 0 ? b.dstCap : lCap, bound, bc ? 1 : 0);
             FR_LAUNCH();
             g_launches++;
             const int mm = (int)m;
@@ -1502,21 +1534,20 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
             }
             return cudaSuccess;
         };
-        if (!linked) {
-            for (int64_t b0 = 0; b0 < nB; b0 += E) {
-                const int64_t m = std::min<int64_t>(E, nB - b0);
-                Batch kb{b.srcBase, t.srcOff + b0, t.len + b0, scratch, eDst, eCap, e.res, m, b.level, b.x32};
-                if (fd) {
-                    FR_TRY(dict_cap(t.len + b0, eCap, m));
-                    kb.dictBase = b.dictBase; kb.dictOff = rowDictOff + b0; kb.dictLen = rowDictLen + b0;
-                    FR_TRY(launch_op(OP_ENCDICT, kb, st));
-                    FR_TRY(dict_raw(t.len + b0, e.res, m));
-                } else {
-                    FR_TRY(launch_op(OP_ENCODE, kb, st));
-                }
-                FR_TRY(place(-1, b0, b0 + m, 0, n, m));
+        for (int64_t b0 = 0; b0 < nI; b0 += E) {
+            const int64_t m = std::min<int64_t>(E, nI - b0);
+            Batch kb{b.srcBase, ti.srcOff + b0, ti.len + b0, scratch, eDst, eCap, e.res, m, b.level, b.x32};
+            if (capm1) FR_TRY(dict_cap(ti.len + b0, eCap, m));
+            if (fd) {
+                kb.dictBase = b.dictBase; kb.dictOff = rowDictOff + b0; kb.dictLen = rowDictLen + b0;
+                FR_TRY(launch_op(OP_ENCDICT, kb, st));
+            } else {
+                FR_TRY(launch_op(OP_ENCODE, kb, st));
             }
-        } else {
+            if (capm1) FR_TRY(dict_raw(ti.len + b0, e.res, m));
+            FR_TRY(place(-1, b0, b0 + m, 0, n, m));
+        }
+        if (linked) {
             uint8_t* state = P.get<uint8_t>(E * K4LZ4_CHAIN_STATE_BYTES);
             int64_t* stOff = P.get<int64_t>(E);
             int64_t* so = P.get<int64_t>(E);
@@ -1526,12 +1557,12 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
             k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(stOff, nullptr, (int)E, K4LZ4_CHAIN_STATE_BYTES, 0);
             FR_LAUNCH();
             g_launches++;
-            for (int f0 = 0; f0 < n; f0 += (int)E) {
-                const int m = (int)std::min<int64_t>(E, n - f0);
+            for (int f0 = 0; f0 < nL; f0 += (int)E) {
+                const int m = (int)std::min<int64_t>(E, nL - f0);
                 // with dictionaries, step 0 loads each frame's state record from its dictionary
                 if (!fd) FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
-                for (int k = 0; k < h.maxSteps; k++) {
-                    k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fr, t, so, sl, pre, bs);
+                for (int k = 0; k < h[0].maxSteps; k++) {
+                    k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fl, t, so, sl, pre, bs);
                     FR_LAUNCH();
                     g_launches++;
                     if (fd && k == 0) {
@@ -1543,16 +1574,19 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
                     } else {
                         Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level, b.x32};
                         kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
-                        if (fd) FR_TRY(dict_cap(sl, eCap, m));
+                        if (capm1) FR_TRY(dict_cap(sl, eCap, m));
                         FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
-                        if (fd) FR_TRY(dict_raw(sl, e.res, m));
+                        if (capm1) FR_TRY(dict_raw(sl, e.res, m));
                     }
                     FR_TRY(place(k, 0, 0, f0, f0 + m, m));
                 }
             }
         }
     }
-    if (fd)
+    if (up)
+        k4::frame_lz4f_finish_kernel<<<grid_of(n), 128, 0, st>>>(fx, fi, fl, n, b.srcLen, b.dstBase, b.dstOff,
+                                                                b.dstCap, csum, b.outLen);
+    else if (fd)
         k4::frame_enc_finish_dict_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header,
                                                                     cc ? 1 : 0, csum, b.outLen, fd->id);
     else
@@ -1563,14 +1597,30 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
     return cudaSuccess;
 }
 
-enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE };
+// FO_LZ4F: upstream's LZ4F_compressFrame (k4lz4_lz4f_compress_batch), an encode.
+enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE, FO_LZ4F };
+inline bool frame_encodes(FrameOp fo) { return fo == FO_ENCODE || fo == FO_LZ4F; }
+
+constexpr int LZ4F_FLAGS = FRAME_FLAGS | K4LZ4_FRAME_CONTENT_SIZE;
+
+// LZ4F_compressFrameBound (lz4frame.c:324-361) for a block size of 64 KiB .. 4 MiB: the 19-byte largest header,
+// per block 4 bytes of length code (+ 4 with block checksums) and at most the raw length, the end mark (+ 4).
+int64_t lz4f_bound_of(int64_t length, int32_t bs, int flags) {
+    const int64_t nb = length / bs + (length % bs ? 1 : 0);
+    return 19 + nb * (4 + ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 4 : 0)) + length + 4 +
+           ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 4 : 0);
+}
 
 cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
                       const FrameDict* fd) {
-    if (fo == FO_ENCODE && b.level >= 3) {
+    if (frame_encodes(fo) && b.level >= 3) {
         k4::frame_fill_kernel<<<grid_of(b.n), 128, 0, st>>>(b.outLen, (int)b.n, K4LZ4_R_DELEGATE);
         g_launches++;
         return cudaGetLastError();
+    }
+    if (fo == FO_LZ4F) {
+        const int f = (flags & FRAME_FLAGS) | ((flags & K4LZ4_FRAME_CONTENT_SIZE) ? k4::FR_CONTENT_SIZE : 0);
+        return frame_encode_dev(b, bs, f, 0, st, nullptr, true);
     }
     return fo == FO_ENCODE ? frame_encode_dev(b, bs, flags, header, st, fd) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
 }
@@ -1584,7 +1634,7 @@ cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_
 int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev, const FrameDict* fd) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
-    if (fo == FO_ENCODE && b.level >= 3) {
+    if (frame_encodes(fo) && b.level >= 3) {
         for (int64_t i = 0; i < b.n; i++) b.outLen[i] = K4LZ4_R_DELEGATE;
         return K4LZ4_OK;
     }
@@ -1597,6 +1647,7 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
         if (!dst) return 0;
         const int64_t c = std::max<int32_t>(b.dstCap[i], 0);
         const int64_t idRoom = fd && fd->id && fd->id[i] ? 4 : 0;
+        if (fo == FO_LZ4F) return std::min<int64_t>(c, lz4f_bound_of(src_size(b, i), bs, flags));
         return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags) + idRoom) : c;
     };
     const bool dict = fd && b.dictBase;
@@ -1663,7 +1714,12 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
 int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memKind, void* stream, int device,
               const FrameDict* fd = nullptr) {
     int32_t bs = 0;
-    if (fo == FO_ENCODE) {
+    if (fo == FO_LZ4F) {
+        if (blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22))
+            return fail(K4LZ4_E_ARG, "bad frame block size %d (64 KiB, 256 KiB, 1 MiB or 4 MiB)", blockSize);
+        if (flags & ~LZ4F_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
+        bs = blockSize;
+    } else if (fo == FO_ENCODE) {
         bs = frame_block_size(blockSize);
         if (fd && blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22))
             bs = 0;
@@ -1672,7 +1728,7 @@ int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memK
         if (flags & ~FRAME_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
     }
     const bool missing = fd && (fo == FO_ENCODE ? !b.dictBase : fo == FO_SIZE ? !fd->outId : false);
-    const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
+    const int rc = check(frame_encodes(fo) ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     const uint64_t header = fo == FO_ENCODE ? frame_header(blockSize, flags) : 0;
     if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, bs, flags, header, device < 0 ? 0 : device, fd);
@@ -2826,6 +2882,22 @@ int32_t k4lz4_frame_encode_batch_x32(const uint8_t* srcBase, const int64_t* srcO
                                      int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level, true};
     return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
+}
+
+int64_t k4lz4_lz4f_compress_bound(int64_t length, int32_t blockSize, int32_t flags) {
+    if ((blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22)) ||
+        length < 0 || (flags & ~LZ4F_FLAGS))
+        return fail(K4LZ4_E_ARG, "bad LZ4F bound arguments");
+    return lz4f_bound_of(length, blockSize, flags);
+}
+
+int32_t k4lz4_lz4f_compress_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                  uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
+                                  int32_t nFrames, int32_t blockSize, int32_t flags, int32_t level, int32_t memKind,
+                                  void* cudaStream, int32_t device) {
+    // levels 0..2 are acceleration 1 (lz4frame.c:768,779); HC levels and accelerations (negative levels) delegate
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level < 0 || level >= 3 ? 3 : level};
+    return frame_run(FO_LZ4F, b, blockSize, flags, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_content_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,

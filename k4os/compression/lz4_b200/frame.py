@@ -264,6 +264,71 @@ class LZ4Frame:
                                                N.MEM_DEVICE, stream or None, int(device)))
 
 
+class LZ4F:
+    """Frames as upstream lz4 writes them (k4lz4_lz4f_compress_batch): LZ4F_compressFrame byte for byte, many frames
+    per call.  Unlike LZ4Frame, each frame's block size shrinks to fit small contents, a one-block frame is written
+    independent, every block is encoded with capacity n - 1 and stored raw when that fails, and the content size can
+    be written (content_size=True, as python-lz4's store_size).  block_size is 64 KiB, 256 KiB, 1 MiB or 4 MiB;
+    level 0..2 (acceleration 1).  The reference has no such call: it is liblz4's, the lz4 CLI's and python-lz4's."""
+
+    BLOCK_SIZES = (1 << 16, 1 << 18, 1 << 20, 1 << 22)
+
+    @staticmethod
+    def flags(linked: bool = True, block_checksum: bool = False, content_checksum: bool = False,
+              content_size: bool = False) -> int:
+        return _flags(linked, block_checksum, content_checksum) | (N.FRAME_CONTENT_SIZE if content_size else 0)
+
+    @staticmethod
+    def bound(length: int, block_size: int = 65536, linked: bool = True, block_checksum: bool = False,
+              content_checksum: bool = False, content_size: bool = False) -> int:
+        """LZ4F_compressFrameBound for these preferences."""
+        r = int(N.lib().k4lz4_lz4f_compress_bound(int(length), int(block_size),
+                                                   LZ4F.flags(linked, block_checksum, content_checksum, content_size)))
+        if r < 0:
+            N.check(r)
+        return r
+
+    @staticmethod
+    def compress_many(datas, block_size: int = 65536, linked: bool = True, block_checksum: bool = False,
+                      content_checksum: bool = False, content_size: bool = False, level: int = 0, device: int = 0):
+        """-> (list of frames, int32 results): the frame's length, or K4LZ4_R_DELEGATE for level >= 3 or < 0."""
+        src, so, sl = _pack([_u8(d) for d in datas])
+        fl = LZ4F.flags(linked, block_checksum, content_checksum, content_size)
+        caps = [LZ4F.bound(int(x), block_size, linked, block_checksum, content_checksum, content_size) for x in sl]
+        dst, do, dc = _slots(caps)
+        out = np.full(len(sl), -1, dtype=np.int32)
+        N.check(N.lib().k4lz4_lz4f_compress_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data,
+                                                  do.ctypes.data, dc.ctypes.data, out.ctypes.data, len(sl),
+                                                  int(block_size), fl, int(level), N.MEM_HOST, None, int(device)))
+        return _slices(dst, do, out), out
+
+    @staticmethod
+    def compress_many_device(src, src_off, src_len, dst, dst_off, dst_cap, out_len, block_size: int = 65536,
+                             linked: bool = True, block_checksum: bool = False, content_checksum: bool = False,
+                             content_size: bool = False, level: int = 0, stream: int = 0, device: int = -1) -> None:
+        """Torch tensors on the GPU (uint8 data, int64 offsets, int32 lengths and results); only enqueues work on
+        `stream`, after one wait for the block and step counts."""
+        N.check(N.lib().k4lz4_lz4f_compress_batch(
+            src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(), dst.data_ptr(), dst_off.data_ptr(),
+            dst_cap.data_ptr(), out_len.data_ptr(), int(src_len.numel()), int(block_size),
+            LZ4F.flags(linked, block_checksum, content_checksum, content_size), int(level), N.MEM_DEVICE,
+            stream or None, int(device)))
+
+
+def lz4f_compress(data, block_size: int = 65536, linked: bool = True, block_checksum: bool = False,
+                  content_checksum: bool = False, content_size: bool = False, level: int = 0,
+                  device: int = 0) -> bytes:
+    """One frame, as LZ4F_compressFrame writes it.  Raises NotImplementedError for HC levels (>= 3) and
+    accelerations (< 0), which this library does not encode."""
+    frames, out = LZ4F.compress_many([data], block_size, linked, block_checksum, content_checksum, content_size,
+                                     level, device)
+    if int(out[0]) == N.R_DELEGATE:
+        raise NotImplementedError(f"LZ4F_compressFrame at level {level} is not implemented")
+    if int(out[0]) < 0:
+        raise RuntimeError("ERROR_dstMaxSize_tooSmall")
+    return frames[0]
+
+
 def write_frames(datas, block_size: int = 65536, block_checksum: bool = False, content_checksum: bool = False,
                  level: int = 0, device: int = 0, chaining: bool = True) -> list:
     """Many LZ4 frames, one per item of `datas` (LZ4FrameWriter with the default Chaining = true, L00_FAST), in one
