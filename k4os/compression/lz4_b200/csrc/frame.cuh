@@ -21,8 +21,8 @@ namespace k4 {
 
 constexpr uint32_t FRAME_MAGIC = 0x184D2204u;
 constexpr int FR_INDEPENDENT = 1, FR_BLOCK_SUM = 2, FR_CONTENT_SUM = 4;   // K4LZ4_FRAME_* (and the parsed FLG bits)
-constexpr int FR_DICT_ID = 8;                // parsed (dictionary calls): the header has a dictID field
-constexpr int FR_CONTENT_SIZE = 16;          // encode (k4lz4_lz4f_compress_batch): write the content size field
+constexpr int FR_DICT_ID = 8;                // the header has a dictID field
+constexpr int FR_CONTENT_SIZE = 16;          // the header has a content size field
 constexpr int FR_CORRUPT = -1000, FR_DELEGATE = -2, FR_DST_SMALL = -1001;   // K4LZ4_R_*
 constexpr unsigned long long FK_NONE = ~0ull;
 constexpr int FK_TRUNC = 0, FK_SUM = 1, FK_RAW = 2, FK_BLOCK = 3;
@@ -33,17 +33,17 @@ constexpr int RK_RAW = 1, RK_SCRATCH = 2, RK_SKIP = 4, RK_LINKED = 8;
 
 struct FrameRec {            // per frame, on the device
     int64_t first;           // first row of the frame in the block table
-    int64_t slot;            // decode: first scratch slot
+    int64_t slot;            // decode: first scratch slot; encode: first independent row
     int64_t pos;             // decode: content size (sum of the walks); encode: bytes laid out so far
     unsigned long long err;  // decode: smallest error key
-    int32_t nb;              // decode: complete blocks; encode: blocks
-    int32_t nslot;           // decode: scratch slots
+    int32_t nb;              // decode: complete blocks; encode: linked blocks (the independent view: its blocks)
+    int32_t nslot;           // decode: scratch slots; encode: independent blocks
     int32_t status;          // 0, or the frame's verdict before any block (R_CORRUPT / R_DELEGATE); encode: -1
-    int32_t flags;           // FR_* as parsed (decode)
-    int32_t maxBlock;        // BD maximum
+    int32_t flags;           // FR_* as parsed (decode) or written (encode)
+    int32_t maxBlock;        // BD maximum (encode: the block size BD declares)
     int32_t k0;              // decode: first block that may need a scratch slot
     uint32_t expect;         // decode: stored content checksum
-    uint32_t dictId;         // decode (dictionary calls): the header's dictID
+    uint32_t dictId;         // the header's dictID (decode: dictionary calls)
 };
 
 struct FrameTotals { int64_t blocks, slots; int32_t maxSteps, maxCap; };
@@ -58,7 +58,7 @@ struct FrameTable {
     int32_t* size;           // decoded length (the walk) or the raw length
     int64_t* fin;            // final position, relative to dstBase
     int64_t* dst;            // where the block is decoded, relative to dstBase (in place or a scratch slot)
-    int32_t* cap;            // the reference's capacity
+    int32_t* cap;            // the reference's capacity (encode: the encoder's)
     int32_t* ilen;           // OP_DECODE source length (independent compressed blocks; 0 elsewhere)
     int32_t* res;            // decoder result
     int32_t* ckLen;          // bytes to checksum (block checksums on)
@@ -71,7 +71,7 @@ constexpr int64_t FRAME_ROW_BYTES = 8 * 5 + 4 * 11;
 __device__ __forceinline__ uint32_t fr_rd32(const uint8_t* p) {
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
-__device__ __forceinline__ void fr_wr32(uint8_t* p, uint32_t v) {
+__host__ __device__ __forceinline__ void fr_wr32(uint8_t* p, uint32_t v) {
     p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
 }
 __host__ __device__ inline int32_t frame_max_block(int code) {   // LZ4FrameReader.cs:55-59
@@ -466,27 +466,106 @@ __global__ void frame_info_kernel(const FrameRec* __restrict__ fr, int n, int64_
 }
 
 // ---- encode ---------------------------------------------------------------------------------------------------
+// The kinds of frame an encode writes differ only in the data of their FrameFormat: the reference's LZ4FrameWriter
+// (k4lz4_frame_encode_batch), upstream's CDict frames (k4lz4_frame_encode_dict_batch: independent blocks each start
+// from LZ4_loadDict of the frame's dictionary, OP_ENCDICT; linked frames load it once, in front of block 0,
+// frame_dict_first_kernel) and upstream's LZ4F_compressFrame (k4lz4_lz4f_compress_batch).
 
-// One thread per frame.  Pass 0: block counts (and the number of steps).  Pass 1: the rows (source offset and
-// length of every block; in FrameTable's srcOff / len) and the frame's starting layout.
-__global__ void frame_enc_plan_kernel(int pass, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
-                                      int n, int32_t bs, FrameRec* __restrict__ fr, FrameTable t,
-                                      FrameTotals* __restrict__ tot) {
+// One encode call's frames, filled once per call by the host.
+struct FrameFormat {
+    int32_t bs;              // encoder block size: every block of a frame is bs bytes but its last
+    int32_t bdSize;          // the block size BD declares (LZ4FrameWriter.cs:183-188: the caller's, not rounded)
+    int32_t flags;           // FR_INDEPENDENT, FR_BLOCK_SUM, FR_CONTENT_SUM and FR_CONTENT_SIZE of the call (an
+                             // empty frame gets no content size field, as upstream writes it)
+    int32_t upstream;        // upstream's rule (lz4frame.c:385-395): BD shrinks to the smallest of 64 KiB, 256 KiB,
+                             // 1 MiB that holds the frame, up to bdSize (LZ4F_optimalBSID), and a frame of one block
+                             // is independent; its blocks stay bs bytes
+    int32_t rawFallback;     // every block is encoded with capacity n - 1 and stored raw when that fails
+                             // (lz4frame.c:747-749); otherwise with the bound, and a block that fails fails the frame
+    int32_t dict;            // the blocks encode against the Batch's dictionaries, which the call requires
+    const uint32_t* dictId;  // per frame, the dictID its header carries (0: none); null: none
+};
+
+// The frame header at d: magic, FLG, BD (the code of bdSize), the content size with FR_CONTENT_SIZE, the dictID
+// with FR_DICT_ID, and HC over FLG .. dictID.  -> its length.
+__host__ __device__ inline int frame_put_header(uint8_t* d, int flags, int32_t bdSize, uint64_t contentSize,
+                                                uint32_t dictId) {
+    fr_wr32(d, FRAME_MAGIC);
+    d[4] = (uint8_t)((1 << 6) | ((flags & FR_INDEPENDENT) ? 1 << 5 : 0) | ((flags & FR_BLOCK_SUM) ? 1 << 4 : 0) |
+                     ((flags & FR_CONTENT_SIZE) ? 1 << 3 : 0) | ((flags & FR_CONTENT_SUM) ? 1 << 2 : 0) |
+                     ((flags & FR_DICT_ID) ? 1 : 0));
+    d[5] = (uint8_t)((bdSize <= (1 << 16) ? 4 : bdSize <= (1 << 18) ? 5 : bdSize <= (1 << 20) ? 6 : 7) << 4);
+    int p = 6;
+    if (flags & FR_CONTENT_SIZE) {
+        fr_wr32(d + p, (uint32_t)contentSize); fr_wr32(d + p + 4, (uint32_t)(contentSize >> 32));
+        p += 8;
+    }
+    if (flags & FR_DICT_ID) { fr_wr32(d + p, dictId); p += 4; }
+    d[p] = (uint8_t)(xx_finish(XXP5 + (uint32_t)(p - 4), d + 4, (size_t)(p - 4)) >> 8);
+    return p + 1;
+}
+
+// One thread per frame.  Pass 0: the frame's record in fr -- mode (FR_INDEPENDENT), BD size (maxBlock), dictID, the
+// header's length (pos: 7, + 8 with a content size, + 4 with a dictID), nb its linked and nslot its independent
+// blocks -- the number of linked steps, and with fx (a call that may mix modes) fx.nb = 1 for a linked frame.
+// Pass 1, after frame_scan_kernel over fr (slots = 1: first = the first linked row, slot = the first independent row)
+// and over fx (first = the linked frame's index in fl): the rows -- source, length and encode capacity (the bound,
+// or n - 1) -- of linked frames in t and of independent ones in ti, each independent row's dictionary, the
+// independent view fi (first = slot, nb = nslot, so 0 for a linked frame), and with fx the linked frames compacted
+// into fl with their destinations lOff / lCap.  Each frame's layout and status then live in the record of its pass.
+__global__ void frame_enc_plan_kernel(int pass, FrameFormat f, const int64_t* __restrict__ srcOff,
+                                      const int32_t* __restrict__ srcLen, const int64_t* __restrict__ dstOff,
+                                      const int32_t* __restrict__ dstCap, const int64_t* __restrict__ dictOff,
+                                      const int32_t* __restrict__ dictLen, int n, FrameRec* __restrict__ fr,
+                                      FrameRec* __restrict__ fx, FrameRec* __restrict__ fi, FrameRec* __restrict__ fl,
+                                      int64_t* __restrict__ lOff, int32_t* __restrict__ lCap, FrameTable t,
+                                      FrameTable ti, int64_t* __restrict__ rowDictOff,
+                                      int32_t* __restrict__ rowDictLen, FrameTotals* __restrict__ tot) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const int32_t bs = f.bs;
     const int64_t L = srcLen[i] > 0 ? srcLen[i] : 0;
     const int nb = (int)((L + bs - 1) / bs);
     if (pass == 0) {
         FrameRec r = {};
-        r.nb = nb; r.pos = 7; r.err = FK_NONE;
+        int32_t size = f.bdSize;
+        if (f.upstream) {
+            size = 1 << 16;
+            while (size < f.bdSize && L > size) size <<= 2;
+        }
+        const bool indep = (f.flags & FR_INDEPENDENT) || (f.upstream && L <= size);
+        const bool cs = (f.flags & FR_CONTENT_SIZE) && L > 0;
+        r.dictId = f.dictId ? f.dictId[i] : 0u;
+        r.flags = (indep ? FR_INDEPENDENT : 0) | (f.flags & (FR_BLOCK_SUM | FR_CONTENT_SUM)) |
+                  (cs ? FR_CONTENT_SIZE : 0) | (r.dictId ? FR_DICT_ID : 0);
+        r.maxBlock = size;
+        r.nb = indep ? 0 : nb; r.nslot = indep ? nb : 0;
+        r.pos = 7 + (cs ? 8 : 0) + (r.dictId ? 4 : 0); r.err = FK_NONE;
         fr[i] = r;
-        atomicMax(&tot->maxSteps, nb);
+        if (fx) fx[i].nb = indep ? 0 : 1;
+        if (!indep) atomicMax(&tot->maxSteps, nb);
         return;
     }
-    const int64_t first = fr[i].first;
+    const FrameRec r = fr[i];
+    const bool indep = r.flags & FR_INDEPENDENT;
+    const int64_t first = indep ? r.slot : r.first;
+    int64_t* const rowOff = (indep ? ti.srcOff : t.srcOff) + first;
+    int32_t* const rowLen = (indep ? ti.len : t.len) + first;
+    int32_t* const rowCap = (indep ? ti.cap : t.cap) + first;
+    const int32_t bound = max_output_size(bs);
     for (int k = 0; k < nb; k++) {
-        t.srcOff[first + k] = srcOff[i] + (int64_t)k * bs;
-        t.len[first + k] = (int32_t)((L - (int64_t)k * bs) < bs ? (L - (int64_t)k * bs) : bs);
+        const int32_t len = (int32_t)((L - (int64_t)k * bs) < bs ? (L - (int64_t)k * bs) : bs);
+        rowOff[k] = srcOff[i] + (int64_t)k * bs;
+        rowLen[k] = len;
+        rowCap[k] = f.rawFallback ? len - 1 : bound;
+        if (f.dict && indep) { rowDictOff[first + k] = dictOff[i]; rowDictLen[first + k] = dictLen[i]; }
+    }
+    FrameRec v = r;
+    v.first = r.slot; v.nb = r.nslot;
+    fi[i] = v;
+    if (fx && !indep) {
+        const int64_t j = fx[i].first;
+        fl[j] = r; lOff[j] = dstOff[i]; lCap[j] = dstCap[i];
     }
 }
 
@@ -500,12 +579,13 @@ struct FrameEnc {
 
 // One thread per frame: lays out the frame's blocks of this launch -- rows [b0, b1) (independent: entry = row - b0)
 // or, with k >= 0, its block k (linked: entry = frame - f0).  Stored = the encoded bytes when they shrink the block,
-// else the raw bytes (LZ4EncoderBase.cs:79-83).  A block that does not fit dstCap fails the frame (-1); nothing is
-// written at or beyond dstCap.
+// else the raw bytes (LZ4EncoderBase.cs:79-83).  rawFallback (FrameFormat): a block the encoder gave <= 0 for is
+// stored raw; otherwise it fails the frame (-1), as does a block that does not fit dstCap.  Nothing is written at or
+// beyond dstCap.
 __global__ void frame_enc_place_kernel(int k, int64_t b0, int64_t b1, int f0, int f1, FrameRec* __restrict__ fr,
                                        FrameTable t, FrameEnc e, uint8_t* __restrict__ dstBase,
                                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                                       int32_t bound, int bc) {
+                                       int32_t bound, int bc, int rawFallback) {
     const int i = f0 + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= f1) return;
     FrameRec r = fr[i];
@@ -521,7 +601,7 @@ __global__ void frame_enc_place_kernel(int k, int64_t b0, int64_t b1, int f0, in
     const int64_t room = dstCap[i] > 0 ? dstCap[i] : 0;
     for (int64_t b = lo; b < hi; b++) {
         const int64_t x = k >= 0 ? i - f0 : b - b0;
-        const int32_t L = t.len[b], res = e.res[x];
+        const int32_t L = t.len[b], res = rawFallback && e.res[x] <= 0 ? L : e.res[x];
         int32_t cl = 0, rl = 0, ck = 0;
         int64_t cd = 0;
         if (!r.status) {
@@ -545,10 +625,11 @@ __global__ void frame_enc_place_kernel(int k, int64_t b0, int64_t b1, int f0, in
     fr[i].status = r.status;
 }
 
-// Linked step k: block k of frame i (entry i - f0) behind the frame's own source; other entries are empty.
+// Linked step k: block k of frame i (entry i - f0) behind the frame's own source, with its row's encode capacity;
+// other entries are empty.
 __global__ void frame_enc_step_kernel(int k, int f0, int f1, const FrameRec* __restrict__ fr, FrameTable t,
-                                      int64_t* __restrict__ so, int32_t* __restrict__ sl, int32_t* __restrict__ pre,
-                                      int32_t bs) {
+                                      int64_t* __restrict__ so, int32_t* __restrict__ sl, int32_t* __restrict__ cap,
+                                      int32_t* __restrict__ pre, int32_t bs) {
     const int i = f0 + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= f1) return;
     const int x = i - f0;
@@ -556,6 +637,7 @@ __global__ void frame_enc_step_kernel(int k, int f0, int f1, const FrameRec* __r
     const bool on = k < r.nb && !r.status;
     so[x] = on ? t.srcOff[r.first + k] : 0;
     sl[x] = on ? t.len[r.first + k] : 0;
+    cap[x] = on ? t.cap[r.first + k] : 0;
     const int64_t p = (int64_t)k * bs;
     pre[x] = (int32_t)(p < 0x7FFFFFFF ? p : 0x7FFFFFFF);
 }
@@ -567,80 +649,31 @@ __global__ void frame_put_sum_kernel(uint8_t* __restrict__ dstBase, FrameEnc e, 
     fr_wr32(dstBase + e.ckOff[x] + e.ckLen[x], e.ckSum[x]);
 }
 
-// One thread per frame: header, end mark, content checksum, result.  DICT: a frame whose dictId is not 0 gets the
-// dictionary flag and the 4-byte ID in front of HC, which covers it (dictId may be null: no IDs).
-template <bool DICT>
-__device__ __forceinline__ void frame_enc_finish_body(const FrameRec* __restrict__ fr, int n,
-                                                      uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff,
-                                                      const int32_t* __restrict__ dstCap, uint64_t header, int cc,
-                                                      const uint32_t* __restrict__ csum, int32_t* __restrict__ outLen,
-                                                      const uint32_t* __restrict__ dictId) {
+// One thread per frame: header, end mark, content checksum, result.  The frame's record is fi[i] for an independent
+// frame, else its linked one: fl[fx[i].first], or fl[i] without fx (fl is then fr).
+__global__ void frame_enc_finish_kernel(const FrameRec* __restrict__ fi, const FrameRec* __restrict__ fl,
+                                        const FrameRec* __restrict__ fx, int n, const int32_t* __restrict__ srcLen,
+                                        uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff,
+                                        const int32_t* __restrict__ dstCap, const uint32_t* __restrict__ csum,
+                                        int32_t* __restrict__ outLen) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const FrameRec& r = fr[i];
+    const FrameRec& r = (fi[i].flags & FR_INDEPENDENT) ? fi[i] : fl[fx ? fx[i].first : i];
+    const bool cc = r.flags & FR_CONTENT_SUM;
     const int64_t total = r.pos + 4 + (cc ? 4 : 0);
     if (r.status || total > (dstCap[i] > 0 ? dstCap[i] : 0) || total > 0x7FFFFFFF) { outLen[i] = -1; return; }
     uint8_t* d = dstBase + dstOff[i];
-    const uint32_t id = DICT && dictId ? dictId[i] : 0u;
-    if (DICT && id) {
-        uint8_t h[6] = {(uint8_t)((header >> 32) | 1), (uint8_t)(header >> 40), (uint8_t)id, (uint8_t)(id >> 8),
-                        (uint8_t)(id >> 16), (uint8_t)(id >> 24)};
-        fr_wr32(d, FRAME_MAGIC);
-        for (int j = 0; j < 6; j++) d[4 + j] = h[j];
-        d[10] = (uint8_t)(xx_finish(XXP5 + 6u, h, 6) >> 8);
-    } else {
-        for (int j = 0; j < 7; j++) d[j] = (uint8_t)(header >> (8 * j));
-    }
+    frame_put_header(d, r.flags, r.maxBlock, (uint64_t)(srcLen[i] > 0 ? srcLen[i] : 0), r.dictId);
     fr_wr32(d + r.pos, 0);
     if (cc) fr_wr32(d + r.pos + 4, csum[i]);
     outLen[i] = (int32_t)total;
-}
-__global__ void frame_enc_finish_kernel(const FrameRec* __restrict__ fr, int n, uint8_t* __restrict__ dstBase,
-                                        const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                                        uint64_t header, int cc, const uint32_t* __restrict__ csum,
-                                        int32_t* __restrict__ outLen) {
-    frame_enc_finish_body<false>(fr, n, dstBase, dstOff, dstCap, header, cc, csum, outLen, nullptr);
-}
-__global__ void frame_enc_finish_dict_kernel(const FrameRec* __restrict__ fr, int n, uint8_t* __restrict__ dstBase,
-                                             const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap,
-                                             uint64_t header, int cc, const uint32_t* __restrict__ csum,
-                                             int32_t* __restrict__ outLen, const uint32_t* __restrict__ dictId) {
-    frame_enc_finish_body<true>(fr, n, dstBase, dstOff, dstCap, header, cc, csum, outLen, dictId);
-}
-
-// ---- dictionary encode (k4lz4_frame_encode_dict_batch): upstream's CDict frames ------------------------------
-// Every block is LZ4_compress_fast_continue with capacity n - 1 and is stored raw when that fails
-// (lz4frame.c:747-749); independent blocks each start from LZ4_loadDict of the frame's dictionary (OP_ENCDICT),
-// linked frames load it once, in front of block 0 (frame_dict_first_kernel).
-
-// One thread per frame, after the plan: the header grows by the dictID field where the ID is not 0, and every row
-// gets its frame's dictionary.
-__global__ void frame_enc_dict_plan_kernel(FrameRec* __restrict__ fr, int n, const int64_t* __restrict__ dictOff,
-                                           const int32_t* __restrict__ dictLen, const uint32_t* __restrict__ dictId,
-                                           int64_t* __restrict__ rowDictOff, int32_t* __restrict__ rowDictLen) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const FrameRec r = fr[i];
-    if (dictId && dictId[i]) fr[i].pos = r.pos + 4;
-    for (int k = 0; k < r.nb; k++) { rowDictOff[r.first + k] = dictOff[i]; rowDictLen[r.first + k] = dictLen[i]; }
-}
-
-// Before an encode launch: capacity n - 1 for every entry.  After it: an entry that did not fit is stored raw
-// (frame_enc_place_kernel stores the source when the result is >= n).
-__global__ void frame_dict_cap_kernel(const int32_t* __restrict__ len, int32_t* __restrict__ cap, int m) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    if (x < m) cap[x] = len[x] > 0 ? len[x] - 1 : 0;
-}
-__global__ void frame_dict_raw_kernel(const int32_t* __restrict__ len, int32_t* __restrict__ res, int m) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    if (x < m && len[x] > 0 && res[x] <= 0) res[x] = len[x];
 }
 
 // Linked step 0, one warp per entry x (frame f0 + x): LZ4_loadDict of the frame's dictionary into its state record,
 // then block 0 in the usingExtDict mode against it (encode_dict_warp, capacity n0 - 1), then what
 // LZ4_compress_fast_continue leaves for the blocks behind it: currentOffset = 65 536 + n0 (lz4.c:918) and
-// dictSize = n0 (lz4.c:1633-1634), also when the block did not fit (its table stops where upstream's does).  The
-// result is as frame_dict_raw_kernel leaves it; steps 1.. are the chained encoder's (OP_ENCCHAIN).
+// dictSize = n0 (lz4.c:1633-1634), also when the block did not fit (its table stops where upstream's does).  A
+// block that did not fit gives n0: it is stored raw.  Steps 1.. are the chained encoder's (OP_ENCCHAIN).
 __global__ void __launch_bounds__(32)
 frame_dict_first_kernel(int f0, const uint8_t* __restrict__ srcBase, const int64_t* __restrict__ so,
                         const int32_t* __restrict__ sl, uint8_t* __restrict__ dstBase, int64_t bound,
@@ -665,102 +698,6 @@ frame_dict_first_kernel(int f0, const uint8_t* __restrict__ srcBase, const int64
         r = r <= 0 ? n0 : r;
     }
     if (lane == 0) res[x] = r;
-}
-
-// ---- upstream's LZ4F_compressFrame (k4lz4_lz4f_compress_batch) ----------------------------------------------
-// Per frame of n bytes (lz4frame.c:385-395): the block size shrinks to the smallest of 64 KiB, 256 KiB, 1 MiB that
-// holds n, up to the caller's (LZ4F_optimalBSID); a frame of one block (n <= block size) is independent; the content
-// size field is written when asked for and n > 0.  Every block is encoded with capacity n - 1 and stored raw when
-// that fails (frame_dict_cap_kernel / frame_dict_raw_kernel): independent blocks as LZ4_compress_fast, linked
-// blocks as LZ4_compress_fast_continue on one fresh stream.  A frame of more than one block keeps the caller's block
-// size, so every frame's blocks are bs bytes but its last.
-
-// Each frame is in one of two passes, and the existing encode kernels see it through the record of its pass:
-// fi, the independent view over all frames (frame_enc_place_kernel with k < 0; nb = 0 for a linked frame, first = its
-// first row of the compact table of independent blocks), and fl, the linked frames alone, compacted with their
-// destinations (lOff / lCap), so that the linked steps run over linked frames only.  A frame's layout and status live
-// in the record of its pass.
-// One thread per frame.  Pass 0: fr gets the frame's mode, block size and header length, nb its linked blocks and
-// nslot its independent blocks; fx.nb is 1 for a linked frame; the number of steps is the largest linked block count.
-// Pass 1, after frame_scan_kernel over fr (slots = 1: fr.first = first linked row, fr.slot = first independent row)
-// and over fx (fx.first = the linked frame's index in fl): the linked frames' rows in t, the independent frames' in
-// ti, fi, and fl / lOff / lCap.  `flags`: FR_* of the call plus FR_CONTENT_SIZE.
-__global__ void frame_lz4f_plan_kernel(int pass, const int64_t* __restrict__ srcOff, const int32_t* __restrict__ srcLen,
-                                       const int64_t* __restrict__ dstOff, const int32_t* __restrict__ dstCap, int n,
-                                       int32_t bs, int flags, FrameRec* __restrict__ fr, FrameRec* __restrict__ fx,
-                                       FrameRec* __restrict__ fi, FrameRec* __restrict__ fl,
-                                       int64_t* __restrict__ lOff, int32_t* __restrict__ lCap, FrameTable t,
-                                       FrameTable ti, FrameTotals* __restrict__ tot) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int64_t L = srcLen[i] > 0 ? srcLen[i] : 0;
-    const int nb = (int)((L + bs - 1) / bs);
-    if (pass == 0) {
-        FrameRec r = {};
-        int32_t size = 1 << 16;                          // LZ4F_optimalBSID
-        while (size < bs && L > size) size <<= 2;
-        const bool indep = (flags & FR_INDEPENDENT) || L <= size;
-        const bool cs = (flags & FR_CONTENT_SIZE) && L > 0;
-        r.flags = (indep ? FR_INDEPENDENT : 0) | (flags & (FR_BLOCK_SUM | FR_CONTENT_SUM)) | (cs ? FR_CONTENT_SIZE : 0);
-        r.maxBlock = size;
-        r.nb = indep ? 0 : nb; r.nslot = indep ? nb : 0; r.pos = cs ? 15 : 7; r.err = FK_NONE;
-        fr[i] = r;
-        fx[i].nb = indep ? 0 : 1;
-        if (!indep) atomicMax(&tot->maxSteps, nb);
-        return;
-    }
-    const FrameRec r = fr[i];
-    const bool indep = r.flags & FR_INDEPENDENT;
-    const int64_t first = indep ? r.slot : r.first;
-    int64_t* const rowOff = (indep ? ti.srcOff : t.srcOff) + first;
-    int32_t* const rowLen = (indep ? ti.len : t.len) + first;
-    for (int k = 0; k < nb; k++) {
-        rowOff[k] = srcOff[i] + (int64_t)k * bs;
-        rowLen[k] = (int32_t)((L - (int64_t)k * bs) < bs ? (L - (int64_t)k * bs) : bs);
-    }
-    FrameRec v = r;
-    v.first = r.slot; v.nb = r.nslot;
-    fi[i] = v;
-    if (!indep) {
-        const int64_t j = fx[i].first;
-        fl[j] = r; lOff[j] = dstOff[i]; lCap[j] = dstCap[i];
-    }
-}
-
-// One thread per frame: header (magic, FLG, BD of the frame's block size, the content size where the frame has
-// one, HC over FLG .. content size), end mark, content checksum, result.
-__global__ void frame_lz4f_finish_kernel(const FrameRec* __restrict__ fx, const FrameRec* __restrict__ fi,
-                                         const FrameRec* __restrict__ fl, int n, const int32_t* __restrict__ srcLen,
-                                         uint8_t* __restrict__ dstBase, const int64_t* __restrict__ dstOff,
-                                         const int32_t* __restrict__ dstCap, const uint32_t* __restrict__ csum,
-                                         int32_t* __restrict__ outLen) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const FrameRec& r = (fi[i].flags & FR_INDEPENDENT) ? fi[i] : fl[fx[i].first];
-    const bool cc = r.flags & FR_CONTENT_SUM, cs = r.flags & FR_CONTENT_SIZE;
-    const int64_t total = r.pos + 4 + (cc ? 4 : 0);
-    if (r.status || total > (dstCap[i] > 0 ? dstCap[i] : 0) || total > 0x7FFFFFFF) { outLen[i] = -1; return; }
-    const int code = r.maxBlock == (1 << 16) ? 4 : r.maxBlock == (1 << 18) ? 5 : r.maxBlock == (1 << 20) ? 6 : 7;
-    uint8_t h[10];
-    h[0] = (uint8_t)((1 << 6) | ((r.flags & FR_INDEPENDENT) ? 1 << 5 : 0) | ((r.flags & FR_BLOCK_SUM) ? 1 << 4 : 0) |
-                     (cs ? 1 << 3 : 0) | (cc ? 1 << 2 : 0));
-    h[1] = (uint8_t)(code << 4);
-    const uint64_t size = (uint64_t)(srcLen[i] > 0 ? srcLen[i] : 0);
-#pragma unroll
-    for (int j = 0; j < 8; j++) h[2 + j] = (uint8_t)(size >> (8 * j));
-    uint8_t* d = dstBase + dstOff[i];
-    fr_wr32(d, FRAME_MAGIC);
-    if (cs) {                                        // constant lengths: h stays in registers
-#pragma unroll
-        for (int j = 0; j < 10; j++) d[4 + j] = h[j];
-        d[14] = (uint8_t)(xx_finish(XXP5 + 10u, h, 10) >> 8);
-    } else {
-        d[4] = h[0]; d[5] = h[1];
-        d[6] = (uint8_t)(xx_finish(XXP5 + 2u, h, 2) >> 8);
-    }
-    fr_wr32(d + r.pos, 0);
-    if (cc) fr_wr32(d + r.pos + 4, csum[i]);
-    outLen[i] = (int32_t)total;
 }
 
 // off[x] = x * stride and, when cap is given, cap[x] = capValue: the fixed slots of a launch.

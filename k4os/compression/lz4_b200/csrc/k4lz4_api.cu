@@ -1234,28 +1234,40 @@ int32_t frame_block_size(int32_t blockSize) {
     return std::max<int32_t>(1024, (blockSize + 1023) / 1024 * 1024);
 }
 
-int64_t frame_bound_of(int64_t length, int32_t bs, int flags) {
-    const int64_t nb = (length + bs - 1) / bs;
-    return 7 + nb * (4 + ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 4 : 0)) + length + 4 +
-           ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 4 : 0);
+// One of upstream's four block sizes (LZ4F_blockSizeID_t): 64 KiB, 256 KiB, 1 MiB, 4 MiB.
+bool upstream_block_size(int32_t s) { return s == (1 << 16) || s == (1 << 18) || s == (1 << 20) || s == (1 << 22); }
+
+// The formats of the frame encoders (frame.cuh, FrameFormat), from the caller's block size and flags; bs = 0 where
+// the format does not take them.
+// The reference's LZ4FrameWriter: any block size of 1 B .. 4 MiB, rounded (frame_block_size).
+k4::FrameFormat writer_format(int32_t blockSize, int flags) {
+    return {(flags & ~FRAME_FLAGS) ? 0 : frame_block_size(blockSize), blockSize, flags, 0, 0, 0, nullptr};
+}
+// Upstream's CDict frames (LZ4F_compressFrame_usingCDict) against the Batch's dictionaries, `dictId` may be null.
+k4::FrameFormat cdict_format(int32_t blockSize, int flags, const uint32_t* dictId) {
+    return {(flags & ~FRAME_FLAGS) || !upstream_block_size(blockSize) ? 0 : blockSize, blockSize, flags, 0, 1, 1,
+            dictId};
+}
+// Upstream's LZ4F_compressFrame, with K4LZ4_FRAME_CONTENT_SIZE.
+constexpr int LZ4F_FLAGS = FRAME_FLAGS | K4LZ4_FRAME_CONTENT_SIZE;
+k4::FrameFormat lz4f_format(int32_t blockSize, int flags) {
+    return {(flags & ~LZ4F_FLAGS) || !upstream_block_size(blockSize) ? 0 : blockSize, blockSize,
+            (flags & FRAME_FLAGS) | ((flags & K4LZ4_FRAME_CONTENT_SIZE) ? k4::FR_CONTENT_SIZE : 0), 1, 1, 0, nullptr};
 }
 
-// Magic, FLG, BD (LZ4FrameWriter.cs:183-188: the code of the caller's block size) and HC, little-endian.
-uint64_t frame_header(int32_t blockSize, int flags) {
-    const int code = blockSize <= (1 << 16) ? 4 : blockSize <= (1 << 18) ? 5 : blockSize <= (1 << 20) ? 6 : 7;
-    const uint8_t fb[2] = {(uint8_t)((1 << 6) | ((flags & K4LZ4_FRAME_INDEPENDENT) ? 1 << 5 : 0) |
-                                     ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 1 << 4 : 0) |
-                                     ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 1 << 2 : 0)),
-                           (uint8_t)(code << 4)};
-    const uint8_t hc = (uint8_t)(k4::xxh32_host(fb, 2, 0) >> 8);
-    return (uint64_t)k4::FRAME_MAGIC | ((uint64_t)fb[0] << 32) | ((uint64_t)fb[1] << 40) | ((uint64_t)hc << 48);
+// The most bytes a frame of `length` bytes takes in format f, whose dictID is `id`: the header, per block 4 bytes of
+// length code (+ 4 with block checksums) and at most the raw length, the end mark (+ 4 with a content checksum).
+// Upstream's rule counts the largest header, 19 bytes, as LZ4F_compressFrameBound does (lz4frame.c:324-361).
+int64_t frame_bound_of(const k4::FrameFormat& f, int64_t length, uint32_t id = 0) {
+    const int64_t nb = length / f.bs + (length % f.bs ? 1 : 0);
+    return (f.upstream ? 19 : 7 + (id ? 4 : 0)) + nb * (4 + ((f.flags & k4::FR_BLOCK_SUM) ? 4 : 0)) + length + 4 +
+           ((f.flags & k4::FR_CONTENT_SUM) ? 4 : 0);
 }
 
-// The dictionary calls (k4lz4_frame_*_dict_batch, k4lz4_frame_info_batch): frame i's dictionary is the Batch's
-// dictBase[dictOff[i] .. + dictLen[i]) (decode: dictBase may be null, no dictionaries); `id` the IDs an encode writes
-// (may be null: none), `outId` where the info call puts the headers' IDs.  A null FrameDict is the frame calls as
-// they were without dictionaries.
-struct FrameDict { const uint32_t* id = nullptr; int64_t* outId = nullptr; };
+// The dictionary calls' decode side (k4lz4_frame_decode_dict_batch, k4lz4_frame_info_batch): frame i's dictionary is
+// the Batch's dictBase[dictOff[i] .. + dictLen[i]) (dictBase may be null, no dictionaries); `outId` where the info
+// call puts the headers' IDs.  A null FrameDict is the decode calls as they were without dictionaries.
+struct FrameDict { int64_t* outId = nullptr; };
 
 // Stream-ordered allocations of one frame call, from the device's private pool; freed (in stream order) at the end.
 struct FramePool {
@@ -1411,97 +1423,67 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
     return cudaSuccess;
 }
 
-// Encode b.n frames in device memory on `st` (level < 3): plan, scan, one host synchronisation for the block and
-// step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of at most
-// FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.  With fd: against
-// the Batch's dictionaries, upstream's CDict frames (frame.cuh, "dictionary encode").  With up: upstream's
-// LZ4F_compressFrame (frame.cuh, "upstream's LZ4F_compressFrame"), each frame independent or linked by its own size,
-// so one call may run both passes; `flags` may then carry FR_CONTENT_SIZE.
-cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
-                             const FrameDict* fd = nullptr, bool up = false) {
+// Encode b.n frames of format f in device memory on `st` (level < 3): plan, scan, one host synchronisation for the
+// block and step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of
+// at most FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.  A call
+// with upstream's rule that is not independent may mix both; its linked frames are compacted (fx numbers them), so
+// that the linked steps run over them alone.
+cudaError_t frame_encode_dev(const Batch& b, const k4::FrameFormat& f, cudaStream_t st) {
     int dev = 0;
     cudaGetDevice(&dev);
     const Dev* D = dev_state(dev);
     if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
     const int n = (int)b.n;
-    const bool bc = flags & K4LZ4_FRAME_BLOCK_CHECKSUM, cc = flags & K4LZ4_FRAME_CONTENT_CHECKSUM;
+    const bool bc = f.flags & k4::FR_BLOCK_SUM, cc = f.flags & k4::FR_CONTENT_SUM;
+    const bool mixed = f.upstream && !(f.flags & k4::FR_INDEPENDENT);
     FramePool P(D->pool, st);
     k4::FrameRec* fr = P.get<k4::FrameRec>(n);
-    // up (frame_lz4f_plan_kernel): fx numbers the linked frames, fi is the independent view, fl the linked frames
-    // alone with their destinations lOff / lCap; otherwise all three are fr and the caller's destinations
-    k4::FrameRec* fx = up ? P.get<k4::FrameRec>(n) : fr;
-    k4::FrameRec* fi = up ? P.get<k4::FrameRec>(n) : fr;
+    k4::FrameRec* fi = P.get<k4::FrameRec>(n);
+    k4::FrameRec* fx = mixed ? P.get<k4::FrameRec>(n) : nullptr;
     k4::FrameTotals* tot = P.get<k4::FrameTotals>(2);
     FR_TRY(P.err);
     FR_TRY(cudaMemsetAsync(tot, 0, 2 * sizeof(k4::FrameTotals), st));
+    // fl: the records of the linked pass, with their destinations lOff / lCap; fr and the caller's unless mixed
     k4::FrameTable t{}, ti{};
     k4::FrameRec* fl = fr;
     int64_t* flOff = nullptr;
     int32_t* flCap = nullptr;
+    int64_t* rowDictOff = nullptr;
+    int32_t* rowDictLen = nullptr;
     auto plan = [&](int pass) {
-        if (up)
-            k4::frame_lz4f_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, b.srcOff, b.srcLen, b.dstOff, b.dstCap, n, bs,
-                                                                  flags, fr, fx, fi, fl, flOff, flCap, t, ti, tot);
-        else k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, b.srcOff, b.srcLen, n, bs, fr, t, tot);
+        k4::frame_enc_plan_kernel<<<grid_of(n), 128, 0, st>>>(pass, f, b.srcOff, b.srcLen, b.dstOff, b.dstCap,
+                                                              b.dictOff, b.dictLen, n, fr, fx, fi, fl, flOff, flCap,
+                                                              t, ti, rowDictOff, rowDictLen, tot);
     };
     plan(0);
     FR_LAUNCH();
-    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, up ? 1 : 0);
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, 1);
     FR_LAUNCH();
     g_launches += 2;
-    if (up) {
+    if (mixed) {
         k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fx, n, tot + 1, 0);
         FR_LAUNCH();
         g_launches++;
     }
     k4::FrameTotals h[2] = {};
-    FR_TRY(cudaMemcpyAsync(h, tot, (up ? 2 : 1) * sizeof(k4::FrameTotals), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaMemcpyAsync(h, tot, (mixed ? 2 : 1) * sizeof(k4::FrameTotals), cudaMemcpyDeviceToHost, st));
     FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size and the number of steps
-    const int64_t nB = h[0].blocks;
-    const bool linked = up ? h[0].maxSteps > 0 : !(flags & K4LZ4_FRAME_INDEPENDENT);
-    const int64_t nI = up ? h[0].slots : linked ? 0 : nB;    // blocks of the independent pass (up: in ti, nB in t)
-    const int64_t nL = up ? h[1].blocks : n;                  // frames of the linked pass
-    t.srcOff = P.get<int64_t>(nB);
-    t.len = P.get<int32_t>(nB);
-    if (up) {
-        ti.srcOff = P.get<int64_t>(nI); ti.len = P.get<int32_t>(nI);
-        fl = P.get<k4::FrameRec>(nL); flOff = P.get<int64_t>(nL); flCap = P.get<int32_t>(nL);
-    } else {
-        ti = t;
-    }
-    const int64_t* lOff = up ? flOff : b.dstOff;
-    const int32_t* lCap = up ? flCap : b.dstCap;
+    const int64_t nB = h[0].blocks, nI = h[0].slots;    // rows of the linked pass (in t) and the independent one (ti)
+    const int64_t nL = mixed ? h[1].blocks : n;         // frames of the linked pass
+    const bool linked = h[0].maxSteps > 0;
+    t.srcOff = P.get<int64_t>(nB); t.len = P.get<int32_t>(nB); t.cap = P.get<int32_t>(nB);
+    ti.srcOff = P.get<int64_t>(nI); ti.len = P.get<int32_t>(nI); ti.cap = P.get<int32_t>(nI);
+    if (mixed) { fl = P.get<k4::FrameRec>(nL); flOff = P.get<int64_t>(nL); flCap = P.get<int32_t>(nL); }
+    if (f.dict) { rowDictOff = P.get<int64_t>(nI); rowDictLen = P.get<int32_t>(nI); }
+    const int64_t* lOff = mixed ? flOff : b.dstOff;
+    const int32_t* lCap = mixed ? flCap : b.dstCap;
     uint32_t* csum = P.get<uint32_t>(n);
     FR_TRY(P.err);
     plan(1);
     FR_LAUNCH();
     g_launches++;
-    int64_t* rowDictOff = nullptr;
-    int32_t* rowDictLen = nullptr;
-    if (fd) {
-        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
-        FR_TRY(P.err);
-        k4::frame_enc_dict_plan_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dictOff, b.dictLen, fd->id, rowDictOff,
-                                                                  rowDictLen);
-        FR_LAUNCH();
-        g_launches++;
-    }
-    // capacity n - 1 in front of a dictionary encode, raw where it did not fit behind it
-    auto dict_cap = [&](const int32_t* len, int32_t* cap, int64_t m) -> cudaError_t {
-        k4::frame_dict_cap_kernel<<<grid_of(m), 128, 0, st>>>(len, cap, (int)m);
-        FR_LAUNCH();
-        g_launches++;
-        return cudaSuccess;
-    };
-    auto dict_raw = [&](const int32_t* len, int32_t* res, int64_t m) -> cudaError_t {
-        k4::frame_dict_raw_kernel<<<grid_of(m), 128, 0, st>>>(len, res, (int)m);
-        FR_LAUNCH();
-        g_launches++;
-        return cudaSuccess;
-    };
     if (cc) FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, b.srcOff, b.srcLen, nullptr, nullptr, nullptr, (int32_t*)csum, n}, st));
-    const bool capm1 = fd || up;                       // capacity n - 1, raw where that fails (lz4frame.c:747-749)
-    const int32_t bound = k4::max_output_size(bs);
+    const int32_t bound = k4::max_output_size(f.bs);
     const int64_t per = std::max<int64_t>(FRAME_SCRATCH / bound, 1);
     const int64_t E = std::max<int64_t>(std::min<int64_t>(per, std::max<int64_t>(linked ? nL : 0, nI)), 1);
     if (nB > 0 || nI > 0) {
@@ -1513,14 +1495,15 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
         e.cLen = P.get<int32_t>(E); e.rLen = P.get<int32_t>(E); e.ckLen = P.get<int32_t>(E); e.ckSum = P.get<uint32_t>(E);
         e.res = P.get<int32_t>(E);
         FR_TRY(P.err);
-        k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(eDst, eCap, (int)E, bound, bound);
+        k4::frame_slots_kernel<<<grid_of(E), 128, 0, st>>>(eDst, nullptr, (int)E, bound, 0);
         FR_LAUNCH();
         g_launches++;
         // the bodies into place, then the block checksums over them
         auto place = [&](int k, int64_t b0, int64_t b1, int f0, int f1, int64_t m) -> cudaError_t {
             k4::frame_enc_place_kernel<<<grid_of(f1 - f0), 128, 0, st>>>(k, b0, b1, f0, f1, k < 0 ? fi : fl, k < 0 ? ti : t,
                                                                          e, b.dstBase, k < 0 ? b.dstOff : lOff,
-                                                                         k < 0 ? b.dstCap : lCap, bound, bc ? 1 : 0);
+                                                                         k < 0 ? b.dstCap : lCap, bound, bc ? 1 : 0,
+                                                                         f.rawFallback);
             FR_LAUNCH();
             g_launches++;
             const int mm = (int)m;
@@ -1536,15 +1519,9 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
         };
         for (int64_t b0 = 0; b0 < nI; b0 += E) {
             const int64_t m = std::min<int64_t>(E, nI - b0);
-            Batch kb{b.srcBase, ti.srcOff + b0, ti.len + b0, scratch, eDst, eCap, e.res, m, b.level, b.x32};
-            if (capm1) FR_TRY(dict_cap(ti.len + b0, eCap, m));
-            if (fd) {
-                kb.dictBase = b.dictBase; kb.dictOff = rowDictOff + b0; kb.dictLen = rowDictLen + b0;
-                FR_TRY(launch_op(OP_ENCDICT, kb, st));
-            } else {
-                FR_TRY(launch_op(OP_ENCODE, kb, st));
-            }
-            if (capm1) FR_TRY(dict_raw(ti.len + b0, e.res, m));
+            Batch kb{b.srcBase, ti.srcOff + b0, ti.len + b0, scratch, eDst, ti.cap + b0, e.res, m, b.level, b.x32};
+            if (f.dict) { kb.dictBase = b.dictBase; kb.dictOff = rowDictOff + b0; kb.dictLen = rowDictLen + b0; }
+            FR_TRY(launch_op(f.dict ? OP_ENCDICT : OP_ENCODE, kb, st));
             FR_TRY(place(-1, b0, b0 + m, 0, n, m));
         }
         if (linked) {
@@ -1560,12 +1537,12 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
             for (int f0 = 0; f0 < nL; f0 += (int)E) {
                 const int m = (int)std::min<int64_t>(E, nL - f0);
                 // with dictionaries, step 0 loads each frame's state record from its dictionary
-                if (!fd) FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
+                if (!f.dict) FR_TRY(cudaMemsetAsync(state, 0, (size_t)m * K4LZ4_CHAIN_STATE_BYTES, st));
                 for (int k = 0; k < h[0].maxSteps; k++) {
-                    k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fl, t, so, sl, pre, bs);
+                    k4::frame_enc_step_kernel<<<grid_of(m), 128, 0, st>>>(k, f0, f0 + m, fl, t, so, sl, eCap, pre, f.bs);
                     FR_LAUNCH();
                     g_launches++;
-                    if (fd && k == 0) {
+                    if (f.dict && k == 0) {
                         k4::frame_dict_first_kernel<<<m, 32, 0, st>>>(f0, b.srcBase, so, sl, scratch, bound, b.dictBase,
                                                                       b.dictOff, b.dictLen,
                                                                       reinterpret_cast<k4::ChainState*>(state), e.res);
@@ -1574,67 +1551,42 @@ cudaError_t frame_encode_dev(const Batch& b, int32_t bs, int flags, uint64_t hea
                     } else {
                         Batch kb{b.srcBase, so, sl, scratch, eDst, eCap, e.res, m, b.level, b.x32};
                         kb.prefixLen = pre; kb.stateBase = state; kb.stateOff = stOff;
-                        if (capm1) FR_TRY(dict_cap(sl, eCap, m));
                         FR_TRY(launch_op(OP_ENCCHAIN, kb, st));
-                        if (capm1) FR_TRY(dict_raw(sl, e.res, m));
                     }
                     FR_TRY(place(k, 0, 0, f0, f0 + m, m));
                 }
             }
         }
     }
-    if (up)
-        k4::frame_lz4f_finish_kernel<<<grid_of(n), 128, 0, st>>>(fx, fi, fl, n, b.srcLen, b.dstBase, b.dstOff,
-                                                                b.dstCap, csum, b.outLen);
-    else if (fd)
-        k4::frame_enc_finish_dict_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header,
-                                                                    cc ? 1 : 0, csum, b.outLen, fd->id);
-    else
-        k4::frame_enc_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, b.dstBase, b.dstOff, b.dstCap, header,
-                                                               cc ? 1 : 0, csum, b.outLen);
+    k4::frame_enc_finish_kernel<<<grid_of(n), 128, 0, st>>>(fi, fl, fx, n, b.srcLen, b.dstBase, b.dstOff, b.dstCap,
+                                                           csum, b.outLen);
     FR_LAUNCH();
     g_launches++;
     return cudaSuccess;
 }
 
-// FO_LZ4F: upstream's LZ4F_compressFrame (k4lz4_lz4f_compress_batch), an encode.
-enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE, FO_LZ4F };
-inline bool frame_encodes(FrameOp fo) { return fo == FO_ENCODE || fo == FO_LZ4F; }
+enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE };
 
-constexpr int LZ4F_FLAGS = FRAME_FLAGS | K4LZ4_FRAME_CONTENT_SIZE;
-
-// LZ4F_compressFrameBound (lz4frame.c:324-361) for a block size of 64 KiB .. 4 MiB: the 19-byte largest header,
-// per block 4 bytes of length code (+ 4 with block checksums) and at most the raw length, the end mark (+ 4).
-int64_t lz4f_bound_of(int64_t length, int32_t bs, int flags) {
-    const int64_t nb = length / bs + (length % bs ? 1 : 0);
-    return 19 + nb * (4 + ((flags & K4LZ4_FRAME_BLOCK_CHECKSUM) ? 4 : 0)) + length + 4 +
-           ((flags & K4LZ4_FRAME_CONTENT_CHECKSUM) ? 4 : 0);
-}
-
-cudaError_t frame_dev(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, cudaStream_t st,
-                      const FrameDict* fd) {
-    if (frame_encodes(fo) && b.level >= 3) {
+// f: the format of an encode (unused by the decode calls).
+cudaError_t frame_dev(FrameOp fo, const Batch& b, const k4::FrameFormat& f, cudaStream_t st, const FrameDict* fd) {
+    if (fo == FO_ENCODE && b.level >= 3) {
         k4::frame_fill_kernel<<<grid_of(b.n), 128, 0, st>>>(b.outLen, (int)b.n, K4LZ4_R_DELEGATE);
         g_launches++;
         return cudaGetLastError();
     }
-    if (fo == FO_LZ4F) {
-        const int f = (flags & FRAME_FLAGS) | ((flags & K4LZ4_FRAME_CONTENT_SIZE) ? k4::FR_CONTENT_SIZE : 0);
-        return frame_encode_dev(b, bs, f, 0, st, nullptr, true);
-    }
-    return fo == FO_ENCODE ? frame_encode_dev(b, bs, flags, header, st, fd) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
+    return fo == FO_ENCODE ? frame_encode_dev(b, f, st) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
 }
 
 // Host memory, one GPU, synchronous: chunks of whole frames (a frame is never split: its linked blocks and its
 // content checksum need all of it) through the device's staging, the device path on each, on the legacy default
 // stream.  The device region of a frame is min(dstCap, frame bound) when encoding (a frame never needs more) and
-// dstCap when decoding; content sizes have none.  With fd: each distinct dictionary of a chunk is staged once, only
-// its last 64 KiB (all that encode and decode read), and the IDs travel in the rows' aux column; the info call's
-// IDs come back behind the sizes.
-int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t header, int dev, const FrameDict* fd) {
+// dstCap when decoding; content sizes have none.  With dictionaries, each distinct one of a chunk is staged once,
+// only its last 64 KiB (all that encode and decode read); an encode's dictIDs travel in the rows' aux column, and the
+// info call's IDs come back behind the sizes.
+int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, const FrameDict* fd) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
-    if (frame_encodes(fo) && b.level >= 3) {
+    if (fo == FO_ENCODE && b.level >= 3) {
         for (int64_t i = 0; i < b.n; i++) b.outLen[i] = K4LZ4_R_DELEGATE;
         return K4LZ4_OK;
     }
@@ -1646,11 +1598,9 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
     auto room = [&](int64_t i) -> int64_t {
         if (!dst) return 0;
         const int64_t c = std::max<int32_t>(b.dstCap[i], 0);
-        const int64_t idRoom = fd && fd->id && fd->id[i] ? 4 : 0;
-        if (fo == FO_LZ4F) return std::min<int64_t>(c, lz4f_bound_of(src_size(b, i), bs, flags));
-        return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(src_size(b, i), bs, flags) + idRoom) : c;
+        return fo == FO_ENCODE ? std::min<int64_t>(c, frame_bound_of(f, src_size(b, i), f.dictId ? f.dictId[i] : 0)) : c;
     };
-    const bool dict = fd && b.dictBase;
+    const bool dict = b.dictBase;
     auto dlen = [&](int64_t i) -> int32_t { return dict ? std::min<int32_t>(std::max<int32_t>(b.dictLen[i], 0), 65536) : 0; };
     auto dkey = [&](int64_t i) { return std::make_pair(b.dictBase + b.dictOff[i] + (b.dictLen[i] - dlen(i)), dlen(i)); };
     std::map<std::pair<const uint8_t*, int32_t>, int64_t> first;   // a chunk's first row of each distinct dictionary
@@ -1679,7 +1629,7 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
         const int64_t resInts = ids ? 4 : 1;          // the info call: the int64 IDs at res + 2 nb
         int rc = stage_up(D->stage, nb, resInts, 0, [&](int64_t k) {
             const int64_t x = i + k, s = src_size(b, x), r = room(x);
-            UpRow u{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, fd && fd->id ? (int32_t)fd->id[x] : 0,
+            UpRow u{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, f.dictId ? (int32_t)f.dictId[x] : 0,
                     dst ? b.dstBase + b.dstOff[x] : nullptr};
             if (dict) { u.blob = dkey(x).first; u.blobLen = dlen(x); u.blobFrom = from[(size_t)k]; }
             return u;
@@ -1690,12 +1640,11 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
         kb.dstBase = up.dst; kb.dstOff = up.dstOff; kb.dstCap = dst ? up.cap : nullptr;
         kb.outLen = up.res; kb.n = nb;
         if (dict) { kb.dictBase = up.blob; kb.dictOff = up.blobOff; kb.dictLen = up.blobLen; }
+        k4::FrameFormat kf = f;
+        kf.dictId = f.dictId ? reinterpret_cast<const uint32_t*>(up.aux) : nullptr;
         FrameDict kd;
-        if (fd) {
-            kd.id = fd->id ? reinterpret_cast<const uint32_t*>(up.aux) : nullptr;
-            kd.outId = ids ? reinterpret_cast<int64_t*>(up.res + 2 * nb) : nullptr;
-        }
-        const cudaError_t e = frame_dev(fo, kb, bs, flags, header, nullptr, fd ? &kd : nullptr);
+        kd.outId = ids ? reinterpret_cast<int64_t*>(up.res + 2 * nb) : nullptr;
+        const cudaError_t e = frame_dev(fo, kb, kf, nullptr, fd ? &kd : nullptr);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
         res.resize((size_t)(nb * resInts));
         rc = stage_down(D->stage, up, nb, ids ? res.data() : b.outLen + i, resInts, dst ? up.dst : nullptr, up.dstOff,
@@ -1709,32 +1658,19 @@ int frame_host(FrameOp fo, const Batch& b, int32_t bs, int flags, uint64_t heade
     return K4LZ4_OK;
 }
 
-// Every frame export: its own arguments, then the batch's (check()), then host or device.  fd: the dictionary calls
-// (their encode takes upstream's four block sizes only, and requires the dictionaries; the info call its ID array).
-int frame_run(FrameOp fo, const Batch& b, int32_t blockSize, int flags, int memKind, void* stream, int device,
+// Every frame export: its own arguments (an encode's: bs = 0 where its format refuses them), then the batch's
+// (check()), then host or device.  An encode whose format reads dictionaries requires them; the info call (fd with
+// FO_SIZE) its ID array.
+int frame_run(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int memKind, void* stream, int device,
               const FrameDict* fd = nullptr) {
-    int32_t bs = 0;
-    if (fo == FO_LZ4F) {
-        if (blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22))
-            return fail(K4LZ4_E_ARG, "bad frame block size %d (64 KiB, 256 KiB, 1 MiB or 4 MiB)", blockSize);
-        if (flags & ~LZ4F_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
-        bs = blockSize;
-    } else if (fo == FO_ENCODE) {
-        bs = frame_block_size(blockSize);
-        if (fd && blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22))
-            bs = 0;
-        if (!bs) return fail(K4LZ4_E_ARG, "bad frame block size %d (%s)", blockSize,
-                             fd ? "64 KiB, 256 KiB, 1 MiB or 4 MiB" : "1 .. 4 MiB");
-        if (flags & ~FRAME_FLAGS) return fail(K4LZ4_E_ARG, "unknown frame flags 0x%x", flags);
-    }
-    const bool missing = fd && (fo == FO_ENCODE ? !b.dictBase : fo == FO_SIZE ? !fd->outId : false);
-    const int rc = check(frame_encodes(fo) ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
+    if (fo == FO_ENCODE && !f.bs) return fail(K4LZ4_E_ARG, "bad frame block size %d or flags", f.bdSize);
+    const bool missing = fo == FO_ENCODE ? f.dict && !b.dictBase : fo == FO_SIZE && fd && !fd->outId;
+    const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
-    const uint64_t header = fo == FO_ENCODE ? frame_header(blockSize, flags) : 0;
-    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, bs, flags, header, device < 0 ? 0 : device, fd);
+    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, f, device < 0 ? 0 : device, fd);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    const cudaError_t e = frame_dev(fo, b, bs, flags, header, (cudaStream_t)stream, fd);
+    const cudaError_t e = frame_dev(fo, b, f, (cudaStream_t)stream, fd);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
 }
@@ -2863,9 +2799,9 @@ int32_t k4lz4_copy_blocks_device(const uint8_t* srcBase, const int64_t* srcOff, 
 }
 
 int64_t k4lz4_frame_bound(int64_t length, int32_t blockSize, int32_t flags) {
-    const int32_t bs = frame_block_size(blockSize);
-    if (!bs || length < 0 || (flags & ~FRAME_FLAGS)) return fail(K4LZ4_E_ARG, "bad frame bound arguments");
-    return frame_bound_of(length, bs, flags);
+    const k4::FrameFormat f = writer_format(blockSize, flags);
+    if (!f.bs || length < 0) return fail(K4LZ4_E_ARG, "bad frame bound arguments");
+    return frame_bound_of(f, length);
 }
 
 int32_t k4lz4_frame_encode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2873,7 +2809,7 @@ int32_t k4lz4_frame_encode_batch(const uint8_t* srcBase, const int64_t* srcOff, 
                                  int32_t nFrames, int32_t blockSize, int32_t flags, int32_t level, int32_t memKind,
                                  void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level};
-    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
+    return frame_run(FO_ENCODE, b, writer_format(blockSize, flags), memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_encode_batch_x32(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2881,14 +2817,13 @@ int32_t k4lz4_frame_encode_batch_x32(const uint8_t* srcBase, const int64_t* srcO
                                      int32_t nFrames, int32_t blockSize, int32_t flags, int32_t level,
                                      int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level, true};
-    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device);
+    return frame_run(FO_ENCODE, b, writer_format(blockSize, flags), memKind, cudaStream, device);
 }
 
 int64_t k4lz4_lz4f_compress_bound(int64_t length, int32_t blockSize, int32_t flags) {
-    if ((blockSize != (1 << 16) && blockSize != (1 << 18) && blockSize != (1 << 20) && blockSize != (1 << 22)) ||
-        length < 0 || (flags & ~LZ4F_FLAGS))
-        return fail(K4LZ4_E_ARG, "bad LZ4F bound arguments");
-    return lz4f_bound_of(length, blockSize, flags);
+    const k4::FrameFormat f = lz4f_format(blockSize, flags);
+    if (!f.bs || length < 0) return fail(K4LZ4_E_ARG, "bad LZ4F bound arguments");
+    return frame_bound_of(f, length);
 }
 
 int32_t k4lz4_lz4f_compress_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2897,21 +2832,21 @@ int32_t k4lz4_lz4f_compress_batch(const uint8_t* srcBase, const int64_t* srcOff,
                                   void* cudaStream, int32_t device) {
     // levels 0..2 are acceleration 1 (lz4frame.c:768,779); HC levels and accelerations (negative levels) delegate
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level < 0 || level >= 3 ? 3 : level};
-    return frame_run(FO_LZ4F, b, blockSize, flags, memKind, cudaStream, device);
+    return frame_run(FO_ENCODE, b, lz4f_format(blockSize, flags), memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_content_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                        int32_t* outSize, int32_t nFrames, int32_t memKind, void* cudaStream,
                                        int32_t device) {
     Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
-    return frame_run(FO_SIZE, b, 0, 0, memKind, cudaStream, device);
+    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_decode_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                  uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap, int32_t* outLen,
                                  int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
-    return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device);
+    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_encode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2921,9 +2856,7 @@ int32_t k4lz4_frame_encode_dict_batch(const uint8_t* srcBase, const int64_t* src
                                       int32_t flags, int32_t level, int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames, level};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
-    FrameDict fd;
-    fd.id = dictId;
-    return frame_run(FO_ENCODE, b, blockSize, flags, memKind, cudaStream, device, &fd);
+    return frame_run(FO_ENCODE, b, cdict_format(blockSize, flags, dictId), memKind, cudaStream, device);
 }
 
 int32_t k4lz4_frame_decode_dict_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -2934,7 +2867,7 @@ int32_t k4lz4_frame_decode_dict_batch(const uint8_t* srcBase, const int64_t* src
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
     FrameDict fd;
-    return frame_run(FO_DECODE, b, 0, 0, memKind, cudaStream, device, &fd);
+    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
 }
 
 int32_t k4lz4_frame_info_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen, int32_t* outSize,
@@ -2942,22 +2875,24 @@ int32_t k4lz4_frame_info_batch(const uint8_t* srcBase, const int64_t* srcOff, co
     Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
     FrameDict fd;
     fd.outId = outDictId;
-    return frame_run(FO_SIZE, b, 0, 0, memKind, cudaStream, device, &fd);
+    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
 }
 
 int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int32_t flags, int32_t level,
                                         int32_t device, k4lz4_frame_writer_group** out) {
     if (out) *out = nullptr;
-    const int32_t B = frame_block_size(blockSize);
-    if (!out || nStreams <= 0 || !B || (flags & ~FRAME_FLAGS) || level < 0 || level > 0xFF)
+    const k4::FrameFormat f = writer_format(blockSize, flags);
+    if (!out || nStreams <= 0 || !f.bs || level < 0 || level > 0xFF)
         return fail(K4LZ4_E_ARG, "bad frame writer group arguments (%d streams, block size %d, flags 0x%x, level %d)",
                     nStreams, blockSize, flags, level);
     if (level >= 3) return K4LZ4_R_DELEGATE;
     return group_create(nStreams, device, "frame writer group", out, [&](k4lz4_frame_writer_group& g) {
-        g.blockSize = blockSize; g.B = B; g.flags = flags; g.level = level;
-        g.header = frame_header(blockSize, flags);
-        if (g.linked()) chain_layout(g, B);
-        else g.ring = g.slot = B;     // independent blocks: the slot alone, pos stays 0
+        g.blockSize = blockSize; g.B = f.bs; g.flags = flags; g.level = level;
+        uint8_t h[8] = {};
+        k4::frame_put_header(h, f.flags, f.bdSize, 0, 0);
+        for (int j = 0; j < 8; j++) g.header |= (uint64_t)h[j] << (8 * j);
+        if (g.linked()) chain_layout(g, g.B);
+        else g.ring = g.slot = g.B;     // independent blocks: the slot alone, pos stays 0
         g.fw = g.alloc<k4::FwState>(sizeof(k4::FwState), true);
         if (g.linked()) g.states = g.alloc<uint8_t>(K4LZ4_CHAIN_STATE_BYTES, true);
     });
@@ -3020,9 +2955,7 @@ int64_t k4lz4_frame_writer_close_bound(const k4lz4_frame_writer_group* g) {
 int32_t k4lz4_frame_reader_group_create(int32_t nStreams, int32_t maxBlockSize, int32_t device,
                                         k4lz4_frame_reader_group** out) {
     if (out) *out = nullptr;
-    const bool bd = maxBlockSize == (1 << 16) || maxBlockSize == (1 << 18) || maxBlockSize == (1 << 20) ||
-                    maxBlockSize == (1 << 22);
-    if (!out || nStreams <= 0 || !bd)
+    if (!out || nStreams <= 0 || !upstream_block_size(maxBlockSize))
         return fail(K4LZ4_E_ARG, "bad frame reader group arguments (%d streams, max block size %d)", nStreams,
                     maxBlockSize);
     return group_create(nStreams, device, "frame reader group", out, [&](k4lz4_frame_reader_group& g) {
