@@ -162,6 +162,14 @@ namespace K4os.Compression.LZ4.Engine.Native
         [DllImport(Lib)] public static extern int k4lz4_lz4f_compress_batch(
             byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
             int* outLen, int nFrames, int blockSize, int flags, int level, int memKind, void* cudaStream, int device);
+        // whole .lz4 inputs as upstream's `lz4 -d` reads them (k4lz4.h ".lz4 streams")
+        [DllImport(Lib)] public static extern int k4lz4_lz4f_decompress_batch(
+            byte* srcBase, long* srcOff, int* srcLen, byte* dstBase, long* dstOff, int* dstCap,
+            byte* dictBase, long* dictOff, int* dictLen, int* outLen, int* outErr, int* outEnd, int nStreams,
+            int memKind, void* cudaStream, int device);
+        [DllImport(Lib)] public static extern int k4lz4_lz4f_decompressed_size_batch(
+            byte* srcBase, long* srcOff, int* srcLen, int* outSize, int* outErr, int* outEnd, int nStreams,
+            int memKind, void* cudaStream, int device);
         // LZ4EncoderStream / LZ4FrameWriter written incrementally, batched across streams (k4lz4.h "frame writer group")
         [DllImport(Lib)] public static extern int k4lz4_frame_writer_group_create(
             int nStreams, int blockSize, int flags, int level, int device, void** group);

@@ -84,6 +84,25 @@ namespace K4os.Compression.LZ4
                     flags, (int)level, K4Lz4Native.MEM_HOST, null, 0));
         }
 
+        // Whole .lz4 inputs as upstream's `lz4 -d [-D dict]` reads them (k4lz4_lz4f_decompress_batch): concatenated
+        // frames, skippable frames, legacy members.  lengths[i]: the content length, -1 on an error, R_DST_SMALL;
+        // errors[i]: (cliError << 8) | LZ4F code, 0 on success; ends[i]: where reading stopped.  An empty
+        // dictionaryLengths span: no dictionaries.  Size targets with k4lz4_lz4f_decompressed_size_batch.
+        public static void DecompressFramesUpstream(
+            ReadOnlySpan<byte> sourceBase, ReadOnlySpan<long> sourceOffsets, ReadOnlySpan<int> sourceLengths,
+            Span<byte> targetBase, ReadOnlySpan<long> targetOffsets, ReadOnlySpan<int> targetCapacities,
+            ReadOnlySpan<byte> dictionaryBase, ReadOnlySpan<long> dictionaryOffsets,
+            ReadOnlySpan<int> dictionaryLengths, Span<int> lengths, Span<int> errors, Span<int> ends)
+        {
+            fixed (byte* s = sourceBase) fixed (long* so = sourceOffsets) fixed (int* sl = sourceLengths)
+            fixed (byte* d = targetBase) fixed (long* dof = targetOffsets) fixed (int* dc = targetCapacities)
+            fixed (byte* k = dictionaryBase) fixed (long* ko = dictionaryOffsets) fixed (int* kl = dictionaryLengths)
+            fixed (int* ol = lengths) fixed (int* oe = errors) fixed (int* oz = ends)
+                Check(K4Lz4Native.k4lz4_lz4f_decompress_batch(s, so, sl, d, dof, dc,
+                    dictionaryLengths.IsEmpty ? null : k, ko, kl, ol, oe, oz, lengths.Length,
+                    K4Lz4Native.MEM_HOST, null, 0));
+        }
+
         // LZ4 frames against a dictionary, as upstream's LZ4F_compressBegin_usingCDict writes them
         // (k4lz4_frame_encode_dict_batch): frame i holds source i, encoded against dictionary i, with the dictID
         // dictionaryIds[i] unless it is 0 (an empty span: no IDs).  blockSize: 64 KiB, 256 KiB, 1 MiB or 4 MiB; flags:

@@ -517,6 +517,49 @@ K4LZ4_API int32_t k4lz4_lz4f_compress_batch(const uint8_t *srcBase, const int64_
                                             int32_t *outLen, int32_t nFrames, int32_t blockSize, int32_t flags,
                                             int32_t level, int32_t memKind, void *cudaStream, int32_t device);
 
+/* ---- .lz4 streams as upstream `lz4 -d` reads them (programs/lz4io.c over LZ4F_decompress_usingDict) -------- */
+
+/* Stream i is one whole input file, srcBase[srcOff[i] .. +srcLen[i]), read member by member:
+ *   - LZ4 frames by LZ4F's rules: version 1, reserved FLG / BD bits clear, block-size IDs 4..7 only, header checksum,
+ *     the dictID flag accepted; a block length code above the BD maximum is an error; blocks decode with capacity
+ *     maxBlockSize; a non-zero content-size field must equal the content (checked at the end mark, before the content
+ *     checksum);
+ *   - skippable frames (magic 0x184D2A50..5F) are skipped; a size that reaches past the end ends the stream;
+ *   - legacy members (magic 0x184C2102, lz4 -l): blocks with a 4-byte length, each decoded with capacity 8 MiB; a
+ *     length above 8 421 520 ends the member and is read as the next member's magic;
+ *   - unknown magic: an error on the first member, the end of the stream (success) on any later one.
+ * Linked history never crosses a member boundary.  An empty stream decodes to 0 bytes.
+ * outLen[i] = the decoded length, written to exactly [dstOff, dstOff + outLen); -1 on an error; K4LZ4_R_DST_SMALL when
+ * the content does not fit dstCap[i], unless the stream has an error that needs no decoding (the ones
+ * k4lz4_lz4f_decompressed_size_batch gives), which then wins.  Nothing is ever written outside
+ * [dstOff, dstOff + dstCap); a failed stream's destination is unspecified (the CLI's partial output is not
+ * reproduced).  outErr[i] = 0, or (e << 8) | c for the first error in stream order, where e is the lz4 CLI's error
+ * number (its exit code) and c the LZ4F_errorCodes value for e = 66 (0 otherwise):
+ *   40 1..3 bytes of a magic number; 42 a skippable size cut short; 44 unknown magic on the first member;
+ *   52 a legacy length or block cut short; 53 a legacy block that does not decode (a 0-length one included);
+ *   66 an LZ4F error (a failed block gives ERROR_GENERIC with 64 KiB blocks and ERROR_decompressionFailed with larger
+ *      ones, as the CLI's 64 KiB output buffer makes LZ4F report it); 68 the input ends inside an LZ4 frame.
+ * outEnd[i] = srcLen[i], or the offset of the undecodable data reading stopped at.
+ * dictBase may be NULL; otherwise stream i's dictionary is dictBase[dictOff[i] .. + dictLen[i]), of which the last
+ * 64 KiB count (lz4 -d -D), used by every LZ4 frame (whatever its dictID flag) and by no legacy member.
+ * Argument errors as k4lz4_frame_decode_dict_batch, and outErr / outEnd are required.  Every input gets a verdict
+ * here: there is no K4LZ4_R_DELEGATE. */
+K4LZ4_API int32_t k4lz4_lz4f_decompress_batch(const uint8_t *srcBase, const int64_t *srcOff, const int32_t *srcLen,
+                                              uint8_t *dstBase, const int64_t *dstOff, const int32_t *dstCap,
+                                              const uint8_t *dictBase, const int64_t *dictOff, const int32_t *dictLen,
+                                              int32_t *outLen, int32_t *outErr, int32_t *outEnd, int32_t nStreams,
+                                              int32_t memKind, void *cudaStream, int32_t device);
+/* The decoded length of every stream, from the members' length codes and token chains, to size the buffers of
+ * k4lz4_lz4f_decompress_batch: outSize[i] = the length (K4LZ4_R_CORRUPT above 2^31 - 1), or -1 with outErr[i] for the
+ * errors that need no decoding (headers, structure, truncation, token chains that do not parse, blocks longer than
+ * their capacity); outEnd[i] as k4lz4_lz4f_decompress_batch.  Checksums, match offsets and content-size fields are
+ * not checked, so where decompress fails the two may name different errors.  Wherever decompress succeeds it returns
+ * exactly this length. */
+K4LZ4_API int32_t k4lz4_lz4f_decompressed_size_batch(const uint8_t *srcBase, const int64_t *srcOff,
+                                                     const int32_t *srcLen, int32_t *outSize, int32_t *outErr,
+                                                     int32_t *outEnd, int32_t nStreams,
+                                                     int32_t memKind, void *cudaStream, int32_t device);
+
 /* ---- LZ4 Frame, written incrementally: LZ4EncoderStream / LZ4FrameWriter, batched across streams ------ */
 
 /*

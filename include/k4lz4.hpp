@@ -736,6 +736,61 @@ struct LZ4F {
                                               bool contentSize = false, int device = 0) {
         return CompressMany({source}, s, contentSize, device)[0];
     }
+
+    // Whole .lz4 inputs as `lz4 -d` reads them (k4lz4_lz4f_decompress_batch): per stream the result, its error
+    // ((cli << 8) | LZ4F code, 0 on success) and where reading stopped.
+    struct Stream { int32_t result = -1, error = 0, end = 0; };
+    static std::vector<Stream> DecompressedSizes(const std::vector<std::vector<uint8_t>>& streams, int device = 0) {
+        const size_t n = streams.size();
+        std::vector<int64_t> so(n);
+        std::vector<int32_t> sl(n), out(n), err(n), end(n);
+        std::vector<uint8_t> src;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)streams[i].size();
+            src.insert(src.end(), streams[i].begin(), streams[i].end());
+        }
+        src.resize(src.size() + 1);
+        const int rc = k4lz4_lz4f_decompressed_size_batch(src.data(), so.data(), sl.data(), out.data(), err.data(),
+                                                          end.data(), (int32_t)n, K4LZ4_MEM_HOST, nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        std::vector<Stream> r(n);
+        for (size_t i = 0; i < n; i++) r[i] = {out[i], err[i], end[i]};
+        return r;
+    }
+    // contents[i] of streams[i], against dictionaries[i] when given (empty: no dictionary); info[i] its verdict.
+    static std::vector<std::vector<uint8_t>> Decompress(const std::vector<std::vector<uint8_t>>& streams,
+                                                        std::vector<Stream>* info = nullptr,
+                                                        const std::vector<std::vector<uint8_t>>* dictionaries = nullptr,
+                                                        int device = 0) {
+        const size_t n = streams.size();
+        const std::vector<Stream> sizes = DecompressedSizes(streams, device);
+        std::vector<int64_t> so(n), dofs(n), dko(n);
+        std::vector<int32_t> sl(n), dc(n), dkl(n), out(n), err(n), end(n);
+        std::vector<uint8_t> src, dst, dic;
+        int64_t d = 0;
+        for (size_t i = 0; i < n; i++) {
+            so[i] = (int64_t)src.size(); sl[i] = (int32_t)streams[i].size();
+            src.insert(src.end(), streams[i].begin(), streams[i].end());
+            dofs[i] = d; dc[i] = std::max<int32_t>(sizes[i].result, 0); d += dc[i];
+            if (dictionaries) {
+                dko[i] = (int64_t)dic.size(); dkl[i] = (int32_t)(*dictionaries)[i].size();
+                dic.insert(dic.end(), (*dictionaries)[i].begin(), (*dictionaries)[i].end());
+            }
+        }
+        src.resize(src.size() + 1); dst.resize((size_t)d + 1); dic.resize(dic.size() + 1);
+        const int rc = k4lz4_lz4f_decompress_batch(src.data(), so.data(), sl.data(), dst.data(), dofs.data(), dc.data(),
+                                                   dictionaries ? dic.data() : nullptr, dko.data(), dkl.data(),
+                                                   out.data(), err.data(), end.data(), (int32_t)n, K4LZ4_MEM_HOST,
+                                                   nullptr, device);
+        if (rc != K4LZ4_OK) throw NativeError(rc, k4lz4_last_error());
+        std::vector<std::vector<uint8_t>> contents(n);
+        if (info) info->resize(n);
+        for (size_t i = 0; i < n; i++) {
+            if (info) (*info)[i] = {out[i], err[i], end[i]};
+            if (out[i] > 0) contents[i].assign(dst.begin() + dofs[i], dst.begin() + dofs[i] + out[i]);
+        }
+        return contents;
+    }
 };
 
 }  // namespace k4lz4

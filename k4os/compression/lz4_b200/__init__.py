@@ -16,9 +16,10 @@ from . import batch
 from .encoders import (LZ4BlockEncoder, LZ4BlockDecoder, LZ4ChainDecoder, LZ4Decoder, LZ4Encoder,
                        LZ4FastChainEncoder)
 from .groups import ChainDecoderGroup, ChainEncoderGroup, FrameReaderGroup, FrameWriterGroup
-from .frame import LZ4F, LZ4Frame, lz4f_compress
+from .frame import LZ4F, LZ4Frame, lz4f_compress, lz4f_decompress
 
 __all__ = ["LZ4Codec", "LZ4Level", "LZ4Pickler", "InvalidDataException",
            "DelegateToManagedEngine", "batch", "_native", "LZ4BlockEncoder", "LZ4BlockDecoder",
            "LZ4ChainDecoder", "LZ4Decoder", "LZ4Encoder", "LZ4FastChainEncoder", "ChainEncoderGroup",
-           "ChainDecoderGroup", "LZ4Frame", "FrameWriterGroup", "FrameReaderGroup", "LZ4F", "lz4f_compress"]
+           "ChainDecoderGroup", "LZ4Frame", "FrameWriterGroup", "FrameReaderGroup", "LZ4F", "lz4f_compress",
+           "lz4f_decompress"]

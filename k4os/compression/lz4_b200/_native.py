@@ -85,6 +85,8 @@ SIGNATURES = {
     "k4lz4_frame_info_batch": ([_vp] * 5 + [_i32] + _CALL, _i32),
     "k4lz4_lz4f_compress_bound": ([_i64, _i32, _i32], _i64),
     "k4lz4_lz4f_compress_batch": (_BATCH + [_i32, _i32, _i32, _i32] + _CALL, _i32),
+    "k4lz4_lz4f_decompress_batch": ([_vp] * 12 + [_i32] + _CALL, _i32),
+    "k4lz4_lz4f_decompressed_size_batch": ([_vp] * 6 + [_i32] + _CALL, _i32),
     "k4lz4_frame_writer_group_create": ([_i32, _i32, _i32, _i32, _i32, _vp], _i32),
     "k4lz4_frame_writer_group_destroy": ([_vp], _i32),
     "k4lz4_frame_writer_group_reset": ([_vp, _vp, _i32, _i32, _vp], _i32),

@@ -42,6 +42,7 @@
 #include "frame.cuh"
 #include "frame_writer.cuh"
 #include "frame_reader.cuh"
+#include "lz4f_read.cuh"
 
 namespace {
 
@@ -1267,7 +1268,12 @@ int64_t frame_bound_of(const k4::FrameFormat& f, int64_t length, uint32_t id = 0
 // The dictionary calls' decode side (k4lz4_frame_decode_dict_batch, k4lz4_frame_info_batch): frame i's dictionary is
 // the Batch's dictBase[dictOff[i] .. + dictLen[i]) (dictBase may be null, no dictionaries); `outId` where the info
 // call puts the headers' IDs.  A null FrameDict is the decode calls as they were without dictionaries.
-struct FrameDict { int64_t* outId = nullptr; };
+// lz4f: the calls that read .lz4 streams as `lz4 -d` does (lz4f_decode_dev), with their error codes and end offsets.
+struct FrameDict {
+    int64_t* outId = nullptr;
+    bool lz4f = false;
+    int32_t* outErr = nullptr; int32_t* outEnd = nullptr;
+};
 
 // Stream-ordered allocations of one frame call, from the device's private pool; freed (in stream order) at the end.
 struct FramePool {
@@ -1423,6 +1429,138 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
     return cudaSuccess;
 }
 
+// Read (or, with sizeOnly, only size) b.n .lz4 streams in device memory on `st` as `lz4 -d` does (lz4f_read.cuh):
+// the member walk, the scans of each stream's blocks, scratch units and members, one host synchronisation for those
+// totals and the number of linked steps, then the members' blocks through frame_decode_dev's machinery and the
+// per-stream finish.  outErr / outEnd: the streams' error codes and end offsets.  With b.dictBase, every LZ4F member
+// decodes against its stream's dictionary.
+cudaError_t lz4f_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, int32_t* outErr, int32_t* outEnd) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const Dev* D = dev_state(dev);
+    if (!D || D->err != cudaSuccess) return D ? D->err : cudaErrorInvalidDevice;
+    const int n = (int)b.n;
+    const bool dict = b.dictBase && !sizeOnly;
+    FramePool P(D->pool, st);
+    k4::Lz4fStreams ss;
+    ss.rows = P.get<k4::FrameRec>(n); ss.mems = P.get<k4::FrameRec>(n);
+    ss.code = P.get<int32_t>(n); ss.end = P.get<int32_t>(n); ss.total = P.get<int64_t>(n); ss.lb = P.get<uint64_t>(n);
+    k4::FrameTotals* tot = P.get<k4::FrameTotals>(2);
+    FR_TRY(P.err);
+    FR_TRY(cudaMemsetAsync(tot, 0, 2 * sizeof(k4::FrameTotals), st));
+    k4::Lz4fMembers mb{};
+    k4::FrameRec* fr = nullptr;
+    auto walk = [&](int pass, const k4::FrameTable& t) {
+        k4::lz4f_walk_kernel<<<grid_of(n), 128, 0, st>>>(pass, b.srcBase, b.srcOff, b.srcLen, n, ss, fr, mb, t,
+                                                         b.dictOff, b.dictLen, dict ? 1 : 0, tot);
+    };
+    walk(0, k4::FrameTable{});
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(ss.rows, n, tot, 1);
+    FR_LAUNCH();
+    k4::frame_scan_kernel<<<1, 1024, 0, st>>>(ss.mems, n, tot + 1, 0);
+    FR_LAUNCH();
+    g_launches += 3;
+    k4::FrameTotals h[2] = {};
+    FR_TRY(cudaMemcpyAsync(h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
+    FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size, the members and the steps
+    const int64_t nB = h[0].blocks, nM = h[1].blocks;
+    const int nm = (int)nM;
+    fr = P.get<k4::FrameRec>(nM);
+    mb.stream = P.get<int32_t>(nM); mb.code = P.get<int32_t>(nM); mb.key = P.get<unsigned long long>(nM);
+    mb.size = P.get<uint64_t>(nM); mb.dst = P.get<int64_t>(nM);
+    if (dict) { mb.dictOff = P.get<int64_t>(nM); mb.dictLen = P.get<int32_t>(nM); }
+    uint8_t* rows = P.get<uint8_t>(nB * k4::FRAME_ROW_BYTES + 16 * 16);
+    FR_TRY(P.err);
+    k4::FrameTable t;
+    {
+        uint8_t* p = rows;
+        auto take = [&](int64_t bytes) { uint8_t* q = p; p += (bytes + 15) & ~int64_t(15); return q; };
+        t.srcOff = (int64_t*)take(nB * 8); t.fin = (int64_t*)take(nB * 8); t.dst = (int64_t*)take(nB * 8);
+        t.cpySrc = (int64_t*)take(nB * 8);
+        t.len = (int32_t*)take(nB * 4); t.kind = (int32_t*)take(nB * 4); t.sum = (uint32_t*)take(nB * 4);
+        t.frame = (int32_t*)take(nB * 4); t.idx = (int32_t*)take(nB * 4); t.size = (int32_t*)take(nB * 4);
+        t.cap = (int32_t*)take(nB * 4); t.ilen = (int32_t*)take(nB * 4); t.res = (int32_t*)take(nB * 4);
+        t.ckLen = (int32_t*)take(nB * 4); t.got = (uint32_t*)take(nB * 4); t.cpyLen = (int32_t*)take(nB * 4);
+    }
+    walk(1, t);
+    FR_LAUNCH();
+    g_launches++;
+    if (nB > 0) {
+        k4::block_size_walk_kernel<<<grid_of(nB * 32), 128, 0, st>>>(b.srcBase, t, nB, fr);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    uint8_t* scratch = sizeOnly ? nullptr : P.get<uint8_t>(h[0].slots * k4::LZ4F_SLOT_UNIT);
+    int32_t* ccLen = P.get<int32_t>(nM);
+    uint32_t* ccGot = P.get<uint32_t>(nM);
+    FR_TRY(P.err);
+    const int64_t scratchRel = sizeOnly ? 0 : (int64_t)((uintptr_t)scratch - (uintptr_t)b.dstBase);
+    k4::lz4f_layout_kernel<<<grid_of(n), 128, 0, st>>>(n, ss, fr, mb, t, sizeOnly ? nullptr : b.dstOff,
+                                                       sizeOnly ? nullptr : b.dstCap, scratchRel, ccLen);
+    FR_LAUNCH();
+    g_launches++;
+    int64_t* rowDictOff = nullptr;
+    int32_t* rowDictLen = nullptr;
+    if (dict) {
+        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
+        FR_TRY(P.err);
+        k4::frame_dict_layout_kernel<<<grid_of(nM), 128, 0, st>>>(fr, nm, t, mb.dictOff, mb.dictLen, rowDictOff,
+                                                                 rowDictLen, scratchRel, k4::LZ4F_SLOT_UNIT);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    if (!sizeOnly && nB > 0) {
+        const int nb = (int)nB;
+        // stored blocks first: they are history for the linked blocks after them
+        FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
+        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
+        Batch ib{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb};
+        if (dict) { ib.dictBase = b.dictBase; ib.dictOff = rowDictOff; ib.dictLen = rowDictLen; }
+        FR_TRY(launch_op(OP_DECODE, ib, st));
+        if (h[0].maxSteps > 0) {         // block k of every linked member, so a stream's frames decode in parallel
+            k4::FrameStep s;
+            s.srcOff = P.get<int64_t>(nM); s.dstOff = P.get<int64_t>(nM); s.hSrc = P.get<int64_t>(nM);
+            s.hDst = P.get<int64_t>(nM); s.srcLen = P.get<int32_t>(nM); s.cap = P.get<int32_t>(nM);
+            s.prefix = P.get<int32_t>(nM); s.res = P.get<int32_t>(nM); s.hLen = P.get<int32_t>(nM);
+            k4::FrameStepDict sd{};
+            if (dict) { sd.src = P.get<int64_t>(nM); sd.dst = P.get<int64_t>(nM); sd.len = P.get<int32_t>(nM); }
+            FR_TRY(P.err);
+            for (int k = 0; k < h[0].maxSteps; k++) {
+                if (dict) k4::frame_step_prepare_dict_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s, mb.dst, mb.dictOff, mb.dictLen, sd);
+                else k4::frame_step_prepare_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s, mb.dst);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, nm}, st));
+                Batch cb{b.srcBase, s.srcOff, s.srcLen, b.dstBase, s.dstOff, s.cap, s.res, nm};
+                if (dict && k == 0) {          // block 0 against the dictionary itself
+                    cb.dictBase = b.dictBase; cb.dictOff = mb.dictOff; cb.dictLen = mb.dictLen;
+                    FR_TRY(launch_op(OP_DECODE, cb, st));
+                } else {
+                    if (dict) FR_TRY(launch_op(OP_COPY, Batch{b.dictBase, sd.src, sd.len, b.dstBase, sd.dst, nullptr, nullptr, nm}, st));
+                    cb.prefixLen = s.prefix;
+                    FR_TRY(launch_op(OP_CHAIN, cb, st));
+                }
+                k4::frame_step_commit_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, nm}, st));
+            }
+        }
+        k4::frame_verdict_kernel<<<grid_of(nB), 128, 0, st>>>(fr, t, nB);
+        FR_LAUNCH();
+        g_launches++;
+        FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
+    }
+    if (!sizeOnly && nM > 0)
+        FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, mb.dst, ccLen, nullptr, nullptr, nullptr, (int32_t*)ccGot, nm}, st));
+    k4::lz4f_finish_kernel<<<grid_of(n), 128, 0, st>>>(n, ss, fr, mb, t, sizeOnly ? nullptr : b.dstCap,
+                                                       sizeOnly ? nullptr : ccGot, ccLen, b.outLen, outErr, outEnd);
+    FR_LAUNCH();
+    g_launches++;
+    return cudaSuccess;
+}
+
 // Encode b.n frames of format f in device memory on `st` (level < 3): plan, scan, one host synchronisation for the
 // block and step counts, then everything else enqueued.  Independent frames: the blocks of all frames in launches of
 // at most FRAME_SCRATCH bytes of encoder output; linked frames: one launch per step over chunks of frames.  A call
@@ -1574,6 +1712,7 @@ cudaError_t frame_dev(FrameOp fo, const Batch& b, const k4::FrameFormat& f, cuda
         g_launches++;
         return cudaGetLastError();
     }
+    if (fd && fd->lz4f) return lz4f_decode_dev(b, fo == FO_SIZE, st, fd->outErr, fd->outEnd);
     return fo == FO_ENCODE ? frame_encode_dev(b, f, st) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
 }
 
@@ -1605,7 +1744,7 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
     auto dkey = [&](int64_t i) { return std::make_pair(b.dictBase + b.dictOff[i] + (b.dictLen[i] - dlen(i)), dlen(i)); };
     std::map<std::pair<const uint8_t*, int32_t>, int64_t> first;   // a chunk's first row of each distinct dictionary
     std::vector<int64_t> from;
-    const bool ids = fd && fd->outId;
+    const bool ids = fd && fd->outId, lz4f = fd && fd->lz4f;
     std::vector<int32_t> res;
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
@@ -1626,7 +1765,8 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
         }
         const int64_t nb = j - i;
         StageUp up;
-        const int64_t resInts = ids ? 4 : 1;          // the info call: the int64 IDs at res + 2 nb
+        // the info call: the int64 IDs at res + 2 nb; the lz4f calls: the errors at res + nb, the ends at res + 2 nb
+        const int64_t resInts = ids ? 4 : lz4f ? 3 : 1;
         int rc = stage_up(D->stage, nb, resInts, 0, [&](int64_t k) {
             const int64_t x = i + k, s = src_size(b, x), r = room(x);
             UpRow u{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, f.dictId ? (int32_t)f.dictId[x] : 0,
@@ -1644,15 +1784,22 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
         kf.dictId = f.dictId ? reinterpret_cast<const uint32_t*>(up.aux) : nullptr;
         FrameDict kd;
         kd.outId = ids ? reinterpret_cast<int64_t*>(up.res + 2 * nb) : nullptr;
+        kd.lz4f = lz4f;
+        if (lz4f) { kd.outErr = up.res + nb; kd.outEnd = up.res + 2 * nb; }
         const cudaError_t e = frame_dev(fo, kb, kf, nullptr, fd ? &kd : nullptr);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
         res.resize((size_t)(nb * resInts));
-        rc = stage_down(D->stage, up, nb, ids ? res.data() : b.outLen + i, resInts, dst ? up.dst : nullptr, up.dstOff,
+        rc = stage_down(D->stage, up, nb, ids || lz4f ? res.data() : b.outLen + i, resInts, dst ? up.dst : nullptr, up.dstOff,
                         nullptr, nullptr);
         if (rc != K4LZ4_OK) return rc;
         if (ids) {
             memcpy(b.outLen + i, res.data(), (size_t)nb * 4);
             memcpy(fd->outId + i, res.data() + 2 * nb, (size_t)nb * 8);
+        }
+        if (lz4f) {
+            memcpy(b.outLen + i, res.data(), (size_t)nb * 4);
+            memcpy(fd->outErr + i, res.data() + nb, (size_t)nb * 4);
+            memcpy(fd->outEnd + i, res.data() + 2 * nb, (size_t)nb * 4);
         }
     }
     return K4LZ4_OK;
@@ -1664,7 +1811,8 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
 int frame_run(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int memKind, void* stream, int device,
               const FrameDict* fd = nullptr) {
     if (fo == FO_ENCODE && !f.bs) return fail(K4LZ4_E_ARG, "bad frame block size %d or flags", f.bdSize);
-    const bool missing = fo == FO_ENCODE ? f.dict && !b.dictBase : fo == FO_SIZE && fd && !fd->outId;
+    const bool missing = fo == FO_ENCODE ? f.dict && !b.dictBase
+                       : fd && fd->lz4f ? !fd->outErr || !fd->outEnd : fo == FO_SIZE && fd && !fd->outId;
     const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
     if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, f, device < 0 ? 0 : device, fd);
@@ -2875,6 +3023,27 @@ int32_t k4lz4_frame_info_batch(const uint8_t* srcBase, const int64_t* srcOff, co
     Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
     FrameDict fd;
     fd.outId = outDictId;
+    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+}
+
+int32_t k4lz4_lz4f_decompress_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                    uint8_t* dstBase, const int64_t* dstOff, const int32_t* dstCap,
+                                    const uint8_t* dictBase, const int64_t* dictOff, const int32_t* dictLen,
+                                    int32_t* outLen, int32_t* outErr, int32_t* outEnd, int32_t nStreams,
+                                    int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nStreams};
+    b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
+    FrameDict fd;
+    fd.lz4f = true; fd.outErr = outErr; fd.outEnd = outEnd;
+    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+}
+
+int32_t k4lz4_lz4f_decompressed_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
+                                           int32_t* outSize, int32_t* outErr, int32_t* outEnd, int32_t nStreams,
+                                           int32_t memKind, void* cudaStream, int32_t device) {
+    Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nStreams};
+    FrameDict fd;
+    fd.lz4f = true; fd.outErr = outErr; fd.outEnd = outEnd;
     return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
 }
 

@@ -314,6 +314,72 @@ class LZ4F:
             LZ4F.flags(linked, block_checksum, content_checksum, content_size), int(level), N.MEM_DEVICE,
             stream or None, int(device)))
 
+    @staticmethod
+    def decompressed_sizes(streams, device: int = 0):
+        """-> (int32 sizes, int32 errors, int32 ends) of whole .lz4 streams (k4lz4_lz4f_decompressed_size_batch): the
+        content length, or -1 with the error that needs no decoding; see decompress_many for the codes."""
+        src, so, sl = _pack([_u8(s) for s in streams])
+        out, err, end = (np.zeros(len(sl), dtype=np.int32) for _ in range(3))
+        N.check(N.lib().k4lz4_lz4f_decompressed_size_batch(src.ctypes.data, so.ctypes.data, sl.ctypes.data,
+                                                           out.ctypes.data, err.ctypes.data, end.ctypes.data,
+                                                           len(sl), N.MEM_HOST, None, int(device)))
+        return out, err, end
+
+    @staticmethod
+    def decompress_many(streams, dictionaries=None, caps=None, device: int = 0):
+        """Whole .lz4 streams read as `lz4 -d [-D dict]` reads them (k4lz4_lz4f_decompress_batch): concatenated
+        frames, skippable frames, legacy members, trailing data.  -> (list of contents, int32 results, int32 errors,
+        int32 ends).  A result is the content length, -1 on an error or K4LZ4_R_DST_SMALL; an error is
+        (cli << 8) | lz4f, cli being the lz4 CLI's exit code and lz4f the LZ4F_errorCodes value for cli = 66; an end
+        is where reading stopped (the stream's length, or the start of undecodable trailing data).  caps default to
+        each stream's decompressed size."""
+        streams = [_u8(s) for s in streams]
+        if caps is None:
+            caps = np.maximum(LZ4F.decompressed_sizes(streams, device)[0], 0)
+        src, so, sl = _pack(streams)
+        dic = do_ = dl = None
+        if dictionaries is not None:
+            dic, do_, dl = _pack([_u8(d) for d in dictionaries])
+            if len(dl) != len(sl):
+                raise ValueError("one dictionary per stream")
+        dst, do, dc = _slots(caps)
+        out, err, end = (np.zeros(len(sl), dtype=np.int32) for _ in range(3))
+        N.check(N.lib().k4lz4_lz4f_decompress_batch(
+            src.ctypes.data, so.ctypes.data, sl.ctypes.data, dst.ctypes.data, do.ctypes.data, dc.ctypes.data,
+            None if dic is None else dic.ctypes.data, None if dic is None else do_.ctypes.data,
+            None if dic is None else dl.ctypes.data, out.ctypes.data, err.ctypes.data, end.ctypes.data, len(sl),
+            N.MEM_HOST, None, int(device)))
+        return _slices(dst, do, out), out, err, end
+
+    @staticmethod
+    def decompress_many_device(src, src_off, src_len, dst, dst_off, dst_cap, out_len, out_err, out_end,
+                               dict_base=None, dict_off=None, dict_len=None, stream: int = 0,
+                               device: int = -1) -> None:
+        """Torch tensors on the GPU (uint8 data, int64 offsets, int32 lengths, results, errors and ends); only
+        enqueues work on `stream`, after one wait for the block, member and step counts."""
+        ptr = (lambda t: None if t is None else t.data_ptr())
+        N.check(N.lib().k4lz4_lz4f_decompress_batch(
+            src.data_ptr(), src_off.data_ptr(), src_len.data_ptr(), dst.data_ptr(), dst_off.data_ptr(),
+            dst_cap.data_ptr(), ptr(dict_base), ptr(dict_off), ptr(dict_len), out_len.data_ptr(), out_err.data_ptr(),
+            out_end.data_ptr(), int(src_len.numel()), N.MEM_DEVICE, stream or None, int(device)))
+
+
+class LZ4FError(ValueError):
+    """A .lz4 stream `lz4 -d` refuses: `cli` is the CLI's exit code, `lz4f` the LZ4F_errorCodes value (cli 66)."""
+
+    def __init__(self, cli: int, lz4f: int):
+        super().__init__(f"lz4 -d error {cli}" + (f" (LZ4F error {lz4f})" if lz4f else ""))
+        self.cli, self.lz4f = cli, lz4f
+
+
+def lz4f_decompress(data, dictionary=None, device: int = 0) -> bytes:
+    """One whole .lz4 stream, as `lz4 -d -c [-D dictionary]` decodes it; undecodable data after the first member is
+    ignored, as the CLI does.  Raises LZ4FError where the CLI fails."""
+    contents, out, err, _ = LZ4F.decompress_many([data], None if dictionary is None else [dictionary], None, device)
+    if int(err[0]):
+        raise LZ4FError(int(err[0]) >> 8, int(err[0]) & 0xFF)
+    return contents[0]
+
 
 def lz4f_compress(data, block_size: int = 65536, linked: bool = True, block_checksum: bool = False,
                   content_checksum: bool = False, content_size: bool = False, level: int = 0,
