@@ -3,6 +3,13 @@
 // existing codec kernels (launch_op in k4lz4_api.cu) on block tables these kernels write, moved by
 // copy_blocks_kernel and hashed by xxh32_batch_kernel.
 //
+// Decode has two front ends over one block pass.  The reference's reader (frame_decode_dev in k4lz4_api.cu: the
+// parse, scan and frame_layout_kernel here) and upstream's `lz4 -d` (lz4f_decode_dev: lz4f_read.cuh's walk and
+// layout) each write member records (FrameRec) and the rows of one block table, each row placed by frame_place_row.
+// frame_decode_blocks then runs the same kernels for both: frame_dict_layout_kernel, the stored copies, block XXH32,
+// OP_DECODE, the linked steps (frame_step_prepare_kernel, frame_step_commit_kernel) and frame_verdict_kernel.  Each
+// front end keeps its own rules -- header walk, capacity, scratch slots, dictionaries and verdicts -- and its finish.
+//
 // Format: orig/doc/lz4_Frame_format.md; the reference's writer and reader: Streams/Frames/LZ4FrameWriter.cs:57-189,
 // LZ4FrameReader.cs:55-59, LZ4FrameReader.blocking.cs:57-144.  The CPU restatement of the parse is frame.py's
 // _Frame; of the walk (size_walk.cuh), tests/test_frame_model.py.
@@ -66,7 +73,6 @@ struct FrameTable {
     int64_t* cpySrc;         // raw copy (source in srcBase), then scratch copy-back (source relative to dstBase)
     int32_t* cpyLen;
 };
-constexpr int64_t FRAME_ROW_BYTES = 8 * 5 + 4 * 11;
 
 __device__ __forceinline__ uint32_t fr_rd32(const uint8_t* p) {
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
@@ -266,9 +272,28 @@ __global__ void block_size_walk_kernel(const uint8_t* __restrict__ srcBase, Fram
     t.size[b] = (int32_t)(s < frame_lb(L, raw) ? frame_lb(L, raw) : (s > 0x7FFFFFFF ? 0x7FFFFFFF : s));
 }
 
+// Row b's placement, which both readers' layouts write (frame_layout_kernel, lz4f_layout_kernel): its final position
+// fin, where it decodes (at: fin, or a scratch slot), its capacity, its kind (the parse's RK_RAW / RK_LINKED with
+// RK_SCRATCH and RK_SKIP), the source length of an independent compressed block's OP_DECODE, the stored copy of
+// cpyLen bytes and the checksum over ckLen bytes.  The readers differ in those last two, so the caller passes them.
+__device__ __forceinline__ void frame_place_row(FrameTable t, int64_t b, int32_t L, bool raw, bool linked, bool skip,
+                                                bool scratch, int64_t fin, int64_t at, int32_t cap, int32_t cpyLen,
+                                                int32_t ckLen) {
+    t.fin[b] = fin;
+    t.dst[b] = at;
+    t.cap[b] = cap;
+    t.kind[b] = (t.kind[b] & (RK_RAW | RK_LINKED)) | (scratch ? RK_SCRATCH : 0) | (skip ? RK_SKIP : 0);
+    t.ilen[b] = (!skip && !raw && !linked) ? L : 0;
+    t.cpyLen[b] = cpyLen;
+    t.cpySrc[b] = t.srcOff[b];
+    t.ckLen[b] = ckLen;
+    t.res[b] = 0;
+}
+
 // One thread per frame: content size, positions, where each block decodes (in place when the reference's capacity
 // stays inside dstCap, else in a scratch slot), raw copies, checksum lengths.  dstCap null: sizes only.  A frame
-// with a header verdict or a content larger than dstCap is skipped: nothing of it is written.
+// with a header verdict or a content larger than dstCap is skipped: nothing of it is written, and no block checksum
+// is computed.
 __global__ void frame_layout_kernel(FrameRec* __restrict__ fr, int n, FrameTable t, const int64_t* __restrict__ dstOff,
                                     const int32_t* __restrict__ dstCap, int64_t scratchRel, int64_t slotBytes,
                                     int32_t* __restrict__ ccLen) {
@@ -295,15 +320,8 @@ __global__ void frame_layout_kernel(FrameRec* __restrict__ fr, int n, FrameTable
         const bool scratch = dstCap && !skip && !raw && pos + cap > room;
         int64_t at = fin;
         if (scratch) at = scratchRel + (r.slot + (linked ? 0 : k - r.k0)) * slotBytes + FR_HIST;
-        t.fin[b] = fin;
-        t.dst[b] = at;
-        t.cap[b] = cap;
-        t.kind[b] = (t.kind[b] & (RK_RAW | RK_LINKED)) | (scratch ? RK_SCRATCH : 0) | (skip ? RK_SKIP : 0);
-        t.ilen[b] = (!skip && !raw && !linked) ? L : 0;
-        t.cpyLen[b] = (!skip && raw && L <= rawLimit) ? L : 0;
-        t.cpySrc[b] = t.srcOff[b];
-        t.ckLen[b] = (!skip && bc) ? L : 0;
-        t.res[b] = 0;
+        frame_place_row(t, b, L, raw, linked, skip, scratch, fin, at, cap, (!skip && raw && L <= rawLimit) ? L : 0,
+                        (!skip && bc) ? L : 0);
         pos += sz;
     }
     fr[i].pos = r.pos;
@@ -313,8 +331,8 @@ __global__ void frame_layout_kernel(FrameRec* __restrict__ fr, int n, FrameTable
 // Dictionary decode, one thread per frame, after frame_layout_kernel: every row gets its frame's dictionary
 // (rowDictOff / rowDictLen: independent blocks decode against it), and a linked block k >= 1 whose 64 KiB window
 // reaches back past the content's start into a non-empty dictionary (fewer than 65 535 bytes decoded before it)
-// decodes in the frame's scratch slot, where frame_step_prepare_kernel<true> puts [dictionary tail | output so far]
-// in front of it.  A linked frame with blocks always has its one slot (frame_parse_kernel: k0 < nb).
+// decodes in the frame's scratch slot, where frame_step_prepare_kernel puts [dictionary tail | output so far] in
+// front of it.  A linked frame with blocks always has its one slot (frame_parse_kernel: k0 < nb).
 __global__ void frame_dict_layout_kernel(const FrameRec* __restrict__ fr, int n, FrameTable t,
                                          const int64_t* __restrict__ dictOff, const int32_t* __restrict__ dictLen,
                                          int64_t* __restrict__ rowDictOff, int32_t* __restrict__ rowDictLen,
@@ -345,15 +363,13 @@ struct FrameStep {
     int64_t* hSrc; int64_t* hDst; int32_t* hLen;     // history copy, then copy-back
 };
 struct FrameStepDict { int64_t* src; int64_t* dst; int32_t* len; };   // dictionary tail copy (source in dictBase)
-// DICT (dictionary decode): step 0 decodes against the dictionary itself (no copy: the caller launches the tile
-// decoder's dictionary form); a later block with fewer than 65 535 bytes decoded before it sits in the scratch slot
-// (frame_dict_layout_kernel) and gets the dictionary's last bytes in front of the output copied there, its prefix
-// then spanning both.
-template <bool DICT>
-__device__ __forceinline__ void frame_step_prepare_body(int k, const FrameRec* __restrict__ fr, int n, FrameTable t,
-                                                        FrameStep s, const int64_t* __restrict__ dstOff,
-                                                        const int64_t* __restrict__ dictOff,
-                                                        const int32_t* __restrict__ dictLen, FrameStepDict sd) {
+// With dictionaries (dictLen, not null): step 0 decodes against the dictionary itself (no copy: the caller launches
+// the tile decoder's dictionary form); a later block with fewer than 65 535 bytes decoded before it sits in the
+// scratch slot (frame_dict_layout_kernel) and gets the dictionary's last bytes in front of the output copied there,
+// its prefix then spanning both.
+__global__ void frame_step_prepare_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t, FrameStep s,
+                                          const int64_t* __restrict__ dstOff, const int64_t* __restrict__ dictOff,
+                                          const int32_t* __restrict__ dictLen, FrameStepDict sd) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const FrameRec& r = fr[i];
@@ -372,7 +388,7 @@ __device__ __forceinline__ void frame_step_prepare_body(int k, const FrameRec* _
             }
         }
     }
-    if constexpr (DICT) {
+    if (dictLen) {
         int32_t dc = 0;
         int64_t ds = 0, dd = 0;
         const int32_t dl = dictLen[i] > 0 ? dictLen[i] : 0;
@@ -385,16 +401,6 @@ __device__ __forceinline__ void frame_step_prepare_body(int k, const FrameRec* _
     }
     s.srcOff[i] = so; s.srcLen[i] = len; s.dstOff[i] = dof; s.cap[i] = cap; s.prefix[i] = pre;
     s.hSrc[i] = hs; s.hDst[i] = hd; s.hLen[i] = hl;
-}
-__global__ void frame_step_prepare_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t, FrameStep s,
-                                          const int64_t* __restrict__ dstOff) {
-    frame_step_prepare_body<false>(k, fr, n, t, s, dstOff, nullptr, nullptr, FrameStepDict{});
-}
-__global__ void frame_step_prepare_dict_kernel(int k, const FrameRec* __restrict__ fr, int n, FrameTable t,
-                                               FrameStep s, const int64_t* __restrict__ dstOff,
-                                               const int64_t* __restrict__ dictOff,
-                                               const int32_t* __restrict__ dictLen, FrameStepDict sd) {
-    frame_step_prepare_body<true>(k, fr, n, t, s, dstOff, dictOff, dictLen, sd);
 }
 
 // After the step's decode: the result goes to the row, an accepted block in a scratch slot is copied back.
@@ -434,10 +440,12 @@ __global__ void frame_verdict_kernel(FrameRec* __restrict__ fr, FrameTable t, in
     t.cpyLen[b] = back;
 }
 
-// One thread per frame: the frame's result.  sizeOnly: the content-size call (no checksums, no decoder results).
+// One thread per frame: the frame's result.  ccGot null: the content-size and info calls (no checksums, no decoder
+// results).  outId, where given (k4lz4_frame_info_batch): the header's dictID, or -1 without a dictID field or a
+// valid header.
 __global__ void frame_decode_finish_kernel(const FrameRec* __restrict__ fr, int n, const int32_t* __restrict__ dstCap,
                                            const uint32_t* __restrict__ ccGot, const int32_t* __restrict__ ccLen,
-                                           int32_t* __restrict__ outLen) {
+                                           int32_t* __restrict__ outLen, int64_t* __restrict__ outId) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const FrameRec& r = fr[i];
@@ -455,14 +463,7 @@ __global__ void frame_decode_finish_kernel(const FrameRec* __restrict__ fr, int 
         else out = r.pos > 0x7FFFFFFF ? FR_CORRUPT : (int32_t)r.pos;
     }
     outLen[i] = out;
-}
-
-// One thread per frame (k4lz4_frame_info_batch): the header's dictID, or -1 without a dictID field or a valid header.
-__global__ void frame_info_kernel(const FrameRec* __restrict__ fr, int n, int64_t* __restrict__ outId) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const FrameRec& r = fr[i];
-    outId[i] = (!r.status && (r.flags & FR_DICT_ID)) ? (int64_t)r.dictId : -1;
+    if (outId) outId[i] = (!r.status && (r.flags & FR_DICT_ID)) ? (int64_t)r.dictId : -1;
 }
 
 // ---- encode ---------------------------------------------------------------------------------------------------

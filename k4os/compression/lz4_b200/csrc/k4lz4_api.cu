@@ -1265,14 +1265,37 @@ int64_t frame_bound_of(const k4::FrameFormat& f, int64_t length, uint32_t id = 0
            ((f.flags & k4::FR_CONTENT_SUM) ? 4 : 0);
 }
 
-// The dictionary calls' decode side (k4lz4_frame_decode_dict_batch, k4lz4_frame_info_batch): frame i's dictionary is
-// the Batch's dictBase[dictOff[i] .. + dictLen[i]) (dictBase may be null, no dictionaries); `outId` where the info
-// call puts the headers' IDs.  A null FrameDict is the decode calls as they were without dictionaries.
-// lz4f: the calls that read .lz4 streams as `lz4 -d` does (lz4f_decode_dev), with their error codes and end offsets.
-struct FrameDict {
+// How a whole-frame decode call reads its frames, and what it returns beside outLen.
+struct FrameRead {
+    bool lz4f = false;       // `lz4 -d`'s rules (lz4f_decode_dev), else the reference's LZ4FrameReader (frame_decode_dev)
+    bool dictFlag = false;   // the reference's reader accepts the dictionary flag, and its frames decode against the
+                             // Batch's dictionaries (empty ones without dictBase): the dictionary and info calls
+    bool ids = false;        // the info call: each header's dictID in outId
     int64_t* outId = nullptr;
-    bool lz4f = false;
-    int32_t* outErr = nullptr; int32_t* outEnd = nullptr;
+    int32_t* outErr = nullptr; int32_t* outEnd = nullptr;   // the lz4f calls: each stream's error code and end
+    // Visits each column the call returns, by reference (frame_host points them at its staging).
+    template <class F> void columns(F f) {
+        if (lz4f) { f(outErr); f(outEnd); }
+        if (ids) f(outId);
+    }
+    bool missing() {
+        bool m = false;
+        columns([&](auto* p) { m |= !p; });
+        return m;
+    }
+    // Visits each column the call returns with its offset `at` in frame_host's staged results, counted in int32 words
+    // per entry: outLen is word 0, and a column of w words (1 for int32, 2 for int64) starts at a multiple of w, at
+    // res + at * nb for nb entries.  -> the words per entry in all.
+    template <class F> int64_t staged(F f) {
+        int64_t at = 1;
+        columns([&](auto*& p) {
+            const int64_t w = sizeof(*p) / 4;
+            at = (at + w - 1) / w * w;
+            f(p, at);
+            at += w;
+        });
+        return at;
+    }
 };
 
 // Stream-ordered allocations of one frame call, from the device's private pool; freed (in stream order) at the end.
@@ -1296,12 +1319,97 @@ inline unsigned grid_of(int64_t n, int t = 128) { return (unsigned)std::max<int6
 #define FR_TRY(expr) do { const cudaError_t e__ = (expr); if (e__ != cudaSuccess) return e__; } while (0)
 #define FR_LAUNCH() FR_TRY(cudaGetLastError())
 
-// Decode (or, with sizeOnly, only the content sizes of) b.n frames in device memory on `st`: parse, scan, one
-// host synchronisation for the block and step counts, then everything else enqueued.  b.dstCap may be null
-// (sizeOnly).
-// With fd: the dictionary flag is accepted, every frame decodes against its dictionary (none without b.dictBase),
-// and fd->outId, where given, gets the headers' IDs.
-cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, const FrameDict* fd = nullptr) {
+// The decode block table of nB rows: its columns, each rounded up to 16 bytes, carved from one allocation of P (all
+// null when it fails: P.err).
+k4::FrameTable frame_table(FramePool& P, int64_t nB) {
+    k4::FrameTable t{};
+    auto carve = [&](uint8_t* base) {            // base null: only the size
+        int64_t at = 0;
+        auto col = [&](auto*& c) {
+            c = base ? reinterpret_cast<std::remove_reference_t<decltype(c)>>(base + at) : nullptr;
+            at += (nB * (int64_t)sizeof(*c) + 15) & ~int64_t(15);
+        };
+        col(t.srcOff); col(t.fin); col(t.dst); col(t.cpySrc);
+        col(t.len); col(t.kind); col(t.sum); col(t.frame); col(t.idx); col(t.size);
+        col(t.cap); col(t.ilen); col(t.res); col(t.ckLen); col(t.got); col(t.cpyLen);
+        return at;
+    };
+    carve(P.get<uint8_t>(carve(nullptr)));
+    return t;
+}
+
+// The block pass of every whole-frame decode, after a reader's layout: the nB rows of t, which belong to m.n member
+// records fr.  Member i's content starts at m.dstBase + m.dstOff[i], its dictionary is m.dictBase[m.dictOff[i] ..
+// + m.dictLen[i]) (m.dictBase null: no dictionaries), its scratch slots start at scratchRel + fr[i].slot * slotUnit.
+// In order: the dictionaries' rows and slots, the stored copies (history for the linked blocks after them), the block
+// checksums, OP_DECODE of the independent blocks, the linked steps (step k: block k of every linked member), the
+// verdicts and the copy-back of independent blocks from their slots; then the members' content checksums (ccLen ->
+// ccGot).
+cudaError_t frame_decode_blocks(FramePool& P, const Batch& m, k4::FrameRec* fr, const k4::FrameTable& t, int64_t nB,
+                                int64_t slotUnit, int64_t scratchRel, int maxSteps, int32_t* ccLen, uint32_t* ccGot,
+                                cudaStream_t st) {
+    const int nm = (int)m.n;
+    const bool dict = m.dictBase;
+    int64_t* rowDictOff = nullptr;
+    int32_t* rowDictLen = nullptr;
+    if (dict) {
+        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
+        FR_TRY(P.err);
+        k4::frame_dict_layout_kernel<<<grid_of(nm), 128, 0, st>>>(fr, nm, t, m.dictOff, m.dictLen, rowDictOff,
+                                                                 rowDictLen, scratchRel, slotUnit);
+        FR_LAUNCH();
+        g_launches++;
+    }
+    if (nB > 0) {
+        const int nb = (int)nB;
+        FR_TRY(launch_op(OP_COPY, Batch{m.srcBase, t.cpySrc, t.cpyLen, m.dstBase, t.fin, nullptr, nullptr, nb}, st));
+        FR_TRY(launch_op(OP_XXH32, Batch{m.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
+        Batch ib{m.srcBase, t.srcOff, t.ilen, m.dstBase, t.dst, t.cap, t.res, nb};
+        if (dict) { ib.dictBase = m.dictBase; ib.dictOff = rowDictOff; ib.dictLen = rowDictLen; }
+        FR_TRY(launch_op(OP_DECODE, ib, st));
+        if (maxSteps > 0) {
+            k4::FrameStep s;
+            s.srcOff = P.get<int64_t>(nm); s.dstOff = P.get<int64_t>(nm); s.hSrc = P.get<int64_t>(nm);
+            s.hDst = P.get<int64_t>(nm); s.srcLen = P.get<int32_t>(nm); s.cap = P.get<int32_t>(nm);
+            s.prefix = P.get<int32_t>(nm); s.res = P.get<int32_t>(nm); s.hLen = P.get<int32_t>(nm);
+            k4::FrameStepDict sd{};
+            if (dict) { sd.src = P.get<int64_t>(nm); sd.dst = P.get<int64_t>(nm); sd.len = P.get<int32_t>(nm); }
+            FR_TRY(P.err);
+            for (int k = 0; k < maxSteps; k++) {
+                k4::frame_step_prepare_kernel<<<grid_of(nm), 128, 0, st>>>(k, fr, nm, t, s, m.dstOff, m.dictOff,
+                                                                          m.dictLen, sd);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{m.dstBase, s.hSrc, s.hLen, m.dstBase, s.hDst, nullptr, nullptr, nm}, st));
+                Batch cb{m.srcBase, s.srcOff, s.srcLen, m.dstBase, s.dstOff, s.cap, s.res, nm};
+                if (dict && k == 0) {          // block 0 against the dictionary itself
+                    cb.dictBase = m.dictBase; cb.dictOff = m.dictOff; cb.dictLen = m.dictLen;
+                    FR_TRY(launch_op(OP_DECODE, cb, st));
+                } else {
+                    if (dict) FR_TRY(launch_op(OP_COPY, Batch{m.dictBase, sd.src, sd.len, m.dstBase, sd.dst, nullptr, nullptr, nm}, st));
+                    cb.prefixLen = s.prefix;
+                    FR_TRY(launch_op(OP_CHAIN, cb, st));
+                }
+                k4::frame_step_commit_kernel<<<grid_of(nm), 128, 0, st>>>(k, fr, nm, t, s);
+                FR_LAUNCH();
+                g_launches++;
+                FR_TRY(launch_op(OP_COPY, Batch{m.dstBase, s.hSrc, s.hLen, m.dstBase, s.hDst, nullptr, nullptr, nm}, st));
+            }
+        }
+        k4::frame_verdict_kernel<<<grid_of(nB), 128, 0, st>>>(fr, t, nB);
+        FR_LAUNCH();
+        g_launches++;
+        FR_TRY(launch_op(OP_COPY, Batch{m.dstBase, t.cpySrc, t.cpyLen, m.dstBase, t.fin, nullptr, nullptr, nb}, st));
+    }
+    return launch_op(OP_XXH32, Batch{m.dstBase, m.dstOff, ccLen, nullptr, nullptr, nullptr, (int32_t*)ccGot, nm}, st);
+}
+
+// The reference's LZ4FrameReader over b.n frames in device memory on `st` (or, with sizeOnly, only their content
+// sizes): parse, scan, one host synchronisation for the block and step counts, the size walk and the layout, then the
+// block pass (frame_decode_blocks; a frame is its one member) and the finish.  b.dstCap may be null (sizeOnly).
+// dictFlag: the dictionary flag is accepted, and every frame decodes against its dictionary (an empty one without
+// b.dictBase); outId, where given, gets the headers' IDs.
+cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, bool dictFlag, int64_t* outId) {
     int dev = 0;
     cudaGetDevice(&dev);
     const Dev* D = dev_state(dev);
@@ -1312,7 +1420,7 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
     k4::FrameTotals* tot = P.get<k4::FrameTotals>(1);
     FR_TRY(P.err);
     FR_TRY(cudaMemsetAsync(tot, 0, sizeof(k4::FrameTotals), st));
-    auto parse = fd ? k4::frame_parse_dict_kernel : k4::frame_parse_kernel;
+    auto parse = dictFlag ? k4::frame_parse_dict_kernel : k4::frame_parse_kernel;
     parse<<<grid_of(n), 128, 0, st>>>(0, b.srcBase, b.srcOff, b.srcLen, n, fr, k4::FrameTable{}, tot);
     FR_LAUNCH();
     k4::frame_scan_kernel<<<1, 1024, 0, st>>>(fr, n, tot, sizeOnly ? 0 : 1);
@@ -1322,19 +1430,8 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
     FR_TRY(cudaMemcpyAsync(&h, tot, sizeof(h), cudaMemcpyDeviceToHost, st));
     FR_TRY(cudaStreamSynchronize(st));                 // the one wait: the table's size and the number of steps
     const int64_t nB = h.blocks;
-    uint8_t* rows = P.get<uint8_t>(nB * k4::FRAME_ROW_BYTES + 16 * 16);
+    const k4::FrameTable t = frame_table(P, nB);
     FR_TRY(P.err);
-    k4::FrameTable t;
-    {
-        uint8_t* p = rows;
-        auto take = [&](int64_t bytes) { uint8_t* q = p; p += (bytes + 15) & ~int64_t(15); return q; };
-        t.srcOff = (int64_t*)take(nB * 8); t.fin = (int64_t*)take(nB * 8); t.dst = (int64_t*)take(nB * 8);
-        t.cpySrc = (int64_t*)take(nB * 8);
-        t.len = (int32_t*)take(nB * 4); t.kind = (int32_t*)take(nB * 4); t.sum = (uint32_t*)take(nB * 4);
-        t.frame = (int32_t*)take(nB * 4); t.idx = (int32_t*)take(nB * 4); t.size = (int32_t*)take(nB * 4);
-        t.cap = (int32_t*)take(nB * 4); t.ilen = (int32_t*)take(nB * 4); t.res = (int32_t*)take(nB * 4);
-        t.ckLen = (int32_t*)take(nB * 4); t.got = (uint32_t*)take(nB * 4); t.cpyLen = (int32_t*)take(nB * 4);
-    }
     parse<<<grid_of(n), 128, 0, st>>>(1, b.srcBase, b.srcOff, b.srcLen, n, fr, t, nullptr);
     FR_LAUNCH();
     g_launches++;
@@ -1353,87 +1450,31 @@ cudaError_t frame_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, con
                                                        sizeOnly ? nullptr : b.dstCap, scratchRel, slotBytes, ccLen);
     FR_LAUNCH();
     g_launches++;
-    // the dictionaries: per frame (no dictionaries: empty ones) and per row
-    const uint8_t* dBase = b.dictBase;
-    const int64_t* dOff = b.dictOff;
-    const int32_t* dLen = b.dictLen;
-    int64_t* rowDictOff = nullptr;
-    int32_t* rowDictLen = nullptr;
-    if (fd && !sizeOnly) {
-        if (!dBase) {
-            int64_t* z = P.get<int64_t>(n);
-            FR_TRY(P.err);
-            FR_TRY(cudaMemsetAsync(z, 0, (size_t)n * 8, st));
-            dBase = b.srcBase; dOff = z; dLen = reinterpret_cast<const int32_t*>(z);
-        }
-        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
-        FR_TRY(P.err);
-        k4::frame_dict_layout_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, t, dOff, dLen, rowDictOff, rowDictLen,
-                                                                scratchRel, slotBytes);
-        FR_LAUNCH();
-        g_launches++;
-    }
-    if (!sizeOnly && nB > 0) {
-        const int nb = (int)nB;
-        // stored blocks first: they are history for the linked blocks after them
-        FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
-        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
-        Batch ib{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb};
-        if (fd) { ib.dictBase = dBase; ib.dictOff = rowDictOff; ib.dictLen = rowDictLen; }
-        FR_TRY(launch_op(OP_DECODE, ib, st));
-        if (h.maxSteps > 0) {
-            k4::FrameStep s;
-            s.srcOff = P.get<int64_t>(n); s.dstOff = P.get<int64_t>(n); s.hSrc = P.get<int64_t>(n); s.hDst = P.get<int64_t>(n);
-            s.srcLen = P.get<int32_t>(n); s.cap = P.get<int32_t>(n); s.prefix = P.get<int32_t>(n); s.res = P.get<int32_t>(n);
-            s.hLen = P.get<int32_t>(n);
-            k4::FrameStepDict sd{};
-            if (fd) { sd.src = P.get<int64_t>(n); sd.dst = P.get<int64_t>(n); sd.len = P.get<int32_t>(n); }
-            FR_TRY(P.err);
-            for (int k = 0; k < h.maxSteps; k++) {
-                if (fd) k4::frame_step_prepare_dict_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff, dOff, dLen, sd);
-                else k4::frame_step_prepare_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s, b.dstOff);
-                FR_LAUNCH();
-                g_launches++;
-                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, n}, st));
-                Batch cb{b.srcBase, s.srcOff, s.srcLen, b.dstBase, s.dstOff, s.cap, s.res, n};
-                if (fd && k == 0) {          // block 0 against the dictionary itself
-                    cb.dictBase = dBase; cb.dictOff = dOff; cb.dictLen = dLen;
-                    FR_TRY(launch_op(OP_DECODE, cb, st));
-                } else {
-                    if (fd) FR_TRY(launch_op(OP_COPY, Batch{dBase, sd.src, sd.len, b.dstBase, sd.dst, nullptr, nullptr, n}, st));
-                    cb.prefixLen = s.prefix;
-                    FR_TRY(launch_op(OP_CHAIN, cb, st));
-                }
-                k4::frame_step_commit_kernel<<<grid_of(n), 128, 0, st>>>(k, fr, n, t, s);
-                FR_LAUNCH();
-                g_launches++;
-                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, n}, st));
+    if (!sizeOnly) {
+        Batch m{b.srcBase, nullptr, nullptr, b.dstBase, b.dstOff, nullptr, nullptr, n};
+        if (dictFlag) {
+            m.dictBase = b.dictBase; m.dictOff = b.dictOff; m.dictLen = b.dictLen;
+            if (!b.dictBase) {
+                int64_t* z = P.get<int64_t>(n);
+                FR_TRY(P.err);
+                FR_TRY(cudaMemsetAsync(z, 0, (size_t)n * 8, st));
+                m.dictBase = b.srcBase; m.dictOff = z; m.dictLen = reinterpret_cast<const int32_t*>(z);
             }
         }
-        k4::frame_verdict_kernel<<<grid_of(nB), 128, 0, st>>>(fr, t, nB);
-        FR_LAUNCH();
-        g_launches++;
-        FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
+        FR_TRY(frame_decode_blocks(P, m, fr, t, nB, slotBytes, scratchRel, h.maxSteps, ccLen, ccGot, st));
     }
-    if (!sizeOnly)
-        FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, b.dstOff, ccLen, nullptr, nullptr, nullptr, (int32_t*)ccGot, n}, st));
     k4::frame_decode_finish_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, sizeOnly ? nullptr : b.dstCap,
-                                                              sizeOnly ? nullptr : ccGot, ccLen, b.outLen);
+                                                              sizeOnly ? nullptr : ccGot, ccLen, b.outLen, outId);
     FR_LAUNCH();
     g_launches++;
-    if (fd && fd->outId) {
-        k4::frame_info_kernel<<<grid_of(n), 128, 0, st>>>(fr, n, fd->outId);
-        FR_LAUNCH();
-        g_launches++;
-    }
     return cudaSuccess;
 }
 
 // Read (or, with sizeOnly, only size) b.n .lz4 streams in device memory on `st` as `lz4 -d` does (lz4f_read.cuh):
 // the member walk, the scans of each stream's blocks, scratch units and members, one host synchronisation for those
-// totals and the number of linked steps, then the members' blocks through frame_decode_dev's machinery and the
-// per-stream finish.  outErr / outEnd: the streams' error codes and end offsets.  With b.dictBase, every LZ4F member
-// decodes against its stream's dictionary.
+// totals and the number of linked steps, the size walk and the layout, then the block pass over the members
+// (frame_decode_blocks) and the per-stream finish.  outErr / outEnd: the streams' error codes and end offsets.  With
+// b.dictBase, every LZ4F member decodes against its stream's dictionary.
 cudaError_t lz4f_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, int32_t* outErr, int32_t* outEnd) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1470,19 +1511,8 @@ cudaError_t lz4f_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, int3
     mb.stream = P.get<int32_t>(nM); mb.code = P.get<int32_t>(nM); mb.key = P.get<unsigned long long>(nM);
     mb.size = P.get<uint64_t>(nM); mb.dst = P.get<int64_t>(nM);
     if (dict) { mb.dictOff = P.get<int64_t>(nM); mb.dictLen = P.get<int32_t>(nM); }
-    uint8_t* rows = P.get<uint8_t>(nB * k4::FRAME_ROW_BYTES + 16 * 16);
+    const k4::FrameTable t = frame_table(P, nB);
     FR_TRY(P.err);
-    k4::FrameTable t;
-    {
-        uint8_t* p = rows;
-        auto take = [&](int64_t bytes) { uint8_t* q = p; p += (bytes + 15) & ~int64_t(15); return q; };
-        t.srcOff = (int64_t*)take(nB * 8); t.fin = (int64_t*)take(nB * 8); t.dst = (int64_t*)take(nB * 8);
-        t.cpySrc = (int64_t*)take(nB * 8);
-        t.len = (int32_t*)take(nB * 4); t.kind = (int32_t*)take(nB * 4); t.sum = (uint32_t*)take(nB * 4);
-        t.frame = (int32_t*)take(nB * 4); t.idx = (int32_t*)take(nB * 4); t.size = (int32_t*)take(nB * 4);
-        t.cap = (int32_t*)take(nB * 4); t.ilen = (int32_t*)take(nB * 4); t.res = (int32_t*)take(nB * 4);
-        t.ckLen = (int32_t*)take(nB * 4); t.got = (uint32_t*)take(nB * 4); t.cpyLen = (int32_t*)take(nB * 4);
-    }
     walk(1, t);
     FR_LAUNCH();
     g_launches++;
@@ -1500,60 +1530,11 @@ cudaError_t lz4f_decode_dev(const Batch& b, bool sizeOnly, cudaStream_t st, int3
                                                        sizeOnly ? nullptr : b.dstCap, scratchRel, ccLen);
     FR_LAUNCH();
     g_launches++;
-    int64_t* rowDictOff = nullptr;
-    int32_t* rowDictLen = nullptr;
-    if (dict) {
-        rowDictOff = P.get<int64_t>(nB); rowDictLen = P.get<int32_t>(nB);
-        FR_TRY(P.err);
-        k4::frame_dict_layout_kernel<<<grid_of(nM), 128, 0, st>>>(fr, nm, t, mb.dictOff, mb.dictLen, rowDictOff,
-                                                                 rowDictLen, scratchRel, k4::LZ4F_SLOT_UNIT);
-        FR_LAUNCH();
-        g_launches++;
+    if (!sizeOnly) {
+        Batch m{b.srcBase, nullptr, nullptr, b.dstBase, mb.dst, nullptr, nullptr, nm};
+        if (dict) { m.dictBase = b.dictBase; m.dictOff = mb.dictOff; m.dictLen = mb.dictLen; }
+        FR_TRY(frame_decode_blocks(P, m, fr, t, nB, k4::LZ4F_SLOT_UNIT, scratchRel, h[0].maxSteps, ccLen, ccGot, st));
     }
-    if (!sizeOnly && nB > 0) {
-        const int nb = (int)nB;
-        // stored blocks first: they are history for the linked blocks after them
-        FR_TRY(launch_op(OP_COPY, Batch{b.srcBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
-        FR_TRY(launch_op(OP_XXH32, Batch{b.srcBase, t.srcOff, t.ckLen, nullptr, nullptr, nullptr, (int32_t*)t.got, nb}, st));
-        Batch ib{b.srcBase, t.srcOff, t.ilen, b.dstBase, t.dst, t.cap, t.res, nb};
-        if (dict) { ib.dictBase = b.dictBase; ib.dictOff = rowDictOff; ib.dictLen = rowDictLen; }
-        FR_TRY(launch_op(OP_DECODE, ib, st));
-        if (h[0].maxSteps > 0) {         // block k of every linked member, so a stream's frames decode in parallel
-            k4::FrameStep s;
-            s.srcOff = P.get<int64_t>(nM); s.dstOff = P.get<int64_t>(nM); s.hSrc = P.get<int64_t>(nM);
-            s.hDst = P.get<int64_t>(nM); s.srcLen = P.get<int32_t>(nM); s.cap = P.get<int32_t>(nM);
-            s.prefix = P.get<int32_t>(nM); s.res = P.get<int32_t>(nM); s.hLen = P.get<int32_t>(nM);
-            k4::FrameStepDict sd{};
-            if (dict) { sd.src = P.get<int64_t>(nM); sd.dst = P.get<int64_t>(nM); sd.len = P.get<int32_t>(nM); }
-            FR_TRY(P.err);
-            for (int k = 0; k < h[0].maxSteps; k++) {
-                if (dict) k4::frame_step_prepare_dict_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s, mb.dst, mb.dictOff, mb.dictLen, sd);
-                else k4::frame_step_prepare_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s, mb.dst);
-                FR_LAUNCH();
-                g_launches++;
-                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, nm}, st));
-                Batch cb{b.srcBase, s.srcOff, s.srcLen, b.dstBase, s.dstOff, s.cap, s.res, nm};
-                if (dict && k == 0) {          // block 0 against the dictionary itself
-                    cb.dictBase = b.dictBase; cb.dictOff = mb.dictOff; cb.dictLen = mb.dictLen;
-                    FR_TRY(launch_op(OP_DECODE, cb, st));
-                } else {
-                    if (dict) FR_TRY(launch_op(OP_COPY, Batch{b.dictBase, sd.src, sd.len, b.dstBase, sd.dst, nullptr, nullptr, nm}, st));
-                    cb.prefixLen = s.prefix;
-                    FR_TRY(launch_op(OP_CHAIN, cb, st));
-                }
-                k4::frame_step_commit_kernel<<<grid_of(nM), 128, 0, st>>>(k, fr, nm, t, s);
-                FR_LAUNCH();
-                g_launches++;
-                FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, s.hSrc, s.hLen, b.dstBase, s.hDst, nullptr, nullptr, nm}, st));
-            }
-        }
-        k4::frame_verdict_kernel<<<grid_of(nB), 128, 0, st>>>(fr, t, nB);
-        FR_LAUNCH();
-        g_launches++;
-        FR_TRY(launch_op(OP_COPY, Batch{b.dstBase, t.cpySrc, t.cpyLen, b.dstBase, t.fin, nullptr, nullptr, nb}, st));
-    }
-    if (!sizeOnly && nM > 0)
-        FR_TRY(launch_op(OP_XXH32, Batch{b.dstBase, mb.dst, ccLen, nullptr, nullptr, nullptr, (int32_t*)ccGot, nm}, st));
     k4::lz4f_finish_kernel<<<grid_of(n), 128, 0, st>>>(n, ss, fr, mb, t, sizeOnly ? nullptr : b.dstCap,
                                                        sizeOnly ? nullptr : ccGot, ccLen, b.outLen, outErr, outEnd);
     FR_LAUNCH();
@@ -1705,24 +1686,25 @@ cudaError_t frame_encode_dev(const Batch& b, const k4::FrameFormat& f, cudaStrea
 
 enum FrameOp { FO_ENCODE, FO_DECODE, FO_SIZE };
 
-// f: the format of an encode (unused by the decode calls).
-cudaError_t frame_dev(FrameOp fo, const Batch& b, const k4::FrameFormat& f, cudaStream_t st, const FrameDict* fd) {
+// f: the format of an encode, rd: how a decode reads (each unused by the other).
+cudaError_t frame_dev(FrameOp fo, const Batch& b, const k4::FrameFormat& f, cudaStream_t st, const FrameRead& rd) {
     if (fo == FO_ENCODE && b.level >= 3) {
         k4::frame_fill_kernel<<<grid_of(b.n), 128, 0, st>>>(b.outLen, (int)b.n, K4LZ4_R_DELEGATE);
         g_launches++;
         return cudaGetLastError();
     }
-    if (fd && fd->lz4f) return lz4f_decode_dev(b, fo == FO_SIZE, st, fd->outErr, fd->outEnd);
-    return fo == FO_ENCODE ? frame_encode_dev(b, f, st) : frame_decode_dev(b, fo == FO_SIZE, st, fd);
+    if (fo == FO_ENCODE) return frame_encode_dev(b, f, st);
+    if (rd.lz4f) return lz4f_decode_dev(b, fo == FO_SIZE, st, rd.outErr, rd.outEnd);
+    return frame_decode_dev(b, fo == FO_SIZE, st, rd.dictFlag, rd.outId);
 }
 
 // Host memory, one GPU, synchronous: chunks of whole frames (a frame is never split: its linked blocks and its
 // content checksum need all of it) through the device's staging, the device path on each, on the legacy default
 // stream.  The device region of a frame is min(dstCap, frame bound) when encoding (a frame never needs more) and
 // dstCap when decoding; content sizes have none.  With dictionaries, each distinct one of a chunk is staged once,
-// only its last 64 KiB (all that encode and decode read); an encode's dictIDs travel in the rows' aux column, and the
-// info call's IDs come back behind the sizes.
-int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, const FrameDict* fd) {
+// only its last 64 KiB (all that encode and decode read); an encode's dictIDs travel in the rows' aux column, and a
+// decode's extra columns (FrameRead::columns) come back behind the sizes.
+int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, FrameRead rd) {
     DeviceGuard guard(dev);
     if (!guard.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", dev);
     if (fo == FO_ENCODE && b.level >= 3) {
@@ -1744,7 +1726,7 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
     auto dkey = [&](int64_t i) { return std::make_pair(b.dictBase + b.dictOff[i] + (b.dictLen[i] - dlen(i)), dlen(i)); };
     std::map<std::pair<const uint8_t*, int32_t>, int64_t> first;   // a chunk's first row of each distinct dictionary
     std::vector<int64_t> from;
-    const bool ids = fd && fd->outId, lz4f = fd && fd->lz4f;
+    const int64_t words = rd.staged([](auto*&, int64_t) {});     // per entry: outLen and the extra columns
     std::vector<int32_t> res;
     for (int64_t i = 0, j; i < b.n; i = j) {
         int64_t bytes = 0;
@@ -1765,9 +1747,7 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
         }
         const int64_t nb = j - i;
         StageUp up;
-        // the info call: the int64 IDs at res + 2 nb; the lz4f calls: the errors at res + nb, the ends at res + 2 nb
-        const int64_t resInts = ids ? 4 : lz4f ? 3 : 1;
-        int rc = stage_up(D->stage, nb, resInts, 0, [&](int64_t k) {
+        int rc = stage_up(D->stage, nb, words, 0, [&](int64_t k) {
             const int64_t x = i + k, s = src_size(b, x), r = room(x);
             UpRow u{b.srcBase + b.srcOff[x], s, r, 0, (int32_t)s, (int32_t)r, f.dictId ? (int32_t)f.dictId[x] : 0,
                     dst ? b.dstBase + b.dstOff[x] : nullptr};
@@ -1782,43 +1762,35 @@ int frame_host(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int dev, co
         if (dict) { kb.dictBase = up.blob; kb.dictOff = up.blobOff; kb.dictLen = up.blobLen; }
         k4::FrameFormat kf = f;
         kf.dictId = f.dictId ? reinterpret_cast<const uint32_t*>(up.aux) : nullptr;
-        FrameDict kd;
-        kd.outId = ids ? reinterpret_cast<int64_t*>(up.res + 2 * nb) : nullptr;
-        kd.lz4f = lz4f;
-        if (lz4f) { kd.outErr = up.res + nb; kd.outEnd = up.res + 2 * nb; }
-        const cudaError_t e = frame_dev(fo, kb, kf, nullptr, fd ? &kd : nullptr);
+        FrameRead kr = rd;
+        kr.staged([&](auto*& p, int64_t at) { p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(up.res + at * nb); });
+        const cudaError_t e = frame_dev(fo, kb, kf, nullptr, kr);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
-        res.resize((size_t)(nb * resInts));
-        rc = stage_down(D->stage, up, nb, ids || lz4f ? res.data() : b.outLen + i, resInts, dst ? up.dst : nullptr, up.dstOff,
+        res.resize((size_t)(nb * words));
+        rc = stage_down(D->stage, up, nb, words > 1 ? res.data() : b.outLen + i, words, dst ? up.dst : nullptr, up.dstOff,
                         nullptr, nullptr);
         if (rc != K4LZ4_OK) return rc;
-        if (ids) {
+        if (words > 1) {
             memcpy(b.outLen + i, res.data(), (size_t)nb * 4);
-            memcpy(fd->outId + i, res.data() + 2 * nb, (size_t)nb * 8);
-        }
-        if (lz4f) {
-            memcpy(b.outLen + i, res.data(), (size_t)nb * 4);
-            memcpy(fd->outErr + i, res.data() + nb, (size_t)nb * 4);
-            memcpy(fd->outEnd + i, res.data() + 2 * nb, (size_t)nb * 4);
+            rd.staged([&](auto*& p, int64_t at) { memcpy(p + i, res.data() + at * nb, (size_t)nb * sizeof(*p)); });
         }
     }
     return K4LZ4_OK;
 }
 
 // Every frame export: its own arguments (an encode's: bs = 0 where its format refuses them), then the batch's
-// (check()), then host or device.  An encode whose format reads dictionaries requires them; the info call (fd with
-// FO_SIZE) its ID array.
+// (check()), then host or device.  An encode whose format reads dictionaries requires them; a decode, the columns it
+// returns beside outLen (FrameRead::columns).
 int frame_run(FrameOp fo, const Batch& b, const k4::FrameFormat& f, int memKind, void* stream, int device,
-              const FrameDict* fd = nullptr) {
+              FrameRead rd = {}) {
     if (fo == FO_ENCODE && !f.bs) return fail(K4LZ4_E_ARG, "bad frame block size %d or flags", f.bdSize);
-    const bool missing = fo == FO_ENCODE ? f.dict && !b.dictBase
-                       : fd && fd->lz4f ? !fd->outErr || !fd->outEnd : fo == FO_SIZE && fd && !fd->outId;
+    const bool missing = fo == FO_ENCODE ? f.dict && !b.dictBase : rd.missing();
     const int rc = check(fo == FO_ENCODE ? OP_ENCODE : fo == FO_SIZE ? OP_USIZE : OP_DECODE, b, memKind, device, missing);
     if (rc != K4LZ4_OK || b.n == 0) return rc;
-    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, f, device < 0 ? 0 : device, fd);
+    if (memKind == K4LZ4_MEM_HOST) return frame_host(fo, b, f, device < 0 ? 0 : device, rd);
     DeviceGuard g(device);
     if (!g.ok) return fail(K4LZ4_E_CUDA, "cudaSetDevice(%d) failed", device);
-    const cudaError_t e = frame_dev(fo, b, f, (cudaStream_t)stream, fd);
+    const cudaError_t e = frame_dev(fo, b, f, (cudaStream_t)stream, rd);
     if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(K4LZ4_E_CUDA, "frame call: %s", cudaGetErrorString(e)); }
     return K4LZ4_OK;
 }
@@ -3014,16 +2986,17 @@ int32_t k4lz4_frame_decode_dict_batch(const uint8_t* srcBase, const int64_t* src
                                       int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nFrames};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
-    FrameDict fd;
-    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+    FrameRead rd;
+    rd.dictFlag = true;
+    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, rd);
 }
 
 int32_t k4lz4_frame_info_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen, int32_t* outSize,
                                int64_t* outDictId, int32_t nFrames, int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nFrames};
-    FrameDict fd;
-    fd.outId = outDictId;
-    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+    FrameRead rd;
+    rd.dictFlag = true; rd.ids = true; rd.outId = outDictId;
+    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, rd);
 }
 
 int32_t k4lz4_lz4f_decompress_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
@@ -3033,18 +3006,18 @@ int32_t k4lz4_lz4f_decompress_batch(const uint8_t* srcBase, const int64_t* srcOf
                                     int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, dstBase, dstOff, dstCap, outLen, nStreams};
     b.dictBase = dictBase; b.dictOff = dictOff; b.dictLen = dictLen;
-    FrameDict fd;
-    fd.lz4f = true; fd.outErr = outErr; fd.outEnd = outEnd;
-    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+    FrameRead rd;
+    rd.lz4f = true; rd.outErr = outErr; rd.outEnd = outEnd;
+    return frame_run(FO_DECODE, b, k4::FrameFormat{}, memKind, cudaStream, device, rd);
 }
 
 int32_t k4lz4_lz4f_decompressed_size_batch(const uint8_t* srcBase, const int64_t* srcOff, const int32_t* srcLen,
                                            int32_t* outSize, int32_t* outErr, int32_t* outEnd, int32_t nStreams,
                                            int32_t memKind, void* cudaStream, int32_t device) {
     Batch b{srcBase, srcOff, srcLen, nullptr, nullptr, nullptr, outSize, nStreams};
-    FrameDict fd;
-    fd.lz4f = true; fd.outErr = outErr; fd.outEnd = outEnd;
-    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, &fd);
+    FrameRead rd;
+    rd.lz4f = true; rd.outErr = outErr; rd.outEnd = outEnd;
+    return frame_run(FO_SIZE, b, k4::FrameFormat{}, memKind, cudaStream, device, rd);
 }
 
 int32_t k4lz4_frame_writer_group_create(int32_t nStreams, int32_t blockSize, int32_t flags, int32_t level,

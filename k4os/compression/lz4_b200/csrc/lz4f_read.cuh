@@ -1,7 +1,9 @@
 // lz4f_read.cuh -- reading .lz4 streams as upstream's `lz4 -d` does (k4lz4_lz4f_decompress_batch,
-// k4lz4_lz4f_decompressed_size_batch): the member walk, the layout over a stream's members and the per-stream finish.
-// The blocks themselves go through frame.cuh's machinery (block_size_walk_kernel, the stored copies, OP_DECODE, the
-// linked steps, xxh32, frame_verdict_kernel) with one FrameRec per decodable member.
+// k4lz4_lz4f_decompressed_size_batch): the front end of the whole-frame decode for upstream's rules -- the member
+// walk, the layout over a stream's members and the per-stream finish.  The blocks themselves go through
+// block_size_walk_kernel and the block pass that the reference's frames use too (frame_decode_blocks in
+// k4lz4_api.cu: the stored copies, block XXH32, OP_DECODE, the linked steps, frame_verdict_kernel), with one FrameRec
+// per decodable member.
 //
 // The rules are upstream's: selectDecoder / LZ4IO_decompressLZ4F / LZ4IO_decodeLegacyStream (programs/lz4io.c) over
 // LZ4F_decompress_usingDict (lib/lz4frame.c).  A stream is read member by member:
@@ -254,7 +256,7 @@ __global__ void lz4f_walk_kernel(int pass, const uint8_t* __restrict__ srcBase, 
 }
 
 // One thread per stream, after block_size_walk_kernel: each member's place in the stream's destination (behind the
-// members before it), then frame_layout_kernel's work for its blocks with the member's capacity (maxBlockSize, or
+// members before it), then its blocks' placement (frame_place_row) with the member's capacity (maxBlockSize, or
 // 8 MiB for legacy runs) and its own scratch units.  A block whose walk gives more than that capacity fails as the
 // decoder would.  A stream whose content exceeds dstCap is skipped: nothing of it is written.  dstCap null: sizes.
 __global__ void lz4f_layout_kernel(int n, Lz4fStreams ss, FrameRec* __restrict__ fr, Lz4fMembers mb, FrameTable t,
@@ -287,15 +289,9 @@ __global__ void lz4f_layout_kernel(int n, Lz4fStreams ss, FrameRec* __restrict__
             const bool scratch = dstCap && !skip && !raw && pos + cap > room;
             int64_t at = base + pos;
             if (scratch) at = scratchRel + r.slot * LZ4F_SLOT_UNIT + (linked ? 0 : k - r.k0) * unit + FR_HIST;
-            t.fin[b] = base + pos;
-            t.dst[b] = at;
-            t.cap[b] = cap;
-            t.kind[b] = (t.kind[b] & (RK_RAW | RK_LINKED)) | (scratch ? RK_SCRATCH : 0) | (skip ? RK_SKIP : 0);
-            t.ilen[b] = (!skip && !raw && !linked) ? L : 0;
-            t.cpyLen[b] = (!skip && raw) ? L : 0;
-            t.cpySrc[b] = t.srcOff[b];
-            t.ckLen[b] = bc ? L : 0;        // also when skipped: a block checksum needs no decoding
-            t.res[b] = 0;
+            // the block checksum also when skipped: it needs no decoding, and lz4f_finish_kernel reports its mismatch
+            frame_place_row(t, b, L, raw, linked, skip, scratch, base + pos, at, cap, (!skip && raw) ? L : 0,
+                            bc ? L : 0);
             pos += sz;
         }
         fr[m].pos = pos - start;
